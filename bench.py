@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- short-term feature_extraction throughput on B200 (BASELINE.json metric).
+"""bench.py -- short-term feature_extraction throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload (config.workload): BASELINE.json configs[1] -- 1000 synthetic 16 kHz mono int16 10 s clips per
 GPU, window/step 50/25 ms, full 68-row short-term feature matrix.  One "step" = the whole hot path
@@ -13,9 +13,14 @@ gather fused into the kernel's stores).
 Prints ONE JSON line (rank 0).  `value` = frames/s with inputs resident in HBM; `e2e` = the same metric
 through the C ABI's host entry point b200aa_st_features_host (pinned host clips in, pinned host features
 out, copies inside the timed region); `roofline` = algorithmic bytes / kernel time of the fused kernel
-against the measured HBM peak (plus the FP32-issue fraction of the committed ncu capture);
-`cpu_baseline` = the unmodified reference (staged under oracle/_ref by oracle/make_ref.py) on the host
-cores, one single-threaded process per physical core, bounded sample.
+against the HBM peak; `gpu` = the card's name and power limit; `cpu_baseline` = the unmodified reference
+(staged under oracle/_ref by oracle/make_ref.py) on the host cores, one single-threaded process per physical
+core, bounded sample.
+`--dump-outputs DIR` writes what the last timed step computed (rank 0): DIR/features.npy = a fixed, seeded sample
+of DUMP_CLIPS clips of the [clips, 68, T] float32 feature tensor (with N > 1: of the gathered [N * clips, 68, T]
+tensor), DIR/clip_index.npy = their clip indices (float64: the dump format allows float32 / float64 only; exact for
+any index), DIR/clip_norm.npy = the clip statistics records of rank 0's clips (float32 [clips, 8]; every rank keeps
+its own).  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -37,6 +42,7 @@ WORKLOAD = "1000 synthetic 16 kHz mono int16 10 s clips per GPU, win/step 50/25 
 CONFIG = {"workload": WORKLOAD, "fs": FS, "window": WINDOW, "step": STEP, "clip_samples": CLIP_SAMPLES,
           "clips_per_gpu": CLIPS_PER_GPU, "frames_per_clip": FRAMES_PER_CLIP, "n_features": 68,
           "parallelism": "clips sharded per GPU, feature matrices gathered on rank 0"}
+DUMP_CLIPS, DUMP_SEED = 256, 0      # 256 x 68 x 399 float32 = 27.8 MB
 
 
 # ----------------------------------------------------------------------------- CPU baseline (unmodified reference)
@@ -219,24 +225,19 @@ class ClockSampler:
         return {"sm_mhz": s[len(s) // 2] if s else None, "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
                 "samples": len(s)}
 
+    def power_limit_w(self):
+        try:
+            return self.nv.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
+        except Exception:
+            return None
+
 
 def hbm_peak():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_facts():
-    """Figures of the committed `ncu --set full` capture of the fused kernel (profiles/traffic.json): DRAM bytes per
-    launch, warp instructions per launch, issue-slot utilisation.  Static by nature (a profiler cannot run inside
-    the timed region); the file names the capture they come from."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return {}
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 # ----------------------------------------------------------------------------- reference arm
@@ -307,6 +308,7 @@ def run_ours(args, rank, world, local_rank):
     copy_stream = torch.cuda.Stream(dev) if world > 1 else None
 
     ev = lambda: torch.cuda.Event(enable_timing=True)     # noqa: E731
+    last = {}                                             # the last step's clip statistics and feature tensor (--dump-outputs)
 
     def timed(mode, steps, record_kernel=False):
         """`steps` passes in gather mode `mode` ('ce' | 'p2p_store' | 'none' | 'nccl'); returns (ms total max over ranks, kernel ms)."""
@@ -335,6 +337,8 @@ def run_ours(args, rank, world, local_rank):
             ks[i].record()
             pkg.feature_extraction_batch(clips, FS, WINDOW, STEP, deltas=True, out=out, norm=norm, plan=plan)
             ke[i].record()
+            last["norm"] = norm
+            last["out"] = gathers[i % 2].view(0, world * B) if (mode in ("ce", "p2p_store") and world > 1) else out
             if mode == "ce" and world > 1 and rank != 0:
                 copy_stream.wait_event(ke[i])
                 gathers[i % 2].push(out, rank * B, stream=copy_stream)
@@ -362,11 +366,15 @@ def run_ours(args, rank, world, local_rank):
     with ClockSampler(local_rank) as clk:
         ms_total, kernel_ms = timed(main_mode, args.steps)
         launches = L.b200aa_launch_count() - launches0          # our kernels launched inside the timed region
+        if args.dump_outputs and rank == 0:
+            dumped = dump_sample(last["out"], last["norm"])     # device-side copies, enqueued behind the last step
         # keep the sampler alive for a few more identical steps if the timed region was very short
         t_end = time.time() + 0.25
         while time.time() < t_end and len(clk.samples) < 8:
             pkg.feature_extraction_batch(clips, FS, WINDOW, STEP, deltas=True, out=local_out, plan=plan)
             torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        save_dump(args.dump_outputs, *dumped)                     # host copies and files outside the clock sampler
     ms_per_step = ms_total / args.steps
     frames_per_step = world * B * T
     value = frames_per_step / (ms_per_step * 1e-3)
@@ -389,8 +397,7 @@ def run_ours(args, rank, world, local_rank):
                                           "kernel_store_gather": ms_store / args.steps},
                           "root_ingress_bytes_per_step": gather_bytes,
                           "root_ingress_GBps": gather_bytes / (ms_per_step * 1e-3) / 1e9,
-                          "limiter": "root NVLink ingress: (N-1) blocks of 108.5 MB per step against ~770 GB/s measured per direction "
-                                     "(at N = 8 the gather, not the kernels, sets the step time)"}
+                          "limiter": "root NVLink ingress: (N-1) blocks of 108.5 MB per step"}
         # the gathered tensor on the root holds every rank's block (spot check against the local result)
         timed("ce", 2)
         if rank == 0:
@@ -437,26 +444,18 @@ def run_ours(args, rank, world, local_rank):
     peak, peak_src = hbm_peak()
     alg_bytes = B * ALG_BYTES_PER_CLIP
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
-    nf = ncu_facts()
-    inst = nf.get("st_kernel_warp_instructions_per_launch")
-    sm_clock_hz = 1e6 * (clk.summary()["sm_mhz"] or 1965)
-    issue_frac = (inst / (kernel_ms * 1e-3) / (148 * 4 * sm_clock_hz)) if inst else None
     line = {"metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": max(3, args.warmup),
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic", "impl": "ours", "config": CONFIG,
-            "detail": {"l2": "inputs larger than L2 (320 MB int16 clips + 108 MB output per step vs 126 MB L2); no explicit flush",
+            "detail": {"l2": "inputs larger than L2 (320 MB int16 clips + 108 MB output per step vs 50 MB L2); no explicit flush",
                        "kernel_kind": plan.kernel_kind(), "numa": bound,
                        **({"lib_override": os.environ["B200AA_LIB"]} if os.environ.get("B200AA_LIB") else {})},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": nf.get("st_kernel_dram_bytes_per_launch"), "traffic_source": nf.get("source"),
                          "peak_source": peak_src, "kernel": "fused short-term feature kernel",
                          "kernel_ms": kernel_ms, "algorithmic_bytes_per_launch": alg_bytes,
-                         "binding_bound": "fp32_issue",
-                         "fp32_issue_frac": issue_frac, "inst_per_frame": (inst / (B * T)) if inst else None,
-                         "issue_slot_utilisation_ncu": nf.get("st_kernel_issue_slot_utilisation"),
-                         "note": "the kernel is instruction-issue bound, not HBM bound (DESIGN.md): ~30 kFLOP per 1074 B frame; "
-                                 "fp32_issue_frac = warp instructions per launch (ncu capture) / kernel time / (148 SMs x 4 "
-                                 "schedulers x SM clock)"},
+                         "note": "HBM is not the expected bound (DESIGN.md): ~30 kFLOP per 1074 B frame is above the FP32 ridge "
+                                 "(67 TFLOP/s / 3.35 TB/s = 20 FLOP/B, H100 SXM data sheet); issue utilisation not measured"},
+            "gpu": {"name": torch.cuda.get_device_name(dev), "power_limit_w": clk.power_limit_w()},
             "clocks": clk.summary(), "e2e": e2e, "gpu_launches": int(launches)}
     if scaling_detail:
         line["scaling_detail"] = scaling_detail
@@ -469,14 +468,41 @@ def run_ours(args, rank, world, local_rank):
         dist.destroy_process_group()
 
 
+def dump_sample(feats, norm):
+    """Device-side copies of the last timed step's outputs (see the module docstring): the seeded clip sample of the
+    features, its clip indices, the clip statistics records."""
+    import numpy as np
+    import torch
+    n = feats.shape[0]
+    idx = np.sort(np.random.default_rng(DUMP_SEED).choice(n, size=min(n, DUMP_CLIPS), replace=False))
+    return feats[torch.from_numpy(idx).to(feats.device)], idx, norm.view(torch.float32).clone()   # uint8 [B, 32] = float32 [B, 8]
+
+
+def save_dump(path, sample, idx, norm):
+    """Writes dump_sample's arrays as DIR/<name>.npy."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "features.npy"), sample.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(path, "clip_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(path, "clip_norm.npy"), norm.cpu().numpy())
+
+
+def positive_int(v):
+    n = int(v)
+    if n < 1:
+        raise argparse.ArgumentTypeError("must be >= 1")
+    return n
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=positive_int, default=200, help="timed steps")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg (profiling runs)")
-    ap.add_argument("--no-e2e", action="store_true", help="skip the host-pipeline leg (profiling runs under ncu)")
+    ap.add_argument("--no-e2e", action="store_true", help="skip the host-pipeline leg (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,5 +1,5 @@
 /*
- * b200aa.h -- C ABI of libb200aa.so, the B200 (sm_100a) short-term / mid-term audio
+ * b200aa.h -- C ABI of libb200aa.so, the H100 (sm_90a) short-term / mid-term audio
  * feature extractor that replaces pyAudioAnalysis' NumPy hot path.
  *
  * Boundary rules: extern "C", plain pointers and sizes, no C++ / torch types, no
@@ -36,7 +36,7 @@ typedef enum b200aa_status {
                                      (ShortTermFeatures.py:230-231)                                       */
     B200AA_ERR_CUDA = -5,         /* a CUDA call failed; see b200aa_last_cuda_error()                     */
     B200AA_ERR_UNSUPPORTED = -6,  /* window too large for the on-chip transform buffers                  */
-    B200AA_ERR_NO_DEVICE = -7     /* no CUDA device / not an sm_100 device                                */
+    B200AA_ERR_NO_DEVICE = -7     /* no CUDA device / not an sm_90 device                                 */
 } b200aa_status;
 
 /* sample formats of the clip buffer */
@@ -64,7 +64,7 @@ typedef struct b200aa_plan b200aa_plan;   /* opaque: constant tables of one (fs,
 int         b200aa_abi_version(void);
 const char *b200aa_status_string(int status);
 const char *b200aa_last_cuda_error(void);        /* thread-local text of the last CUDA failure */
-int         b200aa_device_ok(void);              /* B200AA_OK iff the current device is sm_100 */
+int         b200aa_device_ok(void);              /* B200AA_OK iff the current device is sm_90 */
 
 /* ------------------------------------------------------------------ host tables -------
  * Pure host code, usable without a GPU (the CPU test-suite checks them against the oracle).

@@ -1,10 +1,10 @@
-"""B200-native drop-in for pyAudioAnalysis' short-term / mid-term feature path.
+"""H100-native drop-in for pyAudioAnalysis' short-term / mid-term feature path.
 
     from pyaudioanalysis_b200 import ShortTermFeatures, MidTermFeatures
 
 mirror ``pyAudioAnalysis.ShortTermFeatures.{feature_extraction, spectrogram, chromagram}`` and
 ``pyAudioAnalysis.MidTermFeatures.mid_feature_extraction`` (same names, arguments, return
-values and error behaviour) on top of hand-written sm_100a CUDA (``libb200aa.so``, C ABI in
+values and error behaviour) on top of hand-written sm_90a CUDA (``libb200aa.so``, C ABI in
 ``include/b200aa.h``).  ``install()`` rebinds those attributes on an imported pyAudioAnalysis.
 There is no CPU fallback.
 """

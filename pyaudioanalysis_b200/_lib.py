@@ -1,6 +1,6 @@
 """ctypes binding of libb200aa.so (the C ABI declared in include/b200aa.h).
 
-There is no CPU fallback: if the library is missing or the device is not a B200-class GPU the
+There is no CPU fallback: if the library is missing or the device is not an H100-class (sm_90) GPU the
 calls raise.  The library itself is pure C ABI; torch is only used by callers for device memory.
 """
 import ctypes

@@ -1,7 +1,7 @@
 """Batched device API: [B, N] clips resident in HBM -> feature tensors resident in HBM.
 
 torch supplies device memory and the current stream; every operation is a C-ABI call into
-libb200aa.so (hand-written sm_100a kernels).  Nothing here computes on the CPU.
+libb200aa.so (hand-written sm_90a kernels).  Nothing here computes on the CPU.
 """
 import ctypes
 

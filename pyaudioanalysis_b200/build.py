@@ -1,4 +1,4 @@
-"""Compile libb200aa.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Compile libb200aa.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -10,7 +10,7 @@ SOURCES = ["b200aa.cu"]
 DEPS = ["b200aa.cu", "common.cuh", "dft_codelets.cuh", "generic_kernel.cuh", "fast_kernel.cuh", "pair_kernel.cuh", "solo_kernel.cuh", "sched.cuh", "tables.inl",
         os.path.join("..", "..", "include", "b200aa.h")]
 
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-shared", "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 

@@ -1,5 +1,5 @@
-// libb200aa.so -- C ABI (include/b200aa.h) over the sm_100a kernels.
-// Build: see pyaudioanalysis_b200/build.py (nvcc -gencode arch=compute_100a,code=sm_100a).
+// libb200aa.so -- C ABI (include/b200aa.h) over the sm_90a kernels.
+// Build: see pyaudioanalysis_b200/build.py (nvcc -gencode arch=compute_90a,code=sm_90a).
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>      // header-only NVTX 3: ranges around the entry points (visible in nsys / ncu timelines)
 
@@ -66,7 +66,7 @@ extern "C" const char *b200aa_status_string(int s)
     case B200AA_ERR_MEL_RANGE: return "mel filterbank: filter edge beyond num_fft";
     case B200AA_ERR_CUDA: return "CUDA error";
     case B200AA_ERR_UNSUPPORTED: return "window too large for the on-chip transform";
-    case B200AA_ERR_NO_DEVICE: return "no sm_100 CUDA device";
+    case B200AA_ERR_NO_DEVICE: return "no sm_90 CUDA device";
     default: return "unknown status";
     }
 }
@@ -77,7 +77,7 @@ extern "C" int b200aa_device_ok(void)
     if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return B200AA_ERR_NO_DEVICE; }
     cudaDeviceProp pr;
     if (cudaGetDeviceProperties(&pr, dev) != cudaSuccess) { cudaGetLastError(); return B200AA_ERR_NO_DEVICE; }
-    return pr.major == 10 ? B200AA_OK : B200AA_ERR_NO_DEVICE;
+    return (pr.major == 9 && pr.minor == 0) ? B200AA_OK : B200AA_ERR_NO_DEVICE;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -573,7 +573,7 @@ extern "C" int b200aa_clip_stats(const void *d_sig, int dtype, int64_t n_clips, 
     if (!d_sig || !d_norm || n_clips < 0 || n_samples < 0 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
     if (n_clips == 0) return B200AA_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 0;
     CK(cudaGetDevice(&dev));
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int tb = 256;

@@ -1,4 +1,4 @@
-// Small forward DFT codelets on register arrays (compile-time trigonometry, Blackwell FP32x2 butterflies).
+// Small forward DFT codelets on register arrays (compile-time trigonometry, lane-wise float2 butterflies).
 // Shared by the register-tiled kernel (fast_kernel.cuh) and the butterfly passes of the generic kernel.
 #pragma once
 #include "common.cuh"
@@ -58,22 +58,41 @@ __host__ __device__ constexpr int cx_modinv(int a, int m)
 // ----------------------------------------------------------------------------------------------
 // small forward DFTs on register arrays
 // ----------------------------------------------------------------------------------------------
-// Blackwell packed FP32: one FADD2 / FFMA2 instruction handles the (re, im) pair (sm_100 FP32x2 datapath)
-// (the codelets are __host__ __device__ so that tests/test_codelets_cpu.py can run them on the CPU; host code and
-// -DB200AA_NO_F32X2 builds use the scalar forms)
-#if !defined(B200AA_NO_F32X2) && defined(__CUDA_ARCH__)
-__device__ __forceinline__ float2 f2add(float2 a, float2 b) { return __fadd2_rn(a, b); }
-// a - b as one FFMA2 (b * -1 + a: the same single rounding); FADD2 has no per-operand negation, the negated copy cost two
-// extra instructions per subtraction (3 % of the pair kernel's instructions, profiles/pair_r2_v1)
-__device__ __forceinline__ float2 f2sub(float2 a, float2 b) { return __ffma2_rn(b, make_float2(-1.f, -1.f), a); }
-__device__ __forceinline__ float2 f2fma(float c, float2 a, float2 acc) { return __ffma2_rn(make_float2(c, c), a, acc); }
-__device__ __forceinline__ float2 f2mulc(float c, float2 a) { return __fmul2_rn(make_float2(c, c), a); }
+// Lane-wise (re, im) arithmetic: f2add / f2sub / f2mul / f2fma, each with one rounding per lane; a float first operand of
+// f2mul / f2fma multiplies both lanes.  sm_90 has no packed FP32x2 instructions, so each helper is two scalar FP32
+// instructions; on the device they are the explicitly rounded intrinsics, which nvcc never contracts across helpers (a
+// product from f2mul is rounded before the f2add that consumes it).
+// (the codelets are __host__ __device__ so that tests/test_codelets_cpu.py can run them on the CPU with plain arithmetic)
+__host__ __device__ __forceinline__ float2 f2add(float2 a, float2 b)
+{
+#ifdef __CUDA_ARCH__
+    return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #else
-__host__ __device__ __forceinline__ float2 f2add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__host__ __device__ __forceinline__ float2 f2sub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-__host__ __device__ __forceinline__ float2 f2fma(float c, float2 a, float2 acc) { return make_float2(fmaf(c, a.x, acc.x), fmaf(c, a.y, acc.y)); }
-__host__ __device__ __forceinline__ float2 f2mulc(float c, float2 a) { return make_float2(c * a.x, c * a.y); }
+    return make_float2(a.x + b.x, a.y + b.y);
 #endif
+}
+__host__ __device__ __forceinline__ float2 f2sub(float2 a, float2 b)
+{
+#ifdef __CUDA_ARCH__
+    return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y));
+#else
+    return make_float2(a.x - b.x, a.y - b.y);
+#endif
+}
+__host__ __device__ __forceinline__ float2 f2mul(float2 a, float2 b)
+{
+#ifdef __CUDA_ARCH__
+    return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+#else
+    return make_float2(a.x * b.x, a.y * b.y);
+#endif
+}
+__host__ __device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c)
+{
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+__host__ __device__ __forceinline__ float2 f2mul(float c, float2 a) { return f2mul(make_float2(c, c), a); }
+__host__ __device__ __forceinline__ float2 f2fma(float c, float2 a, float2 acc) { return f2fma(make_float2(c, c), a, acc); }
 
 template <int RA, int RB> __host__ __device__ __forceinline__ void fft_pfa(float2 (&v)[RA * RB]);
 template <int RA, int RB> __host__ __device__ __forceinline__ void fft_ct(float2 (&v)[RA * RB]);
@@ -216,7 +235,7 @@ __host__ __device__ __forceinline__ void fft_r(float2 (&v)[R])
 // ----------------------------------------------------------------------------------------------
 // 32-point forward FFT in "two sequences per register pair" form (pair kernel, pass 2).
 // Input: re[m] = (Re x[2m], Re x[2m+1]), im[m] = (Im x[2m], Im x[2m+1]), m < 16 -- the .x halves are the even-indexed
-// samples, the .y halves the odd-indexed ones.  Both 16-point sub-transforms run in the same FP32x2 instructions
+// samples, the .y halves the odd-indexed ones.  Both 16-point sub-transforms run in the same float2 operations
 // (identical twiddles, real constants broadcast to both halves; multiplying by -i is a swap of roles, not an
 // instruction), then X[k] = E[k] + W32^k O[k], X[k+16] = E[k] - W32^k O[k] in scalar FMAs.  ~280 instructions
 // instead of ~440 for the generic (re, im)-packed Cooley-Tukey codelet.
@@ -242,8 +261,8 @@ __host__ __device__ __forceinline__ void soa_twiddle(Soa2 &x)
         const float2 t = x.re; x.re = x.im; x.im = make_float2(-t.x, -t.y);
     } else {
         constexpr float wr = float(cx_cos_turn(e, Q)), wi = float(-cx_sin_turn(e, Q));
-        const float2 r = f2fma(-wi, x.im, f2mulc(wr, x.re));
-        const float2 i = f2fma(wr, x.im, f2mulc(wi, x.re));
+        const float2 r = f2fma(-wi, x.im, f2mul(wr, x.re));
+        const float2 i = f2fma(wr, x.im, f2mul(wi, x.re));
         x.re = r; x.im = i;
     }
 }

@@ -4,7 +4,7 @@
 // The real frame is packed into Nc = R1*R2 complex points z[n] = x[2n] + i x[2n+1] and transformed as an
 // R1 x R2 two-pass FFT: every pass is one small FFT per thread held entirely in registers (prime-factor
 // 4x5 / 3x7 / 2x5 / 3x4 / 3x5 butterflies without internal twiddles, 4x4 Cooley-Tukey for 16; all
-// constants are immediates, butterflies use the sm_100 FP32x2 instructions), with one padded shared-memory
+// constants are immediates, butterflies on float2 (re, im) pairs), with one padded shared-memory
 // transpose between the passes.  max(R1, R2) threads own a frame; 8 frames per CTA step.  Post-processing
 // computes |X[k]| and |X[Nc-k]| from one (Z[k], Z[Nc-k]) pair, so only half of the second-pass outputs
 // travel through shared memory.  Samples arrive by TMA (cp.async.bulk + mbarrier) one step ahead.
@@ -63,7 +63,7 @@ struct DenseLane {
 };
 // ----------------------------------------------------------------------------------------------
 // Half-warp variant of the dense pass: 16 lanes per frame (a warp handles two frames), every lane holds
-// C2 = odd(ceil(K/32)) float2 pairs of consecutive bins, per-bin arithmetic on the FP32x2 pipe.  The
+// C2 = odd(ceil(K/32)) float2 pairs of consecutive bins, per-bin arithmetic on float2 pairs.  The
 // fixed per-frame overhead (reductions, scalar math, stores) is paid once per two frames.
 // ----------------------------------------------------------------------------------------------
 template <int K>
@@ -135,7 +135,7 @@ __device__ __forceinline__ void spectral_features_h(const float *X, const float 
         sx += t;
         s1 = fmaf(float(2 * j + 1), t, s1);          // (2j+1) a + (2j+2) b = (2j+1)(a+b) + b
         sb += x2[j].y;
-        const float2 sq = __fmul2_rn(x2[j], x2[j]);
+        const float2 sq = f2mul(x2[j], x2[j]);
         if (j < dlv.x) plo2 = f2add(plo2, sq); else phi2 = f2add(phi2, sq);
     }
     const float plo = plo2.x + plo2.y, phi = phi2.x + phi2.y, part = plo + phi;
@@ -172,10 +172,10 @@ __device__ __forceinline__ void spectral_features_h(const float *X, const float 
     float run = incl - part, below = 0.f;
 #pragma unroll
     for (int j = 0; j < C2; ++j) {
-        sp2 = __ffma2_rn(__fmul2_rn(d2, d2), x2[j], sp2);
+        sp2 = f2fma(f2mul(d2, d2), x2[j], sp2);
         d2 = f2add(d2, dstep);
-        const float2 df = __ffma2_rn(x2[j], nx2, __fmul2_rn(Xp2[j], mnp2));
-        fl2 = __ffma2_rn(df, df, fl2);
+        const float2 df = f2fma(x2[j], nx2, f2mul(Xp2[j], mnp2));
+        fl2 = f2fma(df, df, fl2);
         // padding bins never count: at the last real bin the running sum equals sxx > thr (or everything is 0)
         run = fmaf(x2[j].x, x2[j].x, run);
         below += run > thr ? 0.f : 1.f;
@@ -917,8 +917,7 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
     occ = occ < 1 ? 1 : occ;
     const int64_t slots = int64_t(sm_count) * occ;
     // work items: >= ~8 per CTA slot for balance, as long as possible to amortise the 2-frame halo, and
-    // seg + 2 a multiple of the 8-frame CTA step so no step runs half empty (scan on B200, 1000 x 399 frames:
-    // seg 30: 1.207 ms, 46: 1.176, 62: 1.165, 102: 1.159, 134: 1.175, 399: 1.240)
+    // seg + 2 a multiple of the 8-frame CTA step so no step runs half empty
     int64_t per_clip = (slots * 8 + p.n_clips - 1) / p.n_clips;
     if (per_clip < 1) per_clip = 1;
     int64_t seg = (T + per_clip - 1) / per_clip;

@@ -29,13 +29,10 @@
 
 namespace b200aa {
 
-// Resident warps per SM.  Measured on B200 (1000 x 10 s @16 kHz, 800 / 400; profiles/ab_diet_r2.jsonl), CTAs x warps:
-//   2 x 8 at 128 registers (round 2's first layout, 11.9 KB of shared memory per warp) 0.904 ms;  the 9.6 KB layout below:
-//   2 x 8 (128 regs) 0.916   2 x 10 (96 regs; 3+3+2+2 warps per scheduler and CTA) 0.923   1 x 22 (80 regs, spills) 0.874
-//   1 x 20 (96 regs, five warps per scheduler) 0.824  <- what the 800-sample window gets (22 warps would fit).  Warps per CTA
-//   stay a multiple of four: a CTA's warps go round-robin to the four schedulers of the SM.  The shorter windows fit 24 warps
-//   (80 registers, no spills to speak of): 640 / 320 0.868 -> 0.851 ms, 512 / 256 1.024 -> 0.984, 320 / 160 1.236 -> 1.191
-//   (profiles/ab_solo_r2.jsonl); 960 and 1024 samples run 16 warps at 128 registers.
+// Resident warps per SM: one CTA per SM, 20 warps (five per scheduler, 96 registers) for the 800-sample window.  Measured on
+// an H100 80GB HBM3 (700 W; 1000 x 10 s @16 kHz, 800 / 400, scripts/ab_run.py): 1 x 20 1.026 ms, 1 x 16 at 128 registers
+// (no spills) 1.077 ms.  Warps per CTA stay a multiple of four: a CTA's warps go round-robin to the four schedulers of the
+// SM.  The shorter windows fit 24 warps (80 registers); 960 and 1024 samples run 16 warps at 128 registers.
 #ifndef B200AA_PAIR_MAXWARPS
 #define B200AA_PAIR_MAXWARPS 24
 #endif
@@ -44,8 +41,8 @@ constexpr int kPairMaxWarps = B200AA_PAIR_MAXWARPS;     // warps per CTA (each o
 #define B200AA_PAIR_MINBLOCKS 1
 #endif
 constexpr int kPairMinBlocks = B200AA_PAIR_MINBLOCKS;   // one CTA per SM: the twiddle / mel / DCT / chroma tables exist once per SM
-// the solo kernel's feature layout (solo_kernel.cuh): config 3 (64 x 60 s @44.1 kHz, 882 / 441) 2 x 8 warps 1.162 ms, 1 x 20 1.067,
-// 1 x 24 (80 registers, no spills) 1.075; 400 / 160 on the bench batch 1.808 / 1.625 / 1.599
+// the solo kernel's feature layout (solo_kernel.cuh): one CTA of 24 warps at 80 registers; config 3 (64 x 60 s @44.1 kHz,
+// 882 / 441) on an H100 80GB HBM3 (700 W): 1 x 24 1.297 ms, 1 x 16 1.281 ms (within the spread of one run)
 #ifndef B200AA_SOLO_MAXWARPS
 #define B200AA_SOLO_MAXWARPS 24
 #endif
@@ -181,13 +178,13 @@ __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, f
         sx += t;
         s1 = fmaf(float(2 * j + 1), t, s1);
         sb += x2[j].y;
-        const float2 sq = __fmul2_rn(x2[j], x2[j]);
+        const float2 sq = f2mul(x2[j], x2[j]);
         if constexpr ((Lb % 2) == 0) {                   // block boundaries fall between (even, odd) bin pairs
             if (2 * j < dlv.x) plo2 = f2add(plo2, sq); else phi2 = f2add(phi2, sq);
         } else {                                         // power-of-two windows: a boundary may split a pair
             const float2 m = make_float2(2 * j < dlv.x ? 1.f : 0.f, 2 * j + 1 < dlv.x ? 1.f : 0.f);
-            plo2 = __ffma2_rn(sq, m, plo2);
-            phi2 = __ffma2_rn(sq, make_float2(1.f - m.x, 1.f - m.y), phi2);
+            plo2 = f2fma(sq, m, plo2);
+            phi2 = f2fma(sq, make_float2(1.f - m.x, 1.f - m.y), phi2);
         }
     }
     const float plo = plo2.x + plo2.y, phi = phi2.x + phi2.y, part = plo + phi;
@@ -241,7 +238,7 @@ __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, f
         for (int t = 0; t < PER; ++t) {
             const int idx = l * PER + t;
             const float2 xc = idx < C2 ? reinterpret_cast<const float2 *>(X)[cl * C2 + idx] : make_float2(0.f, 0.f);
-            sq[t] = __fmul2_rn(xc, xc);
+            sq[t] = f2mul(xc, xc);
             pre += sq[t].x + sq[t].y;
         }
 #pragma unroll
@@ -265,10 +262,10 @@ __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, f
 #endif
 #pragma unroll
     for (int j = 0; j < C2; ++j) {
-        sp2 = __ffma2_rn(__fmul2_rn(d2, d2), x2[j], sp2);
+        sp2 = f2fma(f2mul(d2, d2), x2[j], sp2);
         d2 = f2add(d2, dstep);
-        const float2 df = __ffma2_rn(x2[j], nx2, __fmul2_rn(Xp2[j], mnp2));
-        fl2 = __ffma2_rn(df, df, fl2);
+        const float2 df = f2fma(x2[j], nx2, f2mul(Xp2[j], mnp2));
+        fl2 = f2fma(df, df, fl2);
 #ifdef B200AA_ROLLOFF_SEQ
         run = fmaf(x2[j].x, x2[j].x, run);
         below += run > thr ? 0.f : 1.f;
@@ -419,7 +416,7 @@ __device__ __forceinline__ void td_frame(const float (&u)[R], float cm, const b2
 }
 
 // The same accumulation for BOTH frames of a pair at once (they cover the same rows): u[r] = (sample of a, sample of b),
-// e2[i] = (block sum of a, block sum of b) -- the arithmetic runs in FP32x2 instructions, only the sign masks stay per frame.
+// e2[i] = (block sum of a, block sum of b) -- the arithmetic runs on float2 pairs, only the sign masks stay per frame.
 template <int R, bool FULL, bool TWO>
 __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b200aa_clip_norm &nm, int lane,
                                         float2 *e2 /* [NE] */, int &flips_a, int &link_a, int &flips_b, int &link_b)
@@ -432,7 +429,7 @@ __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b2
     const float2 ncm = make_float2(-cm, -cm), a2 = make_float2(nm.a, nm.a), bp2 = make_float2(nm.bp, nm.bp);
 #pragma unroll
     for (int r = Td::ZROW0; r < R; ++r) {
-        const float2 d = __fadd2_rn(u[r], ncm);
+        const float2 d = f2add(u[r], ncm);
         const unsigned Pa = __ballot_sync(0xffffffffu, d.x > nm.lo), Pb = __ballot_sync(0xffffffffu, d.y > nm.lo);
         unsigned Qa = 0u, Qb = 0u;
         if (TWO) { Qa = __ballot_sync(0xffffffffu, d.x < nm.hi); Qb = __ballot_sync(0xffffffffu, d.y < nm.hi); }
@@ -449,18 +446,18 @@ __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b2
                 fa += __popc(cQa); fb += __popc(cQb);
                 if (!FULL && r == Td::ROW0) { la += int((cQa >> Td::LANE0) & 1u); lb += int((cQb >> Td::LANE0) & 1u); }
             }
-            const float2 y = __ffma2_rn(a2, d, bp2);
+            const float2 y = f2fma(a2, d, bp2);
             const bool live = !(r == Td::ROW0 && Td::LANE0 > 0) || lane >= Td::LANE0;
             const int b0 = (n0 / Lt) < 10 ? (n0 / Lt) : 10;
             const int end = b0 < 10 ? (b0 + 1) * Lt : N;
             const int thr = end - n0;
             const int i0 = b0 - Td::EB, i1 = (b0 + 1 < 10 ? b0 + 1 : 10) - Td::EB;
             if (thr >= 32) {
-                if (i0 >= 0 && i0 < Td::NE) { if (live) e2[i0] = __ffma2_rn(y, y, e2[i0]); }
+                if (i0 >= 0 && i0 < Td::NE) { if (live) e2[i0] = f2fma(y, y, e2[i0]); }
             } else {
                 const bool first = lane < thr;
-                if (i0 >= 0 && i0 < Td::NE) { if (live && first) e2[i0] = __ffma2_rn(y, y, e2[i0]); }
-                if (i1 >= 0 && i1 < Td::NE) { if (live && !first) e2[i1] = __ffma2_rn(y, y, e2[i1]); }
+                if (i0 >= 0 && i0 < Td::NE) { if (live && first) e2[i0] = f2fma(y, y, e2[i0]); }
+                if (i1 >= 0 && i1 < Td::NE) { if (live && !first) e2[i1] = f2fma(y, y, e2[i1]); }
             }
         }
         pPa = Pa; pQa = Qa; pPb = Pb; pQb = Qb;
@@ -677,7 +674,7 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
         const int q1 = qe < NP ? qe : NP;
         // samples: lane l holds samples 32 r + l of both frames of a pair, as exact floats M0 + x.
         // (Measured and rejected: issuing the loads of pair q + 1 in the middle of step q -- the 50 extra live registers
-        // cost more in spills than the hidden latency gains, 0.94 vs 0.89 ms.)
+        // cost more in spills than the hidden latency gains.)
         auto load_pair = [&](int qq, unsigned int (&wa)[R], unsigned int (&wb)[R]) {
             const int ta_ = 2 * qq, tb_ = (ta_ + 1 < T) ? ta_ + 1 : ta_;          // an odd tail pairs the last frame with itself
             if (is16) {
@@ -696,7 +693,7 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
             const bool store = q >= q0;
             const int ta = 2 * q;
             const bool bvalid = ta + 1 < T;
-            float2 uab[R];                      // (sample of a, sample of b) per row: FP32x2 operands
+            float2 uab[R];                      // (sample of a, sample of b) per row: float2 operands
             {
                 unsigned int wa[R], wb[R];
                 load_pair(q, wa, wb);
@@ -816,8 +813,8 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
                 float2 zz = make_float2(0.f, 0.f);
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
-                    z[r] = __ffma2_rn(uab[r], s2, o2);
-                    zz = __ffma2_rn(z[r], z[r], zz);
+                    z[r] = f2fma(uab[r], s2, o2);
+                    zz = f2fma(z[r], z[r], zz);
                 }
                 // A constant frame must come out as exact zeros (the reference's float64 spectrum is ~1e-17 there, and
                 // log10(. + eps) makes that visible): its partner would otherwise leak ~1e-7 of its own level into it
@@ -832,7 +829,7 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
                 }
             }
             __syncwarp();
-            // ---- pass 2 (lane = k1, 32 points over n2, even / odd n2 side by side in FP32x2) -> Z[k1 + R k2] in natural order
+            // ---- pass 2 (lane = k1, 32 points over n2, even / odd n2 side by side in float2) -> Z[k1 + R k2] in natural order
             {
                 float2 v[32];
                 {

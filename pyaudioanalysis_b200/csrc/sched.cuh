@@ -4,9 +4,7 @@
 // contiguous share [w total / W, (w + 1) total / W) and takes it from the front, `chunk` pairs per atomic; a warp that runs
 // dry takes the BACK half of the largest remainder it finds among 256 descriptors at a time and goes on from there.  A
 // contiguous run needs the one-pair halo (flux and the deltas look one frame back) only where it starts, so the redundant
-// work is one pair step per warp and per steal: ~2 % of the steps for BASELINE configs[1] on 2 960 resident warps, where
-// the run lists of round 2's first scheduler (long runs first, short runs last) spent 9.7 %.  Measured (1000 x 10 s @16 kHz,
-// 800 / 400, 20 warps per SM): 0.824 -> 0.796 ms.  What it took to get there (profiles/README.md, DESIGN.md): the scans
+// work is one pair step per warp and per steal.  What it took to get there (DESIGN.md): the scans
 // below must be cheap (the first version's last-warp scans cost more than the halos saved) and every branch must hang on a
 // vote, or ptxas stops trusting the warp's convergence in the step loop that follows.
 //

@@ -124,7 +124,7 @@ __device__ __forceinline__ void td_rows(const float2 (&u)[SoloShape<L, R2>::RT],
 #pragma unroll
     for (int r = 0; r < RT; ++r) {
         const bool live = r < RT - 1 || lane < S::LASTV;
-        const float2 d = __fadd2_rn(u[r], ncm);
+        const float2 d = f2add(u[r], ncm);
         const unsigned Pa = __ballot_sync(0xffffffffu, live && d.x > nm.lo), Pb = __ballot_sync(0xffffffffu, live && d.y > nm.lo);
         unsigned Qa = 0u, Qb = 0u;
         if (TWO) { Qa = __ballot_sync(0xffffffffu, live && d.x < nm.hi); Qb = __ballot_sync(0xffffffffu, live && d.y < nm.hi); }
@@ -136,18 +136,18 @@ __device__ __forceinline__ void td_rows(const float2 (&u)[SoloShape<L, R2>::RT],
             fa += __popc((Qa ^ __funnelshift_l(pQa, Qa, 1)) & valid);
             fb += __popc((Qb ^ __funnelshift_l(pQb, Qb, 1)) & valid);
         }
-        const float2 y = __ffma2_rn(a2, d, bp2);
+        const float2 y = f2fma(a2, d, bp2);
         const int n0 = 32 * r;
         const int b0 = (n0 / Lt) < 10 ? (n0 / Lt) : 10;
         const int end = b0 < 10 ? (b0 + 1) * Lt : N;
         const int thr = end - n0;
         const int i0 = b0, i1 = (b0 + 1 < 10 ? b0 + 1 : 10);
         if (thr >= 32) {
-            if (i0 < S::NE) { if (live) e2[i0] = __ffma2_rn(y, y, e2[i0]); }
+            if (i0 < S::NE) { if (live) e2[i0] = f2fma(y, y, e2[i0]); }
         } else {
             const bool first = lane < thr;
-            if (i0 < S::NE) { if (live && first) e2[i0] = __ffma2_rn(y, y, e2[i0]); }
-            if (i1 < S::NE) { if (live && !first) e2[i1] = __ffma2_rn(y, y, e2[i1]); }
+            if (i0 < S::NE) { if (live && first) e2[i0] = f2fma(y, y, e2[i0]); }
+            if (i1 < S::NE) { if (live && !first) e2[i1] = f2fma(y, y, e2[i1]); }
         }
         pPa = Pa; pQa = Qa; pPb = Pb; pQb = Qb;
     }
@@ -318,13 +318,13 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
 #pragma unroll
                     for (int n1 = 0; n1 < R2; ++n1) {
                         const int64_t m = s0 + 2 * (L * n1 + n2);
-                        z[n1] = __fadd2_rn(make_float2(s16(m), s16(m + 1)), nu0);
+                        z[n1] = f2add(make_float2(s16(m), s16(m + 1)), nu0);
                     }
                 } else {
 #pragma unroll
                     for (int n1 = 0; n1 < R2; ++n1) {
                         const int64_t m = s0 + 2 * (L * n1 + n2);
-                        z[n1] = __fadd2_rn(make_float2(s32(m), s32(m + 1)), nu0);
+                        z[n1] = f2add(make_float2(s32(m), s32(m + 1)), nu0);
                     }
                 }
             };
@@ -409,7 +409,7 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
                 }
             } else {
                 // row modes: rows the reference's loop never reaches are zeros and touch no sample.  (Measured and rejected:
-                // fetching the samples of both frames before the first transform -- 0.685 vs 0.570 ms for config 3's spectrogram.)
+                // fetching the samples of both frames before the first transform: slower for config 3's spectrogram.)
                 float *const g0 = MODE == kModeSpectrogram ? p.out + (size_t(b) * p.rows_total + p.row0 + ta) * K : nullptr;
 #pragma unroll 1
                 for (int f = 0; f < 2; ++f) {

@@ -8,8 +8,7 @@ the only exchange is the final gather of the per-rank [clips, F, T] blocks on on
   (``b200aa_peer_copy``): no collective kernel, no SMs taken on either side, and in a loop the push of batch i rides
   under the kernels of batch i + 1;
 * ``gather="p2p_store"``: the feature kernel writes its slice of the mapped buffer directly (gather fused into the tile
-  store).  Free at 2 GPUs, but 32-byte remote stores from 7 GPUs into one root collapse to ~220 GB/s of ingress at 8
-  (profiles/bench_r2_n8_fused.json), so it is not the default;
+  store); its 32-byte remote stores from many GPUs converge on one root, so it is not the default;
 * ``gather="nccl"`` / gloo: ``torch.distributed.gather`` of padded blocks (the baseline, and what the CPU tests run).
 """
 import ctypes

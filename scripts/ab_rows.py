@@ -1,5 +1,5 @@
 import sys, os, json, torch
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pyaudioanalysis_b200 as pkg
 from pyaudioanalysis_b200.batch import clip_stats
 g = torch.Generator(device="cuda"); g.manual_seed(3)

@@ -19,7 +19,7 @@ def _nvcc():
 @pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
 def test_codelets_and_shapes_on_host(tmp_path):
     exe = str(tmp_path / "codelets_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_100a", "-o", exe, os.path.join(ROOT, "tests", "codelets_host.cu")],
+    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "codelets_host.cu")],
                          capture_output=True, text=True)
     assert res.returncode == 0, res.stderr
     run = subprocess.run([exe], capture_output=True, text=True)

@@ -14,7 +14,7 @@ def P():
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     import pyaudioanalysis_b200 as pkg
     from pyaudioanalysis_b200 import _lib
-    assert _lib.lib().b200aa_device_ok() == 0, "not an sm_100 device"
+    assert _lib.lib().b200aa_device_ok() == 0, "not an sm_90 device"
     pkg.ShortTermFeatures.PRINT_SPECTROGRAM_SHAPE = False
     return pkg
 

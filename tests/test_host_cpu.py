@@ -24,25 +24,28 @@ def test_beat_extraction_matches_reference_golden():
         assert ratio == pytest.approx(float(g["ratio_%d" % i]), rel=1e-12, abs=1e-15), i
 
 
-def test_beat_extraction_against_imported_reference():
-    from oracle.ref_import import reference_available, load_reference
-    if not reference_available():
-        pytest.skip("reference tree not present")
-    S, M, A = load_reference()
-    if not hasattr(np, "Inf"):
-        np.Inf, np.NaN = np.inf, np.nan
-    from pyaudioanalysis_b200.MidTermFeatures import beat_extraction, _peak_positions
-    U = sys.modules["pyAudioAnalysis.utilities"]
+def peak_inputs():
+    """(signal, delta, feature matrix) of the peak-picking comparison, seeded."""
     rng = np.random.default_rng(3)
+    out = []
     for k in range(6):
         v = np.cumsum(rng.standard_normal(400)) * (0.1 + k)
         delta = 2.0 * np.abs(np.diff(v)).mean()
-        assert _peak_positions(v, delta) == [int(p) for p in U.peakdet(v, delta)[0]]
-        st = np.cumsum(rng.standard_normal((34, 200 + 30 * k)), axis=1)
-        for win in (0.05, 0.025, 0.1):
-            assert beat_extraction(st, win) == pytest.approx(M.beat_extraction(st, win), rel=1e-12)
+        out.append((v, delta, np.cumsum(rng.standard_normal((34, 200 + 30 * k)), axis=1)))
+    return out
+
+
+def test_beat_extraction_against_imported_reference():
+    """utilities.peakdet / MidTermFeatures.beat_extraction of the unmodified reference on seeded random walks
+    (tests/golden/reference_checks.npz, oracle/make_golden_reference_checks.py)."""
+    from pyaudioanalysis_b200.MidTermFeatures import beat_extraction, _peak_positions
+    g = load_golden("reference_checks.npz")
+    for k, (v, delta, st) in enumerate(peak_inputs()):
+        assert _peak_positions(v, delta) == [int(p) for p in g["p%d_peaks" % k]]
+        for j, win in enumerate((0.05, 0.025, 0.1)):
+            assert beat_extraction(st, win) == pytest.approx(tuple(g["p%d_beat" % k][j]), rel=1e-12)
     flat = np.ones((34, 100))
-    assert beat_extraction(flat, 0.05) == pytest.approx(M.beat_extraction(flat, 0.05))
+    assert beat_extraction(flat, 0.05) == pytest.approx(tuple(g["flat_beat"]))
 
 
 def _write_wav(path, data, fs, extra_chunk=False):
