@@ -806,7 +806,11 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
             float sa, isa, sb, isb;
             frame_scale(Ea, inv_a2n, sa, isa);
             frame_scale(Eb, inv_a2n, sb, isb);
-            bool a_flat, b_flat;        // every sample equals the frame's first one: the spectrum is exactly zero beyond DC
+            // an odd tail pairs the last frame with itself, and with shared halves Eb came from the ring as if b were the
+            // next frame: a scale from it would bury frame a under its own copy (a loud first half and a quiet second
+            // half put 40 dB between them and mfcc 10x outside the tolerance)
+            if (!bvalid) { sb = sa; isb = isa; }
+            bool a_flat, b_flat;       // every sample equals the frame's first one: the spectrum is exactly zero beyond DC
             {
                 float2 z[R];
                 const float2 s2 = make_float2(sa, sb), o2 = make_float2(-u0a * sa, -u0b * sb);

@@ -16,6 +16,7 @@ sys.path.insert(0, ROOT)
 import pyaudioanalysis_b200 as pkg                      # noqa: E402
 from pyaudioanalysis_b200._lib import Plan             # noqa: E402
 from oracle import st_oracle as O                      # noqa: E402  (checker only)
+from tests import signals as SG                        # noqa: E402
 
 NAMES = O.feature_names(True)
 
@@ -55,26 +56,16 @@ def main():
                 continue
             got = pkg.feature_extraction_batch(d, fs, w, s, plan=pl)[0].cpu().numpy()
             ok &= report("fs=%d w=%d s=%d n=%d kernel %d(%d)" % (fs, w, s, n, kind, pl.kernel_kind()), got, ref, w // 2)
-    # quiet / loud neighbours, silence, DC offset, float input, integer mean (two-sided sign masks)
-    rng = np.random.default_rng(5)
-    x = (rng.normal(0, 3, 40000)).round().astype(np.int16)
-    x[8000:16000] += (8000 * np.sin(np.arange(8000) * 0.21)).astype(np.int16)
-    x[20000:24000] = 0
-    x[30000:] = 11
-    x -= np.int16(round(float(x.mean())))
-    specials = {"quiet/loud/silence": x, "zero mean (two-sided)": (x - np.int16(round(float(x.mean())))).astype(np.int16),
-                "all zero": np.zeros(8000, np.int16), "constant": np.full(8000, 1234, np.int16)}
-    sym = np.concatenate([np.arange(-2000, 2000), np.arange(2000, -2000, -1)]).astype(np.int16)       # mean exactly 0 -> lo == hi
-    specials["integer mean"] = np.tile(sym, 4)
-    for name, xx in specials.items():
-        ref = O.feature_extraction(xx, 16000, 800, 400)[0]
+    # the adversarial signal bank of the test suite (tests/signals.py), int16 and float32
+    bank = dict(SG.bank(16000, 800, 400))
+    bank.update(SG.float_bank(16000, 800, 400))
+    for name, xx in bank.items():
+        ref = SG.patch_noise_defined(O.feature_extraction(xx.astype(np.float64) if xx.dtype == np.float32 else xx, 16000, 800, 400)[0],
+                                     xx, 800, 400)[0]
         d = torch.from_numpy(xx).cuda()[None]
         for kind in (2, 1):
             got = pkg.feature_extraction_batch(d, 16000, 800, 400, plan=Plan(16000, 800, 400).prefer_kernel(kind))[0].cpu().numpy()
             ok &= report("%s kernel %d" % (name, kind), got, ref, 400)
-    xf = (O.synth_clip(3, 30000, 16000).astype(np.float32) * 0.37 + 11.5)
-    got = pkg.feature_extraction_batch(torch.from_numpy(xf).cuda()[None], 16000, 800, 400, plan=Plan(16000, 800, 400).prefer_kernel(2))[0].cpu().numpy()
-    ok &= report("float32 input kernel 2", got, O.feature_extraction(xf.astype(np.float64), 16000, 800, 400)[0], 400)
     # batch / ragged / split independence
     clips = np.stack([O.synth_clip(i, 32000, 16000) for i in range(5)])
     d = torch.from_numpy(clips).cuda()

@@ -7,21 +7,68 @@ mfcc_2..13 and every delta column are differences of near-equal numbers -- see S
 Two rows are discrete: zcr moves in quanta of 0.5/(w-1) and spectral_rolloff in quanta of 1/K; a
 float32-vs-float64 tie may move them by one quantum on a small fraction of frames, which is
 counted and bounded separately.
+
+The absolute term makes the feature check blind below ~1e-5: a quiet frame's energy (~1e-8) passes whatever its value.
+Two row checks close that: ``check_energy_relative`` holds the energy row to RTOL with a negligible floor, and
+``check_zcr_exact`` holds the zcr row of integer input to float32 rounding of the exact count.
 """
 import numpy as np
 
 RTOL, ATOL = 1e-4, 1e-5
-ROLLOFF_ROW = 7
+ZCR_ROW, ENERGY_ROW, ROLLOFF_ROW = 0, 1, 7
 MAX_FLIP_FRACTION = 2e-3
+ENERGY_ATOL = 1e-12
+
+# Known departures from the standard tolerance.  Each entry: the signal of tests/signals.py it applies to, the kernel
+# kinds (2 pair, 3 solo, 1 CTA, 0 generic), the rows, the bound on max err / tol in those rows, and the ratio measured
+# on one H100 80GB HBM3 (400 W power limit) by tests/test_gpu_adversarial.py.  Every other (signal, kernel, row) is held
+# to the standard tolerance.  Constant frames are not an exception: their noise-defined reference values are replaced
+# by the exact ones (tests/signals.patch_noise_defined).
+EXCEPTIONS = [
+    {"signal": "chirp_f32", "kinds": (3,), "rows": (13, 47), "bound": 2.0, "measured": 1.52,
+     "reason": "float32 input, a chirp near 0.45 fs at 44.1 kHz: one frame's mfcc_6 (and its delta) near zero, where the "
+               "absolute term governs, off by 2.0e-5 through the solo kernel's packed-real transform"},
+    {"signal": "edge_impulses_f32", "kinds": (2,), "rows": (42,), "bound": 2.0, "measured": 1.13,
+     "reason": "float32 input, window 960: one delta mfcc_1 near zero off by 1.15e-5 through the pair kernel"},
+    {"signal": "small_f32", "kinds": (0, 2), "rows": (7, 41), "bound": 182.0, "measured": 181.8,
+     "reason": "float32 input at 1e-3 full scale, window 960: a float32 tie moves one frame's rolloff by one quantum (1/K, "
+               "39.5x the tolerance), and its delta on both sides; one flip counts three times against the flip limit"},
+    {"signal": "edge_impulses", "kinds": (1,), "rows": (7, 41), "bound": 501.0, "measured": 500.0,
+     "reason": "window 400, hop 200: a float32 tie moves one frame's rolloff by one quantum through the CTA kernel (50x the "
+               "tolerance) and its delta on both sides (500x); one flip counts three times against the flip limit"},
+]
 
 
-def check_features(gpu, ref, K, what=""):
+def exception_bounds(signal, kind):
+    """{row: bound on err / tol} of the EXCEPTIONS entries for one signal through one kernel kind."""
+    out = {}
+    for e in EXCEPTIONS:
+        if e["signal"] == signal and kind in e["kinds"]:
+            for r in e["rows"]:
+                out[r] = max(out.get(r, 1.0), e["bound"])
+    return out
+
+
+def err_ratio(gpu, ref):
+    """err / tol per entry under the standard tolerance."""
+    gpu = np.asarray(gpu, dtype=np.float64)
+    ref = np.asarray(ref, dtype=np.float64)
+    return np.abs(gpu - ref) / (RTOL * np.abs(ref) + ATOL)
+
+
+def check_features(gpu, ref, K, what="", allow=None):
+    """``allow``: {row: bound on err / tol} for the rows of an EXCEPTIONS entry (exception_bounds)."""
     gpu = np.asarray(gpu, dtype=np.float64)
     ref = np.asarray(ref, dtype=np.float64)
     assert gpu.shape == ref.shape, (what, gpu.shape, ref.shape)
     assert np.isfinite(gpu).all(), what + ": non-finite output"
     err = np.abs(gpu - ref)
     tol = RTOL * np.abs(ref) + ATOL
+    if allow:
+        tol = tol.copy()
+        for r, bound in allow.items():
+            if r < tol.shape[0]:
+                tol[r] *= bound
     bad = err > tol
     F = ref.shape[0]
     flips = 0
@@ -37,6 +84,29 @@ def check_features(gpu, ref, K, what=""):
         worst = [(int(r), float(err[r].max()), float((err[r] / tol[r]).max())) for r in rows]
         raise AssertionError("%s: rows outside tolerance (row, max abs err, max err/tol): %s" % (what, worst))
     return flips
+
+
+def check_zcr_exact(gpu, ref, what=""):
+    """zcr of integer input is an exact count of sign changes: the float32 result is that count rounded once,
+    |gpu - ref| <= 2^-24 |ref|."""
+    g = np.asarray(gpu, dtype=np.float64)[ZCR_ROW]
+    r = np.asarray(ref, dtype=np.float64)[ZCR_ROW]
+    bad = np.abs(g - r) > 2.0 ** -24 * np.abs(r)
+    if bad.any():
+        t = np.nonzero(bad)[0]
+        raise AssertionError("%s: zcr not exact in %d frames, first %d: %r vs %r" % (what, t.size, t[0], g[t[0]], r[t[0]]))
+
+
+def check_energy_relative(gpu, ref, what="", rtol=RTOL, atol=ENERGY_ATOL):
+    """The energy row relative to each frame's own level, so that quiet frames count."""
+    g = np.asarray(gpu, dtype=np.float64)[ENERGY_ROW]
+    r = np.asarray(ref, dtype=np.float64)[ENERGY_ROW]
+    bad = np.abs(g - r) > rtol * np.abs(r) + atol
+    if bad.any():
+        t = np.nonzero(bad)[0]
+        rel = np.abs(g[t] - r[t]) / np.maximum(np.abs(r[t]), 1e-300)
+        raise AssertionError("%s: energy off in %d frames, worst relative error %.3g (frame %d, ref %.3g)"
+                             % (what, t.size, rel.max(), t[np.argmax(rel)], r[t[np.argmax(rel)]]))
 
 
 def check_close(gpu, ref, what="", rtol=RTOL, atol=ATOL):
