@@ -130,6 +130,11 @@ int b200aa_chromagram(const b200aa_plan *plan, const void *d_sig, int dtype, int
 /* Kernel 2: mid-term pooling.  d_st float32 [n_clips, F, t_stride] (n_frames valid columns),
  * d_mid float32 [n_clips, 2F, M], M = b200aa_mid_windows(n_frames, step_ratio): rows 0..F-1 means,
  * F..2F-1 population standard deviations of st[f][c : min(c+ratio, T)], c = j*step_ratio.
+ * The window is a Python slice, as in the reference: ratio may be 0 or negative (the reference's round() of
+ * (mid_window - (short_window - short_step)) / short_step gives that for short mid-term windows).  A negative end
+ * counts from the end of the row (ratio -1: window 0 is st[f][0 : T-1]); an empty window gives mean = std = 0
+ * (np.nan_to_num of the NaNs of an empty slice).  step_ratio < 1 is B200AA_ERR_INVALID: the reference's window
+ * loop never ends there.
  * Replaces: MidTermFeatures.mid_feature_extraction's pooling loops (:110-126). */
 int b200aa_mid_pool(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames,
                     int64_t t_stride, int ratio, int step_ratio, float *d_mid, void *stream);

@@ -21,7 +21,9 @@ def mid_feature_extraction(signal, sampling_rate, mid_window, mid_step, short_wi
 
     Short-term features with deltas (MidTermFeatures.py:93-95), then the mean and population
     standard deviation of every row over runs of ``ratio`` frames every ``step_ratio`` frames
-    (:100-124), ``np.nan_to_num`` (:126).  All window arguments are in samples.
+    (:100-124), ``np.nan_to_num`` (:126).  All window arguments are in samples.  As in the reference, a mid-term
+    window shorter than one short-term step gives ``ratio <= 0``: windows are Python slices, an empty one pools to 0.
+    A mid-term step that rounds to 0 short-term steps raises ValueError (the reference's window loop never ends).
     """
     w, s = int(short_window), int(short_step)
     x, code = _as_clip(signal)
@@ -30,8 +32,8 @@ def mid_feature_extraction(signal, sampling_rate, mid_window, mid_step, short_wi
     if T <= 0:
         ShortTermFeatures._raise_no_frames(plan.fs, w)
     ratio, stepr = mid_ratios(mid_window, mid_step, short_window, short_step)
-    if ratio < 1 or stepr < 1:
-        raise ValueError("mid-term window / step shorter than one short-term step")
+    if stepr < 1:
+        raise ValueError("mid-term step shorter than half a short-term step")
     M = lib().b200aa_mid_windows(T, stepr)
     mid = np.empty((136, M), dtype=np.float32)
     st = np.empty((68, T), dtype=np.float32)

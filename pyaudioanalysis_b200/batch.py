@@ -141,11 +141,12 @@ def mid_ratios(mid_window, mid_step, short_window, short_step):
 
 
 def mid_feature_extraction_batch(signals, sampling_rate, mid_window, mid_step, short_window, short_step):
-    """Batched MidTermFeatures.mid_feature_extraction: returns (mid [B,136,M], st [B,68,T]) on the GPU."""
+    """Batched MidTermFeatures.mid_feature_extraction: returns (mid [B,136,M], st [B,68,T]) on the GPU.  ``ratio <= 0``
+    pools Python slices as the reference does (empty windows give 0); a step ratio < 1 raises ValueError."""
     st = feature_extraction_batch(signals, sampling_rate, short_window, short_step, deltas=True)
     ratio, stepr = mid_ratios(mid_window, mid_step, short_window, short_step)
-    if ratio < 1 or stepr < 1:
-        raise ValueError("mid-term window / step shorter than one short-term step")
+    if stepr < 1:
+        raise ValueError("mid-term step shorter than half a short-term step")
     return mid_pool_batch(st, ratio, stepr), st
 
 

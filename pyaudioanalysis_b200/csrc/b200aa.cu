@@ -613,9 +613,13 @@ __global__ void __launch_bounds__(256) mid_pool_kernel(const float *st, int64_t 
     const int64_t j = wid % M, bf = wid / M;
     const int64_t b = bf / F;
     const int f = int(bf - b * F);
-    const int64_t c0 = j * stepr, c1 = min(T, c0 + ratio);
+    // window j is the Python slice row[c0 : min(c0 + ratio, T)] (:116-120): a negative end counts from the end of
+    // the row (ratio < 0), an end before c0 gives an empty window; n = 0 makes mean and std 0 / 0 -> 0 below
+    const int64_t c0 = j * stepr;
+    int64_t c1 = min(T, c0 + ratio);
+    if (c1 < 0) c1 = max(c1 + T, int64_t(0));
     const float *row = st + (size_t(b) * F + f) * t_stride;
-    const int n = int(c1 - c0);
+    const int n = int(max(c1 - c0, int64_t(0)));
     double s = 0.0;
     for (int64_t c = c0 + lane; c < c1; c += 32) s += double(row[c]);
 #pragma unroll
@@ -641,7 +645,7 @@ extern "C" int b200aa_mid_pool(const float *d_st, int64_t n_clips, int n_feats, 
                                int ratio, int step_ratio, float *d_mid, void *stream)
 {
     NvtxRange nvtx_("b200aa_mid_pool");
-    if (!d_st || !d_mid || n_clips < 0 || n_feats < 1 || n_frames < 1 || ratio < 1 || step_ratio < 1 || t_stride < n_frames)
+    if (!d_st || !d_mid || n_clips < 0 || n_feats < 1 || n_frames < 1 || step_ratio < 1 || t_stride < n_frames)
         return B200AA_ERR_INVALID;
     const int64_t M = b200aa_mid_windows(n_frames, step_ratio);
     const int64_t warps = n_clips * n_feats * M;
@@ -1119,7 +1123,7 @@ extern "C" int b200aa_mid_features_host(const b200aa_plan *plan, const void *h_s
                                         int ratio, int step_ratio, float *h_mid, float *h_st)
 {
     NvtxRange nvtx_("b200aa_mid_features_host");
-    if (!plan || !h_sig || !h_mid || ratio < 1 || step_ratio < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
+    if (!plan || !h_sig || !h_mid || step_ratio < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
     if (plan->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
     const int64_t T = b200aa_host::num_frames(n_samples, plan->window, plan->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;

@@ -11,6 +11,8 @@ counted and bounded separately.
 The absolute term makes the feature check blind below ~1e-5: a quiet frame's energy (~1e-8) passes whatever its value.
 Two row checks close that: ``check_energy_relative`` holds the energy row to RTOL with a negligible floor, and
 ``check_zcr_exact`` holds the zcr row of integer input to float32 rounding of the exact count.
+``check_mid_propagated`` carries the per-frame tolerance through mid-term pooling (mean: mean of the frame tolerances,
+std: their RMS).
 """
 import numpy as np
 
@@ -107,6 +109,60 @@ def check_energy_relative(gpu, ref, what="", rtol=RTOL, atol=ENERGY_ATOL):
         rel = np.abs(g[t] - r[t]) / np.maximum(np.abs(r[t]), 1e-300)
         raise AssertionError("%s: energy off in %d frames, worst relative error %.3g (frame %d, ref %.3g)"
                              % (what, t.size, rel.max(), t[np.argmax(rel)], r[t[np.argmax(rel)]]))
+
+
+def mid_slices(T, ratio, stepr):
+    """(start, stop) of every mid-term window: the Python slice st[c : min(c + ratio, T)], c = 0, stepr, ...
+    (MidTermFeatures.py:116-124; ratio may be 0 or negative there)."""
+    return [slice(c, min(c + ratio, T)).indices(T)[:2] for c in range(0, T, stepr)]
+
+
+def check_mid_propagated(mid, st_gpu, st_ref, ratio, stepr, K, what="", allow=None, ref_mid=None):
+    """Mid-term matrix ``mid`` [2F, M] (pooled from ``st_gpu``) against pooling of the reference's short-term matrix
+    ``st_ref`` [F, T], with the short-term tolerance propagated through the pooling.
+
+    Frame t of row r may be off by tau = RTOL |ref| + ATOL (times the ``allow`` bound of the row, as in check_features);
+    on a rolloff frame that check_features accepts as a flip, by one quantum 1/K (delta rolloff: two) instead.  A window
+    mean may then be off by mean(tau) over the window, and a population std by rms(tau): std is 1-Lipschitz in the RMS
+    norm, |std(x) - std(y)| <= rms(x - y).  Each output is also rounded to float32 once (2^-24 relative).  ``ref_mid``: the
+    reference's own mid-term matrix, compared instead of the pooling of ``st_ref`` (which still gives the bounds)."""
+    mid = np.asarray(mid, dtype=np.float64)
+    g = np.asarray(st_gpu, dtype=np.float64)
+    r = np.asarray(st_ref, dtype=np.float64)
+    F, T = r.shape
+    assert g.shape == r.shape, (what, g.shape, r.shape)
+    win = mid_slices(T, ratio, stepr)
+    assert mid.shape == (2 * F, len(win)), (what, mid.shape, (2 * F, len(win)))
+    tau = RTOL * np.abs(r) + ATOL
+    for row, bound in (allow or {}).items():
+        if row < F:
+            tau[row] *= bound
+    for row in (ROLLOFF_ROW, ROLLOFF_ROW + 34):
+        if row < F:
+            quantum = (1.0 / K) * (2 if row >= 34 else 1) + 1e-6
+            flip = np.abs(g[row] - r[row]) > tau[row]
+            tau[row, flip] = quantum
+    ref = np.zeros_like(mid)
+    bound = np.zeros_like(mid)
+    for j, (a, b) in enumerate(win):
+        if b > a:
+            seg = r[:, a:b]
+            ref[:F, j], ref[F:, j] = seg.mean(axis=1), seg.std(axis=1)
+            bound[:F, j] = tau[:, a:b].mean(axis=1)
+            bound[F:, j] = np.sqrt((tau[:, a:b] ** 2).mean(axis=1))
+    if ref_mid is not None:
+        assert np.shape(ref_mid) == ref.shape, (what, np.shape(ref_mid), ref.shape)
+        ref = np.asarray(ref_mid, dtype=np.float64)
+    bound += 2.0 ** -24 * np.abs(ref)
+    assert np.isfinite(mid).all(), what + ": non-finite mid-term output"
+    err = np.abs(mid - ref)
+    bad = err > bound
+    if bad.any():
+        rows, cols = np.nonzero(bad)
+        k = int(np.argmax(err[bad] / bound[bad]))
+        raise AssertionError("%s: %d mid-term entries outside the propagated tolerance, rows %s; worst (row %d, window %d): "
+                             "%r vs %r, bound %.3g" % (what, rows.size, np.unique(rows)[:10].tolist(), rows[k], cols[k],
+                                                       mid[rows[k], cols[k]], ref[rows[k], cols[k]], bound[rows[k], cols[k]]))
 
 
 def check_close(gpu, ref, what="", rtol=RTOL, atol=ATOL):

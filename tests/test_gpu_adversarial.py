@@ -14,11 +14,11 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
+from tests.kernels import CTA, GENERIC, KIND_NAMES, PAIR, SOLO, plans, ragged
 from tests.parity import (check_close, check_energy_relative, check_features, check_zcr_exact, exception_bounds)
 
 pytestmark = pytest.mark.gpu
 
-PAIR, SOLO, CTA, GENERIC = 2, 3, 1, 0
 # (fs, window, hop): the kernel kinds a plan reaches through prefer_kernel / force_generic
 FEATURE_CONFIGS = [
     (16000, 320, 160, {PAIR, CTA, GENERIC}), (16000, 480, 240, {PAIR, CTA, GENERIC}), (16000, 512, 256, {PAIR, GENERIC}),
@@ -31,7 +31,6 @@ FEATURE_CONFIGS = [
 ]
 ROW_CONFIGS = [(16000, 800, 400), (16000, 800, 333), (44100, 882, 441), (16000, 400, 160), (8000, 600, 300)]
 ODD = 3                 # sample offset of the unaligned view
-KIND_NAMES = {PAIR: "pair", SOLO: "solo", CTA: "CTA", GENERIC: "generic"}
 
 
 @pytest.fixture(scope="module")
@@ -40,36 +39,6 @@ def P():
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     import pyaudioanalysis_b200 as pkg
     return pkg
-
-
-def plans(fs, w, s):
-    """[(kind, Plan)] for every kernel kind a plan for (fs, w, s) reaches, the default choice first."""
-    from pyaudioanalysis_b200._lib import Plan
-    out = [(Plan(fs, w, s).kernel_kind(), Plan(fs, w, s))]
-    for kind in (PAIR, SOLO, CTA):
-        pl = Plan(fs, w, s).prefer_kernel(kind)
-        if pl.kernel_kind() == kind:
-            out.append((kind, pl))
-    pg = Plan(fs, w, s)
-    pg.force_generic(True)
-    assert pg.kernel_kind() == GENERIC
-    out.append((GENERIC, pg))
-    return out
-
-
-def ragged(clips, dtype, offset=0):
-    """[B, Nmax] CUDA batch of the clips (zero padded) and their lengths.  offset 0: a view of a buffer with 16-byte
-    aligned rows (a row stride that is a multiple of 8 samples); offset > 0: a view into a wider buffer whose rows start
-    ``offset`` samples in and whose row stride is not a multiple of 8 samples."""
-    import torch
-    n = max(x.size for x in clips)
-    width = -(-(n + offset) // 8) * 8 + (1 if offset else 0)
-    buf = np.zeros((len(clips), width), dtype=dtype)
-    for i, x in enumerate(clips):
-        buf[i, offset:offset + x.size] = x
-    d = torch.from_numpy(buf).cuda()[:, offset:offset + n]
-    lens = torch.tensor([x.size for x in clips], dtype=torch.int64, device="cuda")
-    return d, lens
 
 
 def oracle_features(x, fs, w, s):

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 from oracle import st_oracle as O
-from tests.parity import check_features, check_close
+from tests.parity import check_close, check_features, check_mid_propagated
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -73,16 +73,9 @@ def test_config4_at_size(P):
     check_features(st, rs, 400, "config 4 short-term")
     # mid-term rows are means / standard deviations over 39 short-term frames.  The pooling itself is held tight against
     # the oracle's pooling of the GPU's own short-term matrix; against the reference's mid-term matrix the short-term
-    # tolerance propagates (a standard deviation of nearly constant values inherits the ABSOLUTE error of its inputs, and
-    # one rolloff quantum flip in a window moves that window's rolloff mean / std), so that comparison uses the short-
-    # term tolerance scaled to each row's magnitude and skips the four rolloff rows.
+    # tolerance of every frame propagates through the pooling (tests/parity.check_mid_propagated), rolloff rows included.
     check_close(mid, O.mid_pool(st, 39, 40), "config 4 pooling of the GPU short-term matrix", rtol=1e-5, atol=1e-6)
-    keep = np.ones(136, bool)
-    keep[[7, 41, 75, 109]] = False
-    scale = np.abs(rs).max(axis=1)                              # per short-term row
-    tol = 1e-4 * np.concatenate([scale, scale])[:, None] + 1e-5 + 1e-4 * np.abs(rm)
-    bad = (np.abs(mid - rm) > tol) & keep[:, None]
-    assert not bad.any(), ("config 4 mid-term rows outside tolerance", np.unique(np.nonzero(bad)[0]))
+    check_mid_propagated(mid, st, rs, 39, 40, 400, "config 4 mid-term", ref_mid=rm)
 
 
 def test_config5_gathered_two_gpus(P):

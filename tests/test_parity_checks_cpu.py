@@ -61,6 +61,58 @@ def test_quiet_frame_energy(REF):
         PA.check_energy_relative(got, F)
 
 
+@pytest.fixture(scope="module")
+def MID(REF):
+    """A short-term matrix within tolerance of REF (every entry off by 0.9 tau, signs alternating; one rolloff flip)
+    and its mid-term matrix at ratio 7 / step 4, pooled in float64 and rounded to float32."""
+    F, w = REF
+    tau = PA.RTOL * np.abs(F) + PA.ATOL
+    sign = np.where((np.arange(F.size) % 2).reshape(F.shape) == 0, 1.0, -1.0)
+    st = F + 0.9 * tau * sign
+    st[PA.ROLLOFF_ROW, 11] = F[PA.ROLLOFF_ROW, 11] + 1.0 / (w // 2)
+    PA.check_features(st, F, w // 2)
+    return st, O.mid_pool(st, 7, 4).astype(np.float32)
+
+
+def test_mid_propagated_passes(REF, MID):
+    F, w = REF
+    st, mid = MID
+    PA.check_mid_propagated(mid, st, F, 7, 4, w // 2)
+    PA.check_mid_propagated(O.mid_pool(F, 7, 4), F, F, 7, 4, w // 2)
+
+
+def mid_bounds(F, ratio, stepr, row, j):
+    """(mean bound, std bound) of window j of short-term row ``row``, as check_mid_propagated derives them."""
+    a, b = PA.mid_slices(F.shape[1], ratio, stepr)[j]
+    tau = PA.RTOL * np.abs(F[row, a:b]) + PA.ATOL
+    return tau.mean(), np.sqrt((tau ** 2).mean())
+
+
+def test_mid_mean_and_std_three_times_bound(REF, MID):
+    F, w = REF
+    st, mid = MID
+    n = F.shape[0]
+    mb, _ = mid_bounds(F, 7, 4, 12, 3)
+    ref = O.mid_pool(F, 7, 4)
+    got = mid.astype(np.float64)
+    got[12, 3] = ref[12, 3] + 3 * mb
+    with pytest.raises(AssertionError, match="propagated tolerance"):
+        PA.check_mid_propagated(got, st, F, 7, 4, w // 2)
+    got = mid.astype(np.float64)
+    _, sb = mid_bounds(F, 7, 4, 40, 5)
+    got[n + 40, 5] = ref[n + 40, 5] - 3 * sb
+    with pytest.raises(AssertionError, match="propagated tolerance"):
+        PA.check_mid_propagated(got, st, F, 7, 4, w // 2)
+
+
+def test_mid_slices_follow_python():
+    assert PA.mid_slices(10, 3, 4) == [(0, 3), (4, 7), (8, 10)]
+    assert PA.mid_slices(10, 0, 4) == [(0, 0), (4, 4), (8, 8)]
+    assert PA.mid_slices(10, -1, 4)[0] == (0, 9) and all(b <= a for a, b in PA.mid_slices(10, -1, 4)[1:])
+    assert PA.mid_slices(10, -20, 20) == [(0, 0)]
+    assert PA.mid_slices(5, 9, 1)[-1] == (4, 5)
+
+
 def test_exception_table():
     names = set(SG.NOTES) | set(SG.float_bank(16000, 800, 400))
     for e in PA.EXCEPTIONS:
