@@ -153,6 +153,16 @@ int b200aa_long_term_mean(const float *d_mid, int64_t n_clips, int n_rows, int64
 int b200aa_normalize_windows(const float *d_mid, int64_t n_clips, int n_rows, int64_t n_windows,
                              const float *d_mean, const float *d_std, float *d_out, void *stream);
 
+/* Kernel 4: beat rate of every clip from its short-term rows 0, 1, 3 .. 18 (SURVEY 8f rank 4).  d_st: float32
+ * [n_clips, n_feats, t_stride], n_feats >= 19; d_frames (nullable, int64 [n_clips]): frames of each clip, clamped to
+ * [0, n_frames]; else n_frames for every clip.  d_out: float64 [n_clips, 2] = (bpm, ratio), bit for bit the host
+ * beat_extraction(st[b, :, :T_b] widened to float64, window_size), NaN where it gives NaN (a clip of 0 frames).
+ * The histogram has round(2 / window_size) bins (half to even); fewer than 1 is B200AA_ERR_INVALID, as are n_feats < 19,
+ * t_stride < n_frames and n_frames >= 2^31 - 1024.  Allocates stream-ordered scratch (at most 256 MiB) on `stream`.
+ * Replaces: MidTermFeatures.beat_extraction (:18-84) and utilities.peakdet (:33-103). */
+int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
+                           const int64_t *d_frames, double window_size, double *d_out, void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

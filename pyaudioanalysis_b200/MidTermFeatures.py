@@ -145,10 +145,12 @@ def _upload_group(clips, n_samples, code):
     return torch.from_numpy(np.stack([c.data for c in clips])).cuda()
 
 
-def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_short=False, want_long_term=False):
+def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_short=False, want_long_term=False,
+                  want_beat=False):
     """Mid-term results of a list of _Clip, in input order: (mid float64 [136 x M] or its long-term mean [136],
-    st float64 [68 x T] | None).  Equal (rate, length, format) clips share launches, in chunks of <= 1 GiB of samples."""
-    from .batch import mid_feature_extraction_batch, long_term_mean_batch
+    st float64 [68 x T] | None, (bpm, ratio) of beat_extraction(st, short_step) | None).  Equal (rate, length, format)
+    clips share launches, in chunks of <= 1 GiB of samples; the beat is computed on the GPU from the resident features."""
+    from .batch import mid_feature_extraction_batch, long_term_mean_batch, beat_extraction_batch
     results = [None] * len(clips)
     groups = {}
     for idx, c in enumerate(clips):
@@ -162,8 +164,9 @@ def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_sh
                                                    round(fs * short_window), round(fs * short_step))
             first = (long_term_mean_batch(mid) if want_long_term else mid).cpu().numpy().astype(np.float64)
             st_h = st.cpu().numpy().astype(np.float64) if want_short else None
+            beat = beat_extraction_batch(st, short_step).cpu().numpy() if want_beat else None
             for k, i in enumerate(part):
-                results[i] = (first[k], st_h[k] if want_short else None)
+                results[i] = (first[k], st_h[k] if want_short else None, tuple(beat[k]) if want_beat else None)
     return results
 
 
@@ -174,7 +177,8 @@ def directory_feature_extraction(folder_path, mid_window, mid_step, short_window
     empty array for none, exactly like the reference's np.vstack logic --, file list, feature names).  Files are
     decoded by ``audioio`` (.wav, .aif / .aiff, and .mp3 / .au / .ogg when pydub is installed, as in the reference; a
     file that cannot be decoded raises instead of silently changing the file list).  ``compute_beat=True`` appends
-    ``beat_extraction`` (this module's own, reference :18-84) of the GPU short-term features: ``bpm`` and ``ratio``.
+    ``bpm`` and ``ratio`` of the GPU short-term features, computed on the GPU (``batch.beat_extraction_batch``, bit for bit
+    this module's ``beat_extraction``, reference :18-84); only those two numbers per file are copied back.
     """
     types = ('*.wav', '*.aif', '*.aiff', '*.mp3', '*.au', '*.ogg')
     files = []
@@ -202,14 +206,13 @@ def directory_feature_extraction(folder_path, mid_window, mid_step, short_window
         return np.array([]), [], names
     st_names = ShortTermFeatures.feature_names(True)
     names = [n + "_mean" for n in st_names] + [n + "_std" for n in st_names]
-    res = _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_short=compute_beat, want_long_term=True)
+    res = _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_long_term=True, want_beat=compute_beat)
     out, out_files = np.array([]), []
     appended = False
-    for c, (v, st) in zip(clips, res):
+    for c, (v, _, beat) in zip(clips, res):
         out_files.append(c.path)
         if (not np.isnan(v).any()) and (not np.isinf(v).any()):      # reference :203-204
-            if compute_beat:
-                beat = beat_extraction(st, short_step)               # reference :191
+            if compute_beat:                                         # beat: reference :191, computed by kernel 4
                 v = np.append(np.append(v, beat[0]), beat[1])        # :205-208
                 if not appended:
                     names = names + ["bpm", "ratio"]
@@ -246,7 +249,7 @@ def directory_feature_extraction_no_avg(folder_path, mid_window, mid_step, short
         clips.append(c)
     mids = _mid_per_clip(clips, mid_window, mid_step, short_window, short_step)
     mid_features, signal_idx = np.array([]), np.array([])
-    for i, (mid, _) in zip(idxs, mids):
+    for i, (mid, _, _) in zip(idxs, mids):
         rows = np.transpose(mid)
         if len(mid_features) == 0:
             mid_features = rows
@@ -261,7 +264,7 @@ def mid_feature_extraction_to_file(file_path, mid_window, mid_step, short_window
                                    store_short_features=False, store_csv=False, plot=False):
     """Reference MidTermFeatures.py:324-362: <output>_mt.npy ([136 x M] float64), optional <output>_st.npy
     ([68 x T]) and transposed CSV copies -- the on-disk formats the reference's CLI consumers read."""
-    (mid, st), = _mid_per_clip([_open_clip(file_path)], mid_window, mid_step, short_window, short_step, want_short=True)
+    (mid, st, _), = _mid_per_clip([_open_clip(file_path)], mid_window, mid_step, short_window, short_step, want_short=True)
     if store_short_features:
         np.save(output_file + "_st", st)
         if plot:

@@ -132,6 +132,37 @@ def long_term_mean_batch(mid):
     return out
 
 
+def beat_extraction_batch(st, window_size, n_frames=None):
+    """Beat rate of every clip (kernel 4): CUDA float32 [B, F >= 19, T] short-term features -> CUDA float64 [B, 2] of
+    (bpm, ratio), bit for bit ``MidTermFeatures.beat_extraction(st[b, :, :n_frames[b]], window_size)`` on the same values
+    widened to float64.  ``n_frames`` (int64 CUDA [B], entries clamped to [0, T]) gives each clip's own frame count in a
+    ragged batch, e.g. the frame counts of ``feature_extraction_batch(..., lengths=)``'s clips.  ``window_size`` is the
+    short-term step in seconds, as in the reference; round(2 / window_size) < 1 raises ValueError like the host function."""
+    _require_cuda(st, "st")
+    if st.dim() != 3 or st.dtype != torch.float32 or not st.is_contiguous() or st.shape[1] < 19:
+        raise ValueError("st must be contiguous float32 [B, F >= 19, T]")
+    max_beat_time = round(2.0 / window_size)
+    if max_beat_time < 1:
+        raise ValueError("round(2 / window_size) = %d: the beat histogram needs at least one bin" % max_beat_time)
+    B, F, T = st.shape
+    fr_ptr = None
+    if n_frames is not None:
+        _require_cuda(n_frames, "n_frames")
+        if n_frames.dtype != torch.int64 or tuple(n_frames.shape) != (B,):
+            raise ValueError("n_frames must be an int64 tensor [B]")
+        n_frames = n_frames.contiguous()
+        fr_ptr = ctypes.c_void_p(n_frames.data_ptr())
+    with torch.cuda.device(st.device):
+        out = torch.empty((B, 2), dtype=torch.float64, device=st.device)
+        if B == 0:
+            return out
+        if T == 0:                  # no frames has an answer too, (60 / window, NaN); give the kernel a valid pointer
+            st, T, fr_ptr = st.new_zeros((B, F, 1)), 0, None
+        check(lib().b200aa_beat_extraction(ctypes.c_void_p(st.data_ptr()), B, F, T, T, fr_ptr, float(window_size),
+                                           ctypes.c_void_p(out.data_ptr()), _stream()))
+    return out
+
+
 def mid_ratios(mid_window, mid_step, short_window, short_step):
     """MidTermFeatures.py:100-102 (Python round(): half to even).  window/step truncation happens
     inside feature_extraction only (ShortTermFeatures.py:563-564); the ratios use the raw arguments."""

@@ -16,9 +16,8 @@ import ctypes
 import numpy as np
 import torch
 
-from . import MidTermFeatures as _mtf
 from ._lib import check, lib
-from .batch import _require_cuda, _stream, long_term_mean_batch, mid_feature_extraction_batch
+from .batch import _require_cuda, _stream, beat_extraction_batch, long_term_mean_batch, mid_feature_extraction_batch
 
 _SKLEARN_TYPES = ("svm", "randomforest", "gradientboosting", "extratrees", "svm_rbf")
 
@@ -96,7 +95,7 @@ def file_classification_vector(signal, sampling_rate, classifier, model_type, me
                                            round(sampling_rate * short_window), round(sampling_rate * short_step))
     vec = long_term_mean_batch(mid)[0].double().cpu().numpy()
     if compute_beat:
-        beat, beat_conf = _mtf.beat_extraction(st[0].double().cpu().numpy(), short_step)
+        beat, beat_conf = beat_extraction_batch(st, short_step)[0].tolist()
         vec = np.append(np.append(vec, beat), beat_conf)
     vec = (vec - np.asarray(mean, dtype=np.float64)) / np.asarray(std, dtype=np.float64)
     ids, post = classify_vectors(classifier, model_type, vec.reshape(1, -1))

@@ -103,7 +103,8 @@ def main():
     emit({"config": "4: mid_feature_extraction, 1 h @16 kHz, mt 1.0/1.0 s, st 50/25 ms (device resident)", "ms": ms4, "st_frames": int(T4),
           "mid_windows": int(m.shape[2]), "st_frames_per_s": T4 / (ms4 * 1e-3), "x_realtime": 3600.0 / (ms4 * 1e-3),
           "algorithmic_GBps": (2 * N4 + 4 * 68 * T4 + 4 * 136 * m.shape[2]) / (ms4 * 1e-3) / 1e9, "hbm_peak_GBps": PEAK})
-    del c4
+    beat_inputs = [("4: 1 h @16 kHz, st 50/25 ms", st)]
+    del c4, m
 
     # ---- other windows on the config-2 batch, per kernel kind
     cg = noise(1000, 160000, 5)
@@ -124,6 +125,20 @@ def main():
     ms0 = timed(lambda: clip_stats(cg), reps=20)
     emit({"config": "kernel 0 (clip statistics) on 1000 x 10 s", "ms": ms0, "GBps": cg.numel() * 2 / (ms0 * 1e-3) / 1e9, "hbm_peak_GBps": PEAK,
           "frac": cg.numel() * 2 / (ms0 * 1e-3) / 1e9 / PEAK})
+
+    # ---- kernel 4 (beat extraction) on config 2's and config 4's short-term features, beside the host function on the
+    # same features (one pass over every clip, wall clock)
+    beat_inputs.insert(0, ("2: 1000 x 10 s @16 kHz, st 50/25 ms", pkg.feature_extraction_batch(cg, 16000, 800, 400)))
+    for name, st in beat_inputs:
+        ms_k = timed(lambda: pkg.beat_extraction_batch(st, 0.025), reps=20, warm=3)
+        st_h = st.cpu().numpy()
+        t0 = time.perf_counter()
+        for b in range(st_h.shape[0]):
+            pkg.MidTermFeatures.beat_extraction(st_h[b].astype(np.float64), 0.025)
+        ms_h = (time.perf_counter() - t0) * 1e3
+        emit({"config": "beat extraction, " + name, "clips": int(st.shape[0]), "frames": int(st.shape[2]), "kernel_ms": ms_k,
+              "host_beat_extraction_ms": ms_h, "host_over_kernel": ms_h / ms_k,
+              "gpu": {"name": torch.cuda.get_device_name(0), "power_limit_w": bench.ClockSampler(0).power_limit_w()}})
 
 
 if __name__ == "__main__":
