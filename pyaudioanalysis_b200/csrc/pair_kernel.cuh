@@ -82,6 +82,8 @@ struct alignas(16) PairWarpMem {
     alignas(16) float rowp[S::Kp];          // |X| row of the previous pair's frame b (the flux of frame a needs it)
     float fv[9 * kFvStride];                // feature rows: row 0 = the frame before the tile, rows 1..8 = the tile
     float blk[24];                          // block energies: a -> [0, 10), b -> [5, 15) (shared halves) or [10, 20); rests at 20, 21
+    float seg_v[2];                         // the segment's clip: 1 / (a^2 N), a / (2 K) (read where a step uses them, not
+                                            // carried in registers)
 };
 
 // warps per CTA such that kPairMinBlocks CTAs fit the 227 KB of an SM (per CTA: kPairCtaCap of pair_launch_t, twiddles, lane
@@ -147,6 +149,7 @@ __device__ __forceinline__ int4 pair_lane_init(int l)
     int4 d;
     d.x = bnd > k0 ? bnd - k0 : 0;
     int ps = 32, pe = 0;
+#pragma unroll 1
     for (int q = 0; q < 16; ++q) {
         const int b0 = q * CB, bb = ((b0 + CB - 1) / Lb) * Lb, sp = bb > b0 ? bb - b0 : 0;
         if (sp > 0 && b0 >= l * Lb && b0 + sp <= (l + 1) * Lb) { ps = min(ps, 2 * q); pe = max(pe, 2 * q + 1); }
@@ -346,7 +349,7 @@ struct MultiReduce {
 };
 
 // ----------------------------------------------------------------------------------------------
-// time-domain accumulation over the 32-sample rows of one frame (u[r] of lane l = sample 32 r + l, as the exact float
+// time-domain accumulation over the 32-sample rows of a frame (u[r] of lane l = sample 32 r + l, as the exact float
 // M0 + x): per-lane sums of y^2 per energy-entropy block, and the number of sign flips from the ballot masks
 //   FULL: all rows, blocks 0..9 (+ the samples beyond 10 blocks);  !FULL: the second half only (blocks 5..9)
 // ----------------------------------------------------------------------------------------------
@@ -362,70 +365,21 @@ struct TdShape {
     static_assert(FULL || S::kShareable, "half-frame sharing needs whole blocks per half");
 };
 
-template <int R, bool FULL, bool TWO>
-__device__ __forceinline__ void td_frame(const float (&u)[R], float cm, const b200aa_clip_norm &nm, int lane,
-                                         float *e /* [NE] */, int &flips, int &link)
-{
-    using S = PairShape<R>;
-    using Td = TdShape<R, FULL>;
-    constexpr int N = S::N, Lt = S::Lt;
-    unsigned prevP = 0u, prevQ = 0u;
-    int fl = 0, lk = 0;
-#pragma unroll
-    for (int r = Td::ZROW0; r < R; ++r) {
-        const float d = u[r] - cm;
-        // ---- sign masks: P = samples above the clip mean, Q = below (complementary unless a sample can equal the mean)
-        const unsigned P = __ballot_sync(0xffffffffu, d > nm.lo);
-        unsigned Q = 0u;
-        if (TWO) Q = __ballot_sync(0xffffffffu, d < nm.hi);
-        if (FULL && r == 0) { prevP = (P & 1u) << 31; prevQ = (Q & 1u) << 31; }      // sample 0 has no predecessor
-        if (r >= Td::ROW0) {
-            const int n0 = 32 * r;
-            // pairs (n - 1, n) counted for n >= max(1, NFIRST)
-            const int nstart = FULL ? 1 : Td::NFIRST;
-            const unsigned valid = n0 >= nstart ? 0xffffffffu : (n0 + 32 <= nstart ? 0u : (0xffffffffu << (nstart - n0)));
-            const unsigned cP = (P ^ __funnelshift_l(prevP, P, 1)) & valid;
-            fl += __popc(cP);
-            if (!FULL && r == Td::ROW0) lk += int((cP >> Td::LANE0) & 1u);
-            if (TWO) {
-                const unsigned cQ = (Q ^ __funnelshift_l(prevQ, Q, 1)) & valid;
-                fl += __popc(cQ);
-                if (!FULL && r == Td::ROW0) lk += int((cQ >> Td::LANE0) & 1u);
-            }
-            // ---- energy of the normalised samples into the row's block(s)
-            // (fused multiply-adds, predicated: bit-identical to td_pair below, whichever of the two handles a frame)
-            const float y = fmaf(nm.a, d, nm.bp);
-            const bool live = !(r == Td::ROW0 && Td::LANE0 > 0) || lane >= Td::LANE0;
-            const int b0 = (n0 / Lt) < 10 ? (n0 / Lt) : 10;
-            const int end = b0 < 10 ? (b0 + 1) * Lt : N;
-            const int thr = end - n0;                     // samples of this row that still belong to block b0
-            const int i0 = b0 - Td::EB, i1 = (b0 + 1 < 10 ? b0 + 1 : 10) - Td::EB;
-            if (thr >= 32) {
-                if (i0 >= 0 && i0 < Td::NE) { if (live) e[i0] = fmaf(y, y, e[i0]); }
-            } else {
-                const bool first = lane < thr;
-                if (i0 >= 0 && i0 < Td::NE) { if (live && first) e[i0] = fmaf(y, y, e[i0]); }
-                if (i1 >= 0 && i1 < Td::NE) { if (live && !first) e[i1] = fmaf(y, y, e[i1]); }
-            }
-        }
-        prevP = P; prevQ = Q;
-    }
-    // one-sided counting saw every change once; |s_n - s_(n-1)| is 2 for a sign change without a zero in between
-    flips = TWO ? fl : 2 * fl;
-    link = TWO ? lk : 2 * lk;
-}
-
-// The same accumulation for BOTH frames of a pair at once (they cover the same rows): u[r] = (sample of a, sample of b),
+// BOTH frames of a pair at once (they cover the same rows): u[r] = (sample of a, sample of b),
 // e2[i] = (block sum of a, block sum of b) -- the arithmetic runs on float2 pairs, only the sign masks stay per frame.
+// FULL also counts, from the same masks, the flips of each frame's second half (pairs (n - 1, n), n >= N / 2) and the
+// link (n = N / 2) among them into half_flips = {a, a's link, b, b's link}: what td_pair<R, false, TWO> returns for them.
 template <int R, bool FULL, bool TWO>
 __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b200aa_clip_norm &nm, int lane,
-                                        float2 *e2 /* [NE] */, int &flips_a, int &link_a, int &flips_b, int &link_b)
+                                        float2 *e2 /* [NE] */, int &flips_a, int &link_a, int &flips_b, int &link_b,
+                                        int (*half_flips)[4] = nullptr)
 {
     using S = PairShape<R>;
     using Td = TdShape<R, FULL>;
-    constexpr int N = S::N, Lt = S::Lt;
+    constexpr int N = S::N, Lt = S::Lt, NH = N / 2, HROW0 = NH / 32, HLANE0 = NH % 32;
     unsigned pPa = 0u, pQa = 0u, pPb = 0u, pQb = 0u;
     int fa = 0, la = 0, fb = 0, lb = 0;
+    int hfa = 0, hla = 0, hfb = 0, hlb = 0;
     const float2 ncm = make_float2(-cm, -cm), a2 = make_float2(nm.a, nm.a), bp2 = make_float2(nm.bp, nm.bp);
 #pragma unroll
     for (int r = Td::ZROW0; r < R; ++r) {
@@ -441,10 +395,19 @@ __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b2
             const unsigned cPa = (Pa ^ __funnelshift_l(pPa, Pa, 1)) & valid, cPb = (Pb ^ __funnelshift_l(pPb, Pb, 1)) & valid;
             fa += __popc(cPa); fb += __popc(cPb);
             if (!FULL && r == Td::ROW0) { la += int((cPa >> Td::LANE0) & 1u); lb += int((cPb >> Td::LANE0) & 1u); }
+            unsigned cQa = 0u, cQb = 0u;
             if (TWO) {
-                const unsigned cQa = (Qa ^ __funnelshift_l(pQa, Qa, 1)) & valid, cQb = (Qb ^ __funnelshift_l(pQb, Qb, 1)) & valid;
+                cQa = (Qa ^ __funnelshift_l(pQa, Qa, 1)) & valid; cQb = (Qb ^ __funnelshift_l(pQb, Qb, 1)) & valid;
                 fa += __popc(cQa); fb += __popc(cQb);
                 if (!FULL && r == Td::ROW0) { la += int((cQa >> Td::LANE0) & 1u); lb += int((cQb >> Td::LANE0) & 1u); }
+            }
+            if (FULL && r >= HROW0) {
+                const unsigned hv = n0 >= NH ? 0xffffffffu : (0xffffffffu << (NH - n0));
+                hfa += __popc(cPa & hv) + __popc(cQa & hv); hfb += __popc(cPb & hv) + __popc(cQb & hv);
+                if (r == HROW0) {
+                    hla += int((cPa >> HLANE0) & 1u) + int((cQa >> HLANE0) & 1u);
+                    hlb += int((cPb >> HLANE0) & 1u) + int((cQb >> HLANE0) & 1u);
+                }
             }
             const float2 y = f2fma(a2, d, bp2);
             const bool live = !(r == Td::ROW0 && Td::LANE0 > 0) || lane >= Td::LANE0;
@@ -462,8 +425,13 @@ __device__ __forceinline__ void td_pair(const float2 (&u)[R], float cm, const b2
         }
         pPa = Pa; pQa = Qa; pPb = Pb; pQb = Qb;
     }
+    // one-sided counting saw every change once; |s_n - s_(n-1)| is 2 for a sign change without a zero in between
     flips_a = TWO ? fa : 2 * fa; link_a = TWO ? la : 2 * la;
     flips_b = TWO ? fb : 2 * fb; link_b = TWO ? lb : 2 * lb;
+    if (FULL && half_flips) {
+        const int m = TWO ? 1 : 2;
+        (*half_flips)[0] = m * hfa; (*half_flips)[1] = m * hla; (*half_flips)[2] = m * hfb; (*half_flips)[3] = m * hlb;
+    }
 }
 
 // power of two s with s * rms(x - x0) ~ 1 (E = sum y^2 of the frame, y = a (x - mean)); its inverse
@@ -563,7 +531,10 @@ __device__ __forceinline__ void tile_store(const float *fv, int tile_n, int tile
 {
     const int c = lane & 7, f0 = lane >> 3;
     if (c < tile_n) {
-        float *const out_b = out_clip + tile_t0 + c;
+        // one 64-bit product per flush: the lane's row f0, then four rows down per store; the delta of row f sits
+        // B200AA_N_BASE rows below it
+        float *out_f = out_clip + f0 * t_stride + (tile_t0 + c);
+        const int64_t step4 = 4 * t_stride, delta = B200AA_N_BASE * t_stride;
         const float *cur_row = fv + (1 + c) * kFvStride, *prv_row = fv + c * kFvStride;
         const bool first = tile_t0 + c == 0;              // frame 0 of the clip: deltas are zero
 #pragma unroll
@@ -571,9 +542,10 @@ __device__ __forceinline__ void tile_store(const float *fv, int tile_n, int tile
             const int f = f0 + 4 * i;
             if (f < B200AA_N_BASE) {
                 const float v = cur_row[f];
-                out_b[size_t(f) * t_stride] = v;
-                if (n_out > B200AA_N_BASE) out_b[size_t(f + B200AA_N_BASE) * t_stride] = first ? 0.f : v - prv_row[f];
+                out_f[0] = v;
+                if (n_out > B200AA_N_BASE) out_f[delta] = first ? 0.f : v - prv_row[f];
             }
+            out_f += step4;
         }
     }
 }
@@ -607,7 +579,10 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
     const StParams &p = pp.st;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int NTHR = 32 * pair_warps<R>();
+    // (once per CTA: rolled loops)
+#pragma unroll 1
     for (int i = tid; i < pp.pbl.words; i += NTHR) blob_s[i] = pp.pblob[i];
+#pragma unroll 1
     for (int i = tid; i < R * 32; i += NTHR) cm_.tw[i] = pp.tw[i];
     if (tid < 16) *reinterpret_cast<int4 *>(cm_.dlane + tid * 4) = pair_lane_init<K>(tid);
     __syncthreads();
@@ -627,76 +602,48 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
     const unsigned wglob = blockIdx.x * unsigned(pair_warps<R>()) + unsigned(warp);
     if (lane == 0) sched_begin(pp.sched, wglob);
     __syncwarp();
-    const int per_clip = int(pp.sched.per_clip);
-    // ---- the run in progress (all of it warp-uniform: the chunk bounds come out of sched_next as lane-0 broadcasts)
-    unsigned run_b = 0xffffffffu, run_q = 0xffffffffu;          // its clip and next pair; run_q = ~0: nothing carried
-    int tile_n = 0, tile_t0 = 0;
-    int zprev = 0;              // sign flips inside the first half of frame a (= second half of the previous b)
-    // pending feature rows -> global memory (tile_flush: always inlined -- an out-of-line call in the step loop costs the
-    // caller-saved registers)
-#define B200AA_PAIR_FLUSH(clip_index) tile_flush(wm.fv, tile_n, tile_t0, p.out + size_t(clip_index) * p.n_out * p.t_stride, p.t_stride, p.n_out, lane)
-
+    const unsigned per_clip = pp.sched.per_clip;
+    const bool is16 = p.dtype == B200AA_DTYPE_I16;
+    const float M0 = is16 ? 8421376.f : 0.f;                       // u = M0 + x exactly (2^23 + 2^15 trick for int16)
+    // One loop, one pair step per pass; where a segment (the part of a chunk inside one clip) ends, the same pass takes the
+    // next one, so that feature rows leave from one place.  All of it is warp-uniform: the chunk bounds come out of
+    // sched_next as lane-0 broadcasts.
     unsigned inc = pp.sched.chunk;      // pairs of the next claim (sched_claim adapts it)
+    unsigned g0 = 0, g1 = 0;            // claimed pairs not begun yet
+    unsigned run_b = 0xffffffffu, run_q = 0xffffffffu;          // the run's clip and next pair; run_q = ~0: nothing carried
+    int q = 0, q0 = 0, q1 = 0;          // next step, first stored pair and end of the segment
+    int tile_n = 0, tile_t0 = 0;
+    int zprev = 0;                      // sign flips inside the first half of frame a (= second half of the previous b)
+    bool fresh = false;                 // no state carried from a previous pair: the run starts one pair early
+    // the clip's values (a handful of cached loads per segment)
+    const char *clip = nullptr;
+    int T = 0, NP = 0;                  // frames and pairs of the clip
+    b200aa_clip_norm nm{};
+    float cmv = 0.f;
+    bool two_sided = false;
     for (;;) {
-        unsigned g0 = 0, g1 = 0;
-        const int got = sched_next(pp.sched, blockIdx.x * unsigned(pair_warps<R>()) + unsigned(warp), lane, inc, g0, g1);
-        if (got == 0) break;
-        if (got == 2) continue;
-        while (g0 < g1) {                                          // a chunk may run over the end of a clip
-        const unsigned cb = g0 / unsigned(per_clip);
-        const int q0 = int(g0 - cb * unsigned(per_clip));
-        int qe = q0 + int(g1 - g0);
-        qe = qe < per_clip ? qe : per_clip;
-        const int64_t b = int64_t(cb);
-        const bool cont = cb == run_b && unsigned(q0) == run_q;     // the run goes on: state carried, no halo
-        if (!cont) B200AA_PAIR_FLUSH(run_b);                        // a new run: the previous one's tile leaves first
-        // the clip's values (a handful of cached loads per chunk; kept local so that nothing but the run state is carried)
-        const int64_t len = p.len ? p.len[b] : p.n_samples;
-        const int T = int(len < N ? 0 : (len - N) / step + 1);
-        const int NP = (T + 1) >> 1;                               // pairs of this clip
-        const b200aa_clip_norm nm = p.norm[b];
-        const bool is16 = p.dtype == B200AA_DTYPE_I16;
-        const char *const clip = reinterpret_cast<const char *>(p.sig) + size_t(b) * p.clip_stride * (is16 ? 2 : 4);
-        const float M0 = is16 ? 8421376.f : 0.f;                   // u = M0 + x exactly (2^23 + 2^15 trick for int16)
-        const float cmv = M0 + nm.m;                                // u - cmv = x - m
-        const bool two_sided = !(nm.hi > nm.lo);                    // a sample may equal the clip mean: count both masks
-        const float inv_a2n = 1.f / (nm.a * nm.a * float(N));
-        const float fscale = nm.a * (0.5f / float(K));
-        bool fresh = !cont;         // no state carried from a previous pair: the run starts one pair early
-        if (!cont) {
-            tile_t0 = 2 * q0;
-            zprev = 0;
-        }
-        g0 += unsigned(qe - q0);
-        run_b = cb;
-        run_q = 0xffffffffu;
-        if (q0 >= NP) continue;                                    // ragged batch: beyond this clip's last pair
-        const int q1 = qe < NP ? qe : NP;
-        // samples: lane l holds samples 32 r + l of both frames of a pair, as exact floats M0 + x.
-        // (Measured and rejected: issuing the loads of pair q + 1 in the middle of step q -- the 50 extra live registers
-        // cost more in spills than the hidden latency gains.)
-        auto load_pair = [&](int qq, unsigned int (&wa)[R], unsigned int (&wb)[R]) {
-            const int ta_ = 2 * qq, tb_ = (ta_ + 1 < T) ? ta_ + 1 : ta_;          // an odd tail pairs the last frame with itself
-            if (is16) {
-                const unsigned short *pa = reinterpret_cast<const unsigned short *>(clip) + size_t(ta_) * step + lane;
-                const unsigned short *pb = reinterpret_cast<const unsigned short *>(clip) + size_t(tb_) * step + lane;
-#pragma unroll
-                for (int r = 0; r < R; ++r) { wa[r] = __ldg(pa + 32 * r); wb[r] = __ldg(pb + 32 * r); }
-            } else {
-                const unsigned int *pa = reinterpret_cast<const unsigned int *>(clip) + size_t(ta_) * step + lane;
-                const unsigned int *pb = reinterpret_cast<const unsigned int *>(clip) + size_t(tb_) * step + lane;
-#pragma unroll
-                for (int r = 0; r < R; ++r) { wa[r] = __ldg(pa + 32 * r); wb[r] = __ldg(pb + 32 * r); }
-            }
-        };
-        for (int q = q0 - ((fresh && q0 > 0) ? 1 : 0); q < q1; ++q) {
+        bool flush = false;
+        if (q < q1) {
             const bool store = q >= q0;
             const int ta = 2 * q;
             const bool bvalid = ta + 1 < T;
+            // samples: lane l holds samples 32 r + l of both frames of a pair, as exact floats M0 + x.
+            // (Measured and rejected: issuing the loads of pair q + 1 in the middle of step q -- the 50 extra live registers
+            // cost more in spills than the hidden latency gains.)
             float2 uab[R];                      // (sample of a, sample of b) per row: float2 operands
             {
                 unsigned int wa[R], wb[R];
-                load_pair(q, wa, wb);
+                // sample offsets fit 32 bits (pair_launch_t); an odd tail pairs the last frame with itself
+                const int oa = ta * step + lane, ob = (bvalid ? ta + 1 : ta) * step + lane;
+                if (is16) {
+                    const unsigned short *const s16 = reinterpret_cast<const unsigned short *>(clip);
+#pragma unroll
+                    for (int r = 0; r < R; ++r) { wa[r] = __ldg(s16 + oa + 32 * r); wb[r] = __ldg(s16 + ob + 32 * r); }
+                } else {
+                    const unsigned int *const s32 = reinterpret_cast<const unsigned int *>(clip);
+#pragma unroll
+                    for (int r = 0; r < R; ++r) { wa[r] = __ldg(s32 + oa + 32 * r); wb[r] = __ldg(s32 + ob + 32 * r); }
+                }
                 if (is16) {
 #pragma unroll
                     for (int r = 0; r < R; ++r)
@@ -734,20 +681,21 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
                     fl_b = (fa_ - la_) + fb_;
                     zprev = fb_ - lb_;
                 } else {
-                    // first step of a run: all of a, the second half of b
-                    float ua[R], ub[R];
+                    // first step of a run: all of a, the second half of b (b's first-half sums and whole-frame flips are
+                    // dead code)
+                    static_assert(NREST == 0, "shared halves: N is a multiple of 10");
+                    float2 e2[NEF];
 #pragma unroll
-                    for (int r = 0; r < R; ++r) { ua[r] = uab[r].x; ub[r] = uab[r].y; }
+                    for (int i = 0; i < NEF; ++i) e2[i] = make_float2(0.f, 0.f);
+                    int fa_, la_, fbw_, lbw_, hf[4];     // hf: flips of a's second half (= b's first half), link; b's
+                    if (two_sided) td_pair<R, true, true>(uab, cmv, nm, lane, e2, fa_, la_, fbw_, lbw_, &hf);
+                    else td_pair<R, true, false>(uab, cmv, nm, lane, e2, fa_, la_, fbw_, lbw_, &hf);
                     float ev[NEF + 5];
 #pragma unroll
-                    for (int i = 0; i < NEF + 5; ++i) ev[i] = 0.f;
-                    int fa_, la_, fb_, lb_;
-                    if (two_sided) { td_frame<R, true, true>(ua, cmv, nm, lane, ev, fa_, la_); td_frame<R, false, true>(ub, cmv, nm, lane, ev + NEF, fb_, lb_); }
-                    else { td_frame<R, true, false>(ua, cmv, nm, lane, ev, fa_, la_); td_frame<R, false, false>(ub, cmv, nm, lane, ev + NEF, fb_, lb_); }
-                    // flips of a's second half alone: b's first half; recount from the shared-half helper
-                    int fh_, lh_;
-                    { float dump[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-                      if (two_sided) td_frame<R, false, true>(ua, cmv, nm, lane, dump, fh_, lh_); else td_frame<R, false, false>(ua, cmv, nm, lane, dump, fh_, lh_); }
+                    for (int i = 0; i < NEF; ++i) ev[i] = e2[i].x;
+#pragma unroll
+                    for (int i = 0; i < 5; ++i) ev[NEF + i] = e2[5 + i].y;
+                    const int fh_ = hf[0], lh_ = hf[1], fb_ = hf[2], lb_ = hf[3];
                     MultiReduce<NEF + 5>::run(ev, lane);
                     __syncwarp();
                     {
@@ -804,6 +752,7 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
 
             // ---- pack the two frames into one complex sequence and transform: pass 1 (lane = n2, R points over n1)
             float sa, isa, sb, isb;
+            const float inv_a2n = wm.seg_v[0];
             frame_scale(Ea, inv_a2n, sa, isa);
             frame_scale(Eb, inv_a2n, sb, isb);
             // an odd tail pairs the last frame with itself, and with shared halves Eb came from the ring as if b were the
@@ -855,6 +804,7 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
             // ---- separate the two spectra: bins k = lane + 32 j
             float xa[C], xb[C];
             {
+                const float fscale = wm.seg_v[1];
                 const float fa = a_flat ? 0.f : fscale * isa, fb = b_flat ? 0.f : fscale * isb;
 #pragma unroll
                 for (int j = 0; j < C; ++j) {
@@ -884,8 +834,8 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
                 for (int j = 0; j < JK; ++j) {
                     const int k = lane + 32 * j;
                     if (k < K) {
-                        pp.dbg[(size_t(b) * p.t_stride + ta) * K + k] = xa[j];
-                        if (bvalid) pp.dbg[(size_t(b) * p.t_stride + ta + 1) * K + k] = xb[j];
+                        pp.dbg[(size_t(run_b) * p.t_stride + ta) * K + k] = xa[j];
+                        if (bvalid) pp.dbg[(size_t(run_b) * p.t_stride + ta + 1) * K + k] = xb[j];
                     }
                 }
             }
@@ -904,17 +854,61 @@ __global__ void __launch_bounds__(32 * pair_warps<R>(), kPairMinBlocks) st_pair_
             // ---- tile bookkeeping: full tiles leave at once, a partial one when the run ends
             if (store) {
                 tile_n += bvalid ? 2 : 1;
-                if (tile_n == 8) B200AA_PAIR_FLUSH(cb);
+                flush = tile_n == 8;
             }
             fresh = false;
+            ++q;
             __syncwarp();                    // the copy above has read the buffer before the next step's pass 1 overwrites it
         }
-        if (q1 < NP) run_q = unsigned(q1);
-        else B200AA_PAIR_FLUSH(cb);          // end of the clip (an odd frame count leaves a partial tile)
+        // ---- the segment is over: the next one starts where the last claim left off, or with a new claim
+        bool begin = false, done = false;
+        unsigned cb = 0;
+        int nq0 = 0, nqe = 0;
+        if (q >= q1) {
+            if (g0 >= g1) {
+                const int got = sched_next(pp.sched, wglob, lane, inc, g0, g1);     // 2: a steal refilled the range
+                done = got == 0;
+            }
+            if (g0 < g1) {                   // a chunk may run over the end of a clip
+                cb = g0 / per_clip;
+                nq0 = int(g0 - cb * per_clip);
+                nqe = nq0 + int(g1 - g0);
+                nqe = nqe < int(per_clip) ? nqe : int(per_clip);
+                g0 += unsigned(nqe - nq0);
+                begin = true;
+            }
+            // a run that does not go on (state carried, no halo) leaves its tile: at the end of a clip (odd frame
+            // counts leave a partial tile), before another run and when the warp is done
+            flush |= done || (begin && !(cb == run_b && unsigned(nq0) == run_q));
+        }
+        if (flush) tile_flush(wm.fv, tile_n, tile_t0, p.out + size_t(run_b) * p.n_out * p.t_stride, p.t_stride, p.n_out, lane);
+        if (done) break;
+        if (begin) {
+            const bool cont = cb == run_b && unsigned(nq0) == run_q;
+            fresh = !cont;
+            if (!cont) {
+                tile_t0 = 2 * nq0;
+                zprev = 0;
+            }
+            run_b = cb;
+            const int64_t len = p.len ? p.len[cb] : p.n_samples;
+            // (len - N) / step in 32 bits: pair_launch_t guarantees (2 per_clip - 1) step < 2^31, so a clamped length
+            // still yields T >= 2 per_clip, which changes neither NP nor any pair step of the clip
+            const unsigned span = unsigned(len - N < int64_t(0x7fffffff) ? len - N : int64_t(0x7fffffff));
+            T = len < N ? 0 : int(span / unsigned(step)) + 1;
+            NP = (T + 1) >> 1;
+            nm = p.norm[cb];
+            clip = reinterpret_cast<const char *>(p.sig) + size_t(cb) * p.clip_stride * (is16 ? 2 : 4);
+            cmv = M0 + nm.m;                                            // u - cmv = x - m
+            two_sided = !(nm.hi > nm.lo);                               // a sample may equal the clip mean: count both masks
+            wm.seg_v[0] = 1.f / (nm.a * nm.a * float(N));
+            wm.seg_v[1] = nm.a * (0.5f / float(K));
+            q0 = nq0;
+            q1 = nqe < NP ? nqe : NP;                                   // ragged batch: nothing beyond the clip's last pair
+            q = q0 < q1 ? q0 - ((fresh && q0 > 0) ? 1 : 0) : q1;
+            run_q = q1 < NP ? unsigned(q1) : 0xffffffffu;
         }
     }
-    B200AA_PAIR_FLUSH(run_b);
-#undef B200AA_PAIR_FLUSH
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -1073,6 +1067,7 @@ inline int pair_launch_t(const PairTables &pt, const StParams &p, int sm_count, 
     const int64_t total = NP * p.n_clips;
     if (total <= 0) return B200AA_OK;                                // no clip has a frame
     if (total >= (int64_t(1) << 31)) return B200AA_ERR_UNSUPPORTED;
+    if ((2 * NP - 1) * p.step + 32 * R > INT32_MAX) return B200AA_ERR_UNSUPPORTED;   // sample offsets in a clip: 32 bits
     // every resident warp gets an equal contiguous share (sched.cuh); small launches use as many warps as they have pairs
     int64_t grid = int64_t(sm_count) * occ;
     if (grid * kPairWarps > total) grid = (total + kPairWarps - 1) / kPairWarps;
