@@ -145,6 +145,32 @@ int b200aa_mid_pool(const float *d_st, int64_t n_clips, int n_feats, int64_t n_f
 int b200aa_long_term_mean(const float *d_mid, int64_t n_clips, int n_rows, int64_t n_windows,
                           float *d_out, void *stream);
 
+/* Per-clip counts of a ragged batch, computed on the device from its lengths: d_len int64 [n_clips] (the lengths given to
+ * b200aa_clip_stats / b200aa_st_features); d_frames int64 [n_clips] = b200aa_num_frames(d_len[b], window, step);
+ * d_windows (nullable) int64 [n_clips] = b200aa_mid_windows(d_frames[b], step_ratio).  NULL d_len / d_frames,
+ * window < 1, step < 1, and step_ratio < 1 with d_windows are B200AA_ERR_INVALID.  Lets a caller that holds the lengths
+ * only on the device pass the counts below without a round trip to the host. */
+int b200aa_frame_counts(const int64_t *d_len, int64_t n_clips, int window, int step, int step_ratio,
+                        int64_t *d_frames, int64_t *d_windows, void *stream);
+
+/* Kernel 2 on a ragged batch: d_st float32 [n_clips, n_feats, t_stride]; d_frames int64 [n_clips]: clip b has
+ * T_b = clamp(d_frames[b], 0, t_stride) frames and M_b = b200aa_mid_windows(T_b, step_ratio) windows.  d_mid float32
+ * [n_clips, 2 * n_feats, M], M = b200aa_mid_windows(t_stride, step_ratio); columns >= M_b of clip b are not written.
+ * Windows, ratio and step_ratio as in b200aa_mid_pool, with T_b for n_frames.  A clip's columns are bit for bit those
+ * b200aa_mid_pool gives for it alone with n_frames = T_b: each window's sums run in an order set by the window's bounds
+ * only.  NULL pointers, n_feats < 1, step_ratio < 1 and t_stride < 0 are B200AA_ERR_INVALID.
+ * Replaces: the pooling loops (MidTermFeatures.py:110-126) of every file of a folder of files of different lengths. */
+int b200aa_mid_pool_ragged(const float *d_st, int64_t n_clips, int n_feats, int64_t t_stride,
+                           const int64_t *d_frames, int ratio, int step_ratio, float *d_mid, void *stream);
+
+/* Long-term average on a ragged batch: d_mid float32 [n_clips, n_rows, m_stride]; d_windows int64 [n_clips]: clip b
+ * averages its first M_b = clamp(d_windows[b], 0, m_stride) columns, NaN for M_b = 0 (0 / 0, as np.mean of an empty
+ * axis).  d_out float32 [n_clips, n_rows], bit for bit b200aa_long_term_mean of the clip alone with n_windows = M_b.
+ * NULL pointers, n_rows < 1 and m_stride < 0 are B200AA_ERR_INVALID.
+ * Replaces: `mid_features.mean(axis=0)` (MidTermFeatures.py:200-201) of every file of a folder. */
+int b200aa_long_term_mean_ragged(const float *d_mid, int64_t n_clips, int n_rows, int64_t m_stride,
+                                 const int64_t *d_windows, float *d_out, void *stream);
+
 /* Feature vectors for the classifiers that consume the mid-term matrix (SURVEY 8f rank 4): d_out float32
  * [n_clips, n_windows, n_rows], vector j of clip b = (d_mid[b, :, j] - mean) / std -- the transpose the per-window loops
  * build one column at a time.  d_mean / d_std: float32 [n_rows] on the device.

@@ -2,7 +2,8 @@
 (:18-84) and the directory wrappers around them (``directory_feature_extraction`` :140-221,
 ``multiple_directory_feature_extraction`` :224-260, ``directory_feature_extraction_no_avg`` :263-309): files are decoded on
 the host (``audioio``: .wav / .aif / .aiff, and .mp3 / .au / .ogg when pydub is installed, as in the reference), files of
-equal sampling rate and length are staged in page-locked memory and batched into single GPU launches."""
+equal sampling rate and sample format, whatever their lengths, are staged in page-locked memory and batched into ragged
+GPU launches."""
 import ctypes
 import glob
 import os
@@ -101,7 +102,8 @@ def beat_extraction(short_features, window_size, plot=False):
     return bpm, ratio
 
 
-_MAX_GROUP_BYTES = 1 << 30       # clips of one (rate, length, format) group go to the GPU in chunks of at most 1 GiB
+_MAX_CHUNK_BYTES = 1 << 30       # padded staging bytes of one chunk; a single larger clip gets a chunk of its own
+_MAX_PADDING = 0.25              # padding samples of a chunk per sample of its clips (DESIGN §7, rank 1)
 
 
 class _Clip:
@@ -126,47 +128,87 @@ def _open_clip(path):
     return _Clip(path, fs, clip.shape[0], clip, code)
 
 
-def _upload_group(clips, n_samples, code):
-    """Clips of one (rate, length, format) group -> one [n, N] device tensor.  int16 clips are staged in page-locked
-    memory (files still on disk are read straight into it) so the H2D copy runs at full PCIe speed."""
+def _plan_chunks(clips, max_bytes=None, max_padding=None):
+    """Cut a list of _Clip into batches: [[index into clips, ...], ...], every index exactly once.  A chunk holds clips
+    of one (rate, format), longest first; it is staged as [len(chunk), n_max] with n_max its first clip's length, so
+    its padding is len(chunk) * n_max - (its clips' samples).  Clips of a (rate, format) are taken longest first and a
+    chunk is closed when the next clip would bring its padded bytes above ``max_bytes`` or its padding above
+    ``max_padding`` times its clips' samples; a clip larger than ``max_bytes`` on its own is a chunk of its own.  The
+    bounds default to _MAX_CHUNK_BYTES and _MAX_PADDING."""
+    from ._lib import DTYPE_I16
+    max_bytes = _MAX_CHUNK_BYTES if max_bytes is None else max_bytes
+    max_padding = _MAX_PADDING if max_padding is None else max_padding
+    groups = {}
+    for idx, c in enumerate(clips):
+        groups.setdefault((c.fs, c.code), []).append(idx)
+    chunks = []
+    for (_, code), idxs in groups.items():
+        item = 2 if code == DTYPE_I16 else 4
+        cur, n_max, payload = [], 0, 0
+        for i in sorted(idxs, key=lambda i: (-clips[i].n, i)):
+            n, k = clips[i].n, len(cur) + 1
+            if cur and (k * n_max * item > max_bytes or k * n_max - (payload + n) > max_padding * (payload + n)):
+                chunks.append(cur)
+                cur = []
+            if not cur:
+                n_max, payload = n, 0
+            cur.append(i)
+            payload += n
+        if cur:
+            chunks.append(cur)
+    return chunks
+
+
+def _upload_chunk(clips, code):
+    """Clips of one chunk, longest first -> ([n, N] device tensor, int64 device lengths [n]), N the first clip's
+    length; each row is zero past its clip.  int16 clips are staged in page-locked memory (files still on disk are
+    read straight into their row) so the H2D copy runs at full PCIe speed."""
     import torch
     from ._lib import DTYPE_I16
+    n_max = clips[0].n
+    lengths = torch.tensor([c.n for c in clips], dtype=torch.int64).cuda()
     if code == DTYPE_I16:
         from .audioio import PinnedBatch
-        pb = PinnedBatch(len(clips), n_samples)
+        pb = PinnedBatch(len(clips), n_max)
         for k, c in enumerate(clips):
-            if c.data is None:
-                pb.fill(k, c.path)
-            else:
-                pb.array[k] = c.data
+            pb.fill(k, c.path, c.data, n=c.n)
         dev = pb.to_device()
         torch.cuda.current_stream().synchronize()          # the staging buffer is released on return
-        return dev
-    return torch.from_numpy(np.stack([c.data for c in clips])).cuda()
+        return dev, lengths
+    x = np.zeros((len(clips), n_max), dtype=np.float32)
+    for k, c in enumerate(clips):
+        x[k, :c.n] = c.data
+    return torch.from_numpy(x).cuda(), lengths
 
 
 def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_short=False, want_long_term=False,
                   want_beat=False):
     """Mid-term results of a list of _Clip, in input order: (mid float64 [136 x M] or its long-term mean [136],
-    st float64 [68 x T] | None, (bpm, ratio) of beat_extraction(st, short_step) | None).  Equal (rate, length, format)
-    clips share launches, in chunks of <= 1 GiB of samples; the beat is computed on the GPU from the resident features."""
-    from .batch import mid_feature_extraction_batch, long_term_mean_batch, beat_extraction_batch
+    st float64 [68 x T] | None, (bpm, ratio) of beat_extraction(st, short_step) | None).  Clips of one (rate, format)
+    share launches as ragged batches (_plan_chunks); every clip's results are bit for bit those of the clip alone.  The
+    long-term mean and the beat are computed on the GPU from the resident features."""
+    from .batch import mid_feature_extraction_batch, long_term_mean_batch, beat_extraction_batch, frame_counts
+    L = lib()
     results = [None] * len(clips)
-    groups = {}
-    for idx, c in enumerate(clips):
-        groups.setdefault((c.fs, c.n, c.code), []).append(idx)
-    for (fs, n, code), idxs in groups.items():
-        per = max(1, int(_MAX_GROUP_BYTES // max(1, n * (2 if code == 0 else 4))))
-        for a in range(0, len(idxs), per):
-            part = idxs[a:a + per]
-            dev = _upload_group([clips[i] for i in part], n, code)
-            mid, st = mid_feature_extraction_batch(dev, fs, round(mid_window * fs), round(mid_step * fs),
-                                                   round(fs * short_window), round(fs * short_step))
-            first = (long_term_mean_batch(mid) if want_long_term else mid).cpu().numpy().astype(np.float64)
-            st_h = st.cpu().numpy().astype(np.float64) if want_short else None
-            beat = beat_extraction_batch(st, short_step).cpu().numpy() if want_beat else None
-            for k, i in enumerate(part):
-                results[i] = (first[k], st_h[k] if want_short else None, tuple(beat[k]) if want_beat else None)
+    for part in _plan_chunks(clips):
+        chunk = [clips[i] for i in part]
+        fs, code = chunk[0].fs, chunk[0].code
+        w, s = round(fs * short_window), round(fs * short_step)
+        mw, ms = round(mid_window * fs), round(mid_step * fs)
+        if L.b200aa_num_frames(chunk[-1].n, w, s) <= 0:
+            check(_lib.ERR_TOO_SHORT)       # alone, the shortest clip has no frames: a ragged batch would give it none
+        dev, lengths = _upload_chunk(chunk, code)
+        mid, st = mid_feature_extraction_batch(dev, fs, mw, ms, w, s, lengths=lengths)
+        stepr = mid_ratios(mw, ms, w, s)[1]
+        if want_long_term or want_beat:
+            n_frames, n_windows = frame_counts(lengths, w, s, stepr)
+        first = (long_term_mean_batch(mid, n_windows=n_windows) if want_long_term else mid).cpu().numpy().astype(np.float64)
+        st_h = st.cpu().numpy().astype(np.float64) if want_short else None
+        beat = beat_extraction_batch(st, short_step, n_frames=n_frames).cpu().numpy() if want_beat else None
+        for k, (i, c) in enumerate(zip(part, chunk)):
+            T = L.b200aa_num_frames(c.n, w, s)
+            results[i] = (first[k] if want_long_term else first[k][:, :L.b200aa_mid_windows(T, stepr)],
+                          st_h[k][:, :T] if want_short else None, tuple(beat[k]) if want_beat else None)
     return results
 
 
@@ -178,8 +220,17 @@ def directory_feature_extraction(folder_path, mid_window, mid_step, short_window
     decoded by ``audioio`` (.wav, .aif / .aiff, and .mp3 / .au / .ogg when pydub is installed, as in the reference; a
     file that cannot be decoded raises instead of silently changing the file list).  ``compute_beat=True`` appends
     ``bpm`` and ``ratio`` of the GPU short-term features, computed on the GPU (``batch.beat_extraction_batch``, bit for bit
-    this module's ``beat_extraction``, reference :18-84); only those two numbers per file are copied back.
+    this module's ``beat_extraction``, reference :18-84); only those two numbers per file are copied back.  Files of
+    any length share launches (ragged batches per sampling rate and sample format).
     """
+    clips = _folder_clips(folder_path)
+    res = _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_long_term=True, want_beat=compute_beat)
+    return _folder_features(clips, res, compute_beat)
+
+
+def _folder_clips(folder_path):
+    """The files of a folder that directory_feature_extraction analyses, as _Clip, with the reference's prints
+    (MidTermFeatures.py:155-190)."""
     types = ('*.wav', '*.aif', '*.aiff', '*.mp3', '*.au', '*.ogg')
     files = []
     for t in types:
@@ -201,12 +252,16 @@ def directory_feature_extraction(folder_path, mid_window, mid_step, short_window
                 print("  (AUDIO FILE TOO SMALL - SKIPPING)")
             continue
         clips.append(c)
+    return clips
+
+
+def _folder_features(clips, res, compute_beat):
+    """directory_feature_extraction's return value from its clips and their _mid_per_clip results (reference :191-221)."""
     names = []
     if not clips:
         return np.array([]), [], names
     st_names = ShortTermFeatures.feature_names(True)
     names = [n + "_mean" for n in st_names] + [n + "_std" for n in st_names]
-    res = _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_long_term=True, want_beat=compute_beat)
     out, out_files = np.array([]), []
     appended = False
     for c, (v, _, beat) in zip(clips, res):
@@ -222,10 +277,16 @@ def directory_feature_extraction(folder_path, mid_window, mid_step, short_window
 
 
 def multiple_directory_feature_extraction(path_list, mid_window, mid_step, short_window, short_step, compute_beat=False):
-    """Reference MidTermFeatures.py:224-260: one feature matrix per class folder."""
+    """Reference MidTermFeatures.py:224-260: one feature matrix per class folder.  Every folder is decoded first (its
+    "Analyzing file" lines print folder by folder), then the files of all folders share launches."""
+    per_dir = [_folder_clips(d) for d in path_list]
+    res = _mid_per_clip([c for clips in per_dir for c in clips], mid_window, mid_step, short_window, short_step,
+                        want_long_term=True, want_beat=compute_beat)
     features, class_names, file_names = [], [], []
-    for d in path_list:
-        f, fn, _ = directory_feature_extraction(d, mid_window, mid_step, short_window, short_step, compute_beat=compute_beat)
+    a = 0
+    for d, clips in zip(path_list, per_dir):
+        f, fn, _ = _folder_features(clips, res[a:a + len(clips)], compute_beat)
+        a += len(clips)
         if f.shape[0] > 0:
             features.append(f)
             file_names.append(fn)
@@ -264,7 +325,12 @@ def mid_feature_extraction_to_file(file_path, mid_window, mid_step, short_window
                                    store_short_features=False, store_csv=False, plot=False):
     """Reference MidTermFeatures.py:324-362: <output>_mt.npy ([136 x M] float64), optional <output>_st.npy
     ([68 x T]) and transposed CSV copies -- the on-disk formats the reference's CLI consumers read."""
-    (mid, st, _), = _mid_per_clip([_open_clip(file_path)], mid_window, mid_step, short_window, short_step, want_short=True)
+    (mid, st, _), = _mid_per_clip([_open_clip(file_path)], mid_window, mid_step, short_window, short_step,
+                                  want_short=store_short_features)
+    _save_features(output_file, mid, st, store_short_features, store_csv, plot)
+
+
+def _save_features(output_file, mid, st, store_short_features, store_csv, plot):
     if store_short_features:
         np.save(output_file + "_st", st)
         if plot:
@@ -284,7 +350,10 @@ def mid_feature_extraction_to_file(file_path, mid_window, mid_step, short_window
 
 def mid_feature_extraction_file_dir(folder_path, mid_window, mid_step, short_window, short_step,
                                     store_short_features=False, store_csv=False, plot=False):
-    """Reference MidTermFeatures.py:365-377."""
-    for f in glob.glob(folder_path + os.sep + '*.wav'):
-        mid_feature_extraction_to_file(f, mid_window, mid_step, short_window, short_step, f,
-                                       store_short_features, store_csv, plot)
+    """Reference MidTermFeatures.py:365-377: mid_feature_extraction_to_file(f, ..., output_file=f) for every .wav file
+    of the folder, the files computed in shared launches and written in the reference's order."""
+    files = glob.glob(folder_path + os.sep + '*.wav')
+    res = _mid_per_clip([_open_clip(f) for f in files], mid_window, mid_step, short_window, short_step,
+                        want_short=store_short_features)
+    for f, (mid, st, _) in zip(files, res):
+        _save_features(f, mid, st, store_short_features, store_csv, plot)

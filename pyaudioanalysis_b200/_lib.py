@@ -45,6 +45,9 @@ SIGNATURES = {
     "b200aa_chromagram": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_mid_pool": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_int, c_int, c_vp, c_vp]),
     "b200aa_long_term_mean": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp]),
+    "b200aa_frame_counts": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "b200aa_mid_pool_ragged": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_int, c_vp, c_vp]),
+    "b200aa_long_term_mean_ragged": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_normalize_windows": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "b200aa_beat_extraction": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),

@@ -140,13 +140,18 @@ class PinnedBatch:
         self.array = self._buf.array
         self.direct = 0                 # files decoded without an intermediate copy
 
-    def fill(self, i, path, decoded=None):
-        if decoded is None and read_wav_into(path, self.array[i]) is not None:
+    def fill(self, i, path, decoded=None, n=None):
+        """Row ``i`` <- the file's samples.  ``n``: the file has that many samples (a ragged batch): they go to
+        ``array[i, :n]`` and the rest of the row is zeroed."""
+        row = self.array[i] if n is None else self.array[i, :n]
+        if n is not None:
+            self.array[i, n:] = 0
+        if decoded is None and read_wav_into(path, row) is not None:
             self.direct += 1
             return
         if decoded is None:
             decoded = stereo_to_mono(read_audio_file(path)[1])
-        self.array[i] = decoded
+        row[...] = decoded
 
     def to_device(self):
         import torch

@@ -105,12 +105,58 @@ def feature_extraction_batch(signals, sampling_rate, window, step, deltas=True, 
     return out
 
 
+def _counts(t, B, name):
+    """A per-clip count argument: an int64 CUDA tensor [B]."""
+    _require_cuda(t, name)
+    if t.dtype != torch.int64 or tuple(t.shape) != (B,):
+        raise ValueError("%s must be an int64 tensor [B]" % name)
+    return t.contiguous()
+
+
+def frame_counts(lengths, window, step, step_ratio=None):
+    """Per-clip counts of a ragged batch, computed on the device: int64 CUDA ``n_frames [B]`` (short-term frames of
+    ``lengths[b]`` samples, ``feature_extraction_batch``'s columns of clip b), and with ``step_ratio`` also
+    ``n_windows [B]`` (its mid-term windows, ``mid_pool_batch``'s columns) as ``(n_frames, n_windows)``."""
+    _require_cuda(lengths, "lengths")
+    if lengths.dim() != 1:
+        raise ValueError("lengths must be a tensor [B]")
+    lengths = lengths.to(torch.int64).contiguous()
+    B = lengths.shape[0]
+    with torch.cuda.device(lengths.device):
+        frames = torch.empty((B,), dtype=torch.int64, device=lengths.device)
+        windows = None if step_ratio is None else torch.empty((B,), dtype=torch.int64, device=lengths.device)
+        if step_ratio is not None and int(step_ratio) < 1:
+            raise ValueError("mid-term step shorter than half a short-term step")
+        if B:
+            check(lib().b200aa_frame_counts(ctypes.c_void_p(lengths.data_ptr()), B, int(window), int(step),
+                                            1 if step_ratio is None else int(step_ratio), ctypes.c_void_p(frames.data_ptr()),
+                                            None if windows is None else ctypes.c_void_p(windows.data_ptr()), _stream()))
+    return frames if windows is None else (frames, windows)
+
+
 def mid_pool_batch(st, ratio, step_ratio, n_frames=None):
-    """Mean / population-std pooling (kernel 2): CUDA float32 [B, F, T] -> [B, 2F, M]."""
+    """Mean / population-std pooling (kernel 2): CUDA float32 [B, F, T] -> [B, 2F, M].
+
+    ``n_frames``: None (every clip has T frames), an int (every clip has that many), or an int64 CUDA tensor [B] of each
+    clip's own frame count, clamped to [0, T], e.g. from ``frame_counts``.  With a tensor the output is zero-filled
+    [B, 2F, mid_windows(T)] and clip b's first M_b = mid_windows(n_frames[b]) columns are bit for bit what the clip gives
+    pooled alone with ``n_frames = n_frames[b]``."""
     _require_cuda(st, "st")
     if st.dim() != 3 or st.dtype != torch.float32 or not st.is_contiguous():
         raise ValueError("st must be contiguous float32 [B, F, T]")
     B, F, Tst = st.shape
+    if isinstance(n_frames, torch.Tensor):
+        n_frames = _counts(n_frames, B, "n_frames")
+        if int(step_ratio) < 1:
+            check(_lib.ERR_INVALID)
+        M = lib().b200aa_mid_windows(Tst, int(step_ratio))
+        with torch.cuda.device(st.device):
+            mid = torch.zeros((B, 2 * F, M), dtype=torch.float32, device=st.device)
+            if mid.numel():
+                check(lib().b200aa_mid_pool_ragged(ctypes.c_void_p(st.data_ptr()), B, F, Tst,
+                                                   ctypes.c_void_p(n_frames.data_ptr()), int(ratio), int(step_ratio),
+                                                   ctypes.c_void_p(mid.data_ptr()), _stream()))
+        return mid
     T = Tst if n_frames is None else int(n_frames)
     M = lib().b200aa_mid_windows(T, int(step_ratio))
     with torch.cuda.device(st.device):
@@ -120,15 +166,27 @@ def mid_pool_batch(st, ratio, step_ratio, n_frames=None):
     return mid
 
 
-def long_term_mean_batch(mid):
-    """Mean over the mid-term windows: CUDA float32 [B, rows, M] -> [B, rows] (MidTermFeatures.py:200-201)."""
+def long_term_mean_batch(mid, n_windows=None):
+    """Mean over the mid-term windows: CUDA float32 [B, rows, M] -> [B, rows] (MidTermFeatures.py:200-201).
+
+    ``n_windows`` (int64 CUDA [B], entries clamped to [0, M]): clip b averages its first n_windows[b] columns, bit for
+    bit as it would alone; a clip of no windows gives NaN, as np.mean of an empty axis does."""
     _require_cuda(mid, "mid")
     if mid.dim() != 3 or mid.dtype != torch.float32 or not mid.is_contiguous():
         raise ValueError("mid must be contiguous float32 [B, rows, M]")
     B, rows, M = mid.shape
     with torch.cuda.device(mid.device):
         out = torch.empty((B, rows), dtype=torch.float32, device=mid.device)
-        check(lib().b200aa_long_term_mean(ctypes.c_void_p(mid.data_ptr()), B, rows, M, ctypes.c_void_p(out.data_ptr()), _stream()))
+        if n_windows is None:
+            check(lib().b200aa_long_term_mean(ctypes.c_void_p(mid.data_ptr()), B, rows, M, ctypes.c_void_p(out.data_ptr()),
+                                              _stream()))
+            return out
+        n_windows = _counts(n_windows, B, "n_windows")
+        if M == 0:                  # no columns to read: give the kernel a valid pointer, every clip averages none
+            mid = mid.new_zeros((1,))
+        check(lib().b200aa_long_term_mean_ragged(ctypes.c_void_p(mid.data_ptr()), B, rows, M,
+                                                 ctypes.c_void_p(n_windows.data_ptr()), ctypes.c_void_p(out.data_ptr()),
+                                                 _stream()))
     return out
 
 
@@ -147,10 +205,7 @@ def beat_extraction_batch(st, window_size, n_frames=None):
     B, F, T = st.shape
     fr_ptr = None
     if n_frames is not None:
-        _require_cuda(n_frames, "n_frames")
-        if n_frames.dtype != torch.int64 or tuple(n_frames.shape) != (B,):
-            raise ValueError("n_frames must be an int64 tensor [B]")
-        n_frames = n_frames.contiguous()
+        n_frames = _counts(n_frames, B, "n_frames")
         fr_ptr = ctypes.c_void_p(n_frames.data_ptr())
     with torch.cuda.device(st.device):
         out = torch.empty((B, 2), dtype=torch.float64, device=st.device)
@@ -171,14 +226,17 @@ def mid_ratios(mid_window, mid_step, short_window, short_step):
     return int(ratio), stepr
 
 
-def mid_feature_extraction_batch(signals, sampling_rate, mid_window, mid_step, short_window, short_step):
+def mid_feature_extraction_batch(signals, sampling_rate, mid_window, mid_step, short_window, short_step, lengths=None):
     """Batched MidTermFeatures.mid_feature_extraction: returns (mid [B,136,M], st [B,68,T]) on the GPU.  ``ratio <= 0``
-    pools Python slices as the reference does (empty windows give 0); a step ratio < 1 raises ValueError."""
-    st = feature_extraction_batch(signals, sampling_rate, short_window, short_step, deltas=True)
+    pools Python slices as the reference does (empty windows give 0); a step ratio < 1 raises ValueError.
+    ``lengths`` (int64 CUDA [B]) makes the batch ragged: clip b is ``signals[b, :lengths[b]]``, its columns past its own
+    frame count in ``st`` and past its own window count in ``mid`` are zero (``frame_counts`` gives both counts)."""
+    st = feature_extraction_batch(signals, sampling_rate, short_window, short_step, deltas=True, lengths=lengths)
     ratio, stepr = mid_ratios(mid_window, mid_step, short_window, short_step)
     if stepr < 1:
         raise ValueError("mid-term step shorter than half a short-term step")
-    return mid_pool_batch(st, ratio, stepr), st
+    n_frames = None if lengths is None else frame_counts(lengths, short_window, short_step)
+    return mid_pool_batch(st, ratio, stepr, n_frames=n_frames), st
 
 
 def spectrogram_batch(signals, sampling_rate, window, step, plan=None, norm=None, out=None):

@@ -114,10 +114,14 @@ extern "C" int64_t b200aa_chromagram_rows(int64_t n, int w, int s)
     if (w < 1 || s < 1) return 0;
     return (n - s - w) / s + 1;     // C division truncates toward zero like int(x / y) (:347)
 }
-extern "C" int64_t b200aa_mid_windows(int64_t n_frames, int stepr)
+// the counts the device needs per clip of a ragged batch; b200aa_num_frames / b200aa_mid_windows on the host
+__host__ __device__ inline int64_t frames_of(int64_t n, int w, int s) { return n < w ? 0 : (n - w) / s + 1; }
+__host__ __device__ inline int64_t windows_of(int64_t n_frames, int stepr)
 {
     return (stepr < 1 || n_frames <= 0) ? 0 : (n_frames + stepr - 1) / stepr;
 }
+
+extern "C" int64_t b200aa_mid_windows(int64_t n_frames, int stepr) { return windows_of(n_frames, stepr); }
 
 // ------------------------------------------------------------------------------------------------
 // plan
@@ -604,8 +608,14 @@ extern "C" int b200aa_clip_stats(const void *d_sig, int dtype, int64_t n_clips, 
 // ------------------------------------------------------------------------------------------------
 // kernel 2: mid-term pooling (MidTermFeatures.py:110-126): one warp per (clip, feature row, window)
 // ------------------------------------------------------------------------------------------------
+// frames (nullable, int64 [n_clips]): clip b has T_b = clamp(frames[b], 0, t_stride) frames and M_b = windows_of(T_b)
+// windows; warps of windows j >= M_b write nothing.  Without frames every clip has T frames.  A warp's sums depend only
+// on (c0, c1, lane), so a clip pooled in a ragged batch gives bit for bit what it gives alone with T = T_b.  RAGGED is
+// a template flag only so that the batch without counts keeps the code (and time) it had before counts existed.
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) mid_pool_kernel(const float *st, int64_t n_clips, int F, int64_t T,
-                                                        int64_t t_stride, int ratio, int stepr, int64_t M, float *mid)
+                                                        int64_t t_stride, const int64_t *frames, int ratio, int stepr,
+                                                        int64_t M, float *mid)
 {
     const int lane = threadIdx.x & 31;
     const int64_t wid = (blockIdx.x * int64_t(blockDim.x) + threadIdx.x) >> 5;
@@ -614,6 +624,10 @@ __global__ void __launch_bounds__(256) mid_pool_kernel(const float *st, int64_t 
     const int64_t j = wid % M, bf = wid / M;
     const int64_t b = bf / F;
     const int f = int(bf - b * F);
+    if (RAGGED) {
+        T = min(max(frames[b], int64_t(0)), t_stride);
+        if (j >= windows_of(T, stepr)) return;              // the whole warp: j is uniform across it
+    }
     // window j is the Python slice row[c0 : min(c0 + ratio, T)] (:116-120): a negative end counts from the end of
     // the row (ratio < 0), an end before c0 gives an empty window; n = 0 makes mean and std 0 / 0 -> 0 below
     const int64_t c0 = j * stepr;
@@ -642,44 +656,103 @@ __global__ void __launch_bounds__(256) mid_pool_kernel(const float *st, int64_t 
     }
 }
 
+// d_mid's row stride is M = windows_of(T): with frames, T = t_stride, the longest any clip can have
+static int mid_pool_launch(const float *d_st, int64_t n_clips, int n_feats, int64_t T, int64_t t_stride, const int64_t *d_frames,
+                           int ratio, int step_ratio, float *d_mid, void *stream)
+{
+    const int64_t M = windows_of(T, step_ratio);
+    const int64_t warps = n_clips * n_feats * M;
+    if (warps == 0) return B200AA_OK;
+    const int64_t blocks = (warps * 32 + 255) / 256;
+    auto kernel = d_frames ? mid_pool_kernel<true> : mid_pool_kernel<false>;
+    kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_st, n_clips, n_feats, T, t_stride, d_frames,
+                                                                             ratio, step_ratio, M, d_mid);
+    CK_LAUNCH("mid_pool_kernel");
+    return B200AA_OK;
+}
+
 extern "C" int b200aa_mid_pool(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
                                int ratio, int step_ratio, float *d_mid, void *stream)
 {
     NvtxRange nvtx_("b200aa_mid_pool");
     if (!d_st || !d_mid || n_clips < 0 || n_feats < 1 || n_frames < 1 || step_ratio < 1 || t_stride < n_frames)
         return B200AA_ERR_INVALID;
-    const int64_t M = b200aa_mid_windows(n_frames, step_ratio);
-    const int64_t warps = n_clips * n_feats * M;
-    if (warps == 0) return B200AA_OK;
-    const int64_t blocks = (warps * 32 + 255) / 256;
-    mid_pool_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_st, n_clips, n_feats, n_frames, t_stride,
-                                                                                       ratio, step_ratio, M, d_mid);
-    CK_LAUNCH("mid_pool_kernel");
-    return B200AA_OK;
+    return mid_pool_launch(d_st, n_clips, n_feats, n_frames, t_stride, nullptr, ratio, step_ratio, d_mid, stream);
 }
 
-// long-term average of the mid-term matrix: one warp per (clip, row), fp64 accumulation
-__global__ void __launch_bounds__(256) long_term_mean_kernel(const float *mid, int64_t rows_total, int64_t M, float *out)
+extern "C" int b200aa_mid_pool_ragged(const float *d_st, int64_t n_clips, int n_feats, int64_t t_stride,
+                                      const int64_t *d_frames, int ratio, int step_ratio, float *d_mid, void *stream)
+{
+    NvtxRange nvtx_("b200aa_mid_pool_ragged");
+    if (!d_st || !d_frames || !d_mid || n_clips < 0 || n_feats < 1 || step_ratio < 1 || t_stride < 0)
+        return B200AA_ERR_INVALID;
+    return mid_pool_launch(d_st, n_clips, n_feats, t_stride, t_stride, d_frames, ratio, step_ratio, d_mid, stream);
+}
+
+// long-term average of the mid-term matrix: one warp per (clip, row), fp64 accumulation.  windows (nullable, int64
+// [n_clips]): clip b averages its first M_b = clamp(windows[b], 0, M) columns (0 / 0 = NaN for none, as np.mean of an
+// empty axis); the sum's order depends only on (M_b, lane), as in mid_pool_kernel.
+__global__ void __launch_bounds__(256) long_term_mean_kernel(const float *mid, int64_t rows_total, int n_rows, int64_t M,
+                                                             const int64_t *windows, float *out)
 {
     const int lane = threadIdx.x & 31;
     const int64_t wid = (blockIdx.x * int64_t(blockDim.x) + threadIdx.x) >> 5;
     if (wid >= rows_total) return;
+    const int64_t Mb = windows ? min(max(windows[wid / n_rows], int64_t(0)), M) : M;
     const float *row = mid + size_t(wid) * M;
     double s = 0.0;
-    for (int64_t c = lane; c < M; c += 32) s += double(row[c]);
+    for (int64_t c = lane; c < Mb; c += 32) s += double(row[c]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) out[wid] = float(s / double(M));
+    if (lane == 0) out[wid] = float(s / double(Mb));
+}
+
+static int long_term_mean_launch(const float *d_mid, int64_t n_clips, int n_rows, int64_t m_stride, const int64_t *d_windows,
+                                 float *d_out, void *stream)
+{
+    const int64_t rows = n_clips * n_rows;
+    if (rows == 0) return B200AA_OK;
+    const int64_t blocks = (rows * 32 + 255) / 256;
+    long_term_mean_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_mid, rows, n_rows, m_stride,
+                                                                                             d_windows, d_out);
+    CK_LAUNCH("long_term_mean_kernel");
+    return B200AA_OK;
 }
 
 extern "C" int b200aa_long_term_mean(const float *d_mid, int64_t n_clips, int n_rows, int64_t n_windows, float *d_out, void *stream)
 {
     if (!d_mid || !d_out || n_clips < 0 || n_rows < 1 || n_windows < 1) return B200AA_ERR_INVALID;
-    const int64_t rows = n_clips * n_rows;
-    if (rows == 0) return B200AA_OK;
-    const int64_t blocks = (rows * 32 + 255) / 256;
-    long_term_mean_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_mid, rows, n_windows, d_out);
-    CK_LAUNCH("long_term_mean_kernel");
+    return long_term_mean_launch(d_mid, n_clips, n_rows, n_windows, nullptr, d_out, stream);
+}
+
+extern "C" int b200aa_long_term_mean_ragged(const float *d_mid, int64_t n_clips, int n_rows, int64_t m_stride,
+                                            const int64_t *d_windows, float *d_out, void *stream)
+{
+    if (!d_mid || !d_windows || !d_out || n_clips < 0 || n_rows < 1 || m_stride < 0) return B200AA_ERR_INVALID;
+    return long_term_mean_launch(d_mid, n_clips, n_rows, m_stride, d_windows, d_out, stream);
+}
+
+// per-clip counts of a ragged batch from its device lengths: one thread per clip
+__global__ void __launch_bounds__(256) frame_counts_kernel(const int64_t *len, int64_t n_clips, int w, int s, int stepr,
+                                                           int64_t *frames, int64_t *windows)
+{
+    const int64_t b = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+    if (b >= n_clips) return;
+    const int64_t T = frames_of(len[b], w, s);
+    frames[b] = T;
+    if (windows) windows[b] = windows_of(T, stepr);
+}
+
+extern "C" int b200aa_frame_counts(const int64_t *d_len, int64_t n_clips, int window, int step, int step_ratio,
+                                   int64_t *d_frames, int64_t *d_windows, void *stream)
+{
+    if (!d_len || !d_frames || n_clips < 0 || window < 1 || step < 1 || (d_windows && step_ratio < 1))
+        return B200AA_ERR_INVALID;
+    if (n_clips == 0) return B200AA_OK;
+    const int64_t blocks = (n_clips + 255) / 256;
+    frame_counts_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_len, n_clips, window, step,
+                                                                                           step_ratio, d_frames, d_windows);
+    CK_LAUNCH("frame_counts_kernel");
     return B200AA_OK;
 }
 
