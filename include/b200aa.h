@@ -127,6 +127,30 @@ int b200aa_chromagram(const b200aa_plan *plan, const void *d_sig, int dtype, int
                       int64_t n_samples, int64_t clip_stride,
                       const b200aa_clip_norm *d_norm, float *d_out, void *stream);
 
+/* Spectrogram / chromagram rows of a ragged batch: clip b is the first d_len[b] samples (int64 [n_clips] on the device,
+ * at most n_samples) of its row of d_sig; d_norm from b200aa_clip_stats with the same d_len.  d_out float32
+ * [n_clips, R, K] (spectrogram) / [n_clips, R, 12] (chromagram) with R = b200aa_spectrogram_rows(n_samples) /
+ * b200aa_chromagram_rows(n_samples), the rows of the widest possible clip.  Clip b's rows below R_b =
+ * b200aa_row_counts(d_len)[b] are bit for bit what b200aa_spectrogram / b200aa_chromagram give for the clip alone
+ * (zero rows included); rows >= R_b are not written, and a clip the single-clip entry point refuses (R_b = 0) gets
+ * nothing written.  NULL pointers, clip_stride < n_samples and a bad dtype are B200AA_ERR_INVALID; R <= 0 is
+ * B200AA_ERR_TOO_SHORT; a plan whose chroma table the reference cannot build makes the chromagram entry point return
+ * B200AA_ERR_CHROMA for the whole batch.  Nothing synchronises: the counts never leave the device.
+ * Replaces: spectrogram() / chromagram() (ShortTermFeatures.py:324-452) of every file of a set of different lengths. */
+int b200aa_spectrogram_ragged(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                              int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                              const b200aa_clip_norm *d_norm, float *d_out, void *stream);
+int b200aa_chromagram_ragged(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                             int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                             const b200aa_clip_norm *d_norm, float *d_out, void *stream);
+
+/* Per-clip rows of a ragged spectrogram (which = 0) or chromagram (which = 1), computed on the device: d_rows int64
+ * [n_clips] = b200aa_spectrogram_rows / b200aa_chromagram_rows(d_len[b]), or 0 for a clip b200aa_spectrogram /
+ * b200aa_chromagram refuse (every accepted clip has at least one row).  NULL pointers, n_clips < 0, window < 1,
+ * step < 1 and another `which` are B200AA_ERR_INVALID.  Nothing synchronises. */
+int b200aa_row_counts(const int64_t *d_len, int64_t n_clips, int window, int step, int which, int64_t *d_rows,
+                      void *stream);
+
 /* Kernel 2: mid-term pooling.  d_st float32 [n_clips, F, t_stride] (n_frames valid columns),
  * d_mid float32 [n_clips, 2F, M], M = b200aa_mid_windows(n_frames, step_ratio): rows 0..F-1 means,
  * F..2F-1 population standard deviations of st[f][c : min(c+ratio, T)], c = j*step_ratio.

@@ -43,6 +43,11 @@ SIGNATURES = {
     "b200aa_st_features": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]),
     "b200aa_spectrogram": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_chromagram": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    # (plan, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out, stream)
+    "b200aa_spectrogram_ragged": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "b200aa_chromagram_ragged": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    # (d_len, n_clips, window, step, which: 0 spectrogram / 1 chromagram, d_rows, stream)
+    "b200aa_row_counts": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp]),
     "b200aa_mid_pool": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_int, c_int, c_vp, c_vp]),
     "b200aa_long_term_mean": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp]),
     "b200aa_frame_counts": (c_int, [c_vp, c_i64, c_int, c_int, c_int, c_vp, c_vp, c_vp]),

@@ -239,39 +239,74 @@ def mid_feature_extraction_batch(signals, sampling_rate, mid_window, mid_step, s
     return mid_pool_batch(st, ratio, stepr, n_frames=n_frames), st
 
 
-def spectrogram_batch(signals, sampling_rate, window, step, plan=None, norm=None, out=None):
+def row_counts(lengths, window, step, which):
+    """Per-clip output rows of a ragged ``spectrogram_batch`` (``which = 0``) or ``chromagram_batch`` (``which = 1``),
+    computed on the device: int64 CUDA [B], ``lengths[b]``'s row count, or 0 for a clip the equal-length call refuses
+    (every accepted clip has at least one row)."""
+    _require_cuda(lengths, "lengths")
+    if lengths.dim() != 1:
+        raise ValueError("lengths must be a tensor [B]")
+    if which not in (0, 1):
+        raise ValueError("which must be 0 (spectrogram) or 1 (chromagram)")
+    lengths = lengths.to(torch.int64).contiguous()
+    B = lengths.shape[0]
+    with torch.cuda.device(lengths.device):
+        rows = torch.empty((B,), dtype=torch.int64, device=lengths.device)
+        if B:
+            check(lib().b200aa_row_counts(ctypes.c_void_p(lengths.data_ptr()), B, int(window), int(step), which,
+                                          ctypes.c_void_p(rows.data_ptr()), _stream()))
+    return rows
+
+
+def spectrogram_batch(signals, sampling_rate, window, step, plan=None, norm=None, out=None, lengths=None):
     """CUDA [B, N] -> CUDA float32 [B, R, K] (ShortTermFeatures.py:389-452 rows, per clip).  ``norm``: records of a previous
-    ``clip_stats`` call on the same clips; ``out``: a contiguous float32 [B, R, K] tensor to write into."""
+    ``clip_stats`` call on the same clips; ``out``: a contiguous float32 [B, R, K] tensor to write into.  ``lengths``
+    (int64 CUDA [B]) makes the batch ragged: clip b is ``signals[b, :lengths[b]]``, R is the row count of N samples, and
+    only clip b's first ``row_counts(lengths, window, step, 0)[b]`` rows are written, bit for bit what the clip gives
+    alone (none for a clip the equal-length call refuses); an output allocated here is zero-filled."""
     window, step = int(window), int(step)
-    signals, B, N, stride, _, _ = _prep(signals, None)
+    signals, B, N, stride, lengths, len_ptr = _prep(signals, lengths)
     with torch.cuda.device(signals.device):
         plan = plan or get_plan(sampling_rate, window, step, signals.device.index)
         R = lib().b200aa_spectrogram_rows(N, window, step)
         if R <= 0:
             check(_lib.ERR_TOO_SHORT)
         if out is None:
-            out = torch.empty((B, R, window // 2), dtype=torch.float32, device=signals.device)
+            alloc = torch.zeros if lengths is not None else torch.empty
+            out = alloc((B, R, window // 2), dtype=torch.float32, device=signals.device)
         elif tuple(out.shape) != (B, R, window // 2) or out.dtype != torch.float32 or not out.is_contiguous() or not out.is_cuda:
             raise ValueError("out must be a contiguous float32 CUDA tensor [B, %d, %d]" % (R, window // 2))
         if norm is None:
-            norm = clip_stats(signals)
-        check(lib().b200aa_spectrogram(plan.handle, ctypes.c_void_p(signals.data_ptr()), _dtype_code(signals), B, N, stride,
-                                       ctypes.c_void_p(norm.data_ptr()), ctypes.c_void_p(out.data_ptr()), _stream()))
+            norm = clip_stats(signals, lengths)
+        args = (plan.handle, ctypes.c_void_p(signals.data_ptr()), _dtype_code(signals), B, N, stride)
+        tail = (ctypes.c_void_p(norm.data_ptr()), ctypes.c_void_p(out.data_ptr()), _stream())
+        if lengths is None:
+            check(lib().b200aa_spectrogram(*args, *tail))
+        else:
+            check(lib().b200aa_spectrogram_ragged(*args, len_ptr, *tail))
     return out
 
 
-def chromagram_batch(signals, sampling_rate, window, step, plan=None, norm=None):
-    """CUDA [B, N] -> CUDA float32 [B, R, 12] (ShortTermFeatures.py:324-386 rows, per clip)."""
+def chromagram_batch(signals, sampling_rate, window, step, plan=None, norm=None, lengths=None):
+    """CUDA [B, N] -> CUDA float32 [B, R, 12] (ShortTermFeatures.py:324-386 rows, per clip).  ``lengths`` (int64 CUDA [B])
+    makes the batch ragged: clip b is ``signals[b, :lengths[b]]``, R is the row count of N samples, and the output is
+    zero-filled; clip b's first ``row_counts(lengths, window, step, 1)[b]`` rows are bit for bit what the clip gives alone,
+    clipped last frames included, and a clip the equal-length call refuses keeps zero rows."""
     window, step = int(window), int(step)
-    signals, B, N, stride, _, _ = _prep(signals, None)
+    signals, B, N, stride, lengths, len_ptr = _prep(signals, lengths)
     with torch.cuda.device(signals.device):
         plan = plan or get_plan(sampling_rate, window, step, signals.device.index)
         R = lib().b200aa_chromagram_rows(N, window, step)
-        if R <= 0 or N - step - window < 0:
+        if R <= 0 or (lengths is None and N - step - window < 0):
             check(_lib.ERR_TOO_SHORT)
-        out = torch.empty((B, R, 12), dtype=torch.float32, device=signals.device)
+        alloc = torch.zeros if lengths is not None else torch.empty
+        out = alloc((B, R, 12), dtype=torch.float32, device=signals.device)
         if norm is None:
-            norm = clip_stats(signals)
-        check(lib().b200aa_chromagram(plan.handle, ctypes.c_void_p(signals.data_ptr()), _dtype_code(signals), B, N, stride,
-                                      ctypes.c_void_p(norm.data_ptr()), ctypes.c_void_p(out.data_ptr()), _stream()))
+            norm = clip_stats(signals, lengths)
+        args = (plan.handle, ctypes.c_void_p(signals.data_ptr()), _dtype_code(signals), B, N, stride)
+        tail = (ctypes.c_void_p(norm.data_ptr()), ctypes.c_void_p(out.data_ptr()), _stream())
+        if lengths is None:
+            check(lib().b200aa_chromagram(*args, *tail))
+        else:
+            check(lib().b200aa_chromagram_ragged(*args, len_ptr, *tail))
     return out

@@ -105,14 +105,11 @@ extern "C" int64_t b200aa_num_frames(int64_t n, int w, int s)
 }
 extern "C" int64_t b200aa_spectrogram_rows(int64_t n, int w, int s)
 {
-    if (w < 1 || s < 1) return 0;
-    // int((N - w) / s) + 1 with Python's truncation toward zero (ShortTermFeatures.py:413)
-    return (n - w) / s + 1;
+    return (w < 1 || s < 1) ? 0 : rows::spectrogram(n, w, s).R;
 }
 extern "C" int64_t b200aa_chromagram_rows(int64_t n, int w, int s)
 {
-    if (w < 1 || s < 1) return 0;
-    return (n - s - w) / s + 1;     // C division truncates toward zero like int(x / y) (:347)
+    return (w < 1 || s < 1) ? 0 : rows::chromagram(n, w, s).R;
 }
 // the counts the device needs per clip of a ragged batch; b200aa_num_frames / b200aa_mid_windows on the host
 __host__ __device__ inline int64_t frames_of(int64_t n, int w, int s) { return n < w ? 0 : (n - w) / s + 1; }
@@ -756,6 +753,27 @@ extern "C" int b200aa_frame_counts(const int64_t *d_len, int64_t n_clips, int wi
     return B200AA_OK;
 }
 
+// per-clip output rows of a ragged spectrogram (which = 0) / chromagram (1): R_b, or 0 where the single-clip entry point
+// refuses the clip
+__global__ void __launch_bounds__(256) row_counts_kernel(const int64_t *len, int64_t n_clips, int w, int s, int which, int64_t *out)
+{
+    const int64_t b = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+    if (b >= n_clips) return;
+    const rows::Rows r = which ? rows::chromagram(len[b], w, s) : rows::spectrogram(len[b], w, s);
+    out[b] = r.refused ? 0 : r.R;
+}
+
+extern "C" int b200aa_row_counts(const int64_t *d_len, int64_t n_clips, int window, int step, int which, int64_t *d_rows,
+                                 void *stream)
+{
+    if (!d_len || !d_rows || n_clips < 0 || window < 1 || step < 1 || (which != 0 && which != 1)) return B200AA_ERR_INVALID;
+    if (n_clips == 0) return B200AA_OK;
+    const int64_t blocks = (n_clips + 255) / 256;
+    row_counts_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_len, n_clips, window, step, which, d_rows);
+    CK_LAUNCH("row_counts_kernel");
+    return B200AA_OK;
+}
+
 // (mid[b, f, j] - mean[f]) / std[f] -> out[b, j, f]: 32 x 32 tiles through shared memory, both sides coalesced
 // (audioSegmentation.py:581-584: one column of the mid-term matrix at a time)
 __global__ void normalize_windows_kernel(const float *__restrict__ mid, int n_rows, int64_t n_windows, const float *__restrict__ mean,
@@ -1000,6 +1018,9 @@ static int launch_generic(const b200aa_plan *pl, StParams &p, int64_t rows_max, 
     if (p.n_items == 0) return B200AA_OK;
     if (big) {
         auto kern = st_generic_kernel<MODE, true>;
+        if constexpr (MODE != kModeFeatures) {
+            if (p.len) kern = st_generic_kernel<MODE, true, true>;
+        }
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
         const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * 2);
         p.scratch_stride = generic_big_bytes(G, p.Nc, p.Kp);
@@ -1014,6 +1035,9 @@ static int launch_generic(const b200aa_plan *pl, StParams &p, int64_t rows_max, 
         return B200AA_OK;
     }
     auto kern = st_generic_kernel<MODE, false>;
+    if constexpr (MODE != kModeFeatures) {
+        if (p.len) kern = st_generic_kernel<MODE, false, true>;
+    }
     CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));   // constant: no race between launching threads
     int occ = 1;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
@@ -1078,49 +1102,130 @@ extern "C" int b200aa_st_features(const b200aa_plan *plan, const void *d_sig, in
     return launch_generic<kModeFeatures>(pl, p, T, st);
 }
 
+// The plan's row kernel over every clip: the per-frame solo kernel, else the register-tiled CTA kernel (the pair kernel
+// has no row mode), else the generic kernel.  p.len set: a ragged batch, every clip with its own rows (ragged_rows).
+template <int MODE>
+static int launch_rows(b200aa_plan *pl, StParams &p, cudaStream_t st)
+{
+    int rc = B200AA_OK;
+    if (use_solo(pl)) {
+        unsigned slot = 0;
+        unsigned int *ctr = nullptr;
+        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
+        rc = solo_launch_mode<MODE>(pl->solo, p, pl->sm_count, p.rows_launch, ctr, b200aa_plan::kSlotBytes, st);
+        const int rc2 = slot_done(pl, st, slot);
+        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "solo kernel") : rc;
+    }
+    if (pl->fast_kind && !pl->force_generic && pl->prefer != 0 && pl->prefer != 3) {
+        unsigned slot = 0;
+        unsigned int *ctr = nullptr;
+        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
+        rc = fast_launch_rows(pl->fast_kind, MODE, pl->fast, p, pl->sm_count, ctr, st);
+        const int rc2 = slot_done(pl, st, slot);
+        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "fast kernel") : rc;
+    }
+    return launch_generic<MODE>(pl, p, p.rows_launch, st);
+}
+
+// Every clipped chromagram frame of the batch in one launch of clipped_chroma_kernel: per_clip candidate rows per clip
+static int launch_clipped(const b200aa_plan *pl, StParams p, int64_t per_clip, cudaStream_t st)
+{
+    constexpr size_t kSmemCap = 226 * 1024;        // the per-CTA opt-in maximum, less the static reserve
+    p.n_items = p.n_clips * per_clip;
+    const size_t bytes = clipped_bytes(p.window, p.K);
+    if (bytes <= kSmemCap) {
+        CK(cudaFuncSetAttribute(clipped_chroma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemCap));
+        const int64_t grid = std::min<int64_t>(p.n_items, int64_t(1) << 30);
+        clipped_chroma_kernel<false><<<(unsigned)grid, kThreads, bytes, st>>>(p, per_clip);
+        CK_LAUNCH("clipped_chroma_kernel");
+        return B200AA_OK;
+    }
+    // large windows: the arrays of every resident CTA in stream-ordered scratch, CTAs loop over the items
+    const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * 2);
+    p.scratch_stride = (bytes + 255) & ~size_t(255);
+    void *scratch = nullptr;
+    CK(cudaMallocAsync(&scratch, p.scratch_stride * size_t(grid), st));
+    p.scratch = static_cast<unsigned char *>(scratch);
+    clipped_chroma_kernel<true><<<(unsigned)grid, kThreads, 0, st>>>(p, per_clip);
+    const cudaError_t e = cudaGetLastError();
+    cudaFreeAsync(scratch, st);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (e != cudaSuccess) return cuda_fail(e, "clipped_chroma_kernel (large window)");
+    return B200AA_OK;
+}
+
+// b200aa_spectrogram and b200aa_spectrogram_ragged (d_len set): the launch is sized by n_samples
+static int spectrogram_launch(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                              int64_t clip_stride, const int64_t *d_len, const b200aa_clip_norm *d_norm, float *d_out,
+                              void *stream)
+{
+    if (!plan || !d_sig || !d_norm || !d_out || n_clips < 0 || (dtype != 0 && dtype != 1) || clip_stride < n_samples)
+        return B200AA_ERR_INVALID;
+    b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
+    const rows::Rows r = rows::spectrogram(n_samples, pl->window, pl->step);
+    if (r.refused) return B200AA_ERR_TOO_SHORT;     // np.zeros with a non-positive row count / empty result
+    if (n_clips == 0) return B200AA_OK;
+    int rc = plan_device_check(pl);
+    if (rc != B200AA_OK) return rc;
+    Transform *t = nullptr;
+    rc = get_transform(pl, pl->window, &t);
+    if (rc != B200AA_OK) return rc;
+    StParams p;
+    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
+    p.mode = kModeSpectrogram;
+    p.origin = pl->window; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
+    return launch_rows<kModeSpectrogram>(pl, p, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int b200aa_spectrogram(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
                                   int64_t n_samples, int64_t clip_stride, const b200aa_clip_norm *d_norm,
                                   float *d_out, void *stream)
 {
     NvtxRange nvtx_("b200aa_spectrogram");
+    return spectrogram_launch(plan, d_sig, dtype, n_clips, n_samples, clip_stride, nullptr, d_norm, d_out, stream);
+}
+
+extern "C" int b200aa_spectrogram_ragged(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                                         int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                                         const b200aa_clip_norm *d_norm, float *d_out, void *stream)
+{
+    NvtxRange nvtx_("b200aa_spectrogram_ragged");
+    if (!d_len) return B200AA_ERR_INVALID;
+    return spectrogram_launch(plan, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out, stream);
+}
+
+// b200aa_chromagram and b200aa_chromagram_ragged (d_len set): the row kernel writes the rows of full frames and zeros
+// after them, then one launch transforms every clipped frame of the batch into its row
+static int chromagram_launch(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                             int64_t clip_stride, const int64_t *d_len, const b200aa_clip_norm *d_norm, float *d_out,
+                             void *stream)
+{
     if (!plan || !d_sig || !d_norm || !d_out || n_clips < 0 || (dtype != 0 && dtype != 1) || clip_stride < n_samples)
         return B200AA_ERR_INVALID;
     b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
     const int w = pl->window, s = pl->step;
-    const int64_t R = b200aa_spectrogram_rows(n_samples, w, s);
-    if (R <= 0) return B200AA_ERR_TOO_SHORT;      // np.zeros with a non-positive row count / empty result
+    const rows::Rows r = rows::chromagram(n_samples, w, s);
+    // a ragged batch is refused only when its width gives no rows: each clip's own refusal leaves its rows unwritten
+    if (r.R <= 0 || (!d_len && n_samples - s - w < 0)) return B200AA_ERR_TOO_SHORT;
+    int rc = pl->tables_status;
+    if (rc == B200AA_ERR_CHROMA) return rc;
     if (n_clips == 0) return B200AA_OK;
-    int rc = plan_device_check(pl);
-    if (rc != B200AA_OK) return rc;
+    if (!d_len && r.refused) return B200AA_ERR_INVALID;     // a clipped frame shorter than K: the reference's scatter raises
+    if ((rc = plan_device_check(pl)) != B200AA_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
     Transform *t = nullptr;
     rc = get_transform(pl, w, &t);
     if (rc != B200AA_OK) return rc;
     StParams p;
-    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, nullptr, d_norm, d_out);
-    p.mode = kModeSpectrogram;
-    p.origin = w; p.row0 = 0; p.rows_total = R; p.rows_launch = R;
-    p.rows_valid = std::min<int64_t>(R, b200aa_host::range_len(w, n_samples - w + 1, s));   // :415
-    if (use_solo(pl)) {
-        cudaStream_t st_ = static_cast<cudaStream_t>(stream);
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st_, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = solo_launch_mode<kModeSpectrogram>(pl->solo, p, pl->sm_count, p.rows_launch, ctr, b200aa_plan::kSlotBytes, st_);
-        const int rc2 = slot_done(pl, st_, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "solo kernel") : rc;
-    }
-    if (pl->fast_kind && !pl->force_generic && pl->prefer != 0 && pl->prefer != 3) {
-        cudaStream_t st_ = static_cast<cudaStream_t>(stream);
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st_, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = fast_launch_rows(pl->fast_kind, kModeSpectrogram, pl->fast, p, pl->sm_count, ctr, st_);
-        const int rc2 = slot_done(pl, st_, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "fast kernel") : rc;
-    }
-    return launch_generic<kModeSpectrogram>(pl, p, R, static_cast<cudaStream_t>(stream));
+    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
+    p.mode = kModeChromagram;
+    p.origin = w; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
+    rc = launch_rows<kModeChromagram>(pl, p, st);
+    if (rc != B200AA_OK) return rc;
+    const int64_t per_clip = d_len ? rows::max_clipped(w, s) : r.n_it - r.n_full;
+    return per_clip > 0 ? launch_clipped(pl, p, per_clip, st) : B200AA_OK;
 }
 
 extern "C" int b200aa_chromagram(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
@@ -1128,66 +1233,16 @@ extern "C" int b200aa_chromagram(const b200aa_plan *plan, const void *d_sig, int
                                  float *d_out, void *stream)
 {
     NvtxRange nvtx_("b200aa_chromagram");
-    if (!plan || !d_sig || !d_norm || !d_out || n_clips < 0 || (dtype != 0 && dtype != 1) || clip_stride < n_samples)
-        return B200AA_ERR_INVALID;
-    b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
-    const int w = pl->window, s = pl->step;
-    const int64_t R = b200aa_chromagram_rows(n_samples, w, s);
-    if (R <= 0 || n_samples - s - w < 0) return B200AA_ERR_TOO_SHORT;
-    int rc = pl->tables_status;
-    if (rc == B200AA_ERR_CHROMA) return rc;
-    if (n_clips == 0) return B200AA_OK;
-    if ((rc = plan_device_check(pl)) != B200AA_OK) return rc;
-    const int64_t n_it = std::min<int64_t>(R, b200aa_host::range_len(w, n_samples - s, s));        // :349
-    // frames that fit entirely: start p = w + i*s with p + w <= N
-    int64_t n_full = 0;
-    if (n_samples - 2 * int64_t(w) >= 0) n_full = std::min<int64_t>(n_it, (n_samples - 2 * int64_t(w)) / s + 1);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    Transform *t = nullptr;
-    rc = get_transform(pl, w, &t);
-    if (rc != B200AA_OK) return rc;
-    StParams p;
-    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, nullptr, d_norm, d_out);
-    p.mode = kModeChromagram;
-    p.origin = w; p.row0 = 0; p.rows_total = R; p.rows_launch = R; p.rows_valid = n_full;
-    rc = B200AA_ERR_UNSUPPORTED;
-    if (use_solo(pl)) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = solo_launch_mode<kModeChromagram>(pl->solo, p, pl->sm_count, p.rows_launch, ctr, b200aa_plan::kSlotBytes, st);
-        if (slot_done(pl, st, slot) != B200AA_OK) return B200AA_ERR_CUDA;
-        if (rc == B200AA_OK) g_launches.fetch_add(1, std::memory_order_relaxed);
-        else if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "solo kernel") : rc;
-    }
-    if (rc == B200AA_ERR_UNSUPPORTED && pl->fast_kind && !pl->force_generic && pl->prefer != 0 && pl->prefer != 3) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = fast_launch_rows(pl->fast_kind, kModeChromagram, pl->fast, p, pl->sm_count, ctr, st);
-        if (slot_done(pl, st, slot) != B200AA_OK) return B200AA_ERR_CUDA;
-        if (rc == B200AA_OK) g_launches.fetch_add(1, std::memory_order_relaxed);
-        else if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "fast kernel") : rc;
-    }
-    if (rc == B200AA_ERR_UNSUPPORTED) rc = launch_generic<kModeChromagram>(pl, p, R, st);
-    if (rc != B200AA_OK) return rc;
-    // frames clipped at the end of the clip: the reference transforms the n < w samples that are
-    // left (ShortTermFeatures.py:352-355); fewer than num_fft samples make its scatter raise.
-    for (int64_t i = n_full; i < n_it; ++i) {
-        const int64_t start = w + i * s;
-        const int64_t n = n_samples - start;
-        if (n < pl->K) return B200AA_ERR_INVALID;
-        Transform *tc = nullptr;
-        rc = get_transform(pl, (int)n, &tc);
-        if (rc != B200AA_OK) return rc;
-        StParams q;
-        fill_common(q, pl, tc, d_sig, dtype, n_clips, n_samples, clip_stride, nullptr, d_norm, d_out);
-        q.mode = kModeChromagram;
-        q.origin = start; q.row0 = i; q.rows_total = R; q.rows_launch = 1; q.rows_valid = 1;
-        rc = launch_generic<kModeChromagram>(pl, q, 1, st);
-        if (rc != B200AA_OK) return rc;
-    }
-    return B200AA_OK;
+    return chromagram_launch(plan, d_sig, dtype, n_clips, n_samples, clip_stride, nullptr, d_norm, d_out, stream);
+}
+
+extern "C" int b200aa_chromagram_ragged(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                                        int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                                        const b200aa_clip_norm *d_norm, float *d_out, void *stream)
+{
+    NvtxRange nvtx_("b200aa_chromagram_ragged");
+    if (!d_len) return B200AA_ERR_INVALID;
+    return chromagram_launch(plan, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out, stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "../../include/b200aa.h"
+#include "rows.cuh"
 
 #define B200AA_EPS 2.220446049250313e-16f   /* sys.float_info.epsilon, ShortTermFeatures.py:11 */
 
@@ -42,12 +43,13 @@ struct StParams {
     int64_t seg_len, segs_per_clip, n_items;
     // spectrogram / chromagram launches: row r of this launch is the frame starting at
     // origin + r*step, stored at output row row0 + r (of rows_total per clip); rows >= rows_valid
-    // of the launch are written as zeros (the reference leaves them unset, ShortTermFeatures.py:413-422)
+    // of the launch are written as zeros (the reference leaves them unset, ShortTermFeatures.py:413-422).
+    // A ragged row launch (len set, the kernels' RAGGED form) takes both counts of clip b from ragged_rows below.
     int64_t origin, row0, rows_total, rows_launch, rows_valid;
     int dtype, deltas, n_out;       // n_out = 34 or 68
     int window;                     // nominal window (frame hop grid, feature tables)
-    int fft_n;                      // samples per frame actually transformed (== window except for a
-                                    // chromagram frame clipped at the end of the clip, :352-355)
+    int fft_n;                      // samples per frame transformed (== window; clipped chromagram frames,
+                                    // :352-355, go to clipped_chroma_kernel)
     int step, K, Kp, Nc, packed;    // K = window/2 bins kept; Nc = complex transform length
     int nrad;
     int radix[kMaxRadix];
@@ -58,6 +60,25 @@ struct StParams {
     unsigned char *scratch;
     size_t scratch_stride;          // bytes per CTA
 };
+
+// Length of clip b of a ragged batch, clamped to the batch width (the clips' samples end there)
+__device__ __forceinline__ int64_t ragged_len(const StParams &p, int64_t b)
+{
+    const int64_t n = p.len[b];
+    return n < 0 ? 0 : (n > p.n_samples ? p.n_samples : n);
+}
+
+// Rows of clip b in a ragged spectrogram / chromagram launch: its own R_b (none when the single-clip entry point refuses
+// the clip), of which the first n_full come from full frames; rows [n_full, R_b) are written as zeros, rows >= R_b not
+// at all.  The launch itself is sized by the batch width, whose row count bounds every clip's.
+template <int MODE>
+__device__ __forceinline__ void ragged_rows(const StParams &p, int64_t b, int64_t &n_rows, int64_t &n_valid)
+{
+    const int64_t n = ragged_len(p, b);
+    const rows::Rows r = MODE == kModeSpectrogram ? rows::spectrogram(n, p.window, p.step) : rows::chromagram(n, p.window, p.step);
+    n_rows = r.refused ? 0 : r.R;
+    n_valid = r.refused ? 0 : r.n_full;
+}
 
 __device__ __forceinline__ float warp_sum(float v)
 {

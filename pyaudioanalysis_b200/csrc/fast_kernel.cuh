@@ -531,7 +531,9 @@ inline size_t fast_smem_bytes(int step, int blob_words, bool runs)
            (runs ? sizeof(short) * (size_t(G) * step + 16) : 0);
 }
 
-template <int R1, int R2, int G, bool STEP_EVEN, bool RUNS, int MODE>
+// RAGGED (row modes only): every clip takes its own row counts from p.len (ragged_rows); a template flag so that the
+// uniform launches keep their code.
+template <int R1, int R2, int G, bool STEP_EVEN, bool RUNS, int MODE, bool RAGGED = false>
 __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fast_kernel(const StParams p, const float2 *__restrict__ g_tw,
                                                                 const float2 *__restrict__ g_twp, unsigned int *work_counter)
 {
@@ -597,8 +599,10 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
         const int64_t len = p.len ? p.len[b] : p.n_samples;
         // features: frames of the clip; spectrogram / chromagram: the rows of this launch (rows >= n_valid are zero)
         typedef int fidx_t;          // frame / row indices inside a clip fit 32 bits (checked on the host)
-        const fidx_t T = fidx_t(MODE == kModeFeatures ? (len < N ? 0 : (len - N) / step + 1) : p.rows_launch);
-        const fidx_t n_valid = MODE == kModeFeatures ? T : fidx_t(p.rows_valid);
+        int64_t rows_b = p.rows_launch, valid_b = p.rows_valid;
+        if constexpr (RAGGED) ragged_rows<MODE>(p, b, rows_b, valid_b);
+        const fidx_t T = fidx_t(MODE == kModeFeatures ? (len < N ? 0 : (len - N) / step + 1) : rows_b);
+        const fidx_t n_valid = MODE == kModeFeatures ? T : fidx_t(valid_b);
         const int64_t origin = MODE == kModeFeatures ? 0 : p.origin;
         const fidx_t t0 = fidx_t(seg * p.seg_len);
         if (t0 >= T) break;
@@ -910,6 +914,9 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
     const size_t smem = fast_smem_bytes<R1, R2, G>(p.step, p.bl.words, RUNS);
     if (smem > 110u * 1024u) return B200AA_ERR_UNSUPPORTED;      // very large hop: leave it to the generic kernel
     auto kern = st_fast_kernel<R1, R2, G, EVEN, RUNS, MODE>;
+    if constexpr (MODE != kModeFeatures) {
+        if (p.len) kern = st_fast_kernel<R1, R2, G, EVEN, RUNS, MODE, true>;
+    }
     // always the same value (the launcher's cap), so concurrent launches of one instantiation cannot undercut each other
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024) != cudaSuccess) return B200AA_ERR_CUDA;
     int occ = 1;
@@ -975,7 +982,7 @@ inline int fast_launch_features(int kind, const FastTables &ft, const StParams &
 {
     return fast_launch_mode<kModeFeatures>(kind, ft, p, sm_count, T, ctr, st);
 }
-// spectrogram / chromagram rows of full-length frames (p.origin, p.rows_* filled by the caller)
+// spectrogram / chromagram rows of full-length frames (p.origin, p.rows_* filled by the caller; p.len set: ragged)
 inline int fast_launch_rows(int kind, int mode, const FastTables &ft, const StParams &p, int sm_count, unsigned int *ctr, cudaStream_t st)
 {
     if (mode == kModeSpectrogram) return fast_launch_mode<kModeSpectrogram>(kind, ft, p, sm_count, p.rows_launch, ctr, st);

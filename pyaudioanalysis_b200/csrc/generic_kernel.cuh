@@ -54,7 +54,9 @@ __device__ __forceinline__ void stockham_pass_bfly(const float2 *src, float2 *ds
 // BIG: windows whose transform does not fit shared memory (e.g. the 1 s windows of music_thumbnailing at 44.1 kHz,
 // audioSegmentation.py:1137-1139): same code, the window-sized arrays of the CTA sit in global memory (L2 resident),
 // __syncthreads() orders the passes as before.
-template <int MODE, bool BIG = false>
+// RAGGED (row modes only): every clip takes its own row counts from p.len (ragged_rows); a template flag so that the
+// uniform launches keep their code.
+template <int MODE, bool BIG = false, bool RAGGED = false>
 __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams p)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -86,6 +88,7 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
         } else {
             n_rows = p.rows_launch;
             n_valid = p.rows_valid;
+            if constexpr (RAGGED) ragged_rows<MODE>(p, b, n_rows, n_valid);
             origin = p.origin;
         }
         const int64_t t0 = seg * p.seg_len;
@@ -273,6 +276,81 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
             if (tid < kFvStride) fvrows[tid] = fvrows[size_t(ng) * kFvStride + tid];
             if (tid == 0) rowsum[0] = rowsum[ng];
             __syncthreads();
+        }
+    }
+}
+
+// bytes of the clipped-frame kernel's per-CTA arrays: |X| row [K] (16-byte padded), twiddles [w] double2, samples [w] double
+inline size_t clipped_bytes(int w, int K)
+{
+    return ((size_t(K) * sizeof(float) + 15) & ~size_t(15)) + size_t(w) * (sizeof(double2) + sizeof(double));
+}
+
+// Chromagram rows of the frames clipped at the end of a clip (ShortTermFeatures.py:349-355): row i >= n_full of clip b
+// transforms the n = len - (w + i*s) samples left, K <= n < w (rows::chromagram).  Work item = (clip b, candidate c <
+// per_clip): the row is n_full + c, and an item without such a row does nothing, so one launch serves every clip and
+// every clipped length whether the lengths are known on the host or only on the device (p.len).
+// Direct DFT of length n: z[j] = x[j] - x[0] in fp64, the phase index j*k mod n advances exactly in integers over a
+// table of the n twiddles the CTA builds for this n, fp64 accumulation.  Then |X|[0:K] / K of y = a*(x - m) + bp (the
+// DC bin adds n*(a*(x[0] - m) + bp)) rounded to float, and the chroma row with the plan's taps / sum(X^2) as in
+// st_generic_kernel's chromagram mode.
+// BIG: windows whose arrays do not fit shared memory keep them in global scratch (p.scratch, p.scratch_stride per CTA).
+template <bool BIG>
+__global__ void __launch_bounds__(kThreads, 2) clipped_chroma_kernel(const StParams p, int64_t per_clip)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int w = p.window, s = p.step, K = p.K;
+    const int tid = threadIdx.x, lane = tid & 31;
+    unsigned char *const base = BIG ? p.scratch + size_t(blockIdx.x) * p.scratch_stride : smem_raw;
+    float *const X = reinterpret_cast<float *>(base);
+    double2 *const tw = reinterpret_cast<double2 *>(base + ((size_t(K) * sizeof(float) + 15) & ~size_t(15)));
+    double *const z = reinterpret_cast<double *>(tw + w);
+    const SmallTables tb = bind_tables(p.blob, p.bl);           // chroma taps straight from global memory
+    const bool is16 = p.dtype == B200AA_DTYPE_I16;
+
+    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+        const int64_t b = item / per_clip, c = item - b * per_clip;
+        const int64_t len = p.len ? ragged_len(p, b) : p.n_samples;
+        const rows::Rows r = rows::chromagram(len, w, s);
+        const int64_t i = r.n_full + c;
+        if (r.refused || i >= r.n_it) continue;                 // uniform across the CTA
+        const int64_t start = rows::frame_start(w, s, i);
+        const int n = int(len - start);
+        const char *clip = reinterpret_cast<const char *>(p.sig) + size_t(b) * p.clip_stride * (is16 ? 2 : 4);
+        auto x = [&](int64_t j) -> double {
+            return is16 ? double(reinterpret_cast<const short *>(clip)[start + j]) : double(reinterpret_cast<const float *>(clip)[start + j]);
+        };
+        const double x0 = x(0);
+        __syncthreads();                                        // the previous item is done with X, tw and z
+        for (int j = tid; j < n; j += kThreads) {
+            z[j] = x(j) - x0;                                   // exact: a difference of two int16 / float32 values
+            double sn, cs;
+            sincospi(2.0 * double(j) / double(n), &sn, &cs);
+            tw[j] = make_double2(cs, -sn);
+        }
+        __syncthreads();
+        const b200aa_clip_norm nm = p.norm[b];
+        const double a = nm.a;
+        for (int k = tid; k < K; k += kThreads) {
+            double re = 0.0, im = 0.0;
+            int ph = 0;                                         // j*k mod n; k < K <= n
+            for (int j = 0; j < n; ++j) {
+                const double2 t = tw[ph];
+                re = fma(z[j], t.x, re);
+                im = fma(z[j], t.y, im);
+                ph += k;
+                if (ph >= n) ph -= n;
+            }
+            const double mag = k == 0 ? fabs(a * re + double(n) * (a * (x0 - double(nm.m)) + double(nm.bp))) : a * sqrt(re * re + im * im);
+            X[k] = float(mag / double(K));
+        }
+        __syncthreads();
+        if (tid < 32) {
+            float sxx = 0.f;
+            for (int k = lane; k < K; k += 32) sxx = fmaf(X[k], X[k], sxx);
+            sxx = warp_sum(sxx);
+            const float ch = chroma_lane(X, sxx, tb, lane);
+            if (lane < 12) p.out[(size_t(b) * p.rows_total + i) * 12 + lane] = ch;
         }
     }
 }

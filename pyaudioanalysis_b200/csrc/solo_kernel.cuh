@@ -155,7 +155,9 @@ __device__ __forceinline__ void td_rows(const float2 (&u)[SoloShape<L, R2>::RT],
     flips_b = TWO ? fb : 2 * fb;
 }
 
-template <int L, int R2, int MODE>
+// RAGGED (row modes only): every clip takes its own row counts from p.len (ragged_rows); a template flag so that the
+// uniform launches keep their code.
+template <int L, int R2, int MODE, bool RAGGED = false>
 __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_blocks<MODE>()) st_solo_kernel(const SoloParams pp)
 {
     using S = SoloShape<L, R2>;
@@ -193,6 +195,7 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
     for (;;) {
         int64_t b;
         int q0, q1, T, NP;
+        int64_t valid_b = 0;        // row modes: rows of clip b from full frames
         bool fresh = true;
         if constexpr (FEAT) {
             if (g0 >= g1) {
@@ -224,14 +227,17 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
             if (int64_t(item) >= p.n_items) break;
             const int seg = int(item / unsigned(p.n_clips));
             b = item - unsigned(seg) * unsigned(p.n_clips);
-            T = int(p.rows_launch);                                 // the rows of this launch (rows >= rows_valid are zero)
+            int64_t rows_b = p.rows_launch;                         // the rows of this launch (rows >= rows_valid are zero)
+            valid_b = p.rows_valid;
+            if constexpr (RAGGED) ragged_rows<MODE>(p, b, rows_b, valid_b);
+            T = int(rows_b);
             NP = (T + 1) >> 1;
             if (seg < pp.n_big) { q0 = seg * pp.seg_big; q1 = q0 + pp.seg_big; }
             else { q0 = pp.n_big * pp.seg_big + (seg - pp.n_big) * pp.seg_small; q1 = q0 + pp.seg_small; }
             if (q0 >= NP) continue;
             q1 = q1 < NP ? q1 : NP;
         }
-        const int n_valid = MODE == kModeFeatures ? T : int(p.rows_valid);
+        const int n_valid = MODE == kModeFeatures ? T : int(valid_b);
         const int64_t origin = MODE == kModeFeatures ? 0 : p.origin;
         const b200aa_clip_norm nm = p.norm[b];
         const bool is16 = p.dtype == B200AA_DTYPE_I16;
@@ -540,6 +546,9 @@ inline int solo_launch_t(const SoloTables &stb, const StParams &p, int sm_count,
     constexpr int cap = MODE == kModeFeatures ? kSoloCtaCap : 113 * 1024;
     if (smem > size_t(cap)) return B200AA_ERR_UNSUPPORTED;
     auto kern = st_solo_kernel<L, R2, MODE>;
+    if constexpr (MODE != kModeFeatures) {
+        if (p.len) kern = st_solo_kernel<L, R2, MODE, true>;
+    }
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return B200AA_ERR_CUDA;
     int occ = 1;
     constexpr int W = solo_warps<L, R2, MODE>();

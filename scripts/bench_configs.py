@@ -48,6 +48,37 @@ def noise(b, n, seed):
     return out
 
 
+def wall(fn, reps=3):
+    fn()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        fn()
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) / reps * 1e3
+
+
+def ragged_config3():
+    """Config 3 as a ragged batch: one spectrogram_batch / chromagram_batch call with lengths= against one call per clip
+    (the only way before lengths= existed); kernel time with the clip statistics done beforehand, wall time with them."""
+    fs, w, s, B = 44100, 882, 441, 64
+    lengths = np.random.default_rng(3).integers(30 * fs, 60 * fs + 1, size=B)
+    sig = noise(B, int(lengths.max()), 33)
+    lens = torch.from_numpy(lengths).cuda()
+    norm = clip_stats(sig, lens)
+    views = [sig[b:b + 1, :int(n)] for b, n in enumerate(lengths)]
+    norms = [clip_stats(v) for v in views]
+    res = {"config": "3 ragged: %d clips @44.1 kHz, 20/10 ms, lengths uniform in 30-60 s (seed 3)" % B,
+           "samples": int(lengths.sum())}
+    for name, fn in (("spectrogram", pkg.spectrogram_batch), ("chromagram", pkg.chromagram_batch)):
+        res[name + "_ragged_kernel_ms"] = timed(lambda: fn(sig, fs, w, s, norm=norm, lengths=lens), reps=5)
+        res[name + "_per_clip_kernel_ms"] = timed(lambda: [fn(v, fs, w, s, norm=nv) for v, nv in zip(views, norms)], reps=3)
+        res[name + "_ragged_wall_ms"] = wall(lambda: fn(sig, fs, w, s, lengths=lens))
+        res[name + "_per_clip_wall_ms"] = wall(lambda: [fn(v, fs, w, s) for v in views])
+    res["gpu"] = {"name": torch.cuda.get_device_name(0), "power_limit_w": bench.ClockSampler(0).power_limit_w()}
+    emit(res)
+
+
 def main():
     torch.cuda.set_device(0)
     pkg.ShortTermFeatures.PRINT_SPECTROGRAM_SHAPE = False
@@ -88,6 +119,7 @@ def main():
           "kernel_only_feature_extraction_frames_per_s": B3 * T3 / (k_fe * 1e-3),
           "combined_algorithmic_GBps": alg / ((ms_sp + ms_ch + ms_fe) * 1e-3) / 1e9, "hbm_peak_GBps": PEAK})
     del c3
+    ragged_config3()
 
     # ---- config 4: mid_feature_extraction over a 1 h recording, mt 1.0/1.0 s, st 50/25 ms
     N4 = 57600000
