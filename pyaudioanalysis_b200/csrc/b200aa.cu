@@ -223,77 +223,6 @@ static int get_transform(b200aa_plan *pl, int n, Transform **out)
     return B200AA_OK;
 }
 
-// pack mel CSR + DCT + chroma entries into one int32 blob
-// Returns the status of the feature tables (mfcc_filter_banks runs before the frame loop, :578 / :230-231, the chroma
-// scatter fails on frame 0, :290-294); the blob is built either way so that spectrogram() still works.
-static int build_blob(int fs, int K, std::vector<int> &blob, BlobLayout &bl)
-{
-    std::vector<double> mel, chr, dct;
-    int rc_mel = b200aa_host::build_mel(fs, K, mel);
-    int rc_chr = b200aa_host::build_chroma(fs, K, chr);
-    b200aa_host::build_dct(dct);
-    std::vector<int> m_start(40, 0), m_count(40, 0), m_off(40, 0);
-    std::vector<float> m_w;
-    if (rc_mel == B200AA_OK)
-        for (int i = 0; i < 40; ++i) {
-            int lo = -1, hi = -1;
-            for (int k = 0; k < K; ++k)
-                if (mel[size_t(i) * K + k] != 0.0) { if (lo < 0) lo = k; hi = k; }
-            m_off[i] = (int)m_w.size();
-            if (lo >= 0) {
-                m_start[i] = lo;
-                m_count[i] = hi - lo + 1;
-                for (int k = lo; k <= hi; ++k) m_w.push_back(float(mel[size_t(i) * K + k]));
-            }
-        }
-    std::vector<int> c_off(13, 0), c_bin;
-    std::vector<float> c_w;
-    if (rc_chr == B200AA_OK)
-        for (int c = 0; c < 12; ++c) {
-            c_off[c] = (int)c_bin.size();
-            for (int k = 0; k < K; ++k)
-                if (chr[size_t(c) * K + k] != 0.0) { c_bin.push_back(k); c_w.push_back(float(chr[size_t(c) * K + k])); }
-            c_off[c + 1] = (int)c_bin.size();
-        }
-    auto put_i = [&](const std::vector<int> &v) { int at = (int)blob.size(); blob.insert(blob.end(), v.begin(), v.end()); return at; };
-    auto put_f = [&](const std::vector<float> &v) {
-        int at = (int)blob.size();
-        for (float f : v) { int w; std::memcpy(&w, &f, 4); blob.push_back(w); }
-        return at;
-    };
-    blob.clear();
-    bl.mel_start = put_i(m_start);
-    bl.mel_count = put_i(m_count);
-    bl.mel_off = put_i(m_off);
-    bl.mel_w = put_f(m_w);
-    std::vector<float> dpad(13 * 41, 0.f);
-    for (int r = 0; r < 13; ++r)
-        for (int n = 0; n < 40; ++n) dpad[r * 41 + n] = float(dct[size_t(r) * 40 + n]);
-    bl.dct = put_f(dpad);
-    bl.chr_off = put_i(c_off);
-    bl.chr_bin = put_i(c_bin);
-    bl.chr_w = put_f(c_w);
-    {
-        std::vector<int> order(40);
-        for (int i = 0; i < 40; ++i) order[i] = i;
-        std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return m_count[a] < m_count[b]; });
-        // 16 groups of <= 3 filters with balanced tap totals (longest-processing-time greedy)
-        std::vector<int> grp(16 * 3, -1), load(16, 0), cntg(16, 0);
-        for (int i = 39; i >= 0; --i) {
-            const int f = order[i];
-            int best = -1;
-            for (int g = 0; g < 16; ++g)
-                if (cntg[g] < 3 && (best < 0 || load[g] < load[best])) best = g;
-            grp[best * 3 + cntg[best]++] = f;
-            load[best] += m_count[f];
-        }
-        bl.mel_grp = put_i(grp);
-    }
-    while (blob.size() % 4) blob.push_back(0);
-    bl.words = (int)blob.size();
-    return (rc_mel != B200AA_OK) ? rc_mel : rc_chr;
-}
-
 extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int step)
 {
     if (!out || fs <= 0 || window < 2 || step < 1) return B200AA_ERR_INVALID;
@@ -305,7 +234,7 @@ extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int ste
     CK(cudaDeviceGetAttribute(&pl->sm_count, cudaDevAttrMultiProcessorCount, pl->device));
     // tables that only feature_extraction / chromagram need may be unbuildable (the reference raises
     // there too); spectrogram must still work, so remember the status instead of failing here.
-    pl->tables_status = build_blob(fs, pl->K, pl->h_blob, pl->bl);
+    pl->tables_status = b200aa_host::build_blob(fs, pl->K, pl->h_blob, pl->bl);
     CK(cudaMalloc(&pl->d_blob, sizeof(int) * pl->h_blob.size()));
     CK(cudaMemcpy(pl->d_blob, pl->h_blob.data(), sizeof(int) * pl->h_blob.size(), cudaMemcpyHostToDevice));
     Transform *t = nullptr;
@@ -989,18 +918,11 @@ static void fill_common(StParams &p, const b200aa_plan *pl, const Transform *t, 
 template <int MODE>
 static int launch_generic(const b200aa_plan *pl, StParams &p, int64_t rows_max, cudaStream_t st)
 {
-    int G = 8;
-    size_t smem = 0;
-    for (; G >= 1; G >>= 1) {
-        smem = generic_smem_bytes(G, p.Nc, p.Kp, p.bl.words);
-        if (smem <= (G == 8 ? 100u * 1024u : 226u * 1024u)) break;   // 227 KB is the per-CTA opt-in maximum
-    }
+    int G = generic_group(p.Nc, p.Kp, p.bl.words);
     const bool big = G < 1;            // one frame does not fit shared memory: window-sized arrays go to global memory
-    if (big) {
-        G = 1;
-        smem = generic_smem_bytes(G, p.Nc, p.Kp, p.bl.words, false);
-        if (p.Nc > (1 << 20)) return B200AA_ERR_UNSUPPORTED;          // 2^21-sample windows: beyond any use of the path
-    }
+    if (big) G = 1;
+    const size_t smem = generic_smem_bytes(G, p.Nc, p.Kp, p.bl.words, !big);
+    if (big && p.Nc > (1 << 20)) return B200AA_ERR_UNSUPPORTED;      // 2^21-sample windows: beyond any use of the path
     p.G = G;
     // segments: long enough to amortise the 2-frame halo, short enough to balance the SMs
     int64_t seg = rows_max;

@@ -24,6 +24,15 @@ inline size_t generic_smem_bytes(int G, int Nc, int Kp, int blob_words, bool big
     b += size_t(blob_words) * sizeof(int);
     return (b + 15) & ~size_t(15);
 }
+// frames per CTA group of the generic kernel: 8 while the arrays fit 100 KB (two CTAs per SM), else the largest of
+// 4, 2, 1 that fits 226 KB (227 KB is the per-CTA opt-in maximum); 0 = one frame does not fit shared memory and the
+// window-sized arrays go to global scratch
+inline int generic_group(int Nc, int Kp, int blob_words)
+{
+    for (int G = 8; G >= 1; G >>= 1)
+        if (generic_smem_bytes(G, Nc, Kp, blob_words) <= (G == 8 ? 100u * 1024u : 226u * 1024u)) return G;
+    return 0;
+}
 
 // One Stockham pass of radix R with one BUTTERFLY per thread (R = 2, 3, 4, 5, 7: register codelets of
 // dft_codelets.cuh); other radices use the one-output-per-thread form inside the kernel.
@@ -153,16 +162,19 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                     int ph = (k * tstep + q * stride) % Nc;   // phase step per input
                     int idx = 0;
                     const float2 *in = src + size_t(f) * Nc + j;
-                    float2 acc = make_float2(0.f, 0.f);
+                    // fp64 accumulation: a float sum of R terms errs by ~sqrt(R) u of its terms' size, which for large
+                    // primes (and for the DC bin, whose partial sums of x - x0 grow with the offset of x0) exceeds the
+                    // log2(N) u of the rest of the transform; products of floats are exact in fp64
+                    double ax = 0.0, ay = 0.0;
                     for (int r = 0; r < R; ++r) {
                         const float2 t = __ldg(p.tw + idx);
                         const float2 v = in[r * stride];
-                        acc.x = fmaf(v.x, t.x, fmaf(-v.y, t.y, acc.x));
-                        acc.y = fmaf(v.x, t.y, fmaf(v.y, t.x, acc.y));
+                        ax = fma(double(v.x), double(t.x), fma(-double(v.y), double(t.y), ax));
+                        ay = fma(double(v.x), double(t.y), fma(double(v.y), double(t.x), ay));
                         idx += ph;
                         if (idx >= Nc) idx -= Nc;
                     }
-                    dst[e] = acc;
+                    dst[e] = make_float2(float(ax), float(ay));
                 }
                 __syncthreads();
                 float2 *t_ = src; src = dst; dst = t_;

@@ -4,6 +4,51 @@ import numpy as np
 PAIR, SOLO, CTA, GENERIC = 2, 3, 1, 0
 KIND_NAMES = {PAIR: "pair", SOLO: "solo", CTA: "CTA", GENERIC: "generic"}
 
+# Windows of the generic kernel's spectrum sweep (tests/test_gpu_spectra.py), each chosen for the code path it reaches:
+# (fs, window, frames per CTA group, path).  The group size G (8, 4, 2, 1; 0 = global scratch) is what launch_generic
+# picks (csrc/generic_kernel.cuh: generic_group) with the tables blob the plan for (fs, window) builds, which grows with
+# the window (the mel taps: about 0.84 K + 900 words at 16 kHz); tests/test_smem_budget_cpu.py holds each claim to the
+# budget formula at that blob and at 256 words either side of it.
+# Even windows transform N/2 packed points, odd windows N real points; radices are 4s first, then primes ascending.
+GENERIC_SWEEP = [
+    (16000, 2, 8, "Nc = 1: empty radix list; K = 1"),
+    (16000, 3, 8, "K = 1, odd: one radix-3 pass, unpacked"),
+    (16000, 5, 8, "small odd window: radix 5"),
+    (16000, 7, 8, "small odd window: radix 7"),
+    (16000, 9, 8, "small odd window: radix 3, 3"),
+    (16000, 8, 8, "4^n: one radix-4 pass"),
+    (16000, 486, 8, "radix 3 alone (Nc = 3^5)"),
+    (16000, 686, 8, "radix 7 alone (Nc = 7^3)"),
+    (16000, 882, 8, "radix 3 and 7 mixed (Nc = 3^2 7^2)"),
+    (16000, 630, 8, "radix 3, 5, 7 mixed (Nc = 3^2 5 7)"),
+    (16000, 22, 8, "prime above 7: direct radix-11 pass"),
+    (16000, 26, 8, "prime above 7: direct radix-13 pass"),
+    (16000, 242, 8, "repeated prime above 7: two radix-11 passes"),
+    (16000, 1688, 4, "4 and a prime above 7 mixed (Nc = 4 211)"),
+    (16000, 1994, 4, "large prime: one direct radix-997 pass"),
+    (16000, 441, 8, "odd composite (3^2 7^2), unpacked; last G = 8 odd window"),
+    (16000, 1000, 8, "even, radix 4, 5 mixed; last G = 8 even window"),
+    (16000, 883, 4, "odd prime, direct radix-883 pass; first G = 4 odd window"),
+    (16000, 1250, 4, "radix 5 alone (Nc = 5^4); first G = 4 even window"),
+    (16000, 1009, 4, "odd prime, direct radix-1009 pass"),
+    (16000, 1323, 4, "odd composite (3^3 7^2)"),
+    (16000, 2048, 4, "4^5"),
+    (16000, 4096, 4, "4^5 2; last G = 4 even window"),
+    (16000, 2401, 4, "odd, radix 7 alone (7^4); last G = 4 odd window"),
+    (16000, 6000, 2, "first G = 2 even window"),
+    (16000, 3375, 2, "odd, radix 3, 5 (3^3 5^3); first G = 2 odd window"),
+    (16000, 9000, 2, "radix 4, 3, 5 (Nc = 4 3^2 5^3); last G = 2 even window"),
+    (16000, 5103, 2, "odd, radix 3, 7 (3^6 7); last G = 2 odd window"),
+    (16000, 11000, 1, "prime 11 among 4s and 5s; first G = 1 even window"),
+    (16000, 6561, 1, "odd, radix 3 alone (3^8); first G = 1 odd window"),
+    (16000, 15360, 1, "radix 4, 2, 3, 5 (Nc = 4^4 2 3 5); last G = 1 even window"),
+    (16000, 10125, 1, "odd, radix 3, 5 (3^4 5^3); last G = 1 odd window"),
+    (16000, 20000, 0, "global scratch, even"),
+    (16000, 12005, 0, "global scratch, odd (5 7^4)"),
+    (16000, 20011, 0, "global scratch, odd prime: one direct radix-20011 pass (its float32 DC sum missed the bound)"),
+    (44100, 11025, 0, "0.25 s at 44.1 kHz, odd: global scratch with its blob of ~2 560 words (G = 1 below ~1 700)"),
+]
+
 
 def plans(fs, w, s):
     """[(kind, Plan)] for every kernel kind a plan for (fs, w, s) reaches, the default choice first."""

@@ -13,7 +13,12 @@ Two row checks close that: ``check_energy_relative`` holds the energy row to RTO
 ``check_zcr_exact`` holds the zcr row of integer input to float32 rounding of the exact count.
 ``check_mid_propagated`` carries the per-frame tolerance through mid-term pooling (mean: mean of the frame tolerances,
 std: their RMS).
+
+``check_spectrum`` holds the magnitude spectrum |X[k]| / K of every frame, which every feature is built from, to a
+float64 DFT under a bound derived from float32 FFT arithmetic (derivation: tests/test_gpu_spectra.py).
 """
+import math
+
 import numpy as np
 
 RTOL, ATOL = 1e-4, 1e-5
@@ -170,3 +175,68 @@ def check_close(gpu, ref, what="", rtol=RTOL, atol=ATOL):
     ref = np.asarray(ref, dtype=np.float64)
     assert gpu.shape == ref.shape, (what, gpu.shape, ref.shape)
     np.testing.assert_allclose(gpu, ref, rtol=rtol, atol=atol, err_msg=what)
+
+
+U32 = 2.0 ** -24        # unit round-off of float32
+SPECTRUM_C = 8.0        # constant of the spectrum bound, fixed by the error analysis in tests/test_gpu_spectra.py
+
+
+def spectrum_reference(x, starts, N):
+    """Per frame (frame j = y[starts[j] : starts[j] + N], y = the normalised clip as O.spectrogram computes it): the
+    float64 magnitudes |DFT|[0:K] / K, the bound on the 2-norm of the error in bins 1 .. K-1, the bound on the error of
+    the DC bin, and whether the frame is constant.
+
+    z = y_frame - y_frame[0] is what every kernel transforms; nu = sqrt(N) |z|_2 / K is the 2-norm of its whole
+    spectrum on the output's scale (Parseval).  Bins:  C u ceil(log2 N) nu.  DC (a sum, then N times the first sample
+    added back):  C u (|z|_1 + N |y_frame[0]|) / K.  float32 input rounds x - x[0] once per sample: u |y_frame|_2 is
+    added to |z|_2."""
+    from oracle import st_oracle as O
+    f32 = np.asarray(x).dtype == np.float32
+    y = O.normalize_clip(np.asarray(x, dtype=np.float64))
+    K = N // 2
+    fr = np.stack([y[s:s + N] for s in starts]) if len(starts) else np.zeros((0, N))
+    z = fr - fr[:, :1]
+    # bins k >= 1 of y_frame and of z are the same numbers; from z a constant frame's are exactly 0, not float64 round-off
+    ref = np.abs(np.fft.fft(z, axis=1)[:, :K]) / K
+    ref[:, 0] = np.abs(fr.sum(axis=1)) / K
+    nz = np.linalg.norm(z, axis=1)
+    if f32:
+        nz = nz + U32 * np.linalg.norm(fr, axis=1)
+    levels = max(1, math.ceil(math.log2(N)))
+    bins = SPECTRUM_C * U32 * levels * math.sqrt(N) * nz / K
+    dc = SPECTRUM_C * U32 * (np.abs(z).sum(axis=1) + N * np.abs(fr[:, 0])) / K
+    return ref, bins, dc, ~z.any(axis=1)
+
+
+def check_spectrum(got, x, starts, N, what=""):
+    """Rows ``got`` [len(starts), K] against spectrum_reference: the 2-norm of the error over bins 1 .. K-1 of every
+    frame within its own bound, the DC bin within its own, and a constant frame's bins 1 .. K-1 exactly zero.
+    Returns (worst bins err / bound, worst DC err / bound)."""
+    got = np.asarray(got, dtype=np.float64)
+    ref, bins, dc, flat = spectrum_reference(x, starts, N)
+    assert got.shape == ref.shape, (what, got.shape, ref.shape)
+    assert np.isfinite(got).all(), what + ": non-finite spectrum"
+    nonzero = np.nonzero(flat & (got[:, 1:] != 0).any(axis=1))[0]
+    assert nonzero.size == 0, "%s: constant frames %s have non-zero bins beyond DC" % (what, nonzero[:10].tolist())
+    e = np.linalg.norm(got[:, 1:] - ref[:, 1:], axis=1)
+    d = np.abs(got[:, 0] - ref[:, 0])
+    r = np.where(bins > 0, e / np.where(bins > 0, bins, 1.0), np.where(e > 0, np.inf, 0.0))
+    rd = np.where(dc > 0, d / np.where(dc > 0, dc, 1.0), np.where(d > 0, np.inf, 0.0))
+    bad = np.nonzero((r > 1.0) | (rd > 1.0))[0]
+    if bad.size:
+        j = bad[np.argmax(np.maximum(r, rd)[bad])]
+        k = int(np.argmax(np.abs(got[j] - ref[j])))
+        raise AssertionError("%s: %d of %d frames outside the spectrum bound; worst frame %d (start %d): bins err / bound "
+                             "%.3g, DC err / bound %.3g, largest error in bin %d: %r vs %r"
+                             % (what, bad.size, len(starts), j, starts[j], r[j], rd[j], k, got[j, k], ref[j, k]))
+    return (float(r.max()) if r.size else 0.0), (float(rd.max()) if rd.size else 0.0)
+
+
+def check_spectrogram_rows(got, x, w, s, what=""):
+    """Spectrogram rows of clip x (row r transforms the frame at w + r s, ShortTermFeatures.py:413-415) under
+    check_spectrum; the rows the reference's loop never reaches are exactly zero."""
+    got = np.asarray(got, dtype=np.float64)
+    starts = np.arange(w, len(x) - w + 1, s)
+    assert got.shape == (int((len(x) - w) / s) + 1, w // 2), (what, got.shape)
+    assert not got[len(starts):].any(), what + ": rows past the last full frame are not zero"
+    return check_spectrum(got[:len(starts)], x, starts, w, what)

@@ -1,9 +1,14 @@
 // Host-side print of the shared-memory footprint of the CTA kernel per (window, hop) shape and of the pair kernel per window
-// (csrc/fast_kernel.cuh: fast_smem_bytes).  Built and read by tests/test_smem_budget_cpu.py; no GPU needed.
+// (csrc/fast_kernel.cuh: fast_smem_bytes), and of the generic kernel's frames per group for the (fs, window) pairs given on
+// the command line (csrc/generic_kernel.cuh: generic_group) at the size of the tables blob their plan builds.  Built and read by
+// tests/test_smem_budget_cpu.py; no GPU needed.
 #include <cstdio>
+#include <cstdlib>
 #define B200AA_LAYOUT_ONLY 1      // skip the launchers: they would instantiate every kernel
 #include "../pyaudioanalysis_b200/csrc/fast_kernel.cuh"
 #include "../pyaudioanalysis_b200/csrc/pair_kernel.cuh"
+#include "../pyaudioanalysis_b200/csrc/generic_kernel.cuh"
+#include "../pyaudioanalysis_b200/csrc/tables.inl"
 using namespace b200aa;
 
 template <int R1, int R2>
@@ -14,8 +19,21 @@ static void row(int step, int blob_words)
     printf("fast %d %d %d %zu\n", N, step, int(runs), fast_smem_bytes<R1, R2, B200AA_FAST_G>(step, blob_words, runs));
 }
 
-int main()
+int main(int argc, char **argv)
 {
+    // generic kernel, per "fs:window" argument: transform points, the blob the plan builds (b200aa_host::build_blob), and
+    // the frames per group with that blob, with 256 words less and with 256 words more, then the shared-memory bytes
+    for (int i = 1; i < argc; ++i) {
+        int fs = 0, w = 0;
+        if (sscanf(argv[i], "%d:%d", &fs, &w) != 2) return 1;
+        const int K = w / 2, Kp = (K + 3) & ~3, Nc = (w % 2 == 0) ? w / 2 : w;
+        std::vector<int> blob;
+        BlobLayout bl{};
+        b200aa_host::build_blob(fs, K, blob, bl);
+        const int words = bl.words, g = generic_group(Nc, Kp, words);
+        printf("generic %d %d %d %d %d %d %d %zu\n", fs, w, Nc, words, generic_group(Nc, Kp, words > 256 ? words - 256 : 0), g,
+               generic_group(Nc, Kp, words + 256), generic_smem_bytes(g ? g : 1, Nc, Kp, words, g != 0));
+    }
     const int words = 1300;     // mel + DCT + chroma blob, upper bound over the supported (fs, window) pairs
     row<20, 20>(400, words); row<20, 20>(800, words); row<20, 20>(160, words);
     row<21, 21>(441, words); row<21, 21>(882, words);

@@ -181,7 +181,11 @@ def test_edges(P, golden_edges):
                                       (48000, 2400, 1200, 60000), (16000, 1024, 512, 20000), (16000, 883, 300, 9000),
                                       (16000, 400, 160, 20000), (16000, 480, 160, 20000), (8000, 600, 300, 12000),
                                       (16000, 400, 133, 9000), (16000, 480, 480, 9600), (16000, 320, 160, 12000),
-                                      (16000, 640, 321, 12000), (8000, 320, 80, 8000)])
+                                      (16000, 640, 321, 12000), (8000, 320, 80, 8000),
+                                      # generic kernel at 2 and 1 frames per CTA group, even and odd (tests/kernels.py:
+                                      # GENERIC_SWEEP): a segment's two-frame halo is a whole group there
+                                      (48000, 6000, 3000, 96000), (44100, 4725, 2205, 70875),
+                                      (44100, 13230, 6615, 145530), (44100, 6615, 3307, 72755)])
 def test_oracle_configs(P, fs, w, s, n):
     x = O.synth_clip(100 + w, n, fs)
     ref, names = O.feature_extraction(x, fs, w, s)

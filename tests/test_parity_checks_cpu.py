@@ -113,6 +113,49 @@ def test_mid_slices_follow_python():
     assert PA.mid_slices(5, 9, 1)[-1] == (4, 5)
 
 
+def float32_spectra(x, starts, N):
+    """|X[k]| / K of z = y_frame - y_frame[0] by numpy's float32 FFT, DC from the float64 sum: a correct float32 transform."""
+    y = O.normalize_clip(np.asarray(x, dtype=np.float64))
+    fr = np.stack([y[s:s + N] for s in starts])
+    z = (fr - fr[:, :1]).astype(np.complex64)
+    got = (np.abs(np.fft.fft(z, axis=1)[:, :N // 2]) / np.float32(N // 2)).astype(np.float64)
+    got[:, 0] = np.abs(fr.sum(axis=1)) / (N // 2)
+    return got
+
+
+@pytest.mark.parametrize("name", ["edge_impulses", "constant_runs", "loud_quiet"])
+def test_spectrum_bound(name):
+    """A float32 FFT passes the spectrum bound; one bin off by 1e-3 relative, a constant frame with a non-zero bin, a
+    constant frame zeroed where one sample differs, and a DC bin off by 1e-4 of the frame's largest bin do not."""
+    N, s = 800, 200
+    x = SG.bank(16000, N, s)[name]
+    starts = np.arange(0, len(x) - N + 1, s)
+    got = float32_spectra(x, starts, N)
+    r, rd = PA.check_spectrum(got, x, starts, N, name)
+    assert r < 0.1 and rd < 0.1, (r, rd)
+    ref, _, _, flat = PA.spectrum_reference(x, starts, N)
+    j = int(np.argmax(ref[:, 1:].sum(axis=1)))
+    k = 1 + int(np.argmax(ref[j, 1:]))
+    for what, edit in (("bin", lambda g: g.__setitem__((j, k), g[j, k] * 1.001)),
+                       ("DC", lambda g: g.__setitem__((j, 0), g[j, 0] + 1e-4 * ref[j, k]))):
+        bad = got.copy()
+        edit(bad)
+        with pytest.raises(AssertionError, match="outside the spectrum bound"):
+            PA.check_spectrum(bad, x, starts, N, what)
+    if name == "constant_runs":
+        c = int(np.nonzero(flat)[0][0])
+        bad = got.copy()
+        bad[c, 5] = 1e-30
+        with pytest.raises(AssertionError, match="constant frames"):
+            PA.check_spectrum(bad, x, starts, N, "constant")
+        one = np.nonzero(~flat & (SG.constant_frames(x, N - 1, starts + 1) | SG.constant_frames(x, N - 1, starts)))[0]
+        assert one.size
+        bad = got.copy()
+        bad[one[0], 1:] = 0.0
+        with pytest.raises(AssertionError, match="outside the spectrum bound"):
+            PA.check_spectrum(bad, x, starts, N, "one differing sample")
+
+
 def test_exception_table():
     names = set(SG.NOTES) | set(SG.float_bank(16000, 800, 400))
     for e in PA.EXCEPTIONS:
