@@ -28,7 +28,8 @@ namespace b200aa {
 // threads per CTA: one warp per frame slot
 __host__ __device__ constexpr int fast_threads(int g) { return 32 * g; }
 
-// ---- cheap math: MUFU-based reciprocal / rsqrt / log2 (2 ulp); the parity tolerance is 1e-4
+// ---- cheap math: MUFU-based reciprocal / rsqrt / log2 (2 ulp); every feature entry stays within its per-entry bound
+// at these documented errors (tests/parity.feature_bounds, error model in tests/test_feature_bounds_cpu.py)
 __device__ __forceinline__ float fdiv(float a, float b) { return __fdividef(a, b); }
 // rsqrtf() is the MUFU.RSQ approximation; __frsqrt_rn() is the correctly rounded (slow) one -- measured 12 % slower
 #ifndef B200AA_NO_FTZ_MUFU

@@ -16,6 +16,8 @@ std: their RMS).
 
 ``check_spectrum`` holds the magnitude spectrum |X[k]| / K of every frame, which every feature is built from, to a
 float64 DFT under a bound derived from float32 FFT arithmetic (derivation: tests/test_gpu_spectra.py).
+``feature_bounds`` / ``check_feature_bounds`` carry that bound, plus the float32 arithmetic of the feature stage, to a
+bound on every entry of the 68 rows (derivation: tests/test_feature_bounds_cpu.py).
 """
 import math
 
@@ -240,3 +242,277 @@ def check_spectrogram_rows(got, x, w, s, what=""):
     assert got.shape == (int((len(x) - w) / s) + 1, w // 2), (what, got.shape)
     assert not got[len(starts):].any(), what + ": rows past the last full frame are not zero"
     return check_spectrum(got[:len(starts)], x, starts, w, what)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Per-entry bound of the 68 feature rows, carried from the spectrum bound (derivation: tests/test_feature_bounds_cpu.py)
+LOG2_ABS = 2.0 ** -22   # lg2.approx.f32 (__log2f): absolute error 2^-22 on [0.5, 2], else 2 ulp of the result
+DIV_REL = 4 * U32       # __fdividef: 2 ulp
+SQRT_REL = 5 * U32      # x * rsqrt.approx(x): 2 ulp and one rounding; sqrt.approx / sqrtf: 2 ulp assumed
+MARGIN = 1.01           # products of (1 + relative error) terms, kept to first order, are covered by 1 %
+F64_REL = 1e-12         # round-off of the float64 reference itself (sums of at most ~10^4 terms)
+ROW_GROUPS = {"time": (0, 1, 2), "spectral": (3, 4, 5, 6, 7), "mfcc": tuple(range(8, 21)), "chroma": tuple(range(21, 34))}
+
+
+def gamma(n):
+    """gamma_n = n u / (1 - n u): a float32 sum of non-negative terms whose every term passes through at most n
+    roundings errs by at most gamma_n times the sum (Higham, Accuracy and Stability, 2nd ed., section 3.1)."""
+    n = np.asarray(n, dtype=np.float64)
+    return n * U32 / (1.0 - n * U32)
+
+
+def sum_depth(n):
+    """Roundings a term of a float32 sum over n values (bins or samples) passes through in any kernel: per-lane
+    sequential chunks of at most ceil(n / 16) terms (16-lane half-warp layouts; 32-lane layouts hold half as many),
+    then at most 5 shuffle levels, the chunk's split into entropy parts and their sum, and the fma / product roundings
+    of the term itself."""
+    return math.ceil(n / 16) + 12
+
+
+def _lin(a, e0, eb):
+    """max |sum_k a_k d_k| over |d_0| <= e0, |d_1..K-1|_2 <= eb; a [..., K], e0 / eb broadcast against a[..., 0]."""
+    return np.abs(a[..., 0]) * e0 + np.linalg.norm(a[..., 1:], axis=-1) * eb
+
+
+def _quad(a, X, e0, eb):
+    """max |sum_k a_k ((X_k + d_k)^2 - X_k^2)| over the same set: 2 |a X|_2 eb + max |a| eb^2, DC apart."""
+    return (np.abs(a[..., 0]) * (2 * X[..., 0] * e0 + e0 ** 2) + 2 * np.linalg.norm((a * X)[..., 1:], axis=-1) * eb
+            + np.abs(a[..., 1:]).max(axis=-1) * eb ** 2)
+
+
+def _ratio_den(den, dden):
+    """den - dden where it stays positive, else nan (the interval of the denominator reaches 0)."""
+    return np.where(den - dden > 0, den - dden, np.nan)
+
+
+def _h(s):
+    return -s * np.log2(s + O_EPS)
+
+
+O_EPS = np.finfo(np.float64).eps
+
+
+def _entropy_bound(s, ds):
+    """Bound on |H' - H|, H = sum_j h(s_j), h(s) = -s log2(s + eps), each s_j' within ds_j of s_j (nan: unbounded).
+    h is concave on [0, inf) with its maximum at ~1/e, so over an interval its extremes are the endpoints and, where
+    the interval holds it, the maximum.  Plus the float32 evaluation of each term: lg2.approx's error times s, and two
+    roundings of the product and of the 10-term sum (gamma_12)."""
+    lo = np.maximum(s - ds, 0.0)
+    hi = s + ds
+    top = np.where((lo <= 1 / math.e) & (hi >= 1 / math.e), _h(1 / math.e), np.maximum(_h(lo), _h(hi)))
+    dev = np.maximum(_h(s) - np.minimum(_h(lo), _h(hi)), top - _h(s))
+    lg = np.maximum(1.0, np.abs(np.log2(lo + O_EPS)))
+    dev = dev + hi * LOG2_ABS * lg + gamma(12) * (np.abs(_h(s)) + dev)
+    return dev.sum(axis=-1)
+
+
+class FeatureBounds:
+    """feature_bounds' result for one clip: ``ref`` [F, T] float64 reference, ``bound`` [F, T] per-entry bound (inf where
+    unbounded), ``roll`` [2, T] admissible rolloff quanta (lo, hi) of every frame, ``unbounded`` {reason: count} and
+    ``K``."""
+
+    def __init__(self, ref, bound, roll, unbounded, K):
+        self.ref, self.bound, self.roll, self.unbounded, self.K = ref, bound, roll, unbounded, K
+
+
+_TABLES = {}
+
+
+def _tables(fs, K):
+    from oracle import st_oracle as O
+    if (fs, K) not in _TABLES:
+        _TABLES[(fs, K)] = (O.mel_filterbank(fs, K), O.dct_matrix(), O.chroma_operator(fs, K))
+    return _TABLES[(fs, K)]
+
+
+def clip_norm(x):
+    """(a, bp, ambiguity) of the kernels' normalisation y = a (x - m) + bp in float64: a = 1 / (max |x - mean| +
+    2^15 1e-10), m the clip centre exact in float (the rounded mean of int16, the float32 mean of float32), bp = a (m -
+    mean)."""
+    xd = np.asarray(x, dtype=np.float64)
+    mean = xd.sum() / xd.size
+    a = 1.0 / (max(xd.max() - mean, mean - xd.min()) + 32768.0 * 1e-10)
+    m = float(np.rint(mean)) if np.asarray(x).dtype == np.int16 else float(np.float32(mean))
+    return a, a * (m - mean)
+
+
+def feature_bounds(x, fs, w, s, deltas=False):
+    """The float64 reference of every short-term feature of clip x at (fs, w, s) and a per-entry bound on what a float32
+    kernel may return: the spectrum bound of spectrum_reference carried through each feature, plus the float32
+    arithmetic of the feature stage.  Derivation and error model: tests/test_feature_bounds_cpu.py."""
+    from oracle import st_oracle as O
+    x = np.asarray(x)
+    f32 = x.dtype == np.float32
+    K = w // 2
+    T = O.frame_count(len(x), w, s)
+    starts = s * np.arange(T)
+    X, eb, e0, flat = spectrum_reference(x, starts, w)
+    eb = np.where(flat, 0.0, eb)                       # a constant frame's bins 1 .. K-1 are exactly zero
+    y = O.normalize_clip(x.astype(np.float64))
+    fr = np.stack([y[a:a + w] for a in starts])
+    ref = O.base_features_from_frames(fr, X, fs)
+    M, D, C = _tables(fs, K)
+    bound = np.zeros_like(ref)
+    unb = {}
+    ebc, e0c = eb[:, None], e0[:, None]
+    gK = gamma(sum_depth(K))
+    k1 = np.arange(1, K + 1) / K
+
+    def unbounded(rows, mask, reason):
+        if mask.any():
+            bound[np.ix_(rows, np.nonzero(mask)[0])] = np.inf
+            unb[reason] = unb.get(reason, 0) + int(mask.sum()) * len(rows)
+
+    # ---- time domain: per-sample error of y = a (x - m) + bp in float32 (a, bp rounded; x - m rounded for float32
+    # input; the generic kernel rebuilds x - m as (x - m - d0) + d0), then float32 sums
+    a, bp = clip_norm(x)
+    beta = MARGIN * 4 * U32 * (np.abs(fr) + np.abs(fr[:, :1]) + abs(bp))
+    dq = 2 * np.abs(fr) * beta + beta ** 2                                   # bound on |y'^2 - y^2| per sample
+    E = (fr ** 2).sum(axis=1)
+    dE = dq.sum(axis=1)
+    gN = gamma(sum_depth(w))
+    flips_amb = (np.abs(fr) <= beta).sum(axis=1) if f32 else 0              # samples whose sign class may differ
+    bound[0] = 2 * U32 * np.abs(ref[0]) + flips_amb * 2.0 / (w - 1)
+    bound[1] = MARGIN * (dE + gN * (E + dE)) / w + 2 * U32 * ref[1]
+    L = w // 10
+    blk = np.arange(w) // L if L > 0 else np.full(w, 10)
+    sj = np.stack([(fr[:, blk == j] ** 2).sum(axis=1) for j in range(10)], axis=1) / (E + O_EPS)[:, None]
+    ind = (blk[None, :] == np.arange(10)[:, None]).astype(np.float64)        # [10, w]
+    num = np.einsum("jn,tn->tj", np.abs(ind), dq) + sj * dE[:, None]         # |1_B - s_j| <= 1_B + s_j
+    ds = num / _ratio_den(E + O_EPS, dE)[:, None] + sj * (2 * gN + 6 * U32)
+    bound[2] = _entropy_bound(sj, ds)
+
+    # ---- spectral rows from |X|: sums, ratios, square roots
+    S = X.sum(axis=1)
+    dS = _lin(np.ones(K), e0, eb)
+    Sd = _ratio_den(S, dS)
+    cen = np.where(S > 0, (X * k1).sum(axis=1) / np.where(S > 0, S, 1), 0.0)
+    dcen_t = _lin(k1[None, :] - cen[:, None], e0, eb) / Sd
+    dcen_a = MARGIN * cen * (2 * gK + 7 * U32)
+    bound[3] = np.where(S > 0, dcen_t + dcen_a, 0.0)
+    V = np.where(S > 0, ((k1[None, :] - cen[:, None]) ** 2 * X).sum(axis=1) / np.where(S > 0, S, 1), 0.0)
+    dV_t = _lin((k1[None, :] - cen[:, None]) ** 2 - V[:, None], e0, eb) / Sd + dcen_t ** 2
+    eta = (math.ceil(K / 16) + 4) * U32              # drift of (k + 1) / K - cen stepped across a lane's bins
+    sp = V * S
+    extra = dcen_a ** 2 * S + eta ** 2 * S + 2 * eta * np.sqrt(sp * S) + 2 * dcen_a * eta * S
+    dV_a = MARGIN * ((extra + gK * (sp + extra)) / np.where(S > 0, S, 1) + (gK + DIV_REL + U32) * (V + extra / np.where(S > 0, S, 1)))
+    dV = dV_t + dV_a
+    spr = np.sqrt(V)
+    # both sides: where V < dV the interval is cut at 0 below and the side above is the larger one
+    bound[4] = np.where(S > 0, np.maximum(np.sqrt(V + dV) - spr, spr - np.sqrt(np.maximum(V - dV, 0.0)))
+                        + SQRT_REL * np.sqrt(V + dV), 0.0)
+    # spectral entropy: 10 blocks of K // 10 bins over the total of all K bins
+    P = X ** 2
+    Et = P.sum(axis=1)
+    dEt = _quad(np.ones(K), X, e0, eb)
+    Lb = K // 10
+    bblk = np.arange(K) // Lb if Lb > 0 else np.full(K, 10)
+    Bm = (bblk[None, :] == np.arange(10)[:, None]).astype(np.float64)       # [10, K]
+    sjs = (P @ Bm.T) / (Et + O_EPS)[:, None]
+    ds = _quad(Bm[None] - sjs[:, :, None], X[:, None, :], e0c, ebc) / _ratio_den(Et + O_EPS, dEt)[:, None]
+    bound[5] = _entropy_bound(sjs, ds + sjs * (2 * gK + 6 * U32))
+    # flux: sqrt(flux) = |X / Sn - Xp / Sp|_2, Sn = S + K eps; each side moves by at most (|d|_2 + |X / Sn|_2 dS) / (Sn - dS)
+    Sn = S + K * O_EPS
+    nrm = np.linalg.norm(X, axis=1) / Sn
+    Dt = (np.sqrt(e0 ** 2 + eb ** 2) + nrm * dS) / _ratio_den(Sn, dS) + MARGIN * (gK + 7 * U32) * nrm
+    Dp = np.concatenate([Dt[:1], Dt[:-1]])
+    rf = np.sqrt(ref[6])
+    bound[6] = (rf + Dt + Dp) ** 2 * (1 + gK + 2 * U32) - ref[6]
+    # rolloff: first k with g_k = cumsum_k(X^2) + eps - 0.9 E > 0; g_k is a weighted sum of squares with weights
+    # 1[j <= k] - 0.9, plus the float32 prefix (lane chunks, a shuffle scan, one subtraction) and 0.90f
+    Pc = np.cumsum(P, axis=1)
+    g = Pc + O_EPS - 0.9 * Et[:, None]
+    aX2 = 0.01 * (Pc - P[:, :1]) + 0.81 * (Et[:, None] - Pc)
+    b = (0.1 * (2 * X[:, :1] * e0c + e0c ** 2) + 2 * np.sqrt(np.maximum(aX2, 0.0)) * ebc + 0.9 * ebc ** 2
+         + MARGIN * (gamma(sum_depth(K) + 2) * (Pc + 0.9 * Et[:, None]) + U32 * 0.9 * Et[:, None]))
+    first = lambda c: np.where(c.any(axis=1), np.argmax(c, axis=1), -1)
+    lo, hi = first(g + b > 0), first(g - b > 0)
+    lo = np.where((lo < 0) | (hi < 0), 0, lo)
+    hi = np.where(hi < 0, K - 1, hi)
+    roll = np.stack([lo, hi])
+    # mfcc: mel bands (linear, non-negative taps; each tap sum sequential in float32), log10 (lg2.approx * log10(2) or
+    # log10f, 2 ulp), DCT (float32 table and sums around a constant offset of the log-mel values)
+    m = X @ M.T                                                                # [T, 40]
+    dm = _lin(M[None], e0c, ebc) + MARGIN * gamma((M > 0).sum(axis=1) + 2)[None, :] * m
+    lm = np.log10(m + O_EPS)
+    lo_m = m - dm
+    mel_unb = (dm > 0) & (lo_m <= 0)
+    dL = np.where(mel_unb, 0.0, lm - np.log10(np.maximum(lo_m, 0.0) + O_EPS))
+    l2 = np.maximum(1.0, np.abs(np.log2(np.maximum(lo_m, 0.0) + O_EPS)))
+    dL = dL + math.log10(2.0) * LOG2_ABS * l2 + 3 * U32 * np.abs(lm)
+    Lrange = lm.max(axis=1) - lm.min(axis=1)
+    Lmax = np.abs(lm).max(axis=1)
+    aD = np.abs(D)
+    g48 = gamma(48)
+    dmf = dL @ aD.T + g48 * aD.sum(axis=1)[None, :] * (Lrange + gamma(8) * Lmax)[:, None]
+    dmf[:, 0] += g48 * 6.33 * Lmax
+    bound[8:21] = dmf.T + F64_REL * (np.abs(lm) @ aD.T).T
+    unbounded(list(range(8, 21)), mel_unb.any(axis=1), "a mel band's interval contains 0 (log10(m + eps))")
+    # chroma: (O X^2)_j / E, E = sum X^2; centred weights O_j - c_j
+    cj = ref[21:33].T                                                          # [T, 12]
+    dc_t = _quad(C[None] - cj[:, :, None], X[:, None, :], e0c, ebc) / _ratio_den(np.where(Et == 0, O_EPS, Et), dEt)[:, None]
+    dc_a = MARGIN * cj * (gamma((C > 0).sum(axis=1) + 3)[None, :] + gK + DIV_REL)
+    dcj = dc_t + dc_a
+    bound[21:33] = dcj.T
+    # chroma_std: 1-Lipschitz in the RMS norm, then its own float32 mean (12 terms), squares and square root
+    mu_e = gamma(6) * cj.mean(axis=1)
+    bound[33] = np.sqrt((dcj ** 2).mean(axis=1)) + MARGIN * (mu_e + (gamma(8) + SQRT_REL) * (ref[33] + mu_e))
+    unbounded([3, 4, 6], np.isnan(Sd), "sum |X| interval contains 0")
+    unbounded([5, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33], np.isnan(_ratio_den(Et + O_EPS, dEt)) & (Et > 0),
+              "sum X^2 interval contains 0")
+    bound = np.where(np.isnan(bound), np.inf, bound)
+    bound += F64_REL * np.abs(ref)
+    if deltas:
+        d = np.zeros_like(ref)
+        d[:, 1:] = ref[:, 1:] - ref[:, :-1]
+        db = np.zeros_like(bound)
+        db[:, 1:] = bound[:, 1:] + bound[:, :-1]
+        db[:, 1:] += 2 * U32 * (np.abs(d[:, 1:]) + db[:, 1:])
+        for reason in list(unb):
+            unb["delta: " + reason] = unb[reason]
+        ref, bound = np.concatenate([ref, d]), np.concatenate([bound, db])
+    return FeatureBounds(ref, bound, roll, unb, K)
+
+
+def check_feature_bounds(got, fb, what=""):
+    """Rows ``got`` [F, T] against a FeatureBounds: every bounded entry within its bound, rolloff (and its delta) a whole
+    number of quanta inside the admissible range, no exception lists and no flip allowance.  Returns ({row group:
+    worst err / bound}, {reason: unbounded entries})."""
+    got = np.asarray(got, dtype=np.float64)
+    assert got.shape == fb.ref.shape, (what, got.shape, fb.ref.shape)
+    assert np.isfinite(got).all(), what + ": non-finite output"
+    F, T = got.shape
+    K = fb.K
+    err = np.abs(got - fb.ref)
+    fin = np.isfinite(fb.bound)
+    ratio = np.where(fin, err / np.where(fb.bound > 0, fb.bound, 1.0), 0.0)
+    ratio = np.where(fin & (fb.bound == 0), np.where(err > 0, np.inf, 0.0), ratio)
+    lo, hi = fb.roll
+    for r in (ROLLOFF_ROW, ROLLOFF_ROW + 34):
+        if r >= F:
+            continue
+        q = np.rint(got[r] * K)
+        if r == ROLLOFF_ROW:
+            qlo, qhi, scale = lo, hi, q
+        else:
+            qlo = np.concatenate([[0], lo[1:] - hi[:-1]])
+            qhi = np.concatenate([[0], hi[1:] - lo[:-1]])
+            scale = np.abs(fb.ref[ROLLOFF_ROW] * K) + np.abs(np.concatenate([[0], fb.ref[ROLLOFF_ROW, :-1] * K]))
+        off = (q < qlo) | (q > qhi) | (np.abs(got[r] * K - q) > 4 * U32 * (scale + 1))
+        if off.any():
+            t = int(np.nonzero(off)[0][0])
+            raise AssertionError("%s: row %d (rolloff) outside its admissible quanta in %d frames, first %d: %r quanta, "
+                                 "admissible %d .. %d" % (what, r, int(off.sum()), t, got[r, t] * K, qlo[t], qhi[t]))
+        ratio[r] = 0.0
+    bad = ratio > 1.0
+    if bad.any():
+        rows, cols = np.nonzero(bad)
+        k = int(np.argmax(ratio[bad]))
+        raise AssertionError("%s: %d entries outside the feature bound, rows %s; worst (row %d, frame %d): %r vs %r, bound "
+                             "%.3g (err / bound %.3g)" % (what, rows.size, np.unique(rows)[:12].tolist(), rows[k], cols[k],
+                                                        got[rows[k], cols[k]], fb.ref[rows[k], cols[k]],
+                                                        fb.bound[rows[k], cols[k]], ratio[rows[k], cols[k]]))
+    worst = {name: float(ratio[[r for r in rows if r < F]].max()) if T else 0.0 for name, rows in ROW_GROUPS.items()}
+    if F > 34:
+        worst["deltas"] = float(ratio[34:].max()) if T else 0.0
+    return worst, dict(fb.unbounded)
