@@ -203,6 +203,37 @@ int b200aa_long_term_mean_ragged(const float *d_mid, int64_t n_clips, int n_rows
 int b200aa_normalize_windows(const float *d_mid, int64_t n_clips, int n_rows, int64_t n_windows,
                              const float *d_mean, const float *d_std, float *d_out, void *stream);
 
+/* PCM WAV decode (SURVEY 8f rank 2): data-chunk formats of a byte arena, as scipy.io.wavfile.read returns them */
+#define B200AA_PCM_U8 0           /* PCM 8-bit, unsigned                                        */
+#define B200AA_PCM_S16 1          /* PCM 16-bit                                                 */
+#define B200AA_PCM_S24 2          /* PCM 24-bit, packed (scipy: int32, the 3 bytes shifted left by 8) */
+#define B200AA_PCM_S32 3          /* PCM 32-bit                                                 */
+#define B200AA_PCM_F32 4          /* IEEE float 32                                              */
+#define B200AA_PCM_F64 5          /* IEEE float 64                                              */
+
+/* One clip of the arena: n_frames interleaved frames of `channels` (1 or 2) little-endian samples of `format`, starting
+ * at byte `offset` (a multiple of 16).  The clip's slot runs from offset to offset + n_frames * block rounded up to a
+ * multiple of 16 (block = channels * sample bytes) and is zero past the frames.  24 bytes. */
+typedef struct b200aa_pcm_clip {
+    int64_t offset;
+    int64_t n_frames;
+    int32_t format;
+    int32_t channels;
+} b200aa_pcm_clip;
+
+/* Decode a ragged batch of WAV data chunks: d_out [n_clips, n_out] of out_dtype (B200AA_DTYPE_I16 / _F32), row b at
+ * d_out + b * out_stride elements.  out[b, i] for i < n_frames of clip b is the frame converted as
+ * _as_clip(stereo_to_mono(wavfile.read(path)[1])) stages it (csrc/pcm.cuh: mono U8 / S16 as int16, every other flavour
+ * as float32; NaN stays NaN, its payload may differ), and 0 for n_frames <= i < n_out; every element is written.
+ * h_clips is HOST memory and every descriptor is checked before any CUDA call: NULL pointers, n_clips < 0, n_out < 0,
+ * out_stride < n_out, an unknown format, channels other than 1 or 2, a negative or misaligned offset, n_frames < 0 or
+ * > n_out, a slot past arena_bytes, and out_dtype int16 for anything but mono U8 / S16 are B200AA_ERR_INVALID.  The
+ * descriptors are then copied to stream-ordered scratch; nothing synchronises.
+ * Replaces: wavfile.read + stereo_to_mono + the float32 cast (audioBasicIO.py:86-110, :156-168) of every file of a
+ * folder, on the host. */
+int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const b200aa_pcm_clip *h_clips, int64_t n_clips,
+                      int out_dtype, void *d_out, int64_t n_out, int64_t out_stride, void *stream);
+
 /* Kernel 4: beat rate of every clip from its short-term rows 0, 1, 3 .. 18 (SURVEY 8f rank 4).  d_st: float32
  * [n_clips, n_feats, t_stride], n_feats >= 19; d_frames (nullable, int64 [n_clips]): frames of each clip, clamped to
  * [0, n_frames]; else n_frames for every clip.  d_out: float64 [n_clips, 2] = (bpm, ratio), bit for bit the host

@@ -1,9 +1,9 @@
 """Drop-in for ``pyAudioAnalysis.MidTermFeatures.mid_feature_extraction`` (MidTermFeatures.py:87-127), ``beat_extraction``
 (:18-84) and the directory wrappers around them (``directory_feature_extraction`` :140-221,
 ``multiple_directory_feature_extraction`` :224-260, ``directory_feature_extraction_no_avg`` :263-309): files are decoded on
-the host (``audioio``: .wav / .aif / .aiff, and .mp3 / .au / .ogg when pydub is installed, as in the reference), files of
-equal sampling rate and sample format, whatever their lengths, are staged in page-locked memory and batched into ragged
-GPU launches."""
+the GPU (PCM / float WAV, mono or stereo: ``audioio.wav_pcm_layout``, ``audioio.stage``) or on the host (other WAV
+files, .aif / .aiff, and .mp3 / .au / .ogg when pydub is installed, as in the reference); files of equal sampling rate and
+sample format, whatever their lengths, are staged in page-locked memory and batched into ragged GPU launches."""
 import ctypes
 import glob
 import os
@@ -107,22 +107,26 @@ _MAX_PADDING = 0.25              # padding samples of a chunk per sample of its 
 
 
 class _Clip:
-    """One audio file of a folder: either still on disk as mono 16-bit PCM (decoded later, straight into page-locked
-    staging memory) or already decoded to a 1-D array."""
-    __slots__ = ("path", "fs", "n", "data", "code")
+    """One audio file of a folder: either still on disk as a WAV file whose data chunk the device decodes (``layout`` =
+    (data_offset, format, channels) of ``audioio.wav_pcm_layout``; read later straight into page-locked staging memory)
+    or already decoded to a 1-D array."""
+    __slots__ = ("path", "fs", "n", "data", "code", "layout")
 
-    def __init__(self, path, fs, n, data, code):
-        self.path, self.fs, self.n, self.data, self.code = path, int(fs), int(n), data, code
+    def __init__(self, path, fs, n, data, code, layout=None):
+        self.path, self.fs, self.n, self.data, self.code, self.layout = path, int(fs), int(n), data, code, layout
 
 
 def _open_clip(path):
-    """audioBasicIO.read_audio_file + stereo_to_mono for one file, lazily for plain mono PCM16 .wav."""
+    """audioBasicIO.read_audio_file + stereo_to_mono for one file, lazily for every WAV flavour audioio.wav_pcm_layout
+    accepts: mono 8 / 16-bit PCM stages as int16, everything else as float32, the code _as_clip gives."""
     from . import audioio
-    from ._lib import DTYPE_I16
+    from ._lib import DTYPE_I16, DTYPE_F32
     if os.path.splitext(path)[1].lower() == ".wav":
-        lay = audioio.wav_pcm16_layout(path)
-        if lay is not None and lay[1] == 1:
-            return _Clip(path, lay[0], lay[2], None, DTYPE_I16)
+        lay = audioio.wav_pcm_layout(path)
+        if lay is not None:
+            fs, ch, n, off, fmt = lay
+            code = DTYPE_I16 if ch == 1 and fmt in (audioio.PCM_U8, audioio.PCM_S16) else DTYPE_F32
+            return _Clip(path, fs, n, None, code, layout=(off, fmt, ch))
     fs, x = audioio.read_audio_file(path)
     clip, code = _as_clip(audioio.stereo_to_mono(x))
     return _Clip(path, fs, clip.shape[0], clip, code)
@@ -159,28 +163,6 @@ def _plan_chunks(clips, max_bytes=None, max_padding=None):
     return chunks
 
 
-def _upload_chunk(clips, code):
-    """Clips of one chunk, longest first -> ([n, N] device tensor, int64 device lengths [n]), N the first clip's
-    length; each row is zero past its clip.  int16 clips are staged in page-locked memory (files still on disk are
-    read straight into their row) so the H2D copy runs at full PCIe speed."""
-    import torch
-    from ._lib import DTYPE_I16
-    n_max = clips[0].n
-    lengths = torch.tensor([c.n for c in clips], dtype=torch.int64).cuda()
-    if code == DTYPE_I16:
-        from .audioio import PinnedBatch
-        pb = PinnedBatch(len(clips), n_max)
-        for k, c in enumerate(clips):
-            pb.fill(k, c.path, c.data, n=c.n)
-        dev = pb.to_device()
-        torch.cuda.current_stream().synchronize()          # the staging buffer is released on return
-        return dev, lengths
-    x = np.zeros((len(clips), n_max), dtype=np.float32)
-    for k, c in enumerate(clips):
-        x[k, :c.n] = c.data
-    return torch.from_numpy(x).cuda(), lengths
-
-
 def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_short=False, want_long_term=False,
                   want_beat=False):
     """Mid-term results of a list of _Clip, in input order: (mid float64 [136 x M] or its long-term mean [136],
@@ -188,16 +170,17 @@ def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_sh
     share launches as ragged batches (_plan_chunks); every clip's results are bit for bit those of the clip alone.  The
     long-term mean and the beat are computed on the GPU from the resident features."""
     from .batch import mid_feature_extraction_batch, long_term_mean_batch, beat_extraction_batch, frame_counts
+    from . import audioio
     L = lib()
     results = [None] * len(clips)
     for part in _plan_chunks(clips):
         chunk = [clips[i] for i in part]
-        fs, code = chunk[0].fs, chunk[0].code
+        fs = chunk[0].fs
         w, s = round(fs * short_window), round(fs * short_step)
         mw, ms = round(mid_window * fs), round(mid_step * fs)
         if L.b200aa_num_frames(chunk[-1].n, w, s) <= 0:
             check(_lib.ERR_TOO_SHORT)       # alone, the shortest clip has no frames: a ragged batch would give it none
-        dev, lengths = _upload_chunk(chunk, code)
+        dev, lengths = audioio.stage(chunk)            # one arena, one H2D copy, one decode launch
         mid, st = mid_feature_extraction_batch(dev, fs, mw, ms, w, s, lengths=lengths)
         stepr = mid_ratios(mw, ms, w, s)[1]
         if want_long_term or want_beat:

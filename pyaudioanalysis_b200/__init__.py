@@ -12,8 +12,9 @@ from . import ShortTermFeatures, MidTermFeatures, consumers  # noqa: F401
 from .batch import (feature_extraction_batch, mid_feature_extraction_batch, clip_stats,  # noqa: F401
                     spectrogram_batch, chromagram_batch, beat_extraction_batch, frame_counts, mid_pool_batch,
                     long_term_mean_batch, row_counts)
+from .audioio import load_batch  # noqa: F401
 from .install import install, uninstall  # noqa: F401
 
 __all__ = ["ShortTermFeatures", "MidTermFeatures", "consumers", "feature_extraction_batch", "mid_feature_extraction_batch",
            "spectrogram_batch", "chromagram_batch", "beat_extraction_batch", "frame_counts", "mid_pool_batch",
-           "long_term_mean_batch", "row_counts", "clip_stats", "install", "uninstall"]
+           "long_term_mean_batch", "row_counts", "clip_stats", "load_batch", "install", "uninstall"]

@@ -54,6 +54,8 @@ SIGNATURES = {
     "b200aa_mid_pool_ragged": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_int, c_vp, c_vp]),
     "b200aa_long_term_mean_ragged": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_normalize_windows": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    # (d_arena, arena_bytes, h_clips, n_clips, out_dtype, d_out, n_out, out_stride, stream)
+    "b200aa_decode_pcm": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_i64, c_i64, c_vp]),
     "b200aa_beat_extraction": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

@@ -20,6 +20,7 @@
 #include "generic_kernel.cuh"
 #include "fast_kernel.cuh"
 #include "pair_kernel.cuh"
+#include "pcm.cuh"
 #include "solo_kernel.cuh"
 #include "tables.inl"
 
@@ -737,6 +738,56 @@ extern "C" int b200aa_normalize_windows(const float *d_mid, int64_t n_clips, int
     normalize_windows_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(d_mid, n_rows, n_windows, d_mean, d_std, d_out);
     CK_LAUNCH("normalize_windows_kernel");
     return B200AA_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// PCM WAV decode (csrc/pcm.cuh): raw data chunks of a byte arena -> the [B, N] int16 / float32 ragged batch
+// ------------------------------------------------------------------------------------------------
+extern "C" int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const b200aa_pcm_clip *h_clips, int64_t n_clips,
+                                 int out_dtype, void *d_out, int64_t n_out, int64_t out_stride, void *stream)
+{
+    NvtxRange nvtx_("b200aa_decode_pcm");
+    if (!d_arena || !h_clips || !d_out || arena_bytes < 0 || n_clips < 0 || n_out < 0 || out_stride < n_out ||
+        (out_dtype != B200AA_DTYPE_I16 && out_dtype != B200AA_DTYPE_F32))
+        return B200AA_ERR_INVALID;
+    for (int64_t b = 0; b < n_clips; ++b) {
+        const b200aa_pcm_clip &c = h_clips[b];
+        const int64_t bytes = pcm::sample_bytes(c.format);
+        if (bytes == 0 || (c.channels != 1 && c.channels != 2) || c.offset < 0 || c.offset % 16 || c.n_frames < 0 ||
+            c.n_frames > n_out)
+            return B200AA_ERR_INVALID;
+        if (out_dtype == B200AA_DTYPE_I16 && (c.channels != 1 || (c.format != B200AA_PCM_U8 && c.format != B200AA_PCM_S16)))
+            return B200AA_ERR_INVALID;
+        const int64_t block = c.channels * bytes;
+        if (c.offset > arena_bytes || c.n_frames > (arena_bytes - c.offset) / block ||
+            (c.n_frames * block + 15) / 16 * 16 > arena_bytes - c.offset)      // the kernel reads whole 16-byte words
+            return B200AA_ERR_INVALID;
+    }
+    if (n_clips == 0 || n_out == 0) return B200AA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    b200aa_pcm_clip *d_clips = nullptr;
+    CK(cudaMallocAsync(reinterpret_cast<void **>(&d_clips), size_t(n_clips) * sizeof(b200aa_pcm_clip), st));
+    const int64_t tiles = (n_out + pcm::kTile - 1) / pcm::kTile;
+    const int64_t items = n_clips * tiles;
+    const unsigned grid = unsigned(std::min<int64_t>(items, int64_t(1) << 30));
+    int rc = B200AA_OK;
+    cudaError_t e = cudaMemcpyAsync(d_clips, h_clips, size_t(n_clips) * sizeof(b200aa_pcm_clip), cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) {
+        rc = cuda_fail(e, "cudaMemcpyAsync");
+    } else {
+        const unsigned char *arena = static_cast<const unsigned char *>(d_arena);
+        if (out_dtype == B200AA_DTYPE_I16)
+            pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
+                                                               static_cast<int16_t *>(d_out));
+        else
+            pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
+                                                               static_cast<float *>(d_out));
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        if ((e = cudaGetLastError()) != cudaSuccess) rc = cuda_fail(e, "pcm::decode_kernel");
+    }
+    e = cudaFreeAsync(d_clips, st);
+    if (e != cudaSuccess && rc == B200AA_OK) rc = cuda_fail(e, "cudaFreeAsync");
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """Small driver for compute-sanitizer: every kernel family once on tiny inputs (pair / CTA / generic feature kernels incl.
-the large-window form, rows, mid-term pooling, the chunked host pipeline)."""
+the large-window form, rows, mid-term pooling, the WAV decode, the chunked host pipeline)."""
 import os
 import sys
 
@@ -52,6 +52,14 @@ if os.environ.get("B200AA_SANITIZE_STEAL"):
     pkg.feature_extraction_batch(big[:, :132300].contiguous(), 44100, 882, 441)
 from pyaudioanalysis_b200.consumers import normalize_windows_batch
 normalize_windows_batch(torch.randn(2, 136, 9, device="cuda"), np.zeros(136), np.ones(136))      # consumers: normalise + transpose
+import tempfile
+from tests import wavgen
+with tempfile.TemporaryDirectory() as d:                                         # WAV decode: all 12 flavours, one launch
+    paths = []
+    for k, (name, ch) in enumerate(wavgen.FLAVOURS):
+        paths.append(os.path.join(d, "%02d.wav" % k))
+        wavgen.write(paths[-1], 16000, wavgen.signal(name, ch, 1000 + 3 * k, k), name)
+    pkg.audioio.stage([pkg.MidTermFeatures._open_clip(p) for p in paths])
 hp = HostPipeline(16000, 800, 400, 24000, max_clips=6, device=0, bind_numa=False)
 hp.h_in[:] = clips.cpu().numpy()
 hp.run()
