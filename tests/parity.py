@@ -18,8 +18,11 @@ std: their RMS).
 float64 DFT under a bound derived from float32 FFT arithmetic (derivation: tests/test_gpu_spectra.py).
 ``feature_bounds`` / ``check_feature_bounds`` carry that bound, plus the float32 arithmetic of the feature stage, to a
 bound on every entry of the 68 rows (derivation: tests/test_feature_bounds_cpu.py).
+``chromagram_bounds`` / ``check_chromagram_bounds`` do the same for chromagram rows: full rows from the spectrum bound,
+clipped rows from a per-bin model of the clipped-frame kernel's fp64 DFT (derivation: tests/test_chroma_bounds_cpu.py).
 """
 import math
+from fractions import Fraction
 
 import numpy as np
 
@@ -306,6 +309,35 @@ def _entropy_bound(s, ds):
     return dev.sum(axis=-1)
 
 
+def _quad_bins(a, X, eps):
+    """max |sum_k a_k ((X_k + d_k)^2 - X_k^2)| over |d_k| <= eps_k, bin by bin: sum |a_k| (2 X_k eps_k + eps_k^2)."""
+    return (np.abs(a) * (2 * X * eps + eps ** 2)).sum(axis=-1)
+
+
+def chroma_bound(X, C, cj, e0=None, eb=None, eps=None):
+    """Per-entry bound [T, 12] on the chroma classes c_j = (C X^2)_j / E, E = sum X^2 (E == 0: divided by eps, as the
+    reference does) that a kernel may return for frames whose float64 spectrum is X [T, K] and whose float64 classes are
+    cj [T, 12]; nan where the interval of E reaches 0 (unbounded).
+
+    Transform error, either the ball of spectrum_reference (|d_0| <= e0, |d_1..K-1|_2 <= eb, a float32 FFT) or per bin
+    (|d_k| <= eps[:, k], the clipped-frame kernel's fp64 DFT): carried with centred weights C_j - c_j through the squares
+    (_quad / _quad_bins) over E - dE.  Float32 chroma stage: each class a sequential fma of its squared taps (gamma(taps +
+    3)), sum X^2 at depth sum_depth(K) (gamma; covers the 16-lane sums of the solo kernel's Kp-padded rows, the deepest
+    layout), and one division (DIV_REL covers IEEE division and __fdividef)."""
+    K = X.shape[1]
+    Et = (X ** 2).sum(axis=1)
+    w = C[None] - cj[:, :, None]                                               # [T, 12, K]
+    if eps is None:
+        dEt = _quad(np.ones(K), X, e0, eb)
+        num = _quad(w, X[:, None, :], e0[:, None], eb[:, None])
+    else:
+        dEt = _quad_bins(np.ones(K), X, eps)
+        num = _quad_bins(w, X[:, None, :], eps[:, None, :])
+    dc_t = num / _ratio_den(np.where(Et == 0, O_EPS, Et), dEt)[:, None]
+    dc_a = MARGIN * cj * (gamma((C > 0).sum(axis=1) + 3)[None, :] + gamma(sum_depth(K)) + DIV_REL)
+    return dc_t + dc_a
+
+
 class FeatureBounds:
     """feature_bounds' result for one clip: ``ref`` [F, T] float64 reference, ``bound`` [F, T] per-entry bound (inf where
     unbounded), ``roll`` [2, T] admissible rolloff quanta (lo, hi) of every frame, ``unbounded`` {reason: count} and
@@ -448,11 +480,8 @@ def feature_bounds(x, fs, w, s, deltas=False):
     dmf[:, 0] += g48 * 6.33 * Lmax
     bound[8:21] = dmf.T + F64_REL * (np.abs(lm) @ aD.T).T
     unbounded(list(range(8, 21)), mel_unb.any(axis=1), "a mel band's interval contains 0 (log10(m + eps))")
-    # chroma: (O X^2)_j / E, E = sum X^2; centred weights O_j - c_j
     cj = ref[21:33].T                                                          # [T, 12]
-    dc_t = _quad(C[None] - cj[:, :, None], X[:, None, :], e0c, ebc) / _ratio_den(np.where(Et == 0, O_EPS, Et), dEt)[:, None]
-    dc_a = MARGIN * cj * (gamma((C > 0).sum(axis=1) + 3)[None, :] + gK + DIV_REL)
-    dcj = dc_t + dc_a
+    dcj = chroma_bound(X, C, cj, e0=e0, eb=eb)
     bound[21:33] = dcj.T
     # chroma_std: 1-Lipschitz in the RMS norm, then its own float32 mean (12 terms), squares and square root
     mu_e = gamma(6) * cj.mean(axis=1)
@@ -516,3 +545,178 @@ def check_feature_bounds(got, fb, what=""):
     if F > 34:
         worst["deltas"] = float(ratio[34:].max()) if T else 0.0
     return worst, dict(fb.unbounded)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Per-entry bound of chromagram rows, full-frame and clipped (derivation: tests/test_chroma_bounds_cpu.py)
+U64 = 2.0 ** -53        # unit round-off of float64
+TWIDDLE_ABS = (4 + 2 * math.pi) * U64   # sincospi(2j / n), per component: 2 ulp (< 4 u64 on [-1, 1]) + the rounded quotient
+REF_FFT_C = 8.0         # numpy's float64 FFT of the reference, the same form as SPECTRUM_C
+ROW_FULL, ROW_CLIPPED, ROW_EMPTY = 0, 1, 2
+ROW_CLASS_NAMES = {ROW_FULL: "full", ROW_CLIPPED: "clipped", ROW_EMPTY: "never filled"}
+
+
+def gamma64(n):
+    n = np.asarray(n, dtype=np.float64)
+    return n * U64 / (1.0 - n * U64)
+
+
+def chromagram_rows(n, w, s):
+    """csrc/rows.cuh's chromagram rule restated: (R, n_it, n_full, refused) for a clip of n samples."""
+    R = int((n - s - w) / s) + 1
+    n_it = min(R, len(range(w, n - s, s))) if R > 0 else 0
+    n_full = min(n_it, (n - 2 * w) // s + 1) if n >= 2 * w else 0
+    refused = R <= 0 or n - s - w < 0 or (n_it > n_full and n - (w + (n_it - 1) * s) < w // 2)
+    return R, n_it, n_full, refused
+
+
+class ChromaBounds:
+    """chromagram_bounds' result for one clip: ``ref`` [R, 12] float64 reference, ``bound`` [R, 12] per-entry bound (inf
+    where unbounded), ``cls`` [R] row class (ROW_FULL, ROW_CLIPPED, ROW_EMPTY), ``refused`` (the single-clip entry point
+    refuses the clip: no rows) and ``unbounded`` {reason: entries}."""
+
+    def __init__(self, ref, bound, cls, refused, unbounded):
+        self.ref, self.bound, self.cls, self.refused, self.unbounded = ref, bound, cls, refused, unbounded
+
+
+def _exact_sum(v):
+    """The exact sum of int16 / float32 values as a Fraction."""
+    v = np.asarray(v)
+    if v.dtype == np.int16:
+        return Fraction(int(v.astype(np.int64).sum()))
+    return sum(map(Fraction, v.astype(np.float64).tolist()), Fraction(0))
+
+
+def clip_record_error(x):
+    """(a, mean, mean_q, alpha, dmean) of the kernels' normalisation record of clip x: the float64 a of clip_norm at the
+    rounded mean, that mean, the exact mean (a Fraction), the relative error alpha of the float32 record value a, and
+    dmean, a bound on the error of the kernels' fp64 mean: an exact int64 sum divided once for int16 input (the same
+    rounded quotient as here), a float64 sum in any order for float32.  The record's a is 1 / (maxdev + c) evaluated in
+    fp64 from that mean (maxdev moves by dmean) and rounded to float32."""
+    xd = np.asarray(x, dtype=np.float64)
+    n = xd.size
+    mean_q = _exact_sum(x) / n
+    mean = float(mean_q)
+    if np.asarray(x).dtype == np.int16:
+        dmean = float(abs(Fraction(mean) - mean_q))
+    else:
+        dmean = float(gamma64(n)) * math.fsum(np.abs(xd)) / n + 2 * U64 * abs(mean)
+    den = max(xd.max() - mean, mean - xd.min()) + 32768.0 * 1e-10
+    a = 1.0 / den
+    alpha = MARGIN * (U32 + dmean / den + 4 * U64)
+    return a, mean, mean_q, alpha, dmean
+
+
+def clipped_spectrum_reference(x, p, K, rec=None):
+    """The clipped frame y[p:] of clip x (n = len(x) - p samples, K <= n): float64 |DFT|[0:K] / K of the normalised
+    frame, and eps [K], a per-bin bound on |kernel - reference| for clipped_chroma_kernel's arithmetic (derivation:
+    tests/test_chroma_bounds_cpu.py), the reference's own error included.  ``rec``: clip_record_error(x), if at hand."""
+    xd = np.asarray(x, dtype=np.float64)
+    f32 = np.asarray(x).dtype == np.float32
+    a, mean, mean_q, alpha, dmean = rec or clip_record_error(x)
+    fr = xd[p:]
+    n = fr.size
+    z = fr - fr[0]                                               # exact: a difference of two int16 / float32 values
+    z1 = np.abs(z).sum()
+    D = np.abs(np.fft.fft(z)[:K])                                # |DFT z|, bins k >= 1 of the frame's DFT
+    S = float(_exact_sum(np.asarray(x)[p:]) - n * mean_q)         # sum of x - mean over the frame, rounded once
+    D[0] = abs(S)
+    X = a * D / K
+    # |m - mean| of the record's centre: for int16 the kernels round the same fp64 mean to the nearest integer, for float32
+    # input they round their own fp64 mean (within dmean) to float
+    dm = U32 * (abs(mean) + dmean) + dmean if f32 else abs(float(np.rint(mean)) - mean) + dmean
+    # bins k >= 1: (re, im) err by (gamma64(n + 2) + twiddle) |z|_1 each; a * sqrt(re^2 + im^2) by 4 u64 more and a's alpha
+    dft = math.sqrt(2.0) * (float(gamma64(n + 2)) + TWIDDLE_ABS) * z1
+    eps = a * (alpha * D + (1 + alpha) * dft + 4 * U64 * D)
+    # DC: a re + n (a (x0 - m) + bp) in fp64 from the float32 record: (a' - a) sum(x - m) + n (bp' - bp), plus the sum
+    # re (n additions) and the roundings of the expression
+    dbp = a * ((U32 + alpha) * dm + dmean)
+    eps[0] = (alpha * a * (abs(S) + n * dm) + n * dbp + a * float(gamma64(n + 2)) * z1
+              + 8 * U64 * a * (z1 + n * (abs(fr[0] - mean) + dm)))
+    # the reference's own error: numpy's FFT of z (bins), the rounding of S and of a S (DC), and a from the rounded mean
+    ref_err = a * REF_FFT_C * U64 * max(1, math.ceil(math.log2(n))) * math.sqrt(n) * np.linalg.norm(z) + 4 * U64 * a * D
+    ref_err[0] = 2 * U64 * a * abs(S)
+    ref_err = ref_err + (2 * U64 * abs(mean) * a + 2 * U64) * a * D          # a = 1 / den moves by dmean / den
+    eps = MARGIN * (eps + ref_err) / K
+    # the float64 magnitude divided by K, rounded to float once
+    eps = eps + U32 * (X + eps) + 2 * U64 * X
+    return X, eps
+
+
+def chromagram_bounds(x, fs, w, s):
+    """The float64 reference of the chromagram rows of clip x at (fs, w, s), a per-entry bound on what the kernels may
+    return, and the row class of each row.
+
+    * full rows (frame at w + r s, all w samples): the spectrum_reference ball at those starts through chroma_bound;
+    * clipped rows (n = len - (w + r s) samples, K <= n < w): clipped_spectrum_reference's per-bin bound through
+      chroma_bound;
+    * rows the reference's loop never fills: exactly 0.
+    A frame whose spectrum is exactly 0 gets exactly 0 (the EPS branch) and a constant frame its DC bin's class weights,
+    both up to the float32 chroma stage only.  Derivation: tests/test_chroma_bounds_cpu.py."""
+    from oracle import st_oracle as O
+    x = np.asarray(x)
+    K = w // 2
+    R, n_it, n_full, refused = chromagram_rows(x.size, w, s)
+    if refused:
+        return ChromaBounds(np.zeros((0, 12)), np.zeros((0, 12)), np.zeros(0, dtype=int), True, {})
+    C = _tables(fs, K)[2]
+    ref = np.zeros((R, 12))
+    bound = np.zeros((R, 12))
+    cls = np.full(R, ROW_EMPTY)
+    unb = {}
+
+    def classes(X):
+        Et = (X ** 2).sum(axis=1)
+        return (X ** 2) @ C.T / np.where(Et == 0, O_EPS, Et)[:, None]
+
+    if n_full:
+        starts = w + s * np.arange(n_full)
+        X, eb, e0, flat = spectrum_reference(x, starts, w)
+        eb = np.where(flat, 0.0, eb)                   # a constant frame's bins 1 .. K-1 are exactly zero
+        cj = classes(X)
+        ref[:n_full] = cj
+        bound[:n_full] = chroma_bound(X, C, cj, e0=e0, eb=eb)
+        cls[:n_full] = ROW_FULL
+    if n_it > n_full:
+        rows = np.arange(n_full, n_it)
+        rec = clip_record_error(x)
+        XE = [clipped_spectrum_reference(x, w + s * i, K, rec) for i in rows]
+        X = np.stack([v[0] for v in XE])
+        eps = np.stack([v[1] for v in XE])
+        cj = classes(X)
+        ref[rows] = cj
+        bound[rows] = chroma_bound(X, C, cj, eps=eps)
+        cls[rows] = ROW_CLIPPED
+    nan = np.isnan(bound).any(axis=1)
+    if nan.any():
+        unb["sum X^2 interval contains 0"] = int(nan.sum()) * 12
+    bound = np.where(np.isnan(bound), np.inf, bound)
+    bound += F64_REL * np.abs(ref)
+    return ChromaBounds(ref, bound, cls, False, unb)
+
+
+def check_chromagram_bounds(got, cb, what=""):
+    """Rows ``got`` [R, 12] against a ChromaBounds: every bounded entry within its bound (a zero bound: exactly equal),
+    rows never filled exactly 0.  Returns ({row class name: worst err / bound}, {reason: unbounded entries})."""
+    got = np.asarray(got, dtype=np.float64)
+    assert got.shape == cb.ref.shape, (what, got.shape, cb.ref.shape)
+    assert np.isfinite(got).all(), what + ": non-finite output"
+    err = np.abs(got - cb.ref)
+    fin = np.isfinite(cb.bound)
+    ratio = np.where(fin, err / np.where(cb.bound > 0, cb.bound, 1.0), 0.0)
+    ratio = np.where(fin & (cb.bound == 0), np.where(err > 0, np.inf, 0.0), ratio)
+    bad = ratio > 1.0
+    if bad.any():
+        rows, cols = np.nonzero(bad)
+        k = int(np.argmax(ratio[bad]))
+        r, c = rows[k], cols[k]
+        raise AssertionError("%s: %d entries outside the chromagram bound in rows %s; worst (%s row %d, class %d): %r vs %r, "
+                             "bound %.3g (err / bound %.3g)" % (what, rows.size, np.unique(rows)[:12].tolist(),
+                                                              ROW_CLASS_NAMES[int(cb.cls[r])], r, c, got[r, c], cb.ref[r, c],
+                                                              cb.bound[r, c], ratio[r, c]))
+    worst = {}
+    for c, name in ROW_CLASS_NAMES.items():
+        sel = cb.cls == c
+        if sel.any():
+            worst[name] = float(ratio[sel].max())
+    return worst, dict(cb.unbounded)
