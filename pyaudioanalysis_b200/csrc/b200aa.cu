@@ -8,7 +8,6 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
-#include <map>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -42,12 +41,50 @@ static int cuda_fail(cudaError_t e, const char *what)
         cudaError_t e_ = (call);                                     \
         if (e_ != cudaSuccess) return cuda_fail(e_, #call);          \
     } while (0)
+// every kernel launch ends here: count it (b200aa_launch_count), then report its launch error
+static int launched(const char *name)
+{
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? B200AA_OK : cuda_fail(e, name);
+}
 #define CK_LAUNCH(name)                                              \
     do {                                                             \
-        g_launches.fetch_add(1, std::memory_order_relaxed);          \
-        cudaError_t e_ = cudaGetLastError();                         \
-        if (e_ != cudaSuccess) return cuda_fail(e_, name);           \
+        const int rc_ = launched(name);                              \
+        if (rc_ != B200AA_OK) return rc_;                            \
     } while (0)
+
+// Stream-ordered device scratch of one entry point, bound to its scope: alloc() takes it with cudaMallocAsync, done(rc)
+// frees it after everything queued on the stream and returns rc, else the free's error.  A scope left early (its error
+// already reported) frees it in the destructor.
+class StreamScratch {
+  public:
+    explicit StreamScratch(cudaStream_t st) : st_(st) {}
+    StreamScratch(const StreamScratch &) = delete;
+    StreamScratch &operator=(const StreamScratch &) = delete;
+    ~StreamScratch() { release(); }
+    int alloc(size_t bytes)
+    {
+        if (bytes) CK(cudaMallocAsync(&p_, bytes, st_));
+        return B200AA_OK;
+    }
+    void *get() const { return p_; }
+    int done(int rc)
+    {
+        const cudaError_t e = release();
+        return (e != cudaSuccess && rc == B200AA_OK) ? cuda_fail(e, "cudaFreeAsync") : rc;
+    }
+
+  private:
+    cudaError_t release()
+    {
+        const cudaError_t e = p_ ? cudaFreeAsync(p_, st_) : cudaSuccess;
+        p_ = nullptr;
+        return e;
+    }
+    cudaStream_t st_;
+    void *p_ = nullptr;
+};
 
 struct NvtxRange {
     explicit NvtxRange(const char *name) { nvtxRangePushA(name); }
@@ -102,7 +139,7 @@ extern "C" int b200aa_host_table(int fs, int window, int which, double *h_out)
 
 extern "C" int64_t b200aa_num_frames(int64_t n, int w, int s)
 {
-    return (w < 1 || s < 1) ? 0 : b200aa_host::num_frames(n, w, s);
+    return (w < 1 || s < 1) ? 0 : rows::frames(n, w, s);
 }
 extern "C" int64_t b200aa_spectrogram_rows(int64_t n, int w, int s)
 {
@@ -112,8 +149,7 @@ extern "C" int64_t b200aa_chromagram_rows(int64_t n, int w, int s)
 {
     return (w < 1 || s < 1) ? 0 : rows::chromagram(n, w, s).R;
 }
-// the counts the device needs per clip of a ragged batch; b200aa_num_frames / b200aa_mid_windows on the host
-__host__ __device__ inline int64_t frames_of(int64_t n, int w, int s) { return n < w ? 0 : (n - w) / s + 1; }
+// mid-term windows of a clip of n_frames frames: b200aa_mid_windows on the host, per clip of a ragged batch on the device
 __host__ __device__ inline int64_t windows_of(int64_t n_frames, int stepr)
 {
     return (stepr < 1 || n_frames <= 0) ? 0 : (n_frames + stepr - 1) / stepr;
@@ -124,15 +160,28 @@ extern "C" int64_t b200aa_mid_windows(int64_t n_frames, int stepr) { return wind
 // ------------------------------------------------------------------------------------------------
 // plan
 // ------------------------------------------------------------------------------------------------
-struct Transform {           // device tables of one transform length
-    int n = 0, Nc = 0, packed = 0;
+struct Transform {           // the window's transform: packed real (even window) or complex, and its device twiddles
+    int Nc = 0, packed = 0;
     std::vector<int> radix;
-    float2 *d_tw = nullptr, *d_tw_post = nullptr;
-    ~Transform()
+    b200aa_host::DeviceMemory tw, tw_post;      // float2 [Nc] each
+};
+
+// Device buffer that only grows, reused across calls (a cudaMalloc / cudaFree pair per call costs more than the kernels
+// for a single clip)
+struct GrowBuffer {
+    b200aa_host::DeviceMemory p;
+    size_t cap = 0;
+    // at least `need` bytes: when it holds fewer, it is reallocated to `want` (>= need) bytes
+    cudaError_t reserve(size_t need, size_t want)
     {
-        if (d_tw) cudaFree(d_tw);
-        if (d_tw_post) cudaFree(d_tw_post);
+        if (cap >= need) return cudaSuccess;
+        clear();
+        const cudaError_t e = b200aa_host::device_alloc(want, p);
+        if (e == cudaSuccess) cap = want;
+        return e;
     }
+    void *get() const { return p.get(); }
+    void clear() { p.reset(); cap = 0; }
 };
 
 struct b200aa_plan {
@@ -142,15 +191,11 @@ struct b200aa_plan {
     int fast_kind = 0;                  // 0 = none, else index of the specialised kernel
     int tables_status = B200AA_OK;      // B200AA_ERR_CHROMA / _MEL_RANGE when the reference cannot build its tables
     BlobLayout bl{};
-    int *d_blob = nullptr;
-    std::vector<int> h_blob;
-    std::mutex mu;
-    std::map<int, std::unique_ptr<Transform>> transforms;   // by transform length
-    // workspace of the host-buffer entry points: grow-only device buffers reused across calls (a cudaMalloc /
-    // cudaFree pair per call costs more than the kernels for a single clip); calls serialise on host_mu
+    b200aa_host::DeviceMemory blob;     // int [bl.words]
+    Transform transform;
+    // workspace of the host-buffer entry points; calls serialise on host_mu
     std::mutex host_mu;
-    void *ws[4] = {nullptr, nullptr, nullptr, nullptr};
-    size_t ws_cap[4] = {0, 0, 0, 0};
+    GrowBuffer ws[4];
     FastTables fast{};                  // extra device tables of the specialised kernel
     PairTables pair{};                  // inter-pass twiddles of the warp-autonomous pair kernel (windows 32 * R)
     SoloTables solo{};                  // tables of the warp-autonomous per-frame kernel (windows 882 / 400 / 600)
@@ -161,68 +206,20 @@ struct b200aa_plan {
     // the whole slot as its per-warp range descriptors (csrc/sched.cuh: 8 bytes per resident warp).
     static constexpr unsigned kSlots = 64;
     static constexpr size_t kSlotBytes = 64 * 1024;
-    unsigned char *d_counters = nullptr;
+    b200aa_host::DeviceMemory counters;
     cudaEvent_t slot_event[kSlots] = {};
     bool slot_used[kSlots] = {};
     unsigned next_slot = 0;
     std::mutex slot_mu;
     static constexpr int kPipe = 3;     // streams of the chunked host pipeline, each with its own clips / records / features buffers
     cudaStream_t pipe_stream[kPipe] = {nullptr, nullptr, nullptr};
-    void *pipe_ws[kPipe][3] = {};
-    size_t pipe_cap[kPipe][3] = {};
+    GrowBuffer pipe_ws[kPipe][3];
     ~b200aa_plan()
     {
-        if (d_blob) cudaFree(d_blob);
-        for (void *w : ws) if (w) cudaFree(w);
-        for (int k = 0; k < kPipe; ++k) {
-            if (pipe_stream[k]) cudaStreamDestroy(pipe_stream[k]);
-            for (void *w : pipe_ws[k]) if (w) cudaFree(w);
-        }
-        fast.release();
-        pair.release();
-        solo.release();
-        if (d_counters) cudaFree(d_counters);
+        for (cudaStream_t s : pipe_stream) if (s) cudaStreamDestroy(s);
         for (cudaEvent_t e : slot_event) if (e) cudaEventDestroy(e);
     }
 };
-
-static int make_transform(int n, std::unique_ptr<Transform> &out)
-{
-    std::unique_ptr<Transform> t(new Transform);
-    t->n = n;
-    t->packed = (n % 2 == 0) ? 1 : 0;
-    t->Nc = t->packed ? n / 2 : n;
-    t->radix = b200aa_host::radix_list(t->Nc);
-    if (t->Nc == 1) t->radix.clear();
-    if ((int)t->radix.size() > kMaxRadix) return B200AA_ERR_UNSUPPORTED;
-    std::vector<float2> tw(t->Nc), tp(t->Nc);
-    for (int j = 0; j < t->Nc; ++j) {
-        const double a = -2.0 * b200aa_host::kPi * double(j) / double(t->Nc);
-        tw[j] = make_float2(float(std::cos(a)), float(std::sin(a)));
-        const double b = -2.0 * b200aa_host::kPi * double(j) / double(n);
-        tp[j] = make_float2(float(std::cos(b)), float(std::sin(b)));
-    }
-    CK(cudaMalloc(&t->d_tw, sizeof(float2) * t->Nc));
-    CK(cudaMalloc(&t->d_tw_post, sizeof(float2) * t->Nc));
-    CK(cudaMemcpy(t->d_tw, tw.data(), sizeof(float2) * t->Nc, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(t->d_tw_post, tp.data(), sizeof(float2) * t->Nc, cudaMemcpyHostToDevice));
-    out = std::move(t);
-    return B200AA_OK;
-}
-
-static int get_transform(b200aa_plan *pl, int n, Transform **out)
-{
-    std::lock_guard<std::mutex> g(pl->mu);
-    auto it = pl->transforms.find(n);
-    if (it == pl->transforms.end()) {
-        std::unique_ptr<Transform> t;
-        int rc = make_transform(n, t);
-        if (rc != B200AA_OK) return rc;
-        it = pl->transforms.emplace(n, std::move(t)).first;
-    }
-    *out = it->second.get();
-    return B200AA_OK;
-}
 
 extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int step)
 {
@@ -235,13 +232,18 @@ extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int ste
     CK(cudaDeviceGetAttribute(&pl->sm_count, cudaDevAttrMultiProcessorCount, pl->device));
     // tables that only feature_extraction / chromagram need may be unbuildable (the reference raises
     // there too); spectrogram must still work, so remember the status instead of failing here.
-    pl->tables_status = b200aa_host::build_blob(fs, pl->K, pl->h_blob, pl->bl);
-    CK(cudaMalloc(&pl->d_blob, sizeof(int) * pl->h_blob.size()));
-    CK(cudaMemcpy(pl->d_blob, pl->h_blob.data(), sizeof(int) * pl->h_blob.size(), cudaMemcpyHostToDevice));
-    Transform *t = nullptr;
-    rc = get_transform(pl.get(), window, &t);
-    if (rc != B200AA_OK) return rc;
-    rc = fast_plan_init(fs, window, step, pl->h_blob, pl->bl, &pl->fast, &pl->fast_kind);
+    std::vector<int> h_blob;
+    pl->tables_status = b200aa_host::build_blob(fs, pl->K, h_blob, pl->bl);
+    CK(b200aa_host::upload(h_blob, pl->blob));
+    Transform &t = pl->transform;
+    t.packed = (window % 2 == 0) ? 1 : 0;
+    t.Nc = t.packed ? window / 2 : window;
+    t.radix = b200aa_host::radix_list(t.Nc);
+    if (t.Nc == 1) t.radix.clear();
+    if ((int)t.radix.size() > kMaxRadix) return B200AA_ERR_UNSUPPORTED;
+    CK(b200aa_host::upload(b200aa_host::twiddles(t.Nc, t.Nc), t.tw));
+    CK(b200aa_host::upload(b200aa_host::twiddles(t.Nc, window), t.tw_post));
+    rc = fast_plan_init(window, &pl->fast, &pl->fast_kind);
     if (rc != B200AA_OK) return rc;
     int sl_ = 0, sr_ = 0;
     if ((pair_r_for_window(window) || solo_shape_for_window(window, &sl_, &sr_)) && pl->tables_status == B200AA_OK) {
@@ -257,7 +259,7 @@ extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int ste
         rc = solo_plan_init(window, pblob, pbl, &pl->solo);
         if (rc != B200AA_OK) return cuda_fail(cudaGetLastError(), "solo_plan_init");
     }
-    CK(cudaMalloc(&pl->d_counters, b200aa_plan::kSlots * b200aa_plan::kSlotBytes));
+    CK(b200aa_host::device_alloc(b200aa_plan::kSlots * b200aa_plan::kSlotBytes, pl->counters));
     *out = pl.release();
     return B200AA_OK;
 }
@@ -271,7 +273,7 @@ static int slot_acquire(b200aa_plan *pl, cudaStream_t st, unsigned *slot, unsign
     if (!pl->slot_event[s]) CK(cudaEventCreateWithFlags(&pl->slot_event[s], cudaEventDisableTiming));
     if (pl->slot_used[s]) CK(cudaStreamWaitEvent(st, pl->slot_event[s], 0));
     *slot = s;
-    *ctr = reinterpret_cast<unsigned int *>(pl->d_counters + size_t(s) * b200aa_plan::kSlotBytes);
+    *ctr = reinterpret_cast<unsigned int *>(static_cast<unsigned char *>(pl->counters.get()) + size_t(s) * b200aa_plan::kSlotBytes);
     return B200AA_OK;
 }
 static int slot_done(b200aa_plan *pl, cudaStream_t st, unsigned slot)
@@ -281,6 +283,25 @@ static int slot_done(b200aa_plan *pl, cudaStream_t st, unsigned slot)
     pl->slot_used[slot] = true;
     return B200AA_OK;
 }
+
+// One launch of a persistent kernel: the constructor takes a work-counter slot (status in rc, counter in ctr), finish()
+// gets the launcher's status, counts the launch, maps the status and records the slot.  B200AA_ERR_UNSUPPORTED = the
+// launcher declined the shape and launched nothing; the caller tries the next kernel.
+struct SlotLaunch {
+    b200aa_plan *pl;
+    cudaStream_t st;
+    unsigned slot = 0;
+    unsigned int *ctr = nullptr;
+    int rc;
+    SlotLaunch(b200aa_plan *plan, cudaStream_t stream) : pl(plan), st(stream) { rc = slot_acquire(pl, st, &slot, &ctr); }
+    int finish(int launch_rc, const char *name)
+    {
+        const int r = launch_rc == B200AA_OK ? launched(name)
+                                             : (launch_rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), name) : launch_rc);
+        const int done = slot_done(pl, st, slot);     // after launched(): a failed record keeps its own message
+        return r != B200AA_OK ? r : done;
+    }
+};
 
 static bool use_pair(const b200aa_plan *pl) { return pl->pair.R && !pl->force_generic && (pl->prefer < 0 || pl->prefer == 2); }
 static bool use_solo(const b200aa_plan *pl) { return pl->solo.L && !pl->force_generic && (pl->prefer < 0 || pl->prefer == 3); }
@@ -315,15 +336,9 @@ extern "C" int b200aa_plan_trim(b200aa_plan *plan)
 {
     if (!plan) return B200AA_ERR_INVALID;
     std::lock_guard<std::mutex> g(plan->host_mu);
-    for (int i = 0; i < 4; ++i) {
-        if (plan->ws[i]) cudaFree(plan->ws[i]);
-        plan->ws[i] = nullptr; plan->ws_cap[i] = 0;
-    }
-    for (int k = 0; k < b200aa_plan::kPipe; ++k)
-        for (int j = 0; j < 3; ++j) {
-            if (plan->pipe_ws[k][j]) cudaFree(plan->pipe_ws[k][j]);
-            plan->pipe_ws[k][j] = nullptr; plan->pipe_cap[k][j] = 0;
-        }
+    for (GrowBuffer &w : plan->ws) w.clear();
+    for (auto &stream_ws : plan->pipe_ws)
+        for (GrowBuffer &w : stream_ws) w.clear();
     return B200AA_OK;
 }
 
@@ -665,7 +680,7 @@ __global__ void __launch_bounds__(256) frame_counts_kernel(const int64_t *len, i
 {
     const int64_t b = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
     if (b >= n_clips) return;
-    const int64_t T = frames_of(len[b], w, s);
+    const int64_t T = rows::frames(len[b], w, s);
     frames[b] = T;
     if (windows) windows[b] = windows_of(T, stepr);
 }
@@ -765,29 +780,24 @@ extern "C" int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const
     }
     if (n_clips == 0 || n_out == 0) return B200AA_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    b200aa_pcm_clip *d_clips = nullptr;
-    CK(cudaMallocAsync(reinterpret_cast<void **>(&d_clips), size_t(n_clips) * sizeof(b200aa_pcm_clip), st));
+    const size_t clip_bytes = size_t(n_clips) * sizeof(b200aa_pcm_clip);
     const int64_t tiles = (n_out + pcm::kTile - 1) / pcm::kTile;
     const int64_t items = n_clips * tiles;
     const unsigned grid = unsigned(std::min<int64_t>(items, int64_t(1) << 30));
-    int rc = B200AA_OK;
-    cudaError_t e = cudaMemcpyAsync(d_clips, h_clips, size_t(n_clips) * sizeof(b200aa_pcm_clip), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) {
-        rc = cuda_fail(e, "cudaMemcpyAsync");
-    } else {
-        const unsigned char *arena = static_cast<const unsigned char *>(d_arena);
-        if (out_dtype == B200AA_DTYPE_I16)
-            pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
-                                                               static_cast<int16_t *>(d_out));
-        else
-            pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
-                                                               static_cast<float *>(d_out));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if ((e = cudaGetLastError()) != cudaSuccess) rc = cuda_fail(e, "pcm::decode_kernel");
-    }
-    e = cudaFreeAsync(d_clips, st);
-    if (e != cudaSuccess && rc == B200AA_OK) rc = cuda_fail(e, "cudaFreeAsync");
-    return rc;
+    StreamScratch scratch(st);
+    int rc = scratch.alloc(clip_bytes);
+    if (rc != B200AA_OK) return rc;
+    const b200aa_pcm_clip *d_clips = static_cast<const b200aa_pcm_clip *>(scratch.get());
+    const cudaError_t e = cudaMemcpyAsync(scratch.get(), h_clips, clip_bytes, cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaMemcpyAsync");
+    const unsigned char *arena = static_cast<const unsigned char *>(d_arena);
+    if (out_dtype == B200AA_DTYPE_I16)
+        pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
+                                                           static_cast<int16_t *>(d_out));
+    else
+        pcm::decode_kernel<<<grid, pcm::kThreads, 0, st>>>(arena, d_clips, items, tiles, n_out, out_stride,
+                                                           static_cast<float *>(d_out));
+    return scratch.done(launched("pcm::decode_kernel"));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -922,47 +932,42 @@ extern "C" int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_
     const size_t per_clip = size_t(beat::kRows) * (size_t(nb) * sizeof(unsigned) + rec_bytes);
     const int64_t slice = std::max<int64_t>(1, std::min<int64_t>({n_clips, int64_t((size_t(256) << 20) / std::max<size_t>(per_clip, 1)),
                                                                    int64_t(INT32_MAX / beat::kRows)}));
-    char *scratch = nullptr;
-    if (per_clip) CK(cudaMallocAsync(reinterpret_cast<void **>(&scratch), size_t(slice) * per_clip, st));
-    unsigned *counts = reinterpret_cast<unsigned *>(scratch);
-    beat::Chunk *recs = reinterpret_cast<beat::Chunk *>(scratch + size_t(slice) * beat::kRows * nb * sizeof(unsigned));
-    int rc = B200AA_OK;
-    for (int64_t b0 = 0; b0 < n_clips && rc == B200AA_OK; b0 += slice) {
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(size_t(slice) * per_clip);
+    if (rc != B200AA_OK) return rc;
+    unsigned *counts = static_cast<unsigned *>(scratch.get());
+    beat::Chunk *recs = reinterpret_cast<beat::Chunk *>(static_cast<char *>(scratch.get()) + size_t(slice) * beat::kRows * nb * sizeof(unsigned));
+    for (int64_t b0 = 0; b0 < n_clips; b0 += slice) {
         const int64_t ns = std::min<int64_t>(slice, n_clips - b0);
-        cudaError_t e = nb ? cudaMemsetAsync(counts, 0, size_t(ns) * beat::kRows * nb * sizeof(unsigned), st) : cudaSuccess;
-        if (e != cudaSuccess) { rc = cuda_fail(e, "cudaMemsetAsync"); break; }
+        const cudaError_t e = nb ? cudaMemsetAsync(counts, 0, size_t(ns) * beat::kRows * nb * sizeof(unsigned), st) : cudaSuccess;
+        if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync");
         beat_rows_kernel<<<(unsigned)(ns * beat::kRows), P, 0, st>>>(d_st, n_feats, n_frames, t_stride, d_frames, b0, mbt, nb, chunk,
                                                                      nch_max, recs, counts);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if ((e = cudaGetLastError()) != cudaSuccess) { rc = cuda_fail(e, "beat_rows_kernel"); break; }
+        CK_LAUNCH("beat_rows_kernel");
         beat_finish_kernel<<<(unsigned)((ns * 32 + 255) / 256), 256, 0, st>>>(d_frames, n_frames, b0, ns, window_size, mbt, nb,
                                                                                counts, d_out);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if ((e = cudaGetLastError()) != cudaSuccess) { rc = cuda_fail(e, "beat_finish_kernel"); break; }
+        CK_LAUNCH("beat_finish_kernel");
     }
-    if (scratch) {
-        const cudaError_t e = cudaFreeAsync(scratch, st);
-        if (e != cudaSuccess && rc == B200AA_OK) rc = cuda_fail(e, "cudaFreeAsync");
-    }
-    return rc;
+    return scratch.done(B200AA_OK);
 }
 
 // ------------------------------------------------------------------------------------------------
 // kernel 1 launchers
 // ------------------------------------------------------------------------------------------------
-static void fill_common(StParams &p, const b200aa_plan *pl, const Transform *t, const void *d_sig, int dtype,
-                        int64_t n_clips, int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
-                        const b200aa_clip_norm *d_norm, float *d_out)
+static void fill_common(StParams &p, const b200aa_plan *pl, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                        int64_t clip_stride, const int64_t *d_len, const b200aa_clip_norm *d_norm, float *d_out)
 {
+    const Transform &t = pl->transform;
     std::memset(&p, 0, sizeof(p));
     p.sig = d_sig; p.len = d_len; p.norm = d_norm; p.out = d_out;
-    p.tw = t->d_tw; p.tw_post = t->d_tw_post; p.blob = pl->d_blob; p.bl = pl->bl;
+    p.tw = static_cast<const float2 *>(t.tw.get()); p.tw_post = static_cast<const float2 *>(t.tw_post.get());
+    p.blob = static_cast<const int *>(pl->blob.get()); p.bl = pl->bl;
     p.n_clips = n_clips; p.n_samples = n_samples; p.clip_stride = clip_stride;
-    p.dtype = dtype; p.window = pl->window; p.fft_n = t->n; p.step = pl->step; p.K = pl->K;
+    p.dtype = dtype; p.window = pl->window; p.fft_n = pl->window; p.step = pl->step; p.K = pl->K;
     p.Kp = (pl->K + 3) & ~3;
-    p.Nc = t->Nc; p.packed = t->packed;
-    p.nrad = (int)t->radix.size();
-    for (int i = 0; i < p.nrad; ++i) p.radix[i] = t->radix[i];
+    p.Nc = t.Nc; p.packed = t.packed;
+    p.nrad = (int)t.radix.size();
+    for (int i = 0; i < p.nrad; ++i) p.radix[i] = t.radix[i];
 }
 
 // choose frames/group and launch the generic kernel
@@ -997,24 +1002,19 @@ static int launch_generic(const b200aa_plan *pl, StParams &p, int64_t rows_max, 
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
         const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * 2);
         p.scratch_stride = generic_big_bytes(G, p.Nc, p.Kp);
-        void *scratch = nullptr;
-        CK(cudaMallocAsync(&scratch, p.scratch_stride * size_t(grid), st));      // stream-ordered: safe across concurrent launches
-        p.scratch = static_cast<unsigned char *>(scratch);
+        StreamScratch scratch(st);             // stream-ordered: safe across concurrent launches
+        const int rc = scratch.alloc(p.scratch_stride * size_t(grid));
+        if (rc != B200AA_OK) return rc;
+        p.scratch = static_cast<unsigned char *>(scratch.get());
         kern<<<(unsigned)grid, kThreads, smem, st>>>(p);
-        const cudaError_t e = cudaGetLastError();
-        cudaFreeAsync(scratch, st);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        if (e != cudaSuccess) return cuda_fail(e, "st_generic_kernel (large window)");
-        return B200AA_OK;
+        return scratch.done(launched("st_generic_kernel (large window)"));
     }
     auto kern = st_generic_kernel<MODE, false>;
     if constexpr (MODE != kModeFeatures) {
         if (p.len) kern = st_generic_kernel<MODE, false, true>;
     }
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));   // constant: no race between launching threads
     int occ = 1;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
-    occ = std::max(1, occ);
+    CK(resident_ctas(kern, kThreads, smem, 226 * 1024, occ));
     const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * occ);
     kern<<<(unsigned)grid, kThreads, smem, st>>>(p);
     CK_LAUNCH("st_generic_kernel");
@@ -1031,46 +1031,35 @@ extern "C" int b200aa_st_features(const b200aa_plan *plan, const void *d_sig, in
     b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
     // error order of the reference: mel bank (before the loop), no frames (:684), chroma (frame 0)
     if (pl->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
-    const int64_t T = b200aa_host::num_frames(n_samples, pl->window, pl->step);
+    const int64_t T = rows::frames(n_samples, pl->window, pl->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;
     int rc = pl->tables_status;
     if (rc != B200AA_OK) return rc;
     if ((rc = plan_device_check(pl)) != B200AA_OK) return rc;
     if (t_stride < T) return B200AA_ERR_INVALID;
     if (n_clips == 0) return B200AA_OK;
-    Transform *t = nullptr;
-    rc = get_transform(pl, pl->window, &t);
-    if (rc != B200AA_OK) return rc;
     StParams p;
-    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
+    fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     p.t_stride = t_stride; p.deltas = deltas ? 1 : 0; p.n_out = deltas ? 68 : 34; p.mode = kModeFeatures;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (use_pair(pl)) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = pair_launch_features(pl->pair, p, pl->sm_count, T, reinterpret_cast<unsigned long long *>(ctr), b200aa_plan::kSlotBytes, g_pair_dump, st);
-        const int rc2 = slot_done(pl, st, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "pair kernel") : rc;
+        SlotLaunch sl(pl, st);
+        if (sl.rc != B200AA_OK) return sl.rc;
+        rc = sl.finish(pair_launch_features(pl->pair, p, pl->sm_count, T, reinterpret_cast<unsigned long long *>(sl.ctr),
+                                            b200aa_plan::kSlotBytes, g_pair_dump, st), "pair kernel");
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     if (use_solo(pl)) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = solo_launch_mode<kModeFeatures>(pl->solo, p, pl->sm_count, T, ctr, b200aa_plan::kSlotBytes, st);
-        const int rc2 = slot_done(pl, st, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "solo kernel") : rc;
+        SlotLaunch sl(pl, st);
+        if (sl.rc != B200AA_OK) return sl.rc;
+        rc = sl.finish(solo_launch_mode<kModeFeatures>(pl->solo, p, pl->sm_count, T, sl.ctr, b200aa_plan::kSlotBytes, st), "solo kernel");
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     if (use_fast(pl)) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = fast_launch_features(pl->fast_kind, pl->fast, p, pl->sm_count, T, ctr, st);
-        const int rc2 = slot_done(pl, st, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "fast kernel") : rc;
+        SlotLaunch sl(pl, st);
+        if (sl.rc != B200AA_OK) return sl.rc;
+        rc = sl.finish(fast_launch_features(pl->fast_kind, pl->fast, p, pl->sm_count, T, sl.ctr, st), "fast kernel");
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     return launch_generic<kModeFeatures>(pl, p, T, st);
 }
@@ -1080,24 +1069,17 @@ extern "C" int b200aa_st_features(const b200aa_plan *plan, const void *d_sig, in
 template <int MODE>
 static int launch_rows(b200aa_plan *pl, StParams &p, cudaStream_t st)
 {
-    int rc = B200AA_OK;
     if (use_solo(pl)) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = solo_launch_mode<MODE>(pl->solo, p, pl->sm_count, p.rows_launch, ctr, b200aa_plan::kSlotBytes, st);
-        const int rc2 = slot_done(pl, st, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "solo kernel") : rc;
+        SlotLaunch sl(pl, st);
+        if (sl.rc != B200AA_OK) return sl.rc;
+        const int rc = sl.finish(solo_launch_mode<MODE>(pl->solo, p, pl->sm_count, p.rows_launch, sl.ctr, b200aa_plan::kSlotBytes, st), "solo kernel");
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     if (pl->fast_kind && !pl->force_generic && pl->prefer != 0 && pl->prefer != 3) {
-        unsigned slot = 0;
-        unsigned int *ctr = nullptr;
-        if ((rc = slot_acquire(pl, st, &slot, &ctr)) != B200AA_OK) return rc;
-        rc = fast_launch_rows(pl->fast_kind, MODE, pl->fast, p, pl->sm_count, ctr, st);
-        const int rc2 = slot_done(pl, st, slot);
-        if (rc == B200AA_OK) { g_launches.fetch_add(1, std::memory_order_relaxed); return rc2; }
-        if (rc != B200AA_ERR_UNSUPPORTED) return rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), "fast kernel") : rc;
+        SlotLaunch sl(pl, st);
+        if (sl.rc != B200AA_OK) return sl.rc;
+        const int rc = sl.finish(fast_launch_rows(pl->fast_kind, MODE, pl->fast, p, pl->sm_count, sl.ctr, st), "fast kernel");
+        if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     return launch_generic<MODE>(pl, p, p.rows_launch, st);
 }
@@ -1118,15 +1100,12 @@ static int launch_clipped(const b200aa_plan *pl, StParams p, int64_t per_clip, c
     // large windows: the arrays of every resident CTA in stream-ordered scratch, CTAs loop over the items
     const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * 2);
     p.scratch_stride = (bytes + 255) & ~size_t(255);
-    void *scratch = nullptr;
-    CK(cudaMallocAsync(&scratch, p.scratch_stride * size_t(grid), st));
-    p.scratch = static_cast<unsigned char *>(scratch);
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(p.scratch_stride * size_t(grid));
+    if (rc != B200AA_OK) return rc;
+    p.scratch = static_cast<unsigned char *>(scratch.get());
     clipped_chroma_kernel<true><<<(unsigned)grid, kThreads, 0, st>>>(p, per_clip);
-    const cudaError_t e = cudaGetLastError();
-    cudaFreeAsync(scratch, st);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    if (e != cudaSuccess) return cuda_fail(e, "clipped_chroma_kernel (large window)");
-    return B200AA_OK;
+    return scratch.done(launched("clipped_chroma_kernel (large window)"));
 }
 
 // b200aa_spectrogram and b200aa_spectrogram_ragged (d_len set): the launch is sized by n_samples
@@ -1140,13 +1119,10 @@ static int spectrogram_launch(const b200aa_plan *plan, const void *d_sig, int dt
     const rows::Rows r = rows::spectrogram(n_samples, pl->window, pl->step);
     if (r.refused) return B200AA_ERR_TOO_SHORT;     // np.zeros with a non-positive row count / empty result
     if (n_clips == 0) return B200AA_OK;
-    int rc = plan_device_check(pl);
-    if (rc != B200AA_OK) return rc;
-    Transform *t = nullptr;
-    rc = get_transform(pl, pl->window, &t);
+    const int rc = plan_device_check(pl);
     if (rc != B200AA_OK) return rc;
     StParams p;
-    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
+    fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     p.mode = kModeSpectrogram;
     p.origin = pl->window; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
     return launch_rows<kModeSpectrogram>(pl, p, static_cast<cudaStream_t>(stream));
@@ -1188,11 +1164,8 @@ static int chromagram_launch(const b200aa_plan *plan, const void *d_sig, int dty
     if (!d_len && r.refused) return B200AA_ERR_INVALID;     // a clipped frame shorter than K: the reference's scatter raises
     if ((rc = plan_device_check(pl)) != B200AA_OK) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    Transform *t = nullptr;
-    rc = get_transform(pl, w, &t);
-    if (rc != B200AA_OK) return rc;
     StParams p;
-    fill_common(p, pl, t, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
+    fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     p.mode = kModeChromagram;
     p.origin = w; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
     rc = launch_rows<kModeChromagram>(pl, p, st);
@@ -1221,18 +1194,11 @@ extern "C" int b200aa_chromagram_ragged(const b200aa_plan *plan, const void *d_s
 // ------------------------------------------------------------------------------------------------
 // host-buffer entry points
 // ------------------------------------------------------------------------------------------------
-// slot `slot` of the plan's workspace, grown to at least n bytes (caller holds host_mu); nullptr = cudaMalloc failed
+// slot `slot` of the plan's workspace, grown to at least n bytes, with room to spare (caller holds host_mu);
+// nullptr = cudaMalloc failed
 static void *workspace(b200aa_plan *pl, int slot, size_t n)
 {
-    if (pl->ws_cap[slot] < n) {
-        if (pl->ws[slot]) cudaFree(pl->ws[slot]);
-        pl->ws[slot] = nullptr;
-        pl->ws_cap[slot] = 0;
-        const size_t want = n + n / 4 + 4096;
-        if (cudaMalloc(&pl->ws[slot], want) != cudaSuccess) return nullptr;
-        pl->ws_cap[slot] = want;
-    }
-    return pl->ws[slot];
+    return pl->ws[slot].reserve(n, n + n / 4 + 4096) == cudaSuccess ? pl->ws[slot].get() : nullptr;
 }
 
 // One host-buffer call: takes the plan's workspace lock, uploads the clips (slot 0) and produces their normalisation
@@ -1283,23 +1249,16 @@ static int st_features_host_pipelined(b200aa_plan *pl, const void *h_sig, int dt
     const size_t need[3] = {size_t(chunk) * n_samples * es, sizeof(b200aa_clip_norm) * size_t(chunk), size_t(chunk) * F * T * 4};
     for (int k = 0; k < b200aa_plan::kPipe; ++k) {
         if (!pl->pipe_stream[k]) CK(cudaStreamCreateWithFlags(&pl->pipe_stream[k], cudaStreamNonBlocking));
-        for (int j = 0; j < 3; ++j)
-            if (pl->pipe_cap[k][j] < need[j]) {
-                if (pl->pipe_ws[k][j]) cudaFree(pl->pipe_ws[k][j]);
-                pl->pipe_ws[k][j] = nullptr;
-                pl->pipe_cap[k][j] = 0;
-                CK(cudaMalloc(&pl->pipe_ws[k][j], need[j]));
-                pl->pipe_cap[k][j] = need[j];
-            }
+        for (int j = 0; j < 3; ++j) CK(pl->pipe_ws[k][j].reserve(need[j], need[j]));
     }
     int64_t c = 0;
     for (int64_t a = 0; a < n_clips && rc == B200AA_OK; a += chunk, ++c) {
         const int k = int(c % b200aa_plan::kPipe);
         const int64_t n = std::min<int64_t>(chunk, n_clips - a);
         cudaStream_t st = pl->pipe_stream[k];      // stream order also protects the buffers: chunk c + kPipe waits for chunk c
-        void *sig = pl->pipe_ws[k][0];
-        b200aa_clip_norm *norm = static_cast<b200aa_clip_norm *>(pl->pipe_ws[k][1]);
-        float *out = static_cast<float *>(pl->pipe_ws[k][2]);
+        void *sig = pl->pipe_ws[k][0].get();
+        b200aa_clip_norm *norm = static_cast<b200aa_clip_norm *>(pl->pipe_ws[k][1].get());
+        float *out = static_cast<float *>(pl->pipe_ws[k][2].get());
         cudaError_t e = cudaMemcpyAsync(sig, static_cast<const char *>(h_sig) + size_t(a) * n_samples * es, size_t(n) * n_samples * es,
                                         cudaMemcpyHostToDevice, st);
         if (e != cudaSuccess) { rc = cuda_fail(e, "cudaMemcpyAsync (clips)"); break; }
@@ -1323,7 +1282,7 @@ extern "C" int b200aa_st_features_host(const b200aa_plan *plan, const void *h_si
     NvtxRange nvtx_("b200aa_st_features_host");
     if (!plan || !h_sig || !h_out || n_clips < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
     if (plan->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
-    const int64_t T = b200aa_host::num_frames(n_samples, plan->window, plan->step);
+    const int64_t T = rows::frames(n_samples, plan->window, plan->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;
     if (plan->tables_status != B200AA_OK) return plan->tables_status;
     {   // chunks of ~32 MB of samples; batches of fewer than two chunks take the single-stream path below
@@ -1384,7 +1343,7 @@ extern "C" int b200aa_mid_features_host(const b200aa_plan *plan, const void *h_s
     NvtxRange nvtx_("b200aa_mid_features_host");
     if (!plan || !h_sig || !h_mid || step_ratio < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
     if (plan->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
-    const int64_t T = b200aa_host::num_frames(n_samples, plan->window, plan->step);
+    const int64_t T = rows::frames(n_samples, plan->window, plan->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;
     if (plan->tables_status != B200AA_OK) return plan->tables_status;
     const int64_t M = b200aa_mid_windows(T, step_ratio);

@@ -16,6 +16,8 @@
 #include <vector>
 #include "common.cuh"
 #include "dft_codelets.cuh"
+#include "sched.cuh"
+#include "tables.inl"
 
 namespace b200aa {
 
@@ -473,15 +475,9 @@ __device__ __forceinline__ void stage_run_smem(const short *raw8, bool has_pred,
 // kernel
 // ----------------------------------------------------------------------------------------------
 struct FastTables {
-    float2 *d_tw = nullptr;      // [R][R]   W_Nc^(k1*n2) stored [k1][n2]
-    float2 *d_twp = nullptr;     // [Nc/2+1] W_N^k
+    b200aa_host::DeviceMemory tw;      // float2 [R][R]   W_Nc^(k1*n2) stored [k1][n2]
+    b200aa_host::DeviceMemory twp;     // float2 [Nc/2+1] W_N^k
     int R = 0;
-    void release()
-    {
-        if (d_tw) cudaFree(d_tw);
-        if (d_twp) cudaFree(d_twp);
-        d_tw = d_twp = nullptr;
-    }
 };
 
 
@@ -879,29 +875,15 @@ inline bool fast_shape_for_window(int window, int *r1, int *r2)
     }
 }
 
-inline int fast_plan_init(int fs, int window, int step, const std::vector<int> &blob, const BlobLayout &bl,
-                          FastTables *ft, int *kind)
+inline int fast_plan_init(int window, FastTables *ft, int *kind)
 {
-    (void)fs; (void)step; (void)blob; (void)bl;
     *kind = 0;
     int R1 = 0, R2 = 0;
     if (!fast_shape_for_window(window, &R1, &R2)) return B200AA_OK;
     const int Nc = R1 * R2, N = 2 * Nc;
-    const double pi = 3.14159265358979323846264338327950288;
-    std::vector<float2> tw(size_t(R1) * R2), twp(Nc / 2 + 1);
-    for (int k1 = 0; k1 < R1; ++k1)
-        for (int n2 = 0; n2 < R2; ++n2) {
-            const double a = -2.0 * pi * double((k1 * n2) % Nc) / double(Nc);
-            tw[size_t(k1) * R2 + n2] = make_float2(float(std::cos(a)), float(std::sin(a)));
-        }
-    for (int k = 0; k <= Nc / 2; ++k) {
-        const double a = -2.0 * pi * double(k) / double(N);
-        twp[k] = make_float2(float(std::cos(a)), float(std::sin(a)));
-    }
-    if (cudaMalloc(&ft->d_tw, tw.size() * sizeof(float2)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMalloc(&ft->d_twp, twp.size() * sizeof(float2)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(ft->d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(ft->d_twp, twp.data(), twp.size() * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
+    if (b200aa_host::upload(b200aa_host::twiddle_grid(R1, R2, Nc), ft->tw) != cudaSuccess ||
+        b200aa_host::upload(b200aa_host::twiddles(Nc / 2 + 1, N), ft->twp) != cudaSuccess)
+        return B200AA_ERR_CUDA;
     ft->R = R1 * 100 + R2;
     *kind = ft->R;
     return B200AA_OK;
@@ -918,11 +900,8 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
     if constexpr (MODE != kModeFeatures) {
         if (p.len) kern = st_fast_kernel<R1, R2, G, EVEN, RUNS, MODE, true>;
     }
-    // always the same value (the launcher's cap), so concurrent launches of one instantiation cannot undercut each other
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024) != cudaSuccess) return B200AA_ERR_CUDA;
     int occ = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, NT, smem) != cudaSuccess) return B200AA_ERR_CUDA;
-    occ = occ < 1 ? 1 : occ;
+    if (resident_ctas(kern, NT, smem, 110 * 1024, occ) != cudaSuccess) return B200AA_ERR_CUDA;
     const int64_t slots = int64_t(sm_count) * occ;
     // work items: >= ~8 per CTA slot for balance, as long as possible to amortise the 2-frame halo, and
     // seg + 2 a multiple of the 8-frame CTA step so no step runs half empty
@@ -945,7 +924,7 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
         fprintf(stderr, "[b200aa] fast kernel %dx%d G=%d runs=%d mode=%d: smem %zu B, %d CTAs/SM, grid %lld, %lld items of %lld frames\n",
                 R1, R2, G, int(RUNS), MODE, smem, occ, (long long)grid, (long long)p.n_items, (long long)seg);
     if (cudaMemsetAsync(ctr, 0, sizeof(unsigned int), st) != cudaSuccess) return B200AA_ERR_CUDA;
-    kern<<<(unsigned)grid, NT, smem, st>>>(p, ft.d_tw, ft.d_twp, ctr);
+    kern<<<(unsigned)grid, NT, smem, st>>>(p, static_cast<const float2 *>(ft.tw.get()), static_cast<const float2 *>(ft.twp.get()), ctr);
     return cudaPeekAtLastError() == cudaSuccess ? B200AA_OK : B200AA_ERR_CUDA;    // the caller fetches (and clears) the text
 }
 

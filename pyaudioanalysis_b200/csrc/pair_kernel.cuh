@@ -929,16 +929,10 @@ inline int pair_r_for_window(int window)
 }
 
 struct PairTables {
-    float2 *d_tw = nullptr;
-    int *d_pblob = nullptr;
+    b200aa_host::DeviceMemory tw;      // float2 [R][32]
+    b200aa_host::DeviceMemory pblob;   // int [pbl.words]
     PairBlobLayout pbl{};
     int R = 0;
-    void release()
-    {
-        if (d_tw) cudaFree(d_tw);
-        if (d_pblob) cudaFree(d_pblob);
-        d_tw = nullptr; d_pblob = nullptr;
-    }
 };
 
 // Pair-kernel tables from the dense host tables (mel [40 x K], chroma [12 x K], dct [13 x 40], all float64):
@@ -1026,18 +1020,9 @@ inline int pair_plan_init(int window, const std::vector<int> &h_pblob, const Pai
     pt->R = 0;
     if (!R) return B200AA_OK;
     if (getenv("B200AA_NO_PAIR")) return B200AA_OK;
-    const int N = 32 * R;
-    const double pi = 3.14159265358979323846264338327950288;
-    std::vector<float2> tw(size_t(R) * 32);
-    for (int k1 = 0; k1 < R; ++k1)
-        for (int n2 = 0; n2 < 32; ++n2) {
-            const double a = -2.0 * pi * double((k1 * n2) % N) / double(N);
-            tw[size_t(k1) * 32 + n2] = make_float2(float(std::cos(a)), float(std::sin(a)));
-        }
-    if (cudaMalloc(&pt->d_tw, tw.size() * sizeof(float2)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(pt->d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMalloc(&pt->d_pblob, h_pblob.size() * sizeof(int)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(pt->d_pblob, h_pblob.data(), h_pblob.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
+    if (b200aa_host::upload(b200aa_host::twiddle_grid(R, 32, 32 * R), pt->tw) != cudaSuccess ||
+        b200aa_host::upload(h_pblob, pt->pblob) != cudaSuccess)
+        return B200AA_ERR_CUDA;
     pt->pbl = pbl;
     pt->R = R;
     return B200AA_OK;
@@ -1051,44 +1036,27 @@ inline int pair_launch_t(const PairTables &pt, const StParams &p, int sm_count, 
     const size_t smem = pair_smem_bytes<R>(pt.pbl.words);
     if (smem > size_t(kPairCtaCap)) return B200AA_ERR_UNSUPPORTED;
     auto kern = st_pair_kernel<R, SHARED>;
-    // always the cap, so concurrent launches of one instantiation cannot undercut each other
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kPairCtaCap) != cudaSuccess) return B200AA_ERR_CUDA;
+    constexpr int kPairWarps = pair_warps<R>();
     int occ = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32 * pair_warps<R>(), smem) != cudaSuccess) return B200AA_ERR_CUDA;
-    occ = occ < 1 ? 1 : occ;
+    if (resident_ctas(kern, 32 * kPairWarps, smem, kPairCtaCap, occ) != cudaSuccess) return B200AA_ERR_CUDA;
     PairParams pp;
     pp.st = p;
-    pp.tw = pt.d_tw;
-    pp.pblob = pt.d_pblob;
+    pp.tw = static_cast<const float2 *>(pt.tw.get());
+    pp.pblob = static_cast<const int *>(pt.pblob.get());
     pp.pbl = pt.pbl;
     pp.dbg = dbg;
     const int64_t NP = (T + 1) / 2;                                  // pairs per (full-length) clip
-    constexpr int kPairWarps = pair_warps<R>();
     const int64_t total = NP * p.n_clips;
     if (total <= 0) return B200AA_OK;                                // no clip has a frame
-    if (total >= (int64_t(1) << 31)) return B200AA_ERR_UNSUPPORTED;
     if ((2 * NP - 1) * p.step + 32 * R > INT32_MAX) return B200AA_ERR_UNSUPPORTED;   // sample offsets in a clip: 32 bits
-    // every resident warp gets an equal contiguous share (sched.cuh); small launches use as many warps as they have pairs
+    // every resident warp gets an equal contiguous share (sched.cuh)
     int64_t grid = int64_t(sm_count) * occ;
-    if (grid * kPairWarps > total) grid = (total + kPairWarps - 1) / kPairWarps;
-    const int64_t n_warps = grid * kPairWarps;
-    if (size_t(n_warps) * sizeof(unsigned long long) > ranges_cap) return B200AA_ERR_UNSUPPORTED;
-    long chunk = 8, min_steal = 2;
-    if (const char *ov = getenv("B200AA_PAIR_STEAL")) {              // tuning override: "chunk,min_steal"
-        long a = 0, b2 = 0;
-        if (sscanf(ov, "%ld,%ld", &a, &b2) == 2 && a > 0 && a <= 65536 && b2 > 1 && b2 <= 65536) { chunk = a; min_steal = b2; }
-    }
-    pp.sched.ranges = ranges;
-    pp.sched.n_warps = unsigned(n_warps);
-    pp.sched.total = unsigned(total);
-    pp.sched.per_clip = unsigned(NP);
-    pp.sched.chunk = unsigned(chunk);
-    pp.sched.min_steal = unsigned(min_steal);
+    const int rc = steal_setup(pp.sched, ranges, ranges_cap, total, NP, kPairWarps, grid, st);
+    if (rc != B200AA_OK) return rc;
     pp.st.n_items = total;
     if (getenv("B200AA_DEBUG"))
-        fprintf(stderr, "[b200aa] pair kernel R=%d shared=%d: smem %zu B, %d CTAs/SM x %d warps, grid %lld, %lld pairs (%lld per clip), chunk %ld, min steal %ld\n",
-                R, int(SHARED), smem, occ, kPairWarps, (long long)grid, (long long)total, (long long)NP, chunk, min_steal);
-    if (cudaMemsetAsync(ranges, 0, size_t(n_warps) * sizeof(unsigned long long), st) != cudaSuccess) return B200AA_ERR_CUDA;
+        fprintf(stderr, "[b200aa] pair kernel R=%d shared=%d: smem %zu B, %d CTAs/SM x %d warps, grid %lld, %lld pairs (%lld per clip), chunk %u, min steal %u\n",
+                R, int(SHARED), smem, occ, kPairWarps, (long long)grid, (long long)total, (long long)NP, pp.sched.chunk, pp.sched.min_steal);
     kern<<<(unsigned)grid, 32 * kPairWarps, smem, st>>>(pp);
     return cudaPeekAtLastError() == cudaSuccess ? B200AA_OK : B200AA_ERR_CUDA;
 }

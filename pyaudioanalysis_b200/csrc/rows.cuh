@@ -1,5 +1,5 @@
-// Row arithmetic of spectrogram() and chromagram() for one clip of n samples (reference ShortTermFeatures.py:413-415 and
-// :347-355): how many rows the output has, which of them the reference's loop fills from full frames or from a frame
+// Frame and row arithmetic of feature_extraction(), spectrogram() and chromagram() for one clip of n samples (reference
+// ShortTermFeatures.py:608, :413-415 and :347-355): how many frames, how many rows the output has, which of them the reference's loop fills from full frames or from a frame
 // clipped at the end of the clip, and whether the single-clip entry points refuse the clip.  The host entry points, the
 // row kernels of a ragged batch, the clipped-frame kernel and b200aa_row_counts all use these, so the rule lives in one
 // place.  __host__ __device__: tests/rows_host.cu runs the same code on the CPU.
@@ -20,6 +20,9 @@ __host__ __device__ inline int64_t min64(int64_t a, int64_t b) { return a < b ? 
 
 // len(range(a, b, s)) for s > 0
 __host__ __device__ inline int64_t range_len(int64_t a, int64_t b, int64_t s) { return b > a ? (b - a + s - 1) / s : 0; }
+
+// frames of feature_extraction's loop (:608): b200aa_num_frames, and the per-clip count of a ragged batch on the device
+__host__ __device__ inline int64_t frames(int64_t n, int w, int s) { return n < w ? 0 : (n - w) / s + 1; }
 
 // first sample of row i: both loops start at cur_p = w (:415, :349)
 __host__ __device__ inline int64_t frame_start(int w, int s, int64_t i) { return int64_t(w) + i * s; }

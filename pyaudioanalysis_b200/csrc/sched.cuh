@@ -12,12 +12,16 @@
 // nobody steals from a warp that has not started -- all CTAs of these launches are resident, so that lasts microseconds); every
 // transition is a single atomic on that word: the owner's claim is an atomicAdd on the front half, a steal is a
 // compare-and-swap that lowers the back half (it fails, harmlessly, if the owner moved in between), and a thief publishes
-// what it took with an atomicExch on its own word.  The functions are host + device so that tests/sched_host.cu can run
-// them with one CPU thread per "warp" (tests/test_sched_cpu.py).
+// what it took with an atomicExch on its own word.  The functions are host + device so that tests/sched_host.cpp can run
+// them with one CPU thread per "warp" (tests/test_sched_cpu.py).  The nvcc-only part below also holds the host side of a
+// launch that the persistent kernels' launchers share: the steal-schedule setup and the resident-CTA count.
 #pragma once
 #include <cstdint>
 #if defined(__CUDACC__)
 #include <cuda_runtime.h>
+#include <cstdio>
+#include <cstdlib>
+#include "../../include/b200aa.h"
 #define B200AA_HD __host__ __device__ __forceinline__
 #else
 #define B200AA_HD inline
@@ -190,6 +194,45 @@ __device__ __forceinline__ int sched_next(const StealParams &sp, unsigned w, int
     }
     inc = 1u;                           // a stolen range starts with a single pair (it is small near the end of a launch)
     return sched_steal(sp, w, lane) ? 2 : 0;
+}
+
+// ---- host side of a launch
+// Steal schedule of one launch of `total` pair steps (per_clip per clip) in CTAs of `warps` warps: small launches shrink
+// `grid` to as many warps as they have pairs, every warp gets a range descriptor in `ranges` (ranges_cap bytes), zeroed
+// in-stream.  B200AA_PAIR_STEAL="chunk,min_steal" overrides the claim size and the smallest remainder worth splitting
+// (tuning).  B200AA_ERR_UNSUPPORTED: the launch does not fit 32-bit steps or the descriptors do not fit `ranges`.
+inline int steal_setup(StealParams &sp, unsigned long long *ranges, size_t ranges_cap, int64_t total, int64_t per_clip,
+                       int warps, int64_t &grid, cudaStream_t st)
+{
+    if (total >= (int64_t(1) << 31)) return B200AA_ERR_UNSUPPORTED;
+    if (grid * warps > total) grid = (total + warps - 1) / warps;
+    const int64_t n_warps = grid * warps;
+    if (size_t(n_warps) * sizeof(unsigned long long) > ranges_cap) return B200AA_ERR_UNSUPPORTED;
+    long chunk = 8, min_steal = 2;
+    if (const char *ov = getenv("B200AA_PAIR_STEAL")) {
+        long a = 0, b2 = 0;
+        if (sscanf(ov, "%ld,%ld", &a, &b2) == 2 && a > 0 && a <= 65536 && b2 > 1 && b2 <= 65536) { chunk = a; min_steal = b2; }
+    }
+    sp.ranges = ranges;
+    sp.n_warps = unsigned(n_warps);
+    sp.total = unsigned(total);
+    sp.per_clip = unsigned(per_clip);
+    sp.chunk = unsigned(chunk);
+    sp.min_steal = unsigned(min_steal);
+    if (cudaMemsetAsync(ranges, 0, size_t(n_warps) * sizeof(unsigned long long), st) != cudaSuccess) return B200AA_ERR_CUDA;
+    return B200AA_OK;
+}
+
+// Resident CTAs per SM of `kern` at `threads` threads and `smem` dynamic shared bytes, at least 1.  The kernel's shared-memory
+// cap is always set to the launcher's constant `cap`, so concurrent launches of one instantiation cannot undercut each other.
+template <class Kernel>
+inline cudaError_t resident_ctas(Kernel kern, int threads, size_t smem, int cap, int &occ)
+{
+    occ = 1;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cap);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
+    if (occ < 1) occ = 1;
+    return e;
 }
 #endif
 

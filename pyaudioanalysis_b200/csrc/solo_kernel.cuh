@@ -495,17 +495,10 @@ inline bool solo_shape_for_window(int window, int *l, int *r2)
 }
 
 struct SoloTables {
-    float2 *d_tw = nullptr, *d_twp = nullptr;
-    int *d_pblob = nullptr;
+    b200aa_host::DeviceMemory tw, twp;  // float2 [R2][L], [Nc/2+1]
+    b200aa_host::DeviceMemory pblob;    // int [pbl.words]
     PairBlobLayout pbl{};
     int L = 0, R2 = 0;
-    void release()
-    {
-        if (d_tw) cudaFree(d_tw);
-        if (d_twp) cudaFree(d_twp);
-        if (d_pblob) cudaFree(d_pblob);
-        d_tw = d_twp = nullptr; d_pblob = nullptr;
-    }
 };
 
 inline int solo_plan_init(int window, const std::vector<int> &h_pblob, const PairBlobLayout &pbl, SoloTables *stb)
@@ -515,23 +508,10 @@ inline int solo_plan_init(int window, const std::vector<int> &h_pblob, const Pai
     if (!solo_shape_for_window(window, &L, &R2)) return B200AA_OK;
     if (getenv("B200AA_NO_SOLO")) return B200AA_OK;
     const int Nc = L * R2, N = 2 * Nc;
-    const double pi = 3.14159265358979323846264338327950288;
-    std::vector<float2> tw(size_t(R2) * L), twp(Nc / 2 + 1);
-    for (int k1 = 0; k1 < R2; ++k1)
-        for (int n2 = 0; n2 < L; ++n2) {
-            const double a = -2.0 * pi * double((k1 * n2) % Nc) / double(Nc);
-            tw[size_t(k1) * L + n2] = make_float2(float(std::cos(a)), float(std::sin(a)));
-        }
-    for (int k = 0; k <= Nc / 2; ++k) {
-        const double a = -2.0 * pi * double(k) / double(N);
-        twp[k] = make_float2(float(std::cos(a)), float(std::sin(a)));
-    }
-    if (cudaMalloc(&stb->d_tw, tw.size() * sizeof(float2)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMalloc(&stb->d_twp, twp.size() * sizeof(float2)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(stb->d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(stb->d_twp, twp.data(), twp.size() * sizeof(float2), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMalloc(&stb->d_pblob, h_pblob.size() * sizeof(int)) != cudaSuccess) return B200AA_ERR_CUDA;
-    if (cudaMemcpy(stb->d_pblob, h_pblob.data(), h_pblob.size() * sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) return B200AA_ERR_CUDA;
+    if (b200aa_host::upload(b200aa_host::twiddle_grid(R2, L, Nc), stb->tw) != cudaSuccess ||
+        b200aa_host::upload(b200aa_host::twiddles(Nc / 2 + 1, N), stb->twp) != cudaSuccess ||
+        b200aa_host::upload(h_pblob, stb->pblob) != cudaSuccess)
+        return B200AA_ERR_CUDA;
     stb->pbl = pbl;
     stb->L = L; stb->R2 = R2;
     return B200AA_OK;
@@ -549,15 +529,13 @@ inline int solo_launch_t(const SoloTables &stb, const StParams &p, int sm_count,
     if constexpr (MODE != kModeFeatures) {
         if (p.len) kern = st_solo_kernel<L, R2, MODE, true>;
     }
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) return B200AA_ERR_CUDA;
-    int occ = 1;
     constexpr int W = solo_warps<L, R2, MODE>();
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32 * W, smem) != cudaSuccess) return B200AA_ERR_CUDA;
-    occ = occ < 1 ? 1 : occ;
+    int occ = 1;
+    if (resident_ctas(kern, 32 * W, smem, cap, occ) != cudaSuccess) return B200AA_ERR_CUDA;
     SoloParams pp;
     pp.st = p;
-    pp.tw = stb.d_tw; pp.twp = stb.d_twp;
-    pp.pblob = stb.d_pblob; pp.pbl = stb.pbl;
+    pp.tw = static_cast<const float2 *>(stb.tw.get()); pp.twp = static_cast<const float2 *>(stb.twp.get());
+    pp.pblob = static_cast<const int *>(stb.pblob.get()); pp.pbl = stb.pbl;
     pp.counter = counter;
     const int64_t NP = (T + 1) / 2;
     const int64_t slots = int64_t(sm_count) * occ * W;
@@ -566,27 +544,13 @@ inline int solo_launch_t(const SoloTables &stb, const StParams &p, int sm_count,
     if (MODE == kModeFeatures) {
         // static shares + steal-half (sched.cuh): the slot is the per-warp range table
         if (total <= 0) return B200AA_OK;
-        if (total >= (int64_t(1) << 31)) return B200AA_ERR_UNSUPPORTED;
-        if (grid * W > total) grid = (total + W - 1) / W;
-        const int64_t n_warps = grid * W;
-        if (size_t(n_warps) * sizeof(unsigned long long) > counter_cap) return B200AA_ERR_UNSUPPORTED;
-        long chunk = 8, min_steal = 2;
-        if (const char *ov = getenv("B200AA_PAIR_STEAL")) {
-            long a = 0, b2 = 0;
-            if (sscanf(ov, "%ld,%ld", &a, &b2) == 2 && a > 0 && a <= 65536 && b2 > 1 && b2 <= 65536) { chunk = a; min_steal = b2; }
-        }
-        pp.sched.ranges = reinterpret_cast<unsigned long long *>(counter);
-        pp.sched.n_warps = unsigned(n_warps);
-        pp.sched.total = unsigned(total);
-        pp.sched.per_clip = unsigned(NP);
-        pp.sched.chunk = unsigned(chunk);
-        pp.sched.min_steal = unsigned(min_steal);
+        const int rc = steal_setup(pp.sched, reinterpret_cast<unsigned long long *>(counter), counter_cap, total, NP, W, grid, st);
+        if (rc != B200AA_OK) return rc;
         pp.seg_big = pp.n_big = pp.seg_small = pp.segs_per_clip = 0;
         pp.st.n_items = total;
         if (getenv("B200AA_DEBUG"))
             fprintf(stderr, "[b200aa] solo kernel %dx%d features: smem %zu B, %d CTAs/SM x %d warps, grid %lld, %lld pairs\n", L, R2, smem, occ, W,
                     (long long)grid, (long long)total);
-        if (cudaMemsetAsync(counter, 0, size_t(n_warps) * sizeof(unsigned long long), st) != cudaSuccess) return B200AA_ERR_CUDA;
         kern<<<(unsigned)grid, 32 * W, smem, st>>>(pp);
         return cudaPeekAtLastError() == cudaSuccess ? B200AA_OK : B200AA_ERR_CUDA;
     }
