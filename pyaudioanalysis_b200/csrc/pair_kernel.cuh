@@ -87,7 +87,9 @@ struct alignas(16) PairWarpMem {
 };
 
 // warps per CTA such that kPairMinBlocks CTAs fit the 227 KB of an SM (per CTA: kPairCtaCap of pair_launch_t, twiddles, lane
-// constants, up to 6.5 KB of mel / DCT / chroma tables)
+// constants, 6.5 KB set aside for the mel / DCT / chroma tables).  The tables outgrow that below ~12 kHz (8.7 KB at 6 854 Hz,
+// window 1024, where the mel filters are longest) and still fit: the warp count is rounded down to whole rounds of four,
+// and with the largest blob every window keeps at least 18 KB of the cap free (tests/test_rates_cpu.py)
 constexpr int kPairCtaCap = (kPairMinBlocks == 1 ? 227 : (kPairMinBlocks == 2 ? 113 : 228 / kPairMinBlocks - 1)) * 1024;
 template <int R>
 __host__ __device__ constexpr int pair_warps()

@@ -28,14 +28,15 @@ __host__ __device__ inline int64_t frames(int64_t n, int w, int s) { return n < 
 __host__ __device__ inline int64_t frame_start(int w, int s, int64_t i) { return int64_t(w) + i * s; }
 
 // C division truncates toward zero like Python's int(x / y) on the reference's float quotient.  Every frame of the
-// spectrogram's loop is full (range(w, n - w + 1, s)).  R <= 0 makes np.zeros raise.
+// spectrogram's loop is full (range(w, n - w + 1, s)).  R <= 0 makes np.zeros raise; so does the normalisation of an
+// empty clip (the max of no samples), which matters where s > w: there int(-w / s) + 1 = 1 row at n = 0.
 __host__ __device__ inline Rows spectrogram(int64_t n, int w, int s)
 {
     Rows r;
     r.R = (n - w) / s + 1;
     r.n_it = r.R > 0 ? min64(r.R, range_len(w, n - w + 1, s)) : 0;
     r.n_full = r.n_it;
-    r.refused = r.R <= 0;
+    r.refused = r.R <= 0 || n == 0;
     return r;
 }
 

@@ -50,6 +50,37 @@ GENERIC_SWEEP = [
 ]
 
 
+# Sample rates of the specialised kernels (tests/test_gpu_rates.py; their tables: tests/test_rates_cpu.py).  The rate reaches a
+# kernel only through its tables, whose layout changes with fs: (fs, window, hop, kernel kinds plans() reaches, what).
+# The mel bank is refused below 6 854 Hz at every specialised window; just above it the last filter reaches bin K - 1, the
+# only place where build_pair_blob moves a four-tap group back inside the row ("clamped").  Layouts: tests/test_rates_cpu.py.
+RATE_CONFIGS = [
+    (48000, 480, 240, {PAIR, CTA, GENERIC}, "10 ms at 48 kHz: 4 empty mel filters"),
+    (44100, 320, 160, {PAIR, CTA, GENERIC}, "9 empty mel filters"),
+    (44100, 512, 256, {PAIR, GENERIC}, "3 empty mel filters, chroma lists of 9 taps"),
+    (24000, 320, 160, {PAIR, CTA, GENERIC}, "1 empty mel filter"),
+    (8000, 800, 400, {PAIR, CTA, GENERIC}, "12 mel steps per lane"),
+    (8000, 1024, 512, {PAIR, GENERIC}, "15 mel steps per lane"),
+    (7000, 960, 480, {PAIR, GENERIC}, "17 mel steps per lane"),
+    (6854, 1024, 512, {PAIR, GENERIC}, "the lowest accepted rate: 18 mel steps per lane (the largest pair blob), a clamped group"),
+    (6854, 800, 400, {PAIR, CTA, GENERIC}, "the lowest accepted rate: a clamped group"),
+    (11025, 1024, 512, {PAIR, GENERIC}, "11.025 kHz: 11 mel steps per lane"),
+    (96000, 960, 480, {PAIR, GENERIC}, "96 kHz: 4 empty mel filters, chroma lists of 9 taps"),
+    (192000, 1024, 512, {PAIR, GENERIC}, "192 kHz: 14 empty mel filters, chroma lists of 10 taps"),
+    (44100, 400, 200, {SOLO, CTA, GENERIC}, "6 empty mel filters"),
+    (48000, 600, 300, {SOLO, CTA, GENERIC}, "2 empty mel filters"),
+    (8000, 882, 441, {SOLO, CTA, GENERIC}, "13 mel steps per lane"),
+    (7000, 600, 300, {SOLO, CTA, GENERIC}, "11 mel steps per lane"),
+    (6854, 600, 300, {SOLO, CTA, GENERIC}, "the lowest accepted rate: a clamped group"),
+    (96000, 882, 441, {SOLO, CTA, GENERIC}, "96 kHz: 6 empty mel filters"),
+    (16000, 800, 1000, {PAIR, CTA, GENERIC}, "hop longer than the window"),
+    (16000, 800, 1600, {PAIR, CTA, GENERIC}, "hop longer than the window: the CTA kernel hands it to the generic kernel"),
+    (16000, 320, 400, {PAIR, CTA, GENERIC}, "hop longer than the window"),
+    (44100, 882, 1323, {SOLO, CTA, GENERIC}, "hop longer than the window"),
+    (16000, 600, 900, {SOLO, CTA, GENERIC}, "hop longer than the window"),
+]
+
+
 def plans(fs, w, s):
     """[(kind, Plan)] for every kernel kind a plan for (fs, w, s) reaches, the default choice first."""
     from pyaudioanalysis_b200._lib import Plan

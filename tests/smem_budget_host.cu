@@ -34,7 +34,9 @@ int main(int argc, char **argv)
         printf("generic %d %d %d %d %d %d %d %zu\n", fs, w, Nc, words, generic_group(Nc, Kp, words > 256 ? words - 256 : 0), g,
                generic_group(Nc, Kp, words + 256), generic_smem_bytes(g ? g : 1, Nc, Kp, words, g != 0));
     }
-    const int words = 1300;     // mel + DCT + chroma blob, upper bound over the supported (fs, window) pairs
+    // mel + DCT + chroma blob: the largest over the supported (fs, window) pairs (6 854 Hz, window 1024: the lowest rate whose
+    // mel bank builds has the longest filters; tests/test_rates_cpu.py: GENERIC_WORDS_MAX)
+    const int words = 1832;
     row<20, 20>(400, words); row<20, 20>(800, words); row<20, 20>(160, words);
     row<21, 21>(441, words); row<21, 21>(882, words);
     row<20, 10>(160, words); row<20, 10>(200, words); row<20, 10>(400, words);
@@ -42,8 +44,9 @@ int main(int argc, char **argv)
     row<20, 15>(300, words);
     row<16, 10>(160, words); row<16, 10>(320, words);
     row<20, 16>(320, words); row<20, 16>(160, words);
-    // pair kernel: bytes per CTA (tables of <= 1 664 words = 6.5 KB) and warps per CTA
-    const int pwords = 1664;
+    // pair kernel: bytes per CTA with the largest pair blob (2 232 words = 8.7 KB at 6 854 Hz, window 1024;
+    // tests/test_rates_cpu.py: PAIR_WORDS_MAX) and warps per CTA
+    const int pwords = 2232;
     printf("pair %d %d %zu\n", 320, pair_warps<10>(), pair_smem_bytes<10>(pwords));
     printf("pair %d %d %zu\n", 480, pair_warps<15>(), pair_smem_bytes<15>(pwords));
     printf("pair %d %d %zu\n", 512, pair_warps<16>(), pair_smem_bytes<16>(pwords));

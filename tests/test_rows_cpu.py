@@ -13,7 +13,8 @@ import pytest
 from oracle import st_oracle as O
 from tests.test_codelets_cpu import ROOT, _nvcc
 
-CONFIGS = [(800, 400), (800, 200), (800, 333), (882, 441), (800, 800), (400, 160)]
+CONFIGS = [(800, 400), (800, 200), (800, 333), (882, 441), (800, 800), (400, 160),
+           (800, 1000), (600, 900), (882, 1323), (320, 400)]          # hops longer than the window: frames skip samples
 FS = {882: 44100}
 
 
