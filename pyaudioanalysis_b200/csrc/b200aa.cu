@@ -20,6 +20,7 @@
 #include "fast_kernel.cuh"
 #include "pair_kernel.cuh"
 #include "pcm.cuh"
+#include "slots.h"
 #include "solo_kernel.cuh"
 #include "tables.inl"
 
@@ -184,6 +185,28 @@ struct GrowBuffer {
     void clear() { p.reset(); cap = 0; }
 };
 
+// the work-slot ring's event operations (csrc/slots.h) on CUDA events
+struct CudaSlotOps {
+    using Event = cudaEvent_t;
+    using Stream = cudaStream_t;
+    static int create(cudaEvent_t &e)
+    {
+        CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        return B200AA_OK;
+    }
+    static int record(cudaEvent_t e, cudaStream_t st)
+    {
+        CK(cudaEventRecord(e, st));
+        return B200AA_OK;
+    }
+    static int wait(cudaStream_t st, cudaEvent_t e)
+    {
+        CK(cudaStreamWaitEvent(st, e, 0));
+        return B200AA_OK;
+    }
+    static void destroy(cudaEvent_t e) { cudaEventDestroy(e); }
+};
+
 struct b200aa_plan {
     int fs = 0, window = 0, step = 0, K = 0;
     int device = 0, sm_count = 0;
@@ -200,24 +223,21 @@ struct b200aa_plan {
     PairTables pair{};                  // inter-pass twiddles of the warp-autonomous pair kernel (windows 32 * R)
     SoloTables solo{};                  // tables of the warp-autonomous per-frame kernel (windows 882 / 400 / 600)
     int prefer = -1;                    // -1 = automatic, 0 / 1 / 2 / 3 = generic / register-tiled CTA / pair / solo kernel only (testing, A/B)
-    // ring of work counters (one per in-flight launch of a persistent kernel).  A slot is handed out again only after
-    // the launch that used it last has finished: that launch recorded the slot's event, the next user's stream waits on it.
+    // ring of work counters (one per in-flight launch of a persistent kernel, csrc/slots.h).  A slot is in flight from
+    // acquire until its launch is queued and has recorded the slot's event; it is never handed to a second launch in that
+    // time, and the next user's stream waits on that event, so it runs after the launch that used the slot last.
     // A slot is kSlotBytes wide: the CTA / solo / generic kernels use its first word as their work counter, the pair kernel
     // the whole slot as its per-warp range descriptors (csrc/sched.cuh: 8 bytes per resident warp).
-    static constexpr unsigned kSlots = 64;
+    static constexpr unsigned kSlots = SlotRing<CudaSlotOps>::kSlots;
     static constexpr size_t kSlotBytes = 64 * 1024;
     b200aa_host::DeviceMemory counters;
-    cudaEvent_t slot_event[kSlots] = {};
-    bool slot_used[kSlots] = {};
-    unsigned next_slot = 0;
-    std::mutex slot_mu;
+    SlotRing<CudaSlotOps> slots;
     static constexpr int kPipe = 3;     // streams of the chunked host pipeline, each with its own clips / records / features buffers
     cudaStream_t pipe_stream[kPipe] = {nullptr, nullptr, nullptr};
     GrowBuffer pipe_ws[kPipe][3];
     ~b200aa_plan()
     {
         for (cudaStream_t s : pipe_stream) if (s) cudaStreamDestroy(s);
-        for (cudaEvent_t e : slot_event) if (e) cudaEventDestroy(e);
     }
 };
 
@@ -265,40 +285,26 @@ extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int ste
 }
 
 extern "C" void b200aa_plan_destroy(b200aa_plan *plan) { delete plan; }
-// work-counter slot for one launch on stream st (see b200aa_plan::slot_event); call slot_done after the launch
-static int slot_acquire(b200aa_plan *pl, cudaStream_t st, unsigned *slot, unsigned int **ctr)
-{
-    std::lock_guard<std::mutex> g(pl->slot_mu);
-    const unsigned s = pl->next_slot++ % b200aa_plan::kSlots;
-    if (!pl->slot_event[s]) CK(cudaEventCreateWithFlags(&pl->slot_event[s], cudaEventDisableTiming));
-    if (pl->slot_used[s]) CK(cudaStreamWaitEvent(st, pl->slot_event[s], 0));
-    *slot = s;
-    *ctr = reinterpret_cast<unsigned int *>(static_cast<unsigned char *>(pl->counters.get()) + size_t(s) * b200aa_plan::kSlotBytes);
-    return B200AA_OK;
-}
-static int slot_done(b200aa_plan *pl, cudaStream_t st, unsigned slot)
-{
-    std::lock_guard<std::mutex> g(pl->slot_mu);
-    CK(cudaEventRecord(pl->slot_event[slot], st));
-    pl->slot_used[slot] = true;
-    return B200AA_OK;
-}
-
-// One launch of a persistent kernel: the constructor takes a work-counter slot (status in rc, counter in ctr), finish()
-// gets the launcher's status, counts the launch, maps the status and records the slot.  B200AA_ERR_UNSUPPORTED = the
-// launcher declined the shape and launched nothing; the caller tries the next kernel.
+// One launch of a persistent kernel: the constructor takes a work-counter slot of the plan's ring (status in rc, counter
+// in ctr), finish() gets the launcher's status, counts the launch, maps the status and frees the slot.
+// B200AA_ERR_UNSUPPORTED = the launcher declined the shape and launched nothing; the caller tries the next kernel.
 struct SlotLaunch {
     b200aa_plan *pl;
     cudaStream_t st;
     unsigned slot = 0;
     unsigned int *ctr = nullptr;
     int rc;
-    SlotLaunch(b200aa_plan *plan, cudaStream_t stream) : pl(plan), st(stream) { rc = slot_acquire(pl, st, &slot, &ctr); }
+    SlotLaunch(b200aa_plan *plan, cudaStream_t stream) : pl(plan), st(stream)
+    {
+        rc = pl->slots.acquire(st, slot);
+        if (rc == B200AA_OK)
+            ctr = reinterpret_cast<unsigned int *>(static_cast<unsigned char *>(pl->counters.get()) + size_t(slot) * b200aa_plan::kSlotBytes);
+    }
     int finish(int launch_rc, const char *name)
     {
         const int r = launch_rc == B200AA_OK ? launched(name)
                                              : (launch_rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), name) : launch_rc);
-        const int done = slot_done(pl, st, slot);     // after launched(): a failed record keeps its own message
+        const int done = pl->slots.done(st, slot);    // after launched(): a failed record keeps its own message
         return r != B200AA_OK ? r : done;
     }
 };

@@ -9,7 +9,8 @@
 // vote, or ptxas stops trusting the warp's convergence in the step loop that follows.
 //
 // State: one 64-bit word per warp, (back << 32) | front, 0 = its warp has not started yet (a memset is all a launch needs;
-// nobody steals from a warp that has not started -- all CTAs of these launches are resident, so that lasts microseconds); every
+// nobody steals from a warp that has not started, and no warp ever waits for another: correctness does not rest on all CTAs
+// being resident at once -- beside another stream's kernels some start only when others have finished); every
 // transition is a single atomic on that word: the owner's claim is an atomicAdd on the front half, a steal is a
 // compare-and-swap that lowers the back half (it fails, harmlessly, if the owner moved in between), and a thief publishes
 // what it took with an atomicExch on its own word.  The functions are host + device so that tests/sched_host.cpp can run
