@@ -640,12 +640,12 @@ extern "C" int b200aa_mid_pool_ragged(const float *d_st, int64_t n_clips, int n_
 // long-term average of the mid-term matrix: one warp per (clip, row), fp64 accumulation.  windows (nullable, int64
 // [n_clips]): clip b averages its first M_b = clamp(windows[b], 0, M) columns (0 / 0 = NaN for none, as np.mean of an
 // empty axis); the sum's order depends only on (M_b, lane), as in mid_pool_kernel.
-__global__ void __launch_bounds__(256) long_term_mean_kernel(const float *mid, int64_t rows_total, int n_rows, int64_t M,
+__global__ void __launch_bounds__(256) long_term_mean_kernel(const float *mid, int64_t all_rows, int n_rows, int64_t M,
                                                              const int64_t *windows, float *out)
 {
     const int lane = threadIdx.x & 31;
     const int64_t wid = (blockIdx.x * int64_t(blockDim.x) + threadIdx.x) >> 5;
-    if (wid >= rows_total) return;
+    if (wid >= all_rows) return;
     const int64_t Mb = windows ? min(max(windows[wid / n_rows], int64_t(0)), M) : M;
     const float *row = mid + size_t(wid) * M;
     double s = 0.0;
@@ -969,7 +969,7 @@ static void fill_common(StParams &p, const b200aa_plan *pl, const void *d_sig, i
     p.tw = static_cast<const float2 *>(t.tw.get()); p.tw_post = static_cast<const float2 *>(t.tw_post.get());
     p.blob = static_cast<const int *>(pl->blob.get()); p.bl = pl->bl;
     p.n_clips = n_clips; p.n_samples = n_samples; p.clip_stride = clip_stride;
-    p.dtype = dtype; p.window = pl->window; p.fft_n = pl->window; p.step = pl->step; p.K = pl->K;
+    p.dtype = dtype; p.window = pl->window; p.step = pl->step; p.K = pl->K;
     p.Kp = (pl->K + 3) & ~3;
     p.Nc = t.Nc; p.packed = t.packed;
     p.nrad = (int)t.radix.size();
@@ -1046,7 +1046,7 @@ extern "C" int b200aa_st_features(const b200aa_plan *plan, const void *d_sig, in
     if (n_clips == 0) return B200AA_OK;
     StParams p;
     fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
-    p.t_stride = t_stride; p.deltas = deltas ? 1 : 0; p.n_out = deltas ? 68 : 34; p.mode = kModeFeatures;
+    p.t_stride = t_stride; p.deltas = deltas ? 1 : 0; p.n_out = deltas ? 68 : 34;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (use_pair(pl)) {
         SlotLaunch sl(pl, st);
@@ -1064,7 +1064,7 @@ extern "C" int b200aa_st_features(const b200aa_plan *plan, const void *d_sig, in
     if (use_fast(pl)) {
         SlotLaunch sl(pl, st);
         if (sl.rc != B200AA_OK) return sl.rc;
-        rc = sl.finish(fast_launch_features(pl->fast_kind, pl->fast, p, pl->sm_count, T, sl.ctr, st), "fast kernel");
+        rc = sl.finish(fast_launch_mode<kModeFeatures>(pl->fast_kind, pl->fast, p, pl->sm_count, T, sl.ctr, st), "fast kernel");
         if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     return launch_generic<kModeFeatures>(pl, p, T, st);
@@ -1084,7 +1084,7 @@ static int launch_rows(b200aa_plan *pl, StParams &p, cudaStream_t st)
     if (pl->fast_kind && !pl->force_generic && pl->prefer != 0 && pl->prefer != 3) {
         SlotLaunch sl(pl, st);
         if (sl.rc != B200AA_OK) return sl.rc;
-        const int rc = sl.finish(fast_launch_rows(pl->fast_kind, MODE, pl->fast, p, pl->sm_count, sl.ctr, st), "fast kernel");
+        const int rc = sl.finish(fast_launch_mode<MODE>(pl->fast_kind, pl->fast, p, pl->sm_count, p.rows_launch, sl.ctr, st), "fast kernel");
         if (rc != B200AA_ERR_UNSUPPORTED) return rc;
     }
     return launch_generic<MODE>(pl, p, p.rows_launch, st);
@@ -1129,8 +1129,7 @@ static int spectrogram_launch(const b200aa_plan *plan, const void *d_sig, int dt
     if (rc != B200AA_OK) return rc;
     StParams p;
     fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
-    p.mode = kModeSpectrogram;
-    p.origin = pl->window; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
+    p.rows_launch = r.R; p.rows_valid = r.n_full;
     return launch_rows<kModeSpectrogram>(pl, p, static_cast<cudaStream_t>(stream));
 }
 
@@ -1172,8 +1171,7 @@ static int chromagram_launch(const b200aa_plan *plan, const void *d_sig, int dty
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StParams p;
     fill_common(p, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
-    p.mode = kModeChromagram;
-    p.origin = w; p.row0 = 0; p.rows_total = r.R; p.rows_launch = r.R; p.rows_valid = r.n_full;
+    p.rows_launch = r.R; p.rows_valid = r.n_full;
     rc = launch_rows<kModeChromagram>(pl, p, st);
     if (rc != B200AA_OK) return rc;
     const int64_t per_clip = d_len ? rows::max_clipped(w, s) : r.n_it - r.n_full;

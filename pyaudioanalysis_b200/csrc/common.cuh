@@ -41,25 +41,31 @@ struct StParams {
     BlobLayout bl;
     int64_t n_clips, n_samples, clip_stride, t_stride;
     int64_t seg_len, segs_per_clip, n_items;
-    // spectrogram / chromagram launches: row r of this launch is the frame starting at
-    // origin + r*step, stored at output row row0 + r (of rows_total per clip); rows >= rows_valid
-    // of the launch are written as zeros (the reference leaves them unset, ShortTermFeatures.py:413-422).
-    // A ragged row launch (len set, the kernels' RAGGED form) takes both counts of clip b from ragged_rows below.
-    int64_t origin, row0, rows_total, rows_launch, rows_valid;
+    // spectrogram / chromagram launches: rows [0, rows_launch) of every clip, row r the full frame that starts at
+    // rows::frame_start(window, step, r), stored at output row b * rows_launch + r; rows >= rows_valid are written as
+    // zeros (the reference leaves them unset, ShortTermFeatures.py:413-422).  Frames clipped at the end of a clip
+    // (:352-355) go to clipped_chroma_kernel.  A ragged row launch (len set, the kernels' RAGGED form) takes both counts
+    // of clip b from ragged_rows below.
+    int64_t rows_launch, rows_valid;
     int dtype, deltas, n_out;       // n_out = 34 or 68
-    int window;                     // nominal window (frame hop grid, feature tables)
-    int fft_n;                      // samples per frame transformed (== window; clipped chromagram frames,
-                                    // :352-355, go to clipped_chroma_kernel)
+    int window;                     // samples per frame
+    int G;                          // frames per group (generic kernel)
     int step, K, Kp, Nc, packed;    // K = window/2 bins kept; Nc = complex transform length
     int nrad;
     int radix[kMaxRadix];
-    int G;                          // frames per group (generic kernel)
-    int mode;
     // large windows (generic kernel, BIG form): the transform ping-pong buffers and the |X| rows of every CTA live in
     // global memory (stream-ordered allocation per launch) instead of shared memory
     unsigned char *scratch;
     size_t scratch_stride;          // bytes per CTA
 };
+
+// first sample of frame r: feature frames start at r * step (ShortTermFeatures.py:608), spectrogram / chromagram rows at
+// rows::frame_start
+template <int MODE>
+__device__ __forceinline__ int64_t frame_first(int w, int s, int64_t r)
+{
+    return MODE == kModeFeatures ? r * s : rows::frame_start(w, s, r);
+}
 
 // Length of clip b of a ragged batch, clamped to the batch width (the clips' samples end there)
 __device__ __forceinline__ int64_t ragged_len(const StParams &p, int64_t b)
@@ -266,66 +272,13 @@ __device__ __forceinline__ void spectral_features(const float *X, const float *X
     __syncwarp();
 }
 
-// time-domain half: zcr, energy, energy entropy  [ShortTermFeatures.py:22-51]
-// D(n) returns sample n of the frame minus the clip centre m.
-template <class Acc>
-__device__ __forceinline__ void time_features(Acc D, int w, const b200aa_clip_norm &nm, float *fv, int lane)
-{
-    const float a = nm.a, bp = nm.bp, lo = nm.lo, hi = nm.hi;
-    const int L = w / 10;
-    float tot = 0.f, ent_acc[10];
-    int flips = 0;   // sum |sign_n - sign_{n-1}|  (each in {0,1,2})
-#pragma unroll
-    for (int j = 0; j < 10; ++j) {
-        float e = 0.f;
-        for (int n = j * L + lane; n < (j + 1) * L; n += 32) {
-            const float d = D(n);
-            const float y = fmaf(a, d, bp);
-            e = fmaf(y, y, e);
-            if (n > 0) {
-                const float q = D(n - 1);
-                const int s1 = (d > lo) - (d < hi), s0 = (q > lo) - (q < hi);
-                flips += abs(s1 - s0);
-            }
-        }
-        ent_acc[j] = e;
-    }
-    float rest = 0.f;
-    for (int n = 10 * L + lane; n < w; n += 32) {
-        const float d = D(n);
-        const float y = fmaf(a, d, bp);
-        rest = fmaf(y, y, rest);
-        const float q = D(n - 1);
-        const int s1 = (d > lo) - (d < hi), s0 = (q > lo) - (q < hi);
-        flips += abs(s1 - s0);
-    }
-#pragma unroll
-    for (int j = 0; j < 10; ++j) {
-        ent_acc[j] = warp_sum(ent_acc[j]);
-        tot += ent_acc[j];
-    }
-    tot += warp_sum(rest);
-    float fl = warp_sum(float(flips));
-    float H = 0.f;
-#pragma unroll
-    for (int j = 0; j < 10; ++j) {
-        const float s = ent_acc[j] / (tot + B200AA_EPS);
-        H -= s * log2f(s + B200AA_EPS);
-    }
-    if (lane == 0) {
-        fv[0] = fl * 0.5f / float(w - 1);
-        fv[1] = tot / float(w);
-        fv[2] = H;
-    }
-}
-
-
 // sign(x - mean) in {-1, 0, +1} as a float, from the exact thresholds of b200aa_clip_norm
 __device__ __forceinline__ float sign_class(float d, float lo, float hi) { return (d > lo ? 1.f : 0.f) - (d < hi ? 1.f : 0.f); }
 
-// ---- chunked form of the same three rows: every lane owns c = ceil(w/32) CONSECUTIVE samples (one load per
+// ---- time-domain rows: zcr, energy, energy entropy  [ShortTermFeatures.py:22-51], one warp per frame.  D(n) returns
+// sample n of the frame minus the clip centre m.  Every lane owns c = ceil(w/32) CONSECUTIVE samples (one load per
 // sample, sequential sign flips, energy split at the single entropy-block boundary a chunk can contain); the block
-// energies are then sums of lane parts.  About half the instructions of time_features() above.
+// energies are then sums of lane parts.
 // Per-lane constants (depend on w and the lane only; computed once per CTA into shared memory as int4):
 //   x = c, y = samples of the chunk that belong to the earlier block, [z, w) = parts that make up block `lane` (< 10)
 __device__ inline int4 time_lane_init(int w, int lane)

@@ -59,11 +59,6 @@ struct DenseShape {
     static constexpr int Lb = K / 10;               // spectral-entropy block length (:94)
 };
 
-// per-lane constants of the dense pass (depend on the lane only; computed once per CTA)
-struct DenseLane {
-    int split;        // bins [0, split) of the lane's chunk belong to the previous entropy block
-    int ps, pe;       // lanes 0..9: range of "parts" (2 per lane, in bin order) that make up block `lane`
-};
 // ----------------------------------------------------------------------------------------------
 // Half-warp variant of the dense pass: 16 lanes per frame (a warp handles two frames), every lane holds
 // C2 = odd(ceil(K/32)) float2 pairs of consecutive bins, per-bin arithmetic on float2 pairs.  The
@@ -77,22 +72,26 @@ struct HalfShape {
     static_assert(16 * CB == DenseShape<K>::Kp, "same padded row length as the warp-per-frame layout");
     static_assert(CB < Lb && (Lb % 2) == 0, "one (even) entropy block boundary per lane at most");
 };
+// per-lane constants of the half-warp dense pass (here and in pair_kernel.cuh / solo_kernel.cuh; depend on the lane only,
+// computed once per CTA), l = lane within the half-warp, 0..15:
+// .x = bins of the lane's chunk that belong to the earlier entropy block, [.y, .z) = parts (2 per lane, in bin order) of block l
 template <int K>
-__device__ __forceinline__ DenseLane dense_lane_init_h(int l)        // l = lane within the half-warp, 0..15
+__device__ __forceinline__ int4 pair_lane_init(int l)
 {
-    constexpr int CB = HalfShape<K>::CB, Lb = HalfShape<K>::Lb;
-    DenseLane d;
+    constexpr int CB = 2 * (((K + 31) / 32) | 1), Lb = K / 10;
     const int k0 = l * CB;
     const int bnd = ((k0 + CB - 1) / Lb) * Lb;
-    d.split = bnd > k0 ? (bnd - k0) / 2 : 0;            // in float2 pairs
-    d.ps = 32; d.pe = 0;
-    const int j = l;
+    int4 d;
+    d.x = bnd > k0 ? bnd - k0 : 0;
+    int ps = 32, pe = 0;
+#pragma unroll 1
     for (int q = 0; q < 16; ++q) {
         const int b0 = q * CB, bb = ((b0 + CB - 1) / Lb) * Lb, sp = bb > b0 ? bb - b0 : 0;
-        if (sp > 0 && b0 >= j * Lb && b0 + sp <= (j + 1) * Lb) { d.ps = min(d.ps, 2 * q); d.pe = max(d.pe, 2 * q + 1); }
-        if (b0 + sp >= j * Lb && b0 + CB <= (j + 1) * Lb) { d.ps = min(d.ps, 2 * q + 1); d.pe = max(d.pe, 2 * q + 2); }
+        if (sp > 0 && b0 >= l * Lb && b0 + sp <= (l + 1) * Lb) { ps = min(ps, 2 * q); pe = max(pe, 2 * q + 1); }
+        if (b0 + sp >= l * Lb && b0 + CB <= (l + 1) * Lb) { ps = min(ps, 2 * q + 1); pe = max(pe, 2 * q + 2); }
     }
-    if (l >= 10) { d.ps = 0; d.pe = 0; }
+    if (l >= 10) { ps = 0; pe = 0; }
+    d.y = ps; d.z = pe; d.w = 0;
     return d;
 }
 __device__ __forceinline__ float half_sum(float v)      // sum over the 16 lanes of a half-warp (both halves at once)
@@ -118,7 +117,7 @@ __device__ __forceinline__ void spectral_features_h(const float *X, const float 
 {
     constexpr int C2 = HalfShape<K>::C2, CB = HalfShape<K>::CB;
     const int k0 = l * CB;
-    const int4 dlv = *reinterpret_cast<const int4 *>(dlp);        // {split (pairs), ps, pe, -}
+    const int4 dlv = *reinterpret_cast<const int4 *>(dlp);        // {split (bins), ps, pe, -}
     const float2 *X2 = reinterpret_cast<const float2 *>(X) + l * C2;
     const float2 *Xp2 = reinterpret_cast<const float2 *>(Xp) + l * C2;
     float2 x2[C2];
@@ -139,7 +138,7 @@ __device__ __forceinline__ void spectral_features_h(const float *X, const float 
         s1 = fmaf(float(2 * j + 1), t, s1);          // (2j+1) a + (2j+2) b = (2j+1)(a+b) + b
         sb += x2[j].y;
         const float2 sq = f2mul(x2[j], x2[j]);
-        if (j < dlv.x) plo2 = f2add(plo2, sq); else phi2 = f2add(phi2, sq);
+        if (2 * j < dlv.x) plo2 = f2add(plo2, sq); else phi2 = f2add(phi2, sq);     // Lb even: boundaries between pairs
     }
     const float plo = plo2.x + plo2.y, phi = phi2.x + phi2.y, part = plo + phi;
     float sk = fmaf(float(k0), sx, s1 + sb);         // sum (k0 + i + 1) x_i
@@ -577,10 +576,7 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
     const int *const blob_t = blob_s;
     const SmallTables tb = bind_tables(blob_t, p.bl);
     if (tid < 32) sm.tlane[tid] = time_lane_init(N, tid);
-    if (tid < 16) {
-        const DenseLane d0_ = dense_lane_init_h<K>(tid);
-        sm.dlane[tid * 4 + 0] = d0_.split; sm.dlane[tid * 4 + 1] = d0_.ps; sm.dlane[tid * 4 + 2] = d0_.pe;
-    }
+    if (MODE == kModeFeatures && tid < 16) *reinterpret_cast<int4 *>(sm.dlane + tid * 4) = pair_lane_init<K>(tid);   // dense pass only
     for (int i = tid; i < 2 * Kp; i += NT) Xprev[i] = 0.f;
     if (RUNS && tid == 0) mbar_init(&sm.mbar, 1);
     unsigned tma_phase = 0;       // parity of the next completion to wait for
@@ -600,7 +596,6 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
         if constexpr (RAGGED) ragged_rows<MODE>(p, b, rows_b, valid_b);
         const fidx_t T = fidx_t(MODE == kModeFeatures ? (len < N ? 0 : (len - N) / step + 1) : rows_b);
         const fidx_t n_valid = MODE == kModeFeatures ? T : fidx_t(valid_b);
-        const int64_t origin = MODE == kModeFeatures ? 0 : p.origin;
         const fidx_t t0 = fidx_t(seg * p.seg_len);
         if (t0 >= T) break;
         const fidx_t t1 = (t0 + fidx_t(p.seg_len)) < T ? (t0 + fidx_t(p.seg_len)) : T;
@@ -624,13 +619,13 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
                 const int width = MODE == kModeSpectrogram ? K : 12;
                 for (int e = tid; e < (nrow - ng) * width; e += NT) {
                     const int f = ng + e / width, k = e % width;
-                    p.out[(size_t(b) * p.rows_total + p.row0 + g0 + f) * width + k] = 0.f;
+                    p.out[(size_t(b) * p.rows_launch + g0 + f) * width + k] = 0.f;
                 }
                 if (ng == 0) continue;
             }
             // ---- stage the sample span of this step as float (x - m)
             const int span = (ng - 1) * step + N;
-            const int64_t sbase = origin + int64_t(g0) * step;
+            const int64_t sbase = frame_first<MODE>(N, step, g0);
             if (RUNS) {
                 // samples shared with the previous step are already converted: move them to the front
                 int keep = 0;
@@ -681,7 +676,7 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
                 const int ngn = int((t1 - gn) < G ? (t1 - gn) : G);
                 const int keepn = N - step;
                 const int cnt = (ngn - 1) * step + N - keepn;                    // new samples of that step
-                const short *src = reinterpret_cast<const short *>(clip) + (origin + int64_t(gn) * step + keepn - 8);
+                const short *src = reinterpret_cast<const short *>(clip) + (frame_first<MODE>(N, step, gn) + keepn - 8);
                 if (tid == 0) tma_load_1d(raw, src, unsigned(cnt + 8) * 2u, &sm.mbar);
                 prefetched = true;
             }
@@ -761,7 +756,7 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
 
             if constexpr (MODE == kModeSpectrogram) {
                 // rows are contiguous in the output: consecutive threads -> consecutive bins
-                float *dst = p.out + (size_t(b) * p.rows_total + p.row0 + g0) * K;
+                float *dst = p.out + (size_t(b) * p.rows_launch + g0) * K;
                 for (int e = tid; e < ng * K; e += NT) {
                     const int f = e / K, k = e - f * K;
                     dst[e] = Xrows[size_t(f) * Kp + k];
@@ -776,7 +771,7 @@ __global__ void __launch_bounds__(fast_threads(G), B200AA_FAST_MINBLOCKS) st_fas
                     for (int i = 0; i < DenseShape<K>::C; ++i) { const float v = X[lane * DenseShape<K>::C + i]; sxx = fmaf(v, v, sxx); }
                     sxx = warp_sum(sxx);
                     const float ch = chroma_lane(X, sxx, tb, lane);
-                    if (lane < 12) p.out[(size_t(b) * p.rows_total + p.row0 + g0 + f) * 12 + lane] = ch;
+                    if (lane < 12) p.out[(size_t(b) * p.rows_launch + g0 + f) * 12 + lane] = ch;
                 }
                 __syncthreads();
                 continue;
@@ -913,7 +908,6 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
     const int64_t min_seg = (T * p.n_clips >= 46 * slots) ? 46 : 6;
     if (seg < min_seg) seg = min_seg;
     seg = ((seg + 2 + G - 1) / G) * G - 2;
-    if (const char *ov = getenv("B200AA_SEG")) { const long v = atol(ov); if (v > 0) seg = v; }   // tuning override
     if (seg > T) seg = T;
     p.seg_len = seg;
     p.segs_per_clip = (T + seg - 1) / seg;
@@ -928,15 +922,16 @@ inline int fast_launch_t(const FastTables &ft, StParams p, int sm_count, int64_t
     return cudaPeekAtLastError() == cudaSuccess ? B200AA_OK : B200AA_ERR_CUDA;    // the caller fetches (and clears) the text
 }
 
-// run staging needs whole 8-sample runs per frame, per entropy block (window % 80 == 0) and per hop
+// run staging needs whole 8-sample runs per frame, per entropy block (window % 80 == 0) and per hop.  Every frame starts
+// at a multiple of the step, or of the step past the (even; with runs, multiple of 8) window.
 template <int R1, int R2, int MODE>
 inline int fast_launch_shape(const FastTables &ft, const StParams &p, int sm_count, int64_t T, unsigned int *ctr, cudaStream_t st)
 {
     constexpr int G = B200AA_FAST_G;
     constexpr int N = 2 * R1 * R2;
-    const bool even = (p.step % 2) == 0 && (p.origin % 2) == 0;
+    const bool even = (p.step % 2) == 0;
     if (N % 80 == 0) {
-        const bool runs = (p.step % 8) == 0 && (p.clip_stride % 8) == 0 && (p.origin % 8) == 0;
+        const bool runs = (p.step % 8) == 0 && (p.clip_stride % 8) == 0;
         if (runs) return fast_launch_t<R1, R2, G, true, N % 80 == 0, MODE>(ft, p, sm_count, T, ctr, st);
     }
     return even ? fast_launch_t<R1, R2, G, true, false, MODE>(ft, p, sm_count, T, ctr, st)
@@ -956,17 +951,6 @@ inline int fast_launch_mode(int kind, const FastTables &ft, const StParams &p, i
     case 2016: return fast_launch_shape<20, 16, MODE>(ft, p, sm_count, T, ctr, st);
     default: return B200AA_ERR_UNSUPPORTED;
     }
-}
-
-inline int fast_launch_features(int kind, const FastTables &ft, const StParams &p, int sm_count, int64_t T, unsigned int *ctr, cudaStream_t st)
-{
-    return fast_launch_mode<kModeFeatures>(kind, ft, p, sm_count, T, ctr, st);
-}
-// spectrogram / chromagram rows of full-length frames (p.origin, p.rows_* filled by the caller; p.len set: ragged)
-inline int fast_launch_rows(int kind, int mode, const FastTables &ft, const StParams &p, int sm_count, unsigned int *ctr, cudaStream_t st)
-{
-    if (mode == kModeSpectrogram) return fast_launch_mode<kModeSpectrogram>(kind, ft, p, sm_count, p.rows_launch, ctr, st);
-    return fast_launch_mode<kModeChromagram>(kind, ft, p, sm_count, p.rows_launch, ctr, st);
 }
 #endif  // B200AA_LAYOUT_ONLY
 

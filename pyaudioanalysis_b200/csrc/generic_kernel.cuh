@@ -69,7 +69,7 @@ template <int MODE, bool BIG = false, bool RAGGED = false>
 __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams p)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int G = p.G, Nc = p.Nc, K = p.K, Kp = p.Kp, w = p.window, fn = p.fft_n;
+    const int G = p.G, Nc = p.Nc, K = p.K, Kp = p.Kp, w = p.window;
     unsigned char *const big = BIG ? p.scratch + size_t(blockIdx.x) * p.scratch_stride : smem_raw;
     float2 *bufA = reinterpret_cast<float2 *>(big);
     float2 *bufB = bufA + size_t(G) * Nc;
@@ -83,22 +83,20 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int i = tid; i < p.bl.words; i += kThreads) blob_s[i] = p.blob[i];
-    if (tid < 32) tlane[tid] = time_lane_init(p.fft_n, tid);
+    if (tid < 32) tlane[tid] = time_lane_init(w, tid);
     __syncthreads();
     const SmallTables tb = bind_tables(blob_s, p.bl);
 
     for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
         const int64_t b = item / p.segs_per_clip, seg = item % p.segs_per_clip;
         const int64_t len = p.len ? p.len[b] : p.n_samples;
-        int64_t n_rows, n_valid, origin;
+        int64_t n_rows, n_valid;
         if (MODE == kModeFeatures) {
             n_rows = n_valid = len < w ? 0 : (len - w) / p.step + 1;     // loop guard :608
-            origin = 0;
         } else {
             n_rows = p.rows_launch;
             n_valid = p.rows_valid;
             if constexpr (RAGGED) ragged_rows<MODE>(p, b, n_rows, n_valid);
-            origin = p.origin;
         }
         const int64_t t0 = seg * p.seg_len;
         if (t0 >= n_rows) continue;
@@ -119,7 +117,7 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                 const int64_t fr = g0 + f;
                 float2 z = make_float2(0.f, 0.f);
                 if (fr < n_valid) {
-                    const int64_t s0 = origin + fr * p.step;
+                    const int64_t s0 = frame_first<MODE>(w, p.step, fr);
                     const float d0 = rd(s0);
                     if (p.packed) z = make_float2(rd(s0 + 2 * n) - d0, rd(s0 + 2 * n + 1) - d0);
                     else z = make_float2(rd(s0 + n) - d0, 0.f);
@@ -132,7 +130,7 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                 // fvrows rows of this step are free: the previous step's store loop finished before its last barrier.
                 for (int f = warp; f < ng; f += kWarps) {
                     const float2 *zf = bufA + size_t(f) * Nc;
-                    const float d0 = rd(origin + (g0 + f) * p.step);
+                    const float d0 = rd(frame_first<MODE>(w, p.step, g0 + f));
                     float *fv = fvrows + size_t(f + 1) * kFvStride;
                     if (p.packed)
                         time_features_chunked([&](int n) { const float2 q = zf[n >> 1]; return ((n & 1) ? q.y : q.x) + d0; }, w, nm,
@@ -180,7 +178,9 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                 float2 *t_ = src; src = dst; dst = t_;
                 Ns = NsR;
             }
-            // ---- magnitudes |X[k]| / K, k < K  (ShortTermFeatures.py:617-621)
+            // ---- magnitudes |X[k]| / K, k < K  (ShortTermFeatures.py:617-621).  Not unrolled: unrolled (and, in the BIG
+            // form, unswitched on p.packed) the loop costs 250-300 instructions more per kernel and more registers.
+#pragma unroll 1
             for (int e = tid; e < ng * K; e += kThreads) {
                 const int f = e / K, k = e - f * K;
                 const int64_t fr = g0 + f;
@@ -190,26 +190,21 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                     const float sc = nm.a / float(K);
                     float2 Xc;
                     if (p.packed) {
-                        // bins above fn/2 (only for a clipped frame with K > fn/2) mirror: |X[k]| = |X[fn-k]|
-                        const int kk = k > Nc ? fn - k : k;
-                        if (kk == Nc) {
-                            Xc = make_float2(Z[0].x - Z[0].y, 0.f);          // Nyquist bin
-                        } else {
-                            const float2 zk = Z[kk];
-                            const float2 zm = Z[kk == 0 ? 0 : Nc - kk];
-                            const float2 ev = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-                            const float2 od = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
-                            const float2 wk = __ldg(p.tw_post + kk);
-                            const float2 t = cmul(od, wk);
-                            Xc = make_float2(ev.x + t.x, ev.y + t.y);
-                        }
+                        // k < K = Nc: X[k] from the pair (Z[k], Z[Nc-k]) of the half-length transform
+                        const float2 zk = Z[k];
+                        const float2 zm = Z[k == 0 ? 0 : Nc - k];
+                        const float2 ev = make_float2(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
+                        const float2 od = make_float2(0.5f * (zk.y + zm.y), -0.5f * (zk.x - zm.x));
+                        const float2 wk = __ldg(p.tw_post + k);
+                        const float2 t = cmul(od, wk);
+                        Xc = make_float2(ev.x + t.x, ev.y + t.y);
                     } else {
                         Xc = Z[k];
                     }
                     if (k == 0) {
                         // DC of y = a*(d - d0) + (a*d0 + bp):  a*sum(d-d0) + w*(a*d0+bp)
-                        const float d0 = rd(origin + fr * p.step);
-                        mag = fabsf(fmaf(nm.a, Xc.x, float(fn) * fmaf(nm.a, d0, nm.bp))) / float(K);
+                        const float d0 = rd(frame_first<MODE>(w, p.step, fr));
+                        mag = fabsf(fmaf(nm.a, Xc.x, float(w) * fmaf(nm.a, d0, nm.bp))) / float(K);
                     } else {
                         const float re = Xc.x * sc, im = Xc.y * sc;
                         mag = sqrtf(fmaf(re, re, im * im));
@@ -222,7 +217,7 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
             if (MODE == kModeSpectrogram) {
                 for (int e = tid; e < ng * K; e += kThreads) {
                     const int f = e / K, k = e - f * K;
-                    p.out[(size_t(b) * p.rows_total + p.row0 + (g0 + f)) * K + k] = Xrows[size_t(f + 1) * Kp + k];
+                    p.out[(size_t(b) * p.rows_launch + (g0 + f)) * K + k] = Xrows[size_t(f + 1) * Kp + k];
                 }
                 __syncthreads();
                 continue;
@@ -234,7 +229,7 @@ __global__ void __launch_bounds__(kThreads, 2) st_generic_kernel(const StParams 
                     for (int k = lane; k < K; k += 32) sxx = fmaf(X[k], X[k], sxx);
                     sxx = warp_sum(sxx);
                     const float ch = (g0 + f < n_valid) ? chroma_lane(X, sxx, tb, lane) : 0.f;
-                    if (lane < 12) p.out[(size_t(b) * p.rows_total + p.row0 + (g0 + f)) * 12 + lane] = ch;
+                    if (lane < 12) p.out[(size_t(b) * p.rows_launch + (g0 + f)) * 12 + lane] = ch;
                 }
                 __syncthreads();
                 continue;
@@ -362,7 +357,7 @@ __global__ void __launch_bounds__(kThreads, 2) clipped_chroma_kernel(const StPar
             for (int k = lane; k < K; k += 32) sxx = fmaf(X[k], X[k], sxx);
             sxx = warp_sum(sxx);
             const float ch = chroma_lane(X, sxx, tb, lane);
-            if (lane < 12) p.out[(size_t(b) * p.rows_total + i) * 12 + lane] = ch;
+            if (lane < 12) p.out[(size_t(b) * p.rows_launch + i) * 12 + lane] = ch;
         }
     }
 }

@@ -41,15 +41,6 @@ constexpr int kPairMaxWarps = B200AA_PAIR_MAXWARPS;     // warps per CTA (each o
 #define B200AA_PAIR_MINBLOCKS 1
 #endif
 constexpr int kPairMinBlocks = B200AA_PAIR_MINBLOCKS;   // one CTA per SM: the twiddle / mel / DCT / chroma tables exist once per SM
-// the solo kernel's feature layout (solo_kernel.cuh): one CTA of 24 warps at 80 registers; config 3 (64 x 60 s @44.1 kHz,
-// 882 / 441) on an H100 80GB HBM3 (700 W): 1 x 24 1.297 ms, 1 x 16 1.281 ms (within the spread of one run)
-#ifndef B200AA_SOLO_MAXWARPS
-#define B200AA_SOLO_MAXWARPS 24
-#endif
-#ifndef B200AA_SOLO_MINBLOCKS
-#define B200AA_SOLO_MINBLOCKS 1
-#endif
-constexpr int kSoloMaxWarps = B200AA_SOLO_MAXWARPS, kSoloMinBlocks = B200AA_SOLO_MINBLOCKS;
 
 template <int R>
 struct PairShape {
@@ -139,29 +130,8 @@ __device__ __forceinline__ float fsqrt_fast(float x)        // MUFU.SQRT (2 ulp,
 // ----------------------------------------------------------------------------------------------
 // Dense spectral rows of two frames per warp (half-warp each): spectral_features_h of fast_kernel.cuh with the previous
 // frame's row sum taken from where it already exists -- half 1 (frame b) receives half 0's (frame a's) sum by shuffle,
-// half 0 the carried sum of the previous pair's b -- instead of re-reading the previous row.
+// half 0 the carried sum of the previous pair's b -- instead of re-reading the previous row.  Lane constants: pair_lane_init.
 // ----------------------------------------------------------------------------------------------
-// per-lane constants: .x = bins of the lane's chunk that belong to the earlier entropy block, [.y, .z) = parts of block l
-template <int K>
-__device__ __forceinline__ int4 pair_lane_init(int l)
-{
-    constexpr int CB = 2 * (((K + 31) / 32) | 1), Lb = K / 10;
-    const int k0 = l * CB;
-    const int bnd = ((k0 + CB - 1) / Lb) * Lb;
-    int4 d;
-    d.x = bnd > k0 ? bnd - k0 : 0;
-    int ps = 32, pe = 0;
-#pragma unroll 1
-    for (int q = 0; q < 16; ++q) {
-        const int b0 = q * CB, bb = ((b0 + CB - 1) / Lb) * Lb, sp = bb > b0 ? bb - b0 : 0;
-        if (sp > 0 && b0 >= l * Lb && b0 + sp <= (l + 1) * Lb) { ps = min(ps, 2 * q); pe = max(pe, 2 * q + 1); }
-        if (b0 + sp >= l * Lb && b0 + CB <= (l + 1) * Lb) { ps = min(ps, 2 * q + 1); pe = max(pe, 2 * q + 2); }
-    }
-    if (l >= 10) { ps = 0; pe = 0; }
-    d.y = ps; d.z = pe; d.w = 0;
-    return d;
-}
-
 template <int K>
 __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, float sxp_carried, bool own_prev, const int *dlp,
                                               float *parts, float *fv, int l, int half)
@@ -225,9 +195,6 @@ __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, f
     const float2 dstep = make_float2(2.f * invK, 2.f * invK);
     const float2 nx2 = make_float2(nx, nx), mnp2 = make_float2(-np_, -np_);
     float2 sp2 = make_float2(0.f, 0.f), fl2 = make_float2(0.f, 0.f);
-#ifdef B200AA_ROLLOFF_SEQ
-    float run = incl - part, below = 0.f;       // (A/B reference: every lane walks its own chunk bin by bin)
-#else
     // rolloff = number of bins whose cumulative energy stays <= thr.  The prefix over the lanes' chunks is monotone, so the
     // lanes before the crossing one count all their CB bins and only the crossing lane's chunk needs a bin-by-bin look: the
     // half-warp takes it together (one or two float2 of that chunk per lane, a 4-step scan) instead of CB dependent steps per lane.
@@ -264,19 +231,12 @@ __device__ __forceinline__ void pair_spectral(const float *X, const float *Xp, f
         }
         if (l == 0) below += float(cl * CB);
     }
-#endif
 #pragma unroll
     for (int j = 0; j < C2; ++j) {
         sp2 = f2fma(f2mul(d2, d2), x2[j], sp2);
         d2 = f2add(d2, dstep);
         const float2 df = f2fma(x2[j], nx2, f2mul(Xp2[j], mnp2));
         fl2 = f2fma(df, df, fl2);
-#ifdef B200AA_ROLLOFF_SEQ
-        run = fmaf(x2[j].x, x2[j].x, run);
-        below += run > thr ? 0.f : 1.f;
-        run = fmaf(x2[j].y, x2[j].y, run);
-        below += run > thr ? 0.f : 1.f;
-#endif
     }
     const float sp = sp2.x + sp2.y, fl = fl2.x + fl2.y;
     __syncwarp();
@@ -1021,7 +981,6 @@ inline int pair_plan_init(int window, const std::vector<int> &h_pblob, const Pai
     const int R = pair_r_for_window(window);
     pt->R = 0;
     if (!R) return B200AA_OK;
-    if (getenv("B200AA_NO_PAIR")) return B200AA_OK;
     if (b200aa_host::upload(b200aa_host::twiddle_grid(R, 32, 32 * R), pt->tw) != cudaSuccess ||
         b200aa_host::upload(h_pblob, pt->pblob) != cudaSuccess)
         return B200AA_ERR_CUDA;

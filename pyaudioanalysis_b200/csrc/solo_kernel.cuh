@@ -54,6 +54,15 @@ struct alignas(16) SoloRowWarpMem {
 template <int L, int R2, int MODE> struct SoloWarpMemFor { using type = SoloRowWarpMem<L, R2, MODE>; };
 template <int L, int R2> struct SoloWarpMemFor<L, R2, kModeFeatures> { using type = SoloWarpMem<L, R2>; };
 
+// the feature layout: one CTA of 24 warps at 80 registers; config 3 (64 x 60 s @44.1 kHz, 882 / 441) on an H100 80GB HBM3
+// (700 W): 1 x 24 1.297 ms, 1 x 16 1.281 ms (within the spread of one run)
+#ifndef B200AA_SOLO_MAXWARPS
+#define B200AA_SOLO_MAXWARPS 24
+#endif
+#ifndef B200AA_SOLO_MINBLOCKS
+#define B200AA_SOLO_MINBLOCKS 1
+#endif
+constexpr int kSoloMaxWarps = B200AA_SOLO_MAXWARPS, kSoloMinBlocks = B200AA_SOLO_MINBLOCKS;
 // Measured on config 3 (64 x 60 s @44.1 kHz), warps per CTA x CTAs per SM -> spectrogram / chromagram ms:
 //   8 x 2 (126 regs, the feature layout) 0.558 / 0.592    5 x 4 (96 regs) 0.543 / 0.558    8 x 3 (80 regs) 0.502 / 0.537
 //   6 x 4 (80) 0.499 / 0.546    7 x 4 (71) 0.490 / 0.561    10 x 3 (64) 0.485 / 0.565    8 x 4 (64 regs, 32 warps) 0.478 / 0.552
@@ -238,7 +247,6 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
             q1 = q1 < NP ? q1 : NP;
         }
         const int n_valid = MODE == kModeFeatures ? T : int(valid_b);
-        const int64_t origin = MODE == kModeFeatures ? 0 : p.origin;
         const b200aa_clip_norm nm = p.norm[b];
         const bool is16 = p.dtype == B200AA_DTYPE_I16;
         const char *clip = reinterpret_cast<const char *>(p.sig) + size_t(b) * p.clip_stride * (is16 ? 2 : 4);
@@ -258,7 +266,7 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
             const int ta = 2 * q;
             const bool bvalid = ta + 1 < T;
             const int tbb = bvalid ? ta + 1 : ta;
-            const int64_t sa0 = origin + int64_t(ta) * step, sb0 = origin + int64_t(tbb) * step;       // first samples
+            const int64_t sa0 = frame_first<MODE>(N, step, ta), sb0 = frame_first<MODE>(N, step, tbb);       // first samples
             float *rowa, *rowb;              // features: frame b's row lands in the transform buffer once its transform is done
             if constexpr (FEAT) { rowa = wm.rowa; rowb = reinterpret_cast<float *>(wm.tz); }
             else { rowa = wm.rows[0]; rowb = wm.rows[1]; }
@@ -416,7 +424,7 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
             } else {
                 // row modes: rows the reference's loop never reaches are zeros and touch no sample.  (Measured and rejected:
                 // fetching the samples of both frames before the first transform: slower for config 3's spectrogram.)
-                float *const g0 = MODE == kModeSpectrogram ? p.out + (size_t(b) * p.rows_total + p.row0 + ta) * K : nullptr;
+                float *const g0 = MODE == kModeSpectrogram ? p.out + (size_t(b) * p.rows_launch + ta) * K : nullptr;
 #pragma unroll 1
                 for (int f = 0; f < 2; ++f) {
                     if (f && !bvalid) break;
@@ -452,7 +460,7 @@ __global__ void __launch_bounds__(32 * solo_warps<L, R2, MODE>(), solo_min_block
                 }
                 ch = ch / (sxx == 0.f ? B200AA_EPS : sxx);
                 if (l16 < 12 && (half == 0 || bvalid))
-                    p.out[(size_t(b) * p.rows_total + p.row0 + ta + half) * 12 + l16] = (half ? b_real : a_real) ? ch : 0.f;
+                    p.out[(size_t(b) * p.rows_launch + ta + half) * 12 + l16] = (half ? b_real : a_real) ? ch : 0.f;
                 __syncwarp();
             } else {
                 float *const msraw = rowb + S::MS0, *const mslog = msraw + 2 * B200AA_N_MEL, *const mfold = mslog + 2 * B200AA_N_MEL;
@@ -506,7 +514,6 @@ inline int solo_plan_init(int window, const std::vector<int> &h_pblob, const Pai
     int L = 0, R2 = 0;
     stb->L = 0;
     if (!solo_shape_for_window(window, &L, &R2)) return B200AA_OK;
-    if (getenv("B200AA_NO_SOLO")) return B200AA_OK;
     const int Nc = L * R2, N = 2 * Nc;
     if (b200aa_host::upload(b200aa_host::twiddle_grid(R2, L, Nc), stb->tw) != cudaSuccess ||
         b200aa_host::upload(b200aa_host::twiddles(Nc / 2 + 1, N), stb->twp) != cudaSuccess ||
