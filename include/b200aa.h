@@ -42,6 +42,7 @@ typedef enum b200aa_status {
 /* sample formats of the clip buffer */
 #define B200AA_DTYPE_I16 0        /* int16 PCM as scipy.io.wavfile.read returns it (audioBasicIO.py:99) */
 #define B200AA_DTYPE_F32 1        /* float32 samples (any scale; the path is scale invariant)           */
+#define B200AA_DTYPE_F64 2        /* float64 (b200aa_knn_classify's query vectors only)                  */
 
 #define B200AA_N_BASE 34          /* ShortTermFeatures.py:580-585 */
 #define B200AA_N_MEL 40           /* ShortTermFeatures.py:191-192 */
@@ -243,6 +244,22 @@ int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const b200aa_pcm
  * Replaces: MidTermFeatures.beat_extraction (:18-84) and utilities.peakdet (:33-103). */
 int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
                            const int64_t *d_frames, double window_size, double *d_out, void *stream);
+
+/* Kernel 5: the library's kNN classifier on a matrix of query vectors (SURVEY 8f rank 4).  Training set on the device:
+ * d_feats float64 [n_train, n_feats]; d_slots int32 [n_train], the class a training row votes for (its label when that is
+ * an integer in [0, n_classes), else -1: never counted); n_classes = len(np.unique(labels)); k = the model's neighbors.
+ * d_query: [n_query] rows of n_feats float32 (B200AA_DTYPE_F32, widened exactly) or float64 (B200AA_DTYPE_F64), row q at
+ * element q * q_stride.  d_ids int64 [n_query], d_P float64 [n_query, n_classes]: row q is Knn.classify(query q) bit for
+ * bit -- distances summed in sequence in fp64 without FMA as scipy's cdist does, the k smallest (distance, training index)
+ * pairs with every NaN after +inf (all n_train of them when k >= n_train), P[c] = count / k, the id the first maximum.
+ * The reference's own argsort leaves only an exact tie at the k-th place between different classes open; there the lower
+ * training index is taken.  NULL pointers, n_train < 1 (or >= 2^31), n_feats < 1, n_classes < 1, k < 1, n_query < 0,
+ * q_stride < n_feats and another dtype are B200AA_ERR_INVALID, checked before any CUDA call; n_query = 0 does nothing.
+ * Allocates stream-ordered scratch of one 8-byte key per (query, training row), queries in slices of at most 256 MiB.
+ * Replaces: audioTrainTest.Knn.classify (:33-49) per window in classifier_wrapper (:52-93). */
+int b200aa_knn_classify(const double *d_feats, const int32_t *d_slots, int64_t n_train, int n_feats, int n_classes,
+                        int64_t k, const void *d_query, int dtype, int64_t n_query, int64_t q_stride, int64_t *d_ids,
+                        double *d_P, void *stream);
 
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the

@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get("B200AA_LIB") or os.path.join(_HERE, "libb200aa.so")  
 
 OK = 0
 ERR_INVALID, ERR_TOO_SHORT, ERR_CHROMA, ERR_MEL_RANGE, ERR_CUDA, ERR_UNSUPPORTED, ERR_NO_DEVICE = -1, -2, -3, -4, -5, -6, -7
-DTYPE_I16, DTYPE_F32 = 0, 1
+DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2
 
 _lib = None
 _lock = threading.Lock()
@@ -57,6 +57,8 @@ SIGNATURES = {
     # (d_arena, arena_bytes, h_clips, n_clips, out_dtype, d_out, n_out, out_stride, stream)
     "b200aa_decode_pcm": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_i64, c_i64, c_vp]),
     "b200aa_beat_extraction": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
+    # (d_feats, d_slots, n_train, n_feats, n_classes, k, d_query, dtype, n_query, q_stride, d_ids, d_P, stream)
+    "b200aa_knn_classify": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_i64, c_vp, c_int, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),
     "b200aa_chromagram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200aa.so")
 SOURCES = ["b200aa.cu"]
-DEPS = ["b200aa.cu", "beat.cuh", "common.cuh", "dft_codelets.cuh", "generic_kernel.cuh", "fast_kernel.cuh", "pair_kernel.cuh", "pcm.cuh", "solo_kernel.cuh", "rows.cuh", "sched.cuh", "slots.h", "tables.inl",
+DEPS = ["b200aa.cu", "beat.cuh", "common.cuh", "dft_codelets.cuh", "generic_kernel.cuh", "fast_kernel.cuh", "knn.cuh", "pair_kernel.cuh", "pcm.cuh", "solo_kernel.cuh", "rows.cuh", "sched.cuh", "slots.h", "tables.inl",
         os.path.join("..", "..", "include", "b200aa.h")]
 
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",

@@ -17,6 +17,7 @@
 #include "beat.cuh"
 #include "common.cuh"
 #include "generic_kernel.cuh"
+#include "knn.cuh"
 #include "fast_kernel.cuh"
 #include "pair_kernel.cuh"
 #include "pcm.cuh"
@@ -953,6 +954,191 @@ extern "C" int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_
         beat_finish_kernel<<<(unsigned)((ns * 32 + 255) / 256), 256, 0, st>>>(d_frames, n_frames, b0, ns, window_size, mbt, nb,
                                                                                counts, d_out);
         CK_LAUNCH("beat_finish_kernel");
+    }
+    return scratch.done(B200AA_OK);
+}
+
+// ------------------------------------------------------------------------------------------------
+// kernel 5: kNN classification (audioTrainTest.py:33-49), bit for bit the reference's Knn.classify per query (csrc/knn.cuh)
+// ------------------------------------------------------------------------------------------------
+// keys[q][i] = key_of(distance(query q, training row i)) for a 64-query x 64-row tile per CTA.  Both tiles are staged
+// 16 features at a time, transposed to [feature][row]; each thread runs 4 x 4 independent chains (queries ty + 16a,
+// rows tx + 16b), so the 136-long dependent DADD chain of one pair is hidden behind 15 others.
+template <class Tq>
+__global__ void __launch_bounds__(knn::kThreads, 3) knn_dist_kernel(const double *__restrict__ feats, int64_t N, int F,
+                                                                 const Tq *__restrict__ q, int64_t q_stride, int64_t n_slice,
+                                                                 uint64_t *__restrict__ keys)
+{
+    static_assert(knn::kQ == knn::kT && knn::kQ == 64 && knn::kThreads == 256, "tile shape");
+    __shared__ double sq[knn::kF][knn::kQ + 1];
+    __shared__ double sv[knn::kF][knn::kT + 1];
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    const int64_t t0 = int64_t(blockIdx.x) * knn::kT;
+    const int64_t q0 = int64_t(blockIdx.y) * knn::kQ;
+    double acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[a][b] = 0.0;
+    for (int f0 = 0; f0 < F; f0 += knn::kF) {
+        const int nf = min(knn::kF, F - f0);
+        __syncthreads();
+        for (int e = threadIdx.x; e < knn::kQ * knn::kF; e += knn::kThreads) {
+            const int r = e / knn::kF, j = e % knn::kF;
+            const int64_t qi = q0 + r, ti = t0 + r;
+            sq[j][r] = (j < nf && qi < n_slice) ? double(q[qi * q_stride + f0 + j]) : 0.0;      // float32: widened exactly
+            sv[j][r] = (j < nf && ti < N) ? feats[ti * F + f0 + j] : 0.0;
+        }
+        __syncthreads();
+#pragma unroll 2
+        for (int j = 0; j < nf; ++j) {
+            double x[4], v[4];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) x[a] = sq[j][ty + 16 * a];
+#pragma unroll
+            for (int b = 0; b < 4; ++b) v[b] = sv[j][tx + 16 * b];
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = 0; b < 4; ++b) acc[a][b] = knn::dist_step(acc[a][b], x[a], v[b]);
+        }
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        const int64_t qi = q0 + ty + 16 * a;
+        if (qi >= n_slice) continue;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            const int64_t ti = t0 + tx + 16 * b;
+            if (ti < N) keys[qi * N + ti] = knn::key_of(knn::dsqrt(acc[a][b]));
+        }
+    }
+}
+
+// One CTA per query: the k-th smallest key by radix select (8 passes of 256 bins over the keys sharing the prefix found so
+// far), then one pass in training-index order that selects the keys below it and the first r equal to it, counting the
+// selected entries' classes in shared memory, kVoteClasses classes per pass.  Writes P[q][0..C) and the first maximum.
+__global__ void __launch_bounds__(knn::kThreads) knn_select_kernel(const uint64_t *__restrict__ keys, int64_t N,
+                                                                   const int32_t *__restrict__ slots, int C, int64_t k,
+                                                                   int64_t q_base, int64_t *__restrict__ ids, double *__restrict__ P)
+{
+    constexpr int kWarps = knn::kThreads / 32;
+    __shared__ unsigned hist[knn::kBins];
+    __shared__ unsigned votes[knn::kVoteClasses];
+    __shared__ unsigned warp_eq[kWarps];
+    __shared__ int64_t warp_best_c[kWarps], warp_best_i[kWarps];
+    __shared__ uint64_t s_prefix;
+    __shared__ int64_t s_rank;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t q = q_base + blockIdx.x;
+    const uint64_t *row = keys + int64_t(blockIdx.x) * N;
+
+    uint64_t thr = knn::kAll;           // k >= N: every entry is selected
+    int64_t r = 0;
+    if (k < N) {
+        uint64_t prefix = 0;
+        int64_t rank = k;
+        for (int shift = 64 - knn::kDigitBits; shift >= 0; shift -= knn::kDigitBits) {
+            const uint64_t mask = knn::prefix_mask(shift);
+            for (int b = tid; b < knn::kBins; b += knn::kThreads) hist[b] = 0;
+            __syncthreads();
+            for (int64_t i = tid; i < N; i += knn::kThreads) {
+                const uint64_t key = row[i];
+                if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & (knn::kBins - 1)], 1u);
+            }
+            __syncthreads();
+            if (tid == 0) {
+                const int d = knn::select_digit(hist, rank);
+                s_prefix = prefix | (uint64_t(d) << shift);
+                s_rank = rank;
+            }
+            __syncthreads();
+            prefix = s_prefix;
+            rank = s_rank;
+        }
+        thr = prefix;
+        r = rank;
+    }
+
+    int64_t best_c = -1, best_i = 0;    // thread 0: the first maximum over the classes done so far
+    for (int c0 = 0; c0 < C; c0 += knn::kVoteClasses) {
+        const int nc = min(knn::kVoteClasses, C - c0);
+        for (int c = tid; c < knn::kVoteClasses; c += knn::kThreads) votes[c] = 0;
+        __syncthreads();
+        int64_t eq_done = 0;            // keys equal to thr at indices below this chunk
+        for (int64_t base = 0; base < N; base += knn::kThreads) {
+            const int64_t i = base + tid;
+            const uint64_t key = i < N ? row[i] : 0;
+            const bool eq = i < N && key == thr;
+            const unsigned m = __ballot_sync(0xffffffffu, eq);
+            if (lane == 0) warp_eq[warp] = __popc(m);
+            __syncthreads();
+            int64_t before = eq_done + __popc(m & ((1u << lane) - 1u)), total = 0;
+#pragma unroll
+            for (int w = 0; w < kWarps; ++w) {
+                if (w < warp) before += warp_eq[w];
+                total += warp_eq[w];
+            }
+            if (i < N && knn::selected(key, thr, before, r)) {
+                const int s = slots[i];
+                if (s >= c0 && s < c0 + nc) atomicAdd(&votes[s - c0], 1u);
+            }
+            eq_done += total;
+            __syncthreads();
+        }
+        int64_t bc = -1, bi = 0;
+        for (int c = tid; c < nc; c += knn::kThreads) {
+            P[q * C + c0 + c] = knn::vote(votes[c], k);
+            if (bc < 0 || knn::better(votes[c], c0 + c, bc, bi)) { bc = votes[c]; bi = c0 + c; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const int64_t oc = __shfl_xor_sync(0xffffffffu, bc, o), oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (oc >= 0 && (bc < 0 || knn::better(oc, oi, bc, bi))) { bc = oc; bi = oi; }
+        }
+        if (lane == 0) { warp_best_c[warp] = bc; warp_best_i[warp] = bi; }
+        __syncthreads();
+        if (tid == 0)
+            for (int w = 0; w < kWarps; ++w)
+                if (warp_best_c[w] >= 0 && (best_c < 0 || knn::better(warp_best_c[w], warp_best_i[w], best_c, best_i))) {
+                    best_c = warp_best_c[w];
+                    best_i = warp_best_i[w];
+                }
+        __syncthreads();
+    }
+    if (tid == 0) ids[q] = best_i;
+}
+
+extern "C" int b200aa_knn_classify(const double *d_feats, const int32_t *d_slots, int64_t n_train, int n_feats, int n_classes,
+                                   int64_t k, const void *d_query, int dtype, int64_t n_query, int64_t q_stride, int64_t *d_ids,
+                                   double *d_P, void *stream)
+{
+    NvtxRange nvtx_("b200aa_knn_classify");
+    if (!d_feats || !d_slots || !d_query || !d_ids || !d_P || n_train < 1 || n_train > INT32_MAX || n_feats < 1 ||
+        n_classes < 1 || k < 1 || n_query < 0 || q_stride < n_feats || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
+        return B200AA_ERR_INVALID;
+    if (n_query == 0) return B200AA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // scratch: one key per (query, training row); queries go in slices whose keys stay below 256 MiB
+    const size_t row_bytes = size_t(n_train) * sizeof(uint64_t);
+    const int64_t slice = std::max<int64_t>(1, std::min<int64_t>({n_query, int64_t((size_t(256) << 20) / row_bytes),
+                                                                   int64_t(65535) * knn::kQ}));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(size_t(slice) * row_bytes);
+    if (rc != B200AA_OK) return rc;
+    uint64_t *keys = static_cast<uint64_t *>(scratch.get());
+    for (int64_t q0 = 0; q0 < n_query; q0 += slice) {
+        const int64_t ns = std::min<int64_t>(slice, n_query - q0);
+        const dim3 grid((unsigned)((n_train + knn::kT - 1) / knn::kT), (unsigned)((ns + knn::kQ - 1) / knn::kQ));
+        if (dtype == B200AA_DTYPE_F32)
+            knn_dist_kernel<<<grid, knn::kThreads, 0, st>>>(d_feats, n_train, n_feats, static_cast<const float *>(d_query) + q0 * q_stride,
+                                                            q_stride, ns, keys);
+        else
+            knn_dist_kernel<<<grid, knn::kThreads, 0, st>>>(d_feats, n_train, n_feats, static_cast<const double *>(d_query) + q0 * q_stride,
+                                                            q_stride, ns, keys);
+        CK_LAUNCH("knn_dist_kernel");
+        knn_select_kernel<<<(unsigned)ns, knn::kThreads, 0, st>>>(keys, n_train, d_slots, n_classes, k, q0, d_ids, d_P);
+        CK_LAUNCH("knn_select_kernel");
     }
     return scratch.done(B200AA_OK);
 }
