@@ -261,6 +261,29 @@ int b200aa_knn_classify(const double *d_feats, const int32_t *d_slots, int64_t n
                         int64_t k, const void *d_query, int dtype, int64_t n_query, int64_t q_stride, int64_t *d_ids,
                         double *d_P, void *stream);
 
+/* Kernel 6: the model selection of audioTrainTest.evaluate_classifier (:576-771) for the library's kNN, every
+ * (neighbour count, train / test split) problem of it in one batch.  Device: d_X float64 [n, n_feats] (row i at
+ * i * n_feats), d_y int32 [n] each row's class index.  Host: per problem p < n_problems, its training rows
+ * h_train_idx[h_train_off[p] .. h_train_off[p + 1]) and test rows h_test_idx[h_test_off[p] .. h_test_off[p + 1]) (int32
+ * row indices, in split order; both offset arrays hold n_problems + 1 entries from 0), its k h_k[p] and the class count
+ * of its training rows h_classes[p] (len(np.unique(y_train))).  Per problem the training rows are standardised as
+ * StandardScaler().fit(X_train).transform does it (scikit-learn 1.9: sequential sums in split order, its constant-column
+ * rule), the test rows with the same mean_ / scale_, and each test row is classified as Knn(X_train, y_train, k).classify
+ * (kernel 5's contract; a training row votes for its class when that is below h_classes[p]; an exact tie at the k-th
+ * place between different classes goes to the lower position in the split).  Writes d_pred int32 [h_test_off[n_problems]],
+ * the predicted class of each test row in the same order, and d_counts int64 [n_problems, n_classes, n_classes], per
+ * problem the count of test rows of class y_test predicted as y_pred at [y_test, y_pred] (a y outside [0, n_classes) is
+ * never counted and never votes).  NULL pointers, n < 1 (or >= 2^31), n_feats < 1, n_classes < 1, n_problems < 0,
+ * offsets not from 0, an empty training or test list, an index outside [0, n), k < 1 and h_classes outside
+ * [1, n_classes] are B200AA_ERR_INVALID, checked before any CUDA call; n_problems = 0 does nothing.  The index lists
+ * are uploaded once; stream-ordered scratch holds the standardised rows and keys of the problems in slices of at most
+ * 256 MiB, a problem too large for one slice cut by its test rows.
+ * Replaces: the param / experiment loop of evaluate_classifier for classifier_name "knn" without SMOTE. */
+int b200aa_knn_cross_validate(const double *d_X, const int32_t *d_y, int64_t n, int n_feats, int n_classes,
+                              int64_t n_problems, const int64_t *h_train_off, const int32_t *h_train_idx,
+                              const int64_t *h_test_off, const int32_t *h_test_idx, const int64_t *h_k,
+                              const int32_t *h_classes, int32_t *d_pred, int64_t *d_counts, void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

@@ -59,6 +59,10 @@ SIGNATURES = {
     "b200aa_beat_extraction": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
     # (d_feats, d_slots, n_train, n_feats, n_classes, k, d_query, dtype, n_query, q_stride, d_ids, d_P, stream)
     "b200aa_knn_classify": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_i64, c_vp, c_int, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    # (d_X, d_y, n, n_feats, n_classes, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx, h_k, h_classes, d_pred,
+    #  d_counts, stream)
+    "b200aa_knn_cross_validate": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                          c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),
     "b200aa_chromagram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

@@ -1,0 +1,186 @@
+"""The kNN model selection of the reference's audioTrainTest.evaluate_classifier (audioTrainTest.py:576-771) on the GPU.
+
+For every neighbour count in `params` and each of `n_exp` experiments the reference draws a train / test split, fits a
+StandardScaler on the training rows, classifies every test row with its Knn and scores the experiment with scikit-learn.
+Here the splits are drawn up front from NumPy's global RNG in the reference's order, all (param, experiment) problems go
+to the GPU in one call (``consumers.knn_cross_validate``, kernel 6), and the per-experiment confusion counts come back.
+The reference's scores follow from those counts: its confusion_matrix is the count block restricted to the classes in
+y_test or y_pred, and its macro f1_score is the mean over those classes of 2 tp / (n_true + n_pred).  The printed table
+and the returned parameter are the reference's, text for text.
+
+Only classifier_name "knn" without SMOTE on finite float64 features runs here (``unsupported`` says why not otherwise);
+``install.install_training`` sends everything else to the reference's own function.
+"""
+import math
+
+import numpy as np
+from sklearn.model_selection import GroupShuffleSplit
+
+
+def features_to_matrix(features):
+    """(X [n, F], y [n] float64 class indices): the class matrices stacked in order (audioTrainTest.py:887-911)."""
+    X = np.vstack([np.asarray(f) for f in features])
+    y = np.concatenate([i * np.ones(len(f)) for i, f in enumerate(features)])
+    return X, y
+
+
+def unsupported(features, classifier_name, params, train_percentage=0.90, smote=False):
+    """None when evaluate_classifier runs on the GPU for these arguments, else the reason it does not."""
+    if classifier_name != "knn":
+        return "classifier %r: only 'knn' runs on the GPU" % (classifier_name,)
+    if smote:
+        return "SMOTE resamples the training rows"
+    if len(features) < 2:
+        return "fewer than two classes"
+    shapes = set()
+    for f in features:
+        a = np.asarray(f)
+        if a.ndim != 2 or a.shape[0] < 1 or a.dtype != np.float64:
+            return "every class needs a non-empty float64 [n, F] matrix"
+        if not np.isfinite(a).all():
+            return "non-finite features"
+        shapes.add(a.shape[1])
+    # StandardScaler's column sums add the rows in sequence only when a row holds more than one value (numpy sums a
+    # single contiguous column pairwise)
+    if len(shapes) != 1 or shapes.pop() < 2:
+        return "the classes need the same number (>= 2) of features"
+    for k in params:
+        if not (isinstance(k, (int, np.integer)) and k >= 1):
+            return "every kNN parameter must be an integer >= 1, got %r" % (k,)
+    if not 0 < 1 - train_percentage < 1:
+        return "train_percentage must leave a test fraction in (0, 1)"
+    return None
+
+
+def split_sizes(n, train_percentage):
+    """(n_train, n_test) of train_test_split(X, y, test_size=1 - train_percentage) on n rows."""
+    n_test = math.ceil((1 - train_percentage) * n)
+    return n - n_test, n_test
+
+
+def draw_splits(X, y, n_params, n_exp, train_percentage, list_of_ids=None):
+    """The (train, test) row indices of every (param, experiment), params outer, drawn as the reference draws them:
+    GroupShuffleSplit(n_splits=n_exp, train_size=.8) once for all params (:624-629), else one
+    train_test_split(X, y, test_size=1 - train_percentage) per (param, experiment) from NumPy's global RNG (:648-649),
+    whose ShuffleSplit takes one permutation: test = perm[:n_test], train = perm[n_test:n_test + n_train]."""
+    if list_of_ids:
+        gss = GroupShuffleSplit(n_splits=n_exp, train_size=.8)
+        fixed = [(train, test) for train, test in gss.split(X, y, list_of_ids)]
+        return fixed * n_params
+    n = X.shape[0]
+    n_train, n_test = split_sizes(n, train_percentage)
+    if n_train < 1:
+        raise ValueError("train_percentage %r leaves no training row of %d" % (train_percentage, n))
+    splits = []
+    for _ in range(n_params * n_exp):
+        perm = np.random.permutation(n)
+        splits.append((perm[n_test:n_test + n_train], perm[:n_test]))
+    return splits
+
+
+def experiment_scores(counts, all_classes):
+    """(cmt, f1t) of one experiment from its [C, C] counts, as the reference has them: confusion_matrix(y_test, y_pred)
+    over the classes present, widened back to C x C by the reference's own insertion (:690-699), and the macro F1."""
+    true, pred = counts.sum(axis=1), counts.sum(axis=0)
+    present = np.flatnonzero(true + pred)
+    cmt = counts[np.ix_(present, present)]
+    f1t = np.mean(2.0 * np.diagonal(cmt) / (1.0 * true[present] + pred[present]))
+    if cmt.size != counts.size:
+        # the reference's set iteration order decides the insertion order; keep it
+        missing = [int(c) for c in all_classes.difference(set(present.tolist()))]
+        for m in missing:
+            cmt = np.insert(cmt, m, 0, axis=0)
+        for m in missing:
+            cmt = np.insert(cmt, m, 0, axis=1)
+    return cmt, f1t
+
+
+def _print_confusion_matrix(cm, class_names):
+    if cm.shape[0] != len(class_names):
+        print("printConfusionMatrix: Wrong argument sizes\n")
+        return
+    short = [c[0:3] if len(c) > 4 else c for c in class_names]
+    print("".join("\t" + c for c in short))
+    total = np.sum(cm)
+    for i, c in enumerate(short):
+        print(c + "".join("\t{0:.2f}".format(100.0 * cm[i][j] / total) for j in range(len(class_names))))
+
+
+def report(y, class_names, params, parameter_mode, n_exp, counts):
+    """Everything evaluate_classifier prints, and its return value, from the confusion counts [len(params) * n_exp, C, C]
+    of its (param, experiment) problems (params outer)."""
+    all_classes = set(y)
+    n_classes = counts.shape[1]
+    pre_all, rec_all, f1_cls_all, ac_all, f1_all, f1_std_all, cms_all = [], [], [], [], [], [], []
+    for ci, C in enumerate(params):
+        cm = np.zeros((n_classes, n_classes))
+        f1_per_exp = []
+        for e in range(n_exp):
+            print("Param = {0:.5f} - classifier Evaluation Experiment {1:d} of {2:d}".format(C, e + 1, n_exp))
+            cmt, f1t = experiment_scores(counts[ci * n_exp + e], all_classes)
+            f1_per_exp.append(f1t)
+            cm = cm + cmt
+        cm = cm + 0.0000000010
+        rec = np.array([cm[i, i] / np.sum(cm[i, :]) for i in range(n_classes)])
+        pre = np.array([cm[i, i] / np.sum(cm[:, i]) for i in range(n_classes)])
+        f1 = 2 * rec * pre / (rec + pre)
+        pre_all.append(pre)
+        rec_all.append(rec)
+        f1_cls_all.append(f1)
+        ac_all.append(np.sum(np.diagonal(cm)) / np.sum(cm))
+        cms_all.append(cm)
+        f1_all.append(np.mean(f1))
+        f1_std_all.append(np.std(f1_per_exp))
+
+    names = ["{0:s}\t\t\t".format(c) for c in class_names[:-1]] + ["{0:s}\t\t".format(c) for c in class_names[-1:]]
+    print("\t\t" + "".join(names) + "OVERALL")
+    print("\tC" + "\tPRE\tREC\tf1" * len(class_names) + "\t{0:s}\t{1:s}".format("ACC", "f1"))
+    best_ac, best_f1 = np.argmax(ac_all), np.argmax(f1_all)
+    for i in range(len(pre_all)):
+        line = "\t{0:.3f}".format(params[i])
+        for c in range(len(pre_all[i])):
+            line += "\t{0:.1f}\t{1:.1f}\t{2:.1f}".format(100.0 * pre_all[i][c], 100.0 * rec_all[i][c], 100.0 * f1_cls_all[i][c])
+        line += "\t{0:.1f}\t{1:.1f}".format(100.0 * ac_all[i], 100.0 * f1_all[i])
+        line += "\t best f1" if i == best_f1 else ""
+        line += "\t best Acc" if i == best_ac else ""
+        print(line)
+    if parameter_mode == 0:
+        print("Confusion Matrix:")
+        _print_confusion_matrix(cms_all[best_ac], class_names)
+        return params[best_ac]
+    if parameter_mode == 1:
+        print("Confusion Matrix:")
+        _print_confusion_matrix(cms_all[best_f1], class_names)
+        print(f"Best macro f1 {100 * f1_all[best_f1]:.1f}")
+        print(f"Best macro f1 std {100 * f1_std_all[best_f1]:.1f}")
+        return params[best_f1]
+    return None
+
+
+def evaluate_classifier(features, class_names, classifier_name, params, parameter_mode, list_of_ids=None, n_exp=-1,
+                        train_percentage=0.90, smote=False):
+    """audioTrainTest.evaluate_classifier (:576-771) for classifier_name "knn": the same prints and return value, every
+    (param, experiment) problem classified on the GPU in one call.  Raises ValueError for arguments it does not cover
+    (``unsupported``); there is no CPU path."""
+    from .consumers import knn_cross_validate
+    why = unsupported(features, classifier_name, params, train_percentage, smote)
+    if why is not None:
+        raise ValueError("evaluate_classifier on the GPU: " + why)
+    X, y = features_to_matrix(features)
+    if n_exp == -1:
+        n_exp = int(50000 / X.shape[0]) + 1
+    splits = draw_splits(X, y, len(params), n_exp, train_percentage, list_of_ids)
+    ks = [int(C) for C in params for _ in range(n_exp)]
+    _, counts = knn_cross_validate(X, y, splits, ks, n_classes=len(features))
+    return report(y, class_names, params, parameter_mode, n_exp, counts.cpu().numpy())
+
+
+def dispatcher(original):
+    """An evaluate_classifier that runs the arguments the GPU covers here and hands the rest to `original`."""
+    def evaluate_classifier_dispatch(features, class_names, classifier_name, params, parameter_mode, list_of_ids=None,
+                                     n_exp=-1, train_percentage=0.90, smote=False):
+        run = evaluate_classifier if unsupported(features, classifier_name, params, train_percentage, smote) is None else original
+        return run(features, class_names, classifier_name, params, parameter_mode, list_of_ids=list_of_ids, n_exp=n_exp,
+                   train_percentage=train_percentage, smote=smote)
+    evaluate_classifier_dispatch.original = original
+    return evaluate_classifier_dispatch

@@ -116,6 +116,52 @@ def knn_classify_batch(model, vectors):
     return ids, P
 
 
+def knn_cross_validate(X, y, splits, ks, n_classes=None):
+    """Knn(X_train, y_train, k).classify of every test row of every (train, test) split, each split's rows standardised by
+    its own StandardScaler fit (audioTrainTest.evaluate_classifier, :631-699), as one batch on the GPU
+    (``b200aa_knn_cross_validate``, DESIGN.md kernel 6).
+
+    X: float64 [n, F] (a CUDA tensor, or host data uploaded to the current device); y: the n class indices in
+    [0, n_classes); splits: (train row indices, test row indices) per problem, in split order; ks: the k of each problem.
+    Returns CUDA (pred int32 [sum of the test counts], the predicted class of each test row, problem after problem;
+    counts int64 [P, n_classes, n_classes], counts[p, y_test, y_pred])."""
+    if not isinstance(X, torch.Tensor):
+        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, F]")
+    X = X.contiguous()
+    n = X.shape[0]
+    y = np.asarray(y.cpu() if isinstance(y, torch.Tensor) else y)
+    if y.shape != (n,) or not np.array_equal(y, np.floor(y)) or (n and y.min() < 0):
+        raise ValueError("y must hold one class index >= 0 per row of X")
+    y = y.astype(np.int64)
+    n_classes = int(y.max()) + 1 if n_classes is None else int(n_classes)
+    if len(splits) != len(ks):
+        raise ValueError("one k per split: %d splits, %d ks" % (len(splits), len(ks)))
+    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
+    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
+    train_off = np.concatenate([[0], np.cumsum([t.size for t in train])]).astype(np.int64)
+    test_off = np.concatenate([[0], np.cumsum([t.size for t in test])]).astype(np.int64)
+    train_idx = np.ascontiguousarray(np.concatenate(train) if train else np.zeros(0), dtype=np.int32)
+    test_idx = np.ascontiguousarray(np.concatenate(test) if test else np.zeros(0), dtype=np.int32)
+    k = np.ascontiguousarray(ks, dtype=np.int64)
+    # Knn.classify's class count: len(np.unique(y_train)) of the split
+    classes = np.array([np.unique(y[t[(t >= 0) & (t < n)]]).size for t in train], dtype=np.int32)
+    with torch.cuda.device(X.device):
+        d_y = torch.from_numpy(y.astype(np.int32)).to(X.device)
+        pred = torch.empty(int(test_off[-1]), dtype=torch.int32, device=X.device)
+        counts = torch.empty((len(splits), n_classes, n_classes), dtype=torch.int64, device=X.device)
+
+        def ptr(a):
+            return ctypes.c_void_p(a.ctypes.data)
+        check(lib().b200aa_knn_cross_validate(
+            ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(d_y.data_ptr()), n, X.shape[1], n_classes, len(splits),
+            ptr(train_off), ptr(train_idx), ptr(test_off), ptr(test_idx), ptr(k), ptr(classes),
+            ctypes.c_void_p(pred.data_ptr()), ctypes.c_void_p(counts.data_ptr()), _stream()))
+    return pred, counts
+
+
 def classify_vectors(classifier, model_type, vectors):
     """classifier_wrapper (audioTrainTest.py:52-93) over the rows of `vectors` [n x F]: (class ids [n], probabilities [n x classes]).
     A CUDA tensor goes to the kNN kernel (``knn_classify_batch``; `classifier` a KnnModel or a Knn-like object) and only the

@@ -32,6 +32,17 @@ constexpr int kVoteClasses = 1024;      // classes counted per pass of the vote 
 constexpr uint64_t kNanKey = 0x7ff8000000000000ull;
 constexpr uint64_t kAll = ~0ull;        // threshold key above every key: all N entries selected (k >= N)
 
+// One problem of a launch of the distance and select kernels (kernel 5 runs one, kernel 6 a batch): training rows
+// [train0, train0 + N) of the training matrix (and of its slots), queries [q0, q0 + n_q) of the query matrix, keys
+// [key0, key0 + n_q * N), results at [out0, out0 + n_q).  Kernel 6 also reads src_train / src_test, the first entries of
+// the problem's training / test row indices, and id, its [C, C] count block.
+struct Problem {
+    int64_t train0, N, q0, n_q, key0, out0, k;
+    int64_t src_train, src_test;
+    int32_t C;                          // classes voted for
+    int32_t id;
+};
+
 __host__ __device__ inline double dsqrt(double a)
 {
 #ifdef __CUDA_ARCH__

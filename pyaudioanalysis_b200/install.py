@@ -28,6 +28,20 @@ def install(pyaudioanalysis_pkg=None):
     return done
 
 
+def install_training(audio_train_test=None):
+    """Rebind an importable ``pyAudioAnalysis.audioTrainTest`` (or the module given) so that its evaluate_classifier runs
+    the kNN model selection on the GPU (``audioTrainTest.evaluate_classifier`` here) and every other classifier, SMOTE
+    and non-finite input through the saved original.  extract_features_and_train looks the function up on the module at
+    call time (audioTrainTest.py:309), so it trains kNN models through the GPU unchanged.  Returns the attribute rebound."""
+    from .audioTrainTest import dispatcher
+    if audio_train_test is None:
+        import importlib
+        audio_train_test = importlib.import_module("pyAudioAnalysis.audioTrainTest")
+    original = _saved.setdefault((audio_train_test, "evaluate_classifier"), audio_train_test.evaluate_classifier)
+    audio_train_test.evaluate_classifier = dispatcher(original)
+    return ["%s.evaluate_classifier" % audio_train_test.__name__]
+
+
 def uninstall():
     for (mod, n), fn in list(_saved.items()):
         setattr(mod, n, fn)
