@@ -284,6 +284,35 @@ int b200aa_knn_cross_validate(const double *d_X, const int32_t *d_y, int64_t n, 
                               const int64_t *h_test_off, const int32_t *h_test_idx, const int64_t *h_k,
                               const int32_t *h_classes, int32_t *d_pred, int64_t *d_counts, void *stream);
 
+/* Kernel 7 (csrc/hmm.cuh): HMM segmentation with the library's diagonal-Gaussian HMMs (audioSegmentation.py:287-344,
+ * :471-492).
+ *
+ * b200aa_hmm_statistics: the means and standard deviations of train_hmm_compute_statistics.  d_mid is a
+ * [n_clips, n_feats, m_stride] batch of float32 (B200AA_DTYPE_F32, widened exactly) or float64 (B200AA_DTYPE_F64); clip b
+ * contributes its first h_n_windows[b] columns (0 .. m_stride) to one concatenated sequence of windows.  Class c's windows
+ * are h_idx[h_class_off[c] .. h_class_off[c + 1]), indices into that sequence in the order NumPy meets them.  Writes d_out
+ * [4, n_classes, n_feats] float64: per (class, feature) the sum, the mean (sum / n), the sum of squared deviations and the
+ * population std, bit for bit NumPy's mean / std of features[:, idx] (a sequential sum over the windows, pairwise for
+ * n_feats == 1).  A class of no windows gives NaN.  NULL pointers, n_clips / n_feats / m_stride / n_classes < 1, a count
+ * outside [0, m_stride], offsets not from 0 or decreasing and an index outside [0, sum of the counts) are
+ * B200AA_ERR_INVALID, checked before any CUDA call.
+ *
+ * b200aa_hmm_decode: GaussianHMM(C, "diag").predict of each clip's windows (hmmlearn's Viterbi; ties: the last state is the
+ * first maximum, every backtrack step the last maximal predecessor).  d_mid [n_clips, n_feats, m_stride] float32, clip b's
+ * first h_n_windows[b] (1 .. m_stride) columns.  The model, on the device, from the host: d_log_start [C] = log pi,
+ * d_log_trans [C, C] = log A (-inf for a zero probability), d_means [C, n_feats], d_vars [C, n_feats] the diagonal
+ * covariances (> 0), d_const [C] = n_feats log 2pi + sum_f log var.  Writes d_ids int32 [n_clips, m_stride], each clip's
+ * states and zeros past its count, and d_bad int32 [n_clips]: 1 for a clip with a non-finite feature, whose ids are not
+ * written.  C = n_states in [1, 2048].  NULL pointers, counts below 1 and a count above m_stride are B200AA_ERR_INVALID,
+ * checked before any CUDA call.  Stream-ordered scratch holds the emissions and backpointers of the clips in slices of at
+ * most 256 MiB (a clip larger than that on its own takes a slice of its own). */
+int b200aa_hmm_statistics(const void *d_mid, int dtype, int64_t n_clips, int n_feats, int64_t m_stride,
+                          const int64_t *h_n_windows, int n_classes, const int64_t *h_class_off, const int64_t *h_idx,
+                          double *d_out, void *stream);
+int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, const int64_t *h_n_windows,
+                      int n_states, const double *d_log_start, const double *d_log_trans, const double *d_means,
+                      const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

@@ -63,6 +63,11 @@ SIGNATURES = {
     #  d_counts, stream)
     "b200aa_knn_cross_validate": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                           c_vp]),
+    # (d_mid, dtype, n_clips, n_feats, m_stride, h_n_windows, n_classes, h_class_off, h_idx, d_out, stream)
+    "b200aa_hmm_statistics": (c_int, [c_vp, c_int, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    # (d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars, d_const, d_ids,
+    #  d_bad, stream)
+    "b200aa_hmm_decode": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),
     "b200aa_chromagram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

@@ -9,8 +9,9 @@ The reference walks the mid-term (or short-term) matrix one column at a time:
 Here all columns are normalised and transposed in ONE kernel (``b200aa_normalize_windows``: [F x M] -> [M x F] feature
 vectors) and the classifier sees the whole matrix at once (scikit-learn's ``predict`` / ``predict_proba`` are row-wise, the
 library's kNN runs as one kernel over a CUDA matrix of test vectors, ``b200aa_knn_classify``, and is restated below for a
-NumPy one), so the results are the loop's results.  The classifiers themselves (training, model files, HMMs) stay out of
-scope; any object with the reference's interface works.
+NumPy one), so the results are the loop's results.  The classifiers themselves (training, model files) stay out of scope; any
+object with the reference's interface works.  The library's HMMs decode a whole ragged batch in one launch pair
+(``hmm_decode_batch``, ``b200aa_hmm_decode``) and train from ``hmm_statistics_batch`` (audioSegmentation.py here).
 """
 import ctypes
 
@@ -160,6 +161,127 @@ def knn_cross_validate(X, y, splits, ks, n_classes=None):
             ptr(train_off), ptr(train_idx), ptr(test_off), ptr(test_idx), ptr(k), ptr(classes),
             ctypes.c_void_p(pred.data_ptr()), ctypes.c_void_p(counts.data_ptr()), _stream()))
     return pred, counts
+
+
+def hmm_model_arrays(hmm):
+    """(startprob [C], transmat [C, C], means [C, F], diagonal covariances [C, F]) of a diagonal GaussianHMM: hmmlearn's
+    object (whose covars_ property expands the diagonal into full matrices; the stored diagonal is _covars_) or anything
+    with its attribute names."""
+    if getattr(hmm, "covariance_type", "diag") != "diag":
+        raise ValueError("only diagonal-covariance HMMs are supported, got covariance_type %r" % (hmm.covariance_type,))
+    cov = getattr(hmm, "_covars_", None)
+    if cov is None:
+        cov = hmm.covars_
+    return (np.asarray(hmm.startprob_, dtype=np.float64), np.asarray(hmm.transmat_, dtype=np.float64),
+            np.asarray(hmm.means_, dtype=np.float64), np.asarray(cov, dtype=np.float64))
+
+
+def hmm_check(start, trans, means, cov):
+    """hmmlearn's model checks before a decode, with its ValueError texts."""
+    C = start.shape[0] if start.ndim == 1 else -1
+    if C < 1:
+        raise ValueError("startprob_ must have shape (n_components,)")
+    if not np.allclose(start.sum(), 1.0):
+        raise ValueError("startprob_ must sum to 1 (got {:.4f})".format(start.sum()))
+    if trans.shape != (C, C):
+        raise ValueError("transmat_ must have shape (n_components, n_components)")
+    if not np.allclose(trans.sum(axis=1), 1.0):
+        raise ValueError("rows of transmat_ must sum to 1 (got {})".format(trans.sum(axis=1)))
+    if means.ndim != 2 or means.shape[0] != C or means.shape[1] < 1:
+        raise ValueError("means_ must have shape (n_components, n_features)")
+    if cov.shape != means.shape:
+        raise ValueError("'diag' covars must have shape (n_components, n_dim)")
+    if np.any(cov <= 0):
+        raise ValueError("'diag' covars must be positive")
+
+
+class HmmModel:
+    """A diagonal GaussianHMM (hmmlearn's, or a look-alike: ``hmm_model_arrays``) checked as hmmlearn checks it before a
+    decode and uploaded once to one CUDA device for ``hmm_decode_batch``.  The logarithms are taken here, with NumPy, as
+    hmmlearn takes them: log pi and log A (-inf for a zero probability), and per state F log 2pi + sum_f log var with
+    var = max(covars, tiny)."""
+
+    def __init__(self, hmm, device=None):
+        start, trans, means, cov = hmm_model_arrays(hmm)
+        hmm_check(start, trans, means, cov)
+        self.n_states, self.n_feats = means.shape
+        var = np.maximum(cov, np.finfo(float).tiny)
+        with np.errstate(divide="ignore"):
+            log_start, log_trans = np.log(start), np.log(trans)
+        const = self.n_feats * np.log(2 * np.pi) + np.log(var).sum(axis=-1)
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != "cuda":
+            raise TypeError("an HmmModel lives on a CUDA device (there is no CPU fallback)")
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+
+        def up(a):
+            return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(self.device)
+        self.log_start, self.log_trans, self.means, self.vars, self.const = (up(a) for a in (log_start, log_trans, means, var,
+                                                                                          const))
+
+
+def _host_counts(n_windows, B, M, lo):
+    if n_windows is None:
+        return np.full(B, M, dtype=np.int64)
+    n = np.ascontiguousarray(n_windows.cpu().numpy() if isinstance(n_windows, torch.Tensor) else n_windows, dtype=np.int64)
+    if n.shape != (B,) or (B and (n.min() < lo or n.max() > M)):
+        raise ValueError("n_windows must hold one count in [%d, %d] per clip" % (lo, M))
+    return n
+
+
+def hmm_decode_batch(mid, model, n_windows=None):
+    """GaussianHMM.predict (hmmlearn's Viterbi) of the windows of every clip of a CUDA float32 [B, F, M] mid-term batch, in
+    one launch pair on the current stream (DESIGN.md, kernel 7).  ``n_windows``: each clip's window count (>= 1), host
+    integers or a CUDA tensor; None: all M.  Returns CUDA (ids int32 [B, M], each clip's states and zeros past its count;
+    bad bool [B], True for a clip with a non-finite feature, whose ids are left unwritten -- hmmlearn raises ValueError
+    for it).  `model`: an HmmModel, or an HMM uploaded for this call."""
+    _require_cuda(mid, "mid")
+    if mid.dim() != 3 or mid.dtype != torch.float32 or not mid.is_contiguous():
+        raise ValueError("mid must be contiguous float32 [B, F, M]")
+    if not isinstance(model, HmmModel):
+        model = HmmModel(model, mid.device)
+    B, F, M = mid.shape
+    if F != model.n_feats:
+        raise ValueError("mid has %d features, the model %d" % (F, model.n_feats))
+    if mid.device != model.device:
+        raise ValueError("mid is on %s, the model on %s" % (mid.device, model.device))
+    counts = _host_counts(n_windows, B, M, 1)
+    with torch.cuda.device(mid.device):
+        ids = torch.zeros((B, M), dtype=torch.int32, device=mid.device)
+        bad = torch.zeros((B,), dtype=torch.int32, device=mid.device)
+        if B:
+            check(lib().b200aa_hmm_decode(
+                ctypes.c_void_p(mid.data_ptr()), B, F, M, ctypes.c_void_p(counts.ctypes.data), model.n_states,
+                ctypes.c_void_p(model.log_start.data_ptr()), ctypes.c_void_p(model.log_trans.data_ptr()),
+                ctypes.c_void_p(model.means.data_ptr()), ctypes.c_void_p(model.vars.data_ptr()),
+                ctypes.c_void_p(model.const.data_ptr()), ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(bad.data_ptr()),
+                _stream()))
+    return ids, bad.bool()
+
+
+def hmm_statistics_batch(mid, class_windows, n_windows=None):
+    """The means and standard deviations of train_hmm_compute_statistics (audioSegmentation.py:328-342) on the GPU.
+
+    mid: a CUDA float32 / float64 [B, F, M] batch whose clips' first n_windows[b] columns (None: all M) form one
+    concatenated sequence of windows; class_windows: per class the indices of its windows in that sequence, in order.
+    Returns CUDA float64 [4, C, F]: per (class, feature) the sum, mean, sum of squared deviations and population std,
+    bit for bit NumPy's features[:, idx].mean(axis=1) / np.std(features[:, idx], axis=1) (DESIGN.md, kernel 7)."""
+    _require_cuda(mid, "mid")
+    if mid.dim() != 3 or mid.dtype not in (torch.float32, torch.float64) or not mid.is_contiguous():
+        raise ValueError("mid must be contiguous float32 / float64 [B, F, M]")
+    B, F, M = mid.shape
+    counts = _host_counts(n_windows, B, M, 0)
+    lists = [np.asarray(w, dtype=np.int64).ravel() for w in class_windows]
+    off = np.concatenate([[0], np.cumsum([w.size for w in lists])]).astype(np.int64)
+    idx = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0), dtype=np.int64)
+    with torch.cuda.device(mid.device):
+        out = torch.empty((4, len(lists), F), dtype=torch.float64, device=mid.device)
+        check(lib().b200aa_hmm_statistics(
+            ctypes.c_void_p(mid.data_ptr()), DTYPE_F32 if mid.dtype == torch.float32 else DTYPE_F64, B, F, M,
+            ctypes.c_void_p(counts.ctypes.data), len(lists), ctypes.c_void_p(off.ctypes.data),
+            ctypes.c_void_p(idx.ctypes.data), ctypes.c_void_p(out.data_ptr()), _stream()))
+    return out
 
 
 def classify_vectors(classifier, model_type, vectors):

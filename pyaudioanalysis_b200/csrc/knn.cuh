@@ -5,8 +5,8 @@
 //   votes     P[c] = count(slot == c among the selected) / k, the id the first maximum (np.argmax).
 // The pieces the result depends on are __host__ __device__: tests/knn_host.cu runs them on the CPU.
 //
-// Every double operation goes through the correctly rounded intrinsics on the device (beat.cuh's dadd / dsub / dmul / ddiv
-// and dsqrt below): nvcc would otherwise contract (x - v) * (x - v) + s into a DFMA, which cdist does not.
+// Every double operation goes through the correctly rounded intrinsics on the device (npsum.cuh's dadd / dsub / dmul / ddiv
+// / dsqrt): nvcc would otherwise contract (x - v) * (x - v) + s into a DFMA, which cdist does not.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -21,6 +21,7 @@ using beat::dadd;
 using beat::ddiv;
 using beat::dmul;
 using beat::dsub;
+using npy::dsqrt;
 
 constexpr int kQ = 64;                  // queries per CTA tile of the distance kernel
 constexpr int kT = 64;                  // training rows per CTA tile
@@ -42,15 +43,6 @@ struct Problem {
     int32_t C;                          // classes voted for
     int32_t id;
 };
-
-__host__ __device__ inline double dsqrt(double a)
-{
-#ifdef __CUDA_ARCH__
-    return __dsqrt_rn(a);
-#else
-    return std::sqrt(a);
-#endif
-}
 
 // one term of the chain: s + (x - v)^2
 __host__ __device__ inline double dist_step(double s, double x, double v)

@@ -42,6 +42,26 @@ def install_training(audio_train_test=None):
     return ["%s.evaluate_classifier" % audio_train_test.__name__]
 
 
+def install_segmentation(audio_segmentation=None):
+    """Rebind an importable ``pyAudioAnalysis.audioSegmentation`` (or the module given) to the HMM segmentation here
+    (``audioSegmentation``: training statistics and decode on the GPU, no hmmlearn needed at run time): the two
+    trainers, hmm_segmentation, train_hmm_compute_statistics, and evaluate_segmentation_classification_dir through a
+    dispatcher that sends the classifier methods to the saved original.  Returns the attributes rebound."""
+    from . import audioSegmentation as ours
+    if audio_segmentation is None:
+        import importlib
+        audio_segmentation = importlib.import_module("pyAudioAnalysis.audioSegmentation")
+    done = []
+    for n in ("train_hmm_compute_statistics", "train_hmm_from_file", "train_hmm_from_directory", "hmm_segmentation"):
+        _saved.setdefault((audio_segmentation, n), getattr(audio_segmentation, n))
+        setattr(audio_segmentation, n, getattr(ours, n))
+        done.append("%s.%s" % (audio_segmentation.__name__, n))
+    n = "evaluate_segmentation_classification_dir"
+    original = _saved.setdefault((audio_segmentation, n), getattr(audio_segmentation, n))
+    setattr(audio_segmentation, n, ours.dispatcher(original))
+    return done + ["%s.%s" % (audio_segmentation.__name__, n)]
+
+
 def uninstall():
     for (mod, n), fn in list(_saved.items()):
         setattr(mod, n, fn)
