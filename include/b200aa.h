@@ -313,6 +313,43 @@ int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feats, int64_t 
                       int n_states, const double *d_log_start, const double *d_log_trans, const double *d_means,
                       const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream);
 
+/* Kernel 8 (csrc/trees.cuh): the tree classifiers of extract_features_and_train (audioTrainTest.py:52-93), bit for bit
+ * scikit-learn 1.9's predict / predict_proba of RandomForestClassifier, ExtraTreesClassifier (mode 0, forest mean) and
+ * GradientBoostingClassifier (mode 1, boosting sum).
+ *
+ * b200aa_trees_create: validates an ensemble on the host and uploads it once to the current device.  h_nodes [n_nodes]:
+ * tree t is nodes [h_roots[t], h_roots[t + 1]) (the last up to n_nodes), h_roots[0] = 0.  An internal node has left / right
+ * indices into h_nodes, both after the node and inside its tree, a feature in [0, n_feats) (bit 31 set: a NaN goes left)
+ * and a float32 threshold, scikit-learn's rounded toward -inf; a leaf has left < 0 and right = its row of h_values, in
+ * [0, n_leaves).  Mode 0: h_values [n_leaves, n_classes], every tree votes for every class, P = the per-class sum over the
+ * trees in order divided by n_trees, h_init ignored (the sums start at 0).  Mode 1: h_values [n_leaves], the learning rate
+ * already applied; tree t adds to class t mod K (K = n_classes) starting from h_init [K].  allow_nan: NaN queries are
+ * walked (else the row is flagged).  Anything else is B200AA_ERR_INVALID, before any CUDA call; a row of more shared
+ * memory than kernel 8 takes is B200AA_ERR_UNSUPPORTED.  Create returns once the model is on the device, so any stream
+ * may use it at once; the model is read-only: any number of streams and threads may classify with it at once.
+ * b200aa_trees_destroy waits for the device's queued work before it frees the model.
+ *
+ * b200aa_trees_classify: d_query [n_query, q_stride], float32 or float64 (B200AA_DTYPE_F32 / F64), n_feats columns
+ * read per row, cast to float32 as scikit-learn casts.  Writes d_ids int64 [n_query] (class index: the first maximum
+ * of the scores, or raw >= 0 for K = 1), d_scores float64 [n_query, n_classes] (P in mode 0, the raw scores in mode 1) and
+ * d_bad int32 [n_query]: 1 for a row scikit-learn refuses (a value that is or becomes +-inf as float32, or NaN unless
+ * allowed), whose other outputs are meaningless.  NULL pointers, n_query < 0, n_feats other than the model's, q_stride <
+ * n_feats, an unknown dtype are B200AA_ERR_INVALID before any CUDA call; a model of another device too.  n_query = 0 does
+ * nothing.  No scratch: every row's work stays in its warp.
+ *
+ * Replaces: classifier.predict / predict_proba in classifier_wrapper for the three tree model types. */
+typedef struct b200aa_tree_node {
+    int32_t left, right, feature;
+    float threshold;
+} b200aa_tree_node;
+typedef struct b200aa_trees b200aa_trees;
+int b200aa_trees_create(b200aa_trees **out, const b200aa_tree_node *h_nodes, int64_t n_nodes, const int32_t *h_roots,
+                        int n_trees, const double *h_values, int64_t n_leaves, int n_classes, int n_feats, int mode,
+                        const double *h_init, int allow_nan);
+int b200aa_trees_classify(const b200aa_trees *model, const void *d_query, int dtype, int64_t n_query, int n_feats,
+                          int64_t q_stride, int64_t *d_ids, double *d_scores, int32_t *d_bad, void *stream);
+int b200aa_trees_destroy(b200aa_trees *model);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

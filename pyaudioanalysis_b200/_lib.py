@@ -68,6 +68,12 @@ SIGNATURES = {
     # (d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars, d_const, d_ids,
     #  d_bad, stream)
     "b200aa_hmm_decode": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (out, h_nodes, n_nodes, h_roots, n_trees, h_values, n_leaves, n_classes, n_feats, mode, h_init, allow_nan)
+    "b200aa_trees_create": (c_int, [ctypes.POINTER(c_vp), c_vp, c_i64, c_vp, c_int, c_vp, c_i64, c_int, c_int, c_int, c_vp,
+                                    c_int]),
+    # (model, d_query, dtype, n_query, n_feats, q_stride, d_ids, d_scores, d_bad, stream)
+    "b200aa_trees_classify": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "b200aa_trees_destroy": (c_int, [c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),
     "b200aa_chromagram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

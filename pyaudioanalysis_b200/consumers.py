@@ -11,14 +11,16 @@ vectors) and the classifier sees the whole matrix at once (scikit-learn's ``pred
 library's kNN runs as one kernel over a CUDA matrix of test vectors, ``b200aa_knn_classify``, and is restated below for a
 NumPy one), so the results are the loop's results.  The classifiers themselves (training, model files) stay out of scope; any
 object with the reference's interface works.  The library's HMMs decode a whole ragged batch in one launch pair
-(``hmm_decode_batch``, ``b200aa_hmm_decode``) and train from ``hmm_statistics_batch`` (audioSegmentation.py here).
+(``hmm_decode_batch``, ``b200aa_hmm_decode``) and train from ``hmm_statistics_batch`` (audioSegmentation.py here).  The
+random forest, extra trees and gradient boosting classifiers run as one kernel over a CUDA matrix (``tree_classify_batch``,
+``b200aa_trees_classify``), bit for bit scikit-learn's predict / predict_proba.
 """
 import ctypes
 
 import numpy as np
 import torch
 
-from ._lib import DTYPE_F32, DTYPE_F64, check, lib
+from ._lib import DTYPE_F32, DTYPE_F64, ERR_UNSUPPORTED, check, lib
 from .batch import _require_cuda, _stream, beat_extraction_batch, long_term_mean_batch, mid_feature_extraction_batch
 
 _SKLEARN_TYPES = ("svm", "randomforest", "gradientboosting", "extratrees", "svm_rbf")
@@ -284,15 +286,175 @@ def hmm_statistics_batch(mid, class_windows, n_windows=None):
     return out
 
 
+TREE_FOREST, TREE_BOOST = 0, 1
+_TREE_TYPES = ("randomforest", "extratrees", "gradientboosting")
+
+
+def _threshold_down(t):
+    """Each float64 threshold rounded toward -inf to float32: for float32 x, x <= t exactly when x <= the result."""
+    with np.errstate(over="ignore"):
+        f = t.astype(np.float32)
+    below = f.astype(np.float64) > t
+    f[below] = np.nextafter(f[below], np.float32(-np.inf))
+    return f
+
+
+def flatten_tree_ensemble(model):
+    """The arrays kernel 8 walks (include/b200aa.h, b200aa_trees_create) of a fitted RandomForestClassifier,
+    ExtraTreesClassifier or GradientBoostingClassifier, in NumPy: a dict of nodes int32 [n_nodes, 4] (left, right, feature
+    with bit 31 set where a NaN goes left, float32 threshold bits; a leaf has left -1 and right its row of values), roots
+    int32 [n_trees], values float64 ([n_leaves, C] class fractions for a forest; [n_leaves] learning rate x leaf value for
+    boosting), mode, n_classes (C, or K raw scores for boosting), n_feats, init (boosting's constant raw start) and
+    allow_nan.  Raises ValueError for anything else: regressors, multi-output forests, a boosting init that is not
+    constant per row."""
+    from sklearn.dummy import DummyClassifier
+    from sklearn.ensemble import ExtraTreesClassifier, GradientBoostingClassifier, RandomForestClassifier
+
+    if isinstance(model, (RandomForestClassifier, ExtraTreesClassifier)):
+        if not hasattr(model, "estimators_"):
+            raise ValueError("the forest is not fitted")
+        if model.n_outputs_ != 1:
+            raise ValueError("multi-output forests are not supported (n_outputs_ = %d)" % model.n_outputs_)
+        mode, C, scale = TREE_FOREST, int(model.n_classes_), None
+        trees = [e.tree_ for e in model.estimators_]
+        init = None
+        allow_nan = bool(model.estimators_[0]._support_missing_values(np.zeros((1, model.n_features_in_), np.float32)))
+    elif isinstance(model, GradientBoostingClassifier):
+        if not hasattr(model, "estimators_"):
+            raise ValueError("the model is not fitted")
+        init_ = model.init_
+        if not (isinstance(init_, str) and init_ == "zero") and not (
+                isinstance(init_, DummyClassifier) and init_.strategy == "prior"):
+            raise ValueError("only a 'zero' or DummyClassifier(strategy='prior') init is supported, got %r" % (init_,))
+        mode, C, scale = TREE_BOOST, int(model.estimators_.shape[1]), float(model.learning_rate)
+        trees = [e.tree_ for e in model.estimators_.ravel()]       # stage-major: tree s * K + k adds to raw score k
+        init = np.ascontiguousarray(model._raw_predict_init(np.zeros((1, model.n_features_in_), np.float32))[0],
+                                    dtype=np.float64)
+        allow_nan = False
+    else:
+        raise ValueError("tree inference supports RandomForestClassifier, ExtraTreesClassifier and "
+                         "GradientBoostingClassifier, got %s" % type(model).__name__)
+    nodes, values, roots = [], [], []
+    base = leaf_base = 0
+    for tr in trees:
+        left = tr.children_left.astype(np.int64)
+        leaf = left < 0
+        n_leaf = int(leaf.sum())
+        nd = np.zeros((tr.node_count, 4), dtype=np.int32)
+        leaf_row = np.cumsum(leaf) - 1 + leaf_base
+        nd[:, 0] = np.where(leaf, -1, left + base)
+        nd[:, 1] = np.where(leaf, leaf_row, tr.children_right.astype(np.int64) + base)
+        feat = np.where(leaf, 0, tr.feature).astype(np.int64)
+        missing = np.asarray(tr.missing_go_to_left, dtype=bool) & ~leaf
+        nd[:, 2] = (feat | np.where(missing, 1 << 31, 0)).astype(np.uint32).view(np.int32)
+        nd[:, 3] = np.where(leaf, np.float32(0), _threshold_down(tr.threshold)).astype(np.float32).view(np.int32)
+        v = tr.value[leaf, 0, :]
+        values.append(v[:, :C] if mode == TREE_FOREST else scale * v[:, 0])
+        nodes.append(nd)
+        roots.append(base)
+        base += tr.node_count
+        leaf_base += n_leaf
+    return {"nodes": np.ascontiguousarray(np.concatenate(nodes)), "roots": np.asarray(roots, dtype=np.int32),
+            "values": np.ascontiguousarray(np.concatenate(values), dtype=np.float64), "mode": mode, "n_classes": C,
+            "n_feats": int(model.n_features_in_), "init": init, "allow_nan": allow_nan}
+
+
+class TreeEnsembleModel:
+    """A fitted RandomForestClassifier, ExtraTreesClassifier or GradientBoostingClassifier (``flatten_tree_ensemble``)
+    uploaded once to one CUDA device for ``tree_classify_batch`` (kernel 8).  Raises ValueError for a model it cannot
+    reproduce bit for bit."""
+
+    def __init__(self, model, device=None):
+        flat = flatten_tree_ensemble(model)
+        self.estimator = model
+        self.classes = np.asarray(model.classes_)
+        self.mode, self.n_classes, self.n_feats = flat["mode"], flat["n_classes"], flat["n_feats"]
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != "cuda":
+            raise TypeError("a TreeEnsembleModel lives on a CUDA device (there is no CPU fallback)")
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        nodes, roots, values, init = flat["nodes"], flat["roots"], flat["values"], flat["init"]
+        h = ctypes.c_void_p()
+        with torch.cuda.device(self.device):
+            status = lib().b200aa_trees_create(
+                ctypes.byref(h), ctypes.c_void_p(nodes.ctypes.data), nodes.shape[0], ctypes.c_void_p(roots.ctypes.data),
+                roots.shape[0], ctypes.c_void_p(values.ctypes.data), values.shape[0], self.n_classes, self.n_feats,
+                self.mode, None if init is None else ctypes.c_void_p(init.ctypes.data), int(flat["allow_nan"]))
+        if status == ERR_UNSUPPORTED:
+            raise ValueError("a row of %d features and %d classes needs more shared memory than the tree kernel takes"
+                             % (self.n_feats, self.n_classes))
+        check(status)
+        self.handle = h
+
+    def __del__(self):
+        h, self.handle = getattr(self, "handle", None), None
+        if h:
+            lib().b200aa_trees_destroy(h)
+
+
+def tree_classify_batch(model, vectors):
+    """predict / predict_proba of a tree ensemble for every row of a CUDA float32 / float64 [n, F] tensor, in one kernel on
+    the current stream (DESIGN.md, kernel 8): CUDA (ids int64 [n], indices into the model's classes_; P float64 [n, C]),
+    bit for bit scikit-learn's.  Gradient boosting's probabilities are its loss's link applied on the host to the raw
+    scores the kernel adds.  A row scikit-learn refuses (inf, a float64 beyond float32, or NaN where the model takes none)
+    raises scikit-learn's own ValueError.  `model`: a TreeEnsembleModel, or an estimator uploaded for this call."""
+    _require_cuda(vectors, "vectors")
+    if not isinstance(model, TreeEnsembleModel):
+        model = TreeEnsembleModel(model, vectors.device)
+    if vectors.dim() != 2 or vectors.dtype not in (torch.float32, torch.float64):
+        raise ValueError("vectors must be float32 / float64 [n, F]")
+    if vectors.shape[1] != model.n_feats:
+        raise ValueError("vectors have %d features, the model %d" % (vectors.shape[1], model.n_feats))
+    if vectors.device != model.device:
+        raise ValueError("vectors are on %s, the model on %s" % (vectors.device, model.device))
+    n = vectors.shape[0]
+    if (model.n_feats > 1 and vectors.stride(1) != 1) or (n > 1 and vectors.stride(0) < model.n_feats):
+        vectors = vectors.contiguous()
+    with torch.cuda.device(vectors.device):
+        ids = torch.empty(n, dtype=torch.int64, device=vectors.device)
+        scores = torch.empty((n, model.n_classes), dtype=torch.float64, device=vectors.device)
+        bad = torch.empty(n, dtype=torch.int32, device=vectors.device)
+        if n:
+            check(lib().b200aa_trees_classify(
+                model.handle, ctypes.c_void_p(vectors.data_ptr()), DTYPE_F32 if vectors.dtype == torch.float32 else DTYPE_F64,
+                n, model.n_feats, vectors.stride(0) if n > 1 else model.n_feats, ctypes.c_void_p(ids.data_ptr()),
+                ctypes.c_void_p(scores.data_ptr()), ctypes.c_void_p(bad.data_ptr()), _stream()))
+            flagged = torch.nonzero(bad)
+            if flagged.numel():
+                row = vectors[int(flagged[0, 0])].reshape(1, -1).cpu().numpy()
+                model.estimator.predict(row)                    # raises scikit-learn's ValueError for this row
+                raise ValueError("row %d holds a value scikit-learn refuses" % int(flagged[0, 0]))
+        if model.mode == TREE_FOREST:
+            return ids, scores
+        raw = scores.cpu().numpy()
+        P = model.estimator._loss.predict_proba(raw[:, 0] if model.n_classes == 1 else raw)
+        return ids, torch.from_numpy(np.ascontiguousarray(P, dtype=np.float64)).to(vectors.device)
+
+
 def classify_vectors(classifier, model_type, vectors):
     """classifier_wrapper (audioTrainTest.py:52-93) over the rows of `vectors` [n x F]: (class ids [n], probabilities [n x classes]).
-    A CUDA tensor goes to the kNN kernel (``knn_classify_batch``; `classifier` a KnnModel or a Knn-like object) and only the
-    results come back; NumPy input runs on the host."""
+    A CUDA tensor goes to the kNN kernel (``knn_classify_batch``; `classifier` a KnnModel or a Knn-like object) or, for the
+    three tree types, to the tree kernel when ``TreeEnsembleModel`` takes the model (``tree_classify_batch``), and only the
+    results come back; other models and NumPy input run on the host.  A plain estimator is flattened and uploaded in every
+    call (tens of ms for a 100-tree forest, DESIGN.md kernel 8); pass a TreeEnsembleModel to classify repeatedly."""
     if isinstance(vectors, torch.Tensor):
         if model_type == "knn" and vectors.is_cuda:
             ids, P = knn_classify_batch(classifier, vectors)
             return ids.cpu().numpy(), P.cpu().numpy()
+        if model_type in _TREE_TYPES and vectors.is_cuda:
+            model = classifier
+            if not isinstance(model, TreeEnsembleModel):
+                try:
+                    model = TreeEnsembleModel(classifier, vectors.device)
+                except ValueError:
+                    model = None
+            if model is not None:
+                ids, P = tree_classify_batch(model, vectors)
+                return model.classes[ids.cpu().numpy()], P.cpu().numpy()
         vectors = vectors.cpu().numpy()
+    if isinstance(classifier, TreeEnsembleModel):
+        classifier = classifier.estimator
     vectors = np.asarray(vectors, dtype=np.float64)
     if model_type == "knn":
         return knn_classify_matrix(classifier, vectors)
