@@ -26,6 +26,38 @@ from .batch import _require_cuda, _stream, beat_extraction_batch, long_term_mean
 _SKLEARN_TYPES = ("svm", "randomforest", "gradientboosting", "extratrees", "svm_rbf")
 
 
+def _cuda_device(device, what):
+    """The CUDA device `what` (a model class, with its article) is uploaded to: `device`, else the current device."""
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    if device.type != "cuda":
+        raise TypeError("%s lives on a CUDA device (there is no CPU fallback)" % what)
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return device
+
+
+def _query_matrix(model, vectors):
+    """A CUDA [n, F] query tensor checked against `model` (its n_feats and device): (the tensor, made contiguous where the
+    kernel cannot read its strides; its row stride; its dtype code)."""
+    if vectors.dim() != 2 or vectors.dtype not in (torch.float32, torch.float64):
+        raise ValueError("vectors must be float32 / float64 [n, F]")
+    if vectors.shape[1] != model.n_feats:
+        raise ValueError("vectors have %d features, the model %d" % (vectors.shape[1], model.n_feats))
+    if vectors.device != model.device:
+        raise ValueError("vectors are on %s, the model on %s" % (vectors.device, model.device))
+    n = vectors.shape[0]
+    if (model.n_feats > 1 and vectors.stride(1) != 1) or (n > 1 and vectors.stride(0) < model.n_feats):
+        vectors = vectors.contiguous()
+    return (vectors, vectors.stride(0) if n > 1 else model.n_feats,
+            DTYPE_F32 if vectors.dtype == torch.float32 else DTYPE_F64)
+
+
+def _concat_indices(lists, dtype):
+    """A list of 1-D int64 index arrays -> (int64 offsets [len + 1], their concatenation as a contiguous `dtype` array)."""
+    off = np.concatenate([[0], np.cumsum([a.size for a in lists])]).astype(np.int64)
+    return off, np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0), dtype=dtype)
+
+
 def normalize_windows_batch(mid, mean, std):
     """CUDA float32 [B, F, M] -> [B, M, F]: vector j of clip b = (mid[b, :, j] - mean) / std."""
     _require_cuda(mid, "mid")
@@ -81,11 +113,7 @@ class KnnModel:
             lf = labels.astype(np.float64)
             ok = (lf == np.floor(lf)) & (lf >= 0) & (lf < self.n_classes)
             slots[ok] = lf[ok].astype(np.int32)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self.device.type != "cuda":
-            raise TypeError("a KnnModel lives on a CUDA device (there is no CPU fallback)")
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.device = _cuda_device(device, "a KnnModel")
         self.features = torch.from_numpy(np.ascontiguousarray(feats)).to(self.device)
         self.slots = torch.from_numpy(slots).to(self.device)
 
@@ -97,15 +125,8 @@ def knn_classify_batch(model, vectors):
     _require_cuda(vectors, "vectors")
     if not isinstance(model, KnnModel):
         model = KnnModel(model, vectors.device)
-    if vectors.dim() != 2 or vectors.dtype not in (torch.float32, torch.float64):
-        raise ValueError("vectors must be float32 / float64 [n, F]")
-    if vectors.shape[1] != model.n_feats:
-        raise ValueError("vectors have %d features, the model %d" % (vectors.shape[1], model.n_feats))
-    if vectors.device != model.device:
-        raise ValueError("vectors are on %s, the model on %s" % (vectors.device, model.device))
+    vectors, stride, dtype = _query_matrix(model, vectors)
     n = vectors.shape[0]
-    if (model.n_feats > 1 and vectors.stride(1) != 1) or (n > 1 and vectors.stride(0) < model.n_feats):
-        vectors = vectors.contiguous()
     with torch.cuda.device(vectors.device):
         ids = torch.empty(n, dtype=torch.int64, device=vectors.device)
         P = torch.empty((n, model.n_classes), dtype=torch.float64, device=vectors.device)
@@ -113,9 +134,8 @@ def knn_classify_batch(model, vectors):
             return ids, P
         check(lib().b200aa_knn_classify(
             ctypes.c_void_p(model.features.data_ptr()), ctypes.c_void_p(model.slots.data_ptr()), model.n_train, model.n_feats,
-            model.n_classes, model.k, ctypes.c_void_p(vectors.data_ptr()),
-            DTYPE_F32 if vectors.dtype == torch.float32 else DTYPE_F64, n, vectors.stride(0) if n > 1 else model.n_feats,
-            ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(P.data_ptr()), _stream()))
+            model.n_classes, model.k, ctypes.c_void_p(vectors.data_ptr()), dtype, n, stride, ctypes.c_void_p(ids.data_ptr()),
+            ctypes.c_void_p(P.data_ptr()), _stream()))
     return ids, P
 
 
@@ -144,10 +164,8 @@ def knn_cross_validate(X, y, splits, ks, n_classes=None):
         raise ValueError("one k per split: %d splits, %d ks" % (len(splits), len(ks)))
     train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
     test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
-    train_off = np.concatenate([[0], np.cumsum([t.size for t in train])]).astype(np.int64)
-    test_off = np.concatenate([[0], np.cumsum([t.size for t in test])]).astype(np.int64)
-    train_idx = np.ascontiguousarray(np.concatenate(train) if train else np.zeros(0), dtype=np.int32)
-    test_idx = np.ascontiguousarray(np.concatenate(test) if test else np.zeros(0), dtype=np.int32)
+    train_off, train_idx = _concat_indices(train, np.int32)
+    test_off, test_idx = _concat_indices(test, np.int32)
     k = np.ascontiguousarray(ks, dtype=np.int64)
     # Knn.classify's class count: len(np.unique(y_train)) of the split
     classes = np.array([np.unique(y[t[(t >= 0) & (t < n)]]).size for t in train], dtype=np.int32)
@@ -211,11 +229,7 @@ class HmmModel:
         with np.errstate(divide="ignore"):
             log_start, log_trans = np.log(start), np.log(trans)
         const = self.n_feats * np.log(2 * np.pi) + np.log(var).sum(axis=-1)
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self.device.type != "cuda":
-            raise TypeError("an HmmModel lives on a CUDA device (there is no CPU fallback)")
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.device = _cuda_device(device, "an HmmModel")
 
         def up(a):
             return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(self.device)
@@ -275,8 +289,7 @@ def hmm_statistics_batch(mid, class_windows, n_windows=None):
     B, F, M = mid.shape
     counts = _host_counts(n_windows, B, M, 0)
     lists = [np.asarray(w, dtype=np.int64).ravel() for w in class_windows]
-    off = np.concatenate([[0], np.cumsum([w.size for w in lists])]).astype(np.int64)
-    idx = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0), dtype=np.int64)
+    off, idx = _concat_indices(lists, np.int64)
     with torch.cuda.device(mid.device):
         out = torch.empty((4, len(lists), F), dtype=torch.float64, device=mid.device)
         check(lib().b200aa_hmm_statistics(
@@ -369,11 +382,7 @@ class TreeEnsembleModel:
         self.estimator = model
         self.classes = np.asarray(model.classes_)
         self.mode, self.n_classes, self.n_feats = flat["mode"], flat["n_classes"], flat["n_feats"]
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self.device.type != "cuda":
-            raise TypeError("a TreeEnsembleModel lives on a CUDA device (there is no CPU fallback)")
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.device = _cuda_device(device, "a TreeEnsembleModel")
         nodes, roots, values, init = flat["nodes"], flat["roots"], flat["values"], flat["init"]
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
@@ -402,24 +411,16 @@ def tree_classify_batch(model, vectors):
     _require_cuda(vectors, "vectors")
     if not isinstance(model, TreeEnsembleModel):
         model = TreeEnsembleModel(model, vectors.device)
-    if vectors.dim() != 2 or vectors.dtype not in (torch.float32, torch.float64):
-        raise ValueError("vectors must be float32 / float64 [n, F]")
-    if vectors.shape[1] != model.n_feats:
-        raise ValueError("vectors have %d features, the model %d" % (vectors.shape[1], model.n_feats))
-    if vectors.device != model.device:
-        raise ValueError("vectors are on %s, the model on %s" % (vectors.device, model.device))
+    vectors, stride, dtype = _query_matrix(model, vectors)
     n = vectors.shape[0]
-    if (model.n_feats > 1 and vectors.stride(1) != 1) or (n > 1 and vectors.stride(0) < model.n_feats):
-        vectors = vectors.contiguous()
     with torch.cuda.device(vectors.device):
         ids = torch.empty(n, dtype=torch.int64, device=vectors.device)
         scores = torch.empty((n, model.n_classes), dtype=torch.float64, device=vectors.device)
         bad = torch.empty(n, dtype=torch.int32, device=vectors.device)
         if n:
             check(lib().b200aa_trees_classify(
-                model.handle, ctypes.c_void_p(vectors.data_ptr()), DTYPE_F32 if vectors.dtype == torch.float32 else DTYPE_F64,
-                n, model.n_feats, vectors.stride(0) if n > 1 else model.n_feats, ctypes.c_void_p(ids.data_ptr()),
-                ctypes.c_void_p(scores.data_ptr()), ctypes.c_void_p(bad.data_ptr()), _stream()))
+                model.handle, ctypes.c_void_p(vectors.data_ptr()), dtype, n, model.n_feats, stride,
+                ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(scores.data_ptr()), ctypes.c_void_p(bad.data_ptr()), _stream()))
             flagged = torch.nonzero(bad)
             if flagged.numel():
                 row = vectors[int(flagged[0, 0])].reshape(1, -1).cpu().numpy()

@@ -1,0 +1,96 @@
+// Host-side plumbing of every C ABI entry point of libb200aa.so: CUDA error reporting and the launch count, stream-ordered
+// scratch, NVTX ranges, scratch alignment and slicing, and the float32 / float64 dispatch of a launch.
+// g_cuda_err and g_launches are defined once, in b200aa.cu, so that b200aa_last_cuda_error() and b200aa_launch_count()
+// see every file's entry points.
+#pragma once
+#include <cuda_runtime.h>
+#include <nvtx3/nvToolsExt.h>      // header-only NVTX 3: ranges around the entry points (visible in nsys / ncu timelines)
+
+#include <atomic>
+#include <cstddef>
+#include <cstdint>
+#include <string>
+
+#include "../../include/b200aa.h"
+
+// ------------------------------------------------------------------------------------------------
+// error plumbing
+// ------------------------------------------------------------------------------------------------
+extern thread_local std::string g_cuda_err;
+extern std::atomic<int64_t> g_launches;
+
+inline int cuda_fail(cudaError_t e, const char *what)
+{
+    g_cuda_err = std::string(what) + ": " + cudaGetErrorString(e);
+    return B200AA_ERR_CUDA;
+}
+#define CK(call)                                                     \
+    do {                                                             \
+        cudaError_t e_ = (call);                                     \
+        if (e_ != cudaSuccess) return cuda_fail(e_, #call);          \
+    } while (0)
+// every kernel launch ends here: count it (b200aa_launch_count), then report its launch error
+inline int launched(const char *name)
+{
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? B200AA_OK : cuda_fail(e, name);
+}
+#define CK_LAUNCH(name)                                              \
+    do {                                                             \
+        const int rc_ = launched(name);                              \
+        if (rc_ != B200AA_OK) return rc_;                            \
+    } while (0)
+
+// Stream-ordered device scratch of one entry point, bound to its scope: alloc() takes it with cudaMallocAsync, done(rc)
+// frees it after everything queued on the stream and returns rc, else the free's error.  A scope left early (its error
+// already reported) frees it in the destructor.
+class StreamScratch {
+  public:
+    explicit StreamScratch(cudaStream_t st) : st_(st) {}
+    StreamScratch(const StreamScratch &) = delete;
+    StreamScratch &operator=(const StreamScratch &) = delete;
+    ~StreamScratch() { release(); }
+    int alloc(size_t bytes)
+    {
+        if (bytes) CK(cudaMallocAsync(&p_, bytes, st_));
+        return B200AA_OK;
+    }
+    void *get() const { return p_; }
+    int done(int rc)
+    {
+        const cudaError_t e = release();
+        return (e != cudaSuccess && rc == B200AA_OK) ? cuda_fail(e, "cudaFreeAsync") : rc;
+    }
+
+  private:
+    cudaError_t release()
+    {
+        const cudaError_t e = p_ ? cudaFreeAsync(p_, st_) : cudaSuccess;
+        p_ = nullptr;
+        return e;
+    }
+    cudaStream_t st_;
+    void *p_ = nullptr;
+};
+
+struct NvtxRange {
+    explicit NvtxRange(const char *name) { nvtxRangePushA(name); }
+    ~NvtxRange() { nvtxRangePop(); }
+};
+
+// ------------------------------------------------------------------------------------------------
+// scratch layout and dispatch
+// ------------------------------------------------------------------------------------------------
+// Bound on one slice of an entry point's stream-ordered scratch: work larger than this is cut into slices run in turn.
+constexpr size_t kScratchSliceBytes = size_t(256) << 20;
+
+inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+// f(float{}) for B200AA_DTYPE_F32, f(double{}) for B200AA_DTYPE_F64 (the caller has checked dtype): a launch over either
+// element type written once
+template <class F>
+auto with_real_type(int dtype, F f)
+{
+    return dtype == B200AA_DTYPE_F32 ? f(float{}) : f(double{});
+}

@@ -12,15 +12,15 @@
 #include <cstdint>
 #include <cstring>
 
-#include "beat.cuh"
+#include "npsum.cuh"
 
 namespace b200aa {
 namespace knn {
 
-using beat::dadd;
-using beat::ddiv;
-using beat::dmul;
-using beat::dsub;
+using npy::dadd;
+using npy::ddiv;
+using npy::dmul;
+using npy::dsub;
 using npy::dsqrt;
 
 constexpr int kQ = 64;                  // queries per CTA tile of the distance kernel

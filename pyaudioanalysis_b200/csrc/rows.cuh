@@ -57,5 +57,11 @@ __host__ __device__ inline Rows chromagram(int64_t n, int w, int s)
 // w - s, which holds at most ceil((w - s) / s) = (w - 1) / s of them
 __host__ __device__ inline int64_t max_clipped(int w, int s) { return w > s ? (int64_t(w) - 1) / s : 0; }
 
+// mid-term windows of a clip of n_frames frames: b200aa_mid_windows on the host, per clip of a ragged batch on the device
+__host__ __device__ inline int64_t windows_of(int64_t n_frames, int stepr)
+{
+    return (stepr < 1 || n_frames <= 0) ? 0 : (n_frames + stepr - 1) / stepr;
+}
+
 }  // namespace rows
 }  // namespace b200aa

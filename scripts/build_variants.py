@@ -7,7 +7,6 @@
 Variants land in pyaudioanalysis_b200/variants/libb200aa_<name>.so and are selected per process with B200AA_LIB.
 """
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -34,15 +33,7 @@ def build(name, verbose=False):
     out_dir = os.path.join(B.HERE, "variants")
     os.makedirs(out_dir, exist_ok=True)
     out = os.path.join(out_dir, "libb200aa_%s.so" % name)
-    flags = [f for f in B.NVCC_FLAGS if not f.startswith("--use_fast_math")]
-    cmd = [B._nvcc()] + flags + VARIANTS[name] + (["-Xptxas", "-v"] if verbose else []) + \
-          ["-o", out] + [os.path.join(B.CSRC, s) for s in B.SOURCES]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building variant " + name)
-    if verbose:
-        sys.stderr.write(res.stderr)
+    B.compile_lib(out, VARIANTS[name], verbose)
     return out
 
 

@@ -1,18 +1,17 @@
 """CPU: the pieces of the beat-extraction kernel (csrc/beat.cuh, __host__ __device__) run on the host by tests/beat_host.cu --
 NumPy's pairwise summation order, the chunked three-phase peak scan, and the whole per-clip computation -- against NumPy and
 the host MidTermFeatures.beat_extraction, bit for bit."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 from pyaudioanalysis_b200.MidTermFeatures import _peak_positions, beat_extraction
+from tests import host_exe
 from tests.conftest import load_golden
-from tests.test_codelets_cpu import ROOT, _nvcc
 from tests.test_host_cpu import peak_inputs
 
-pytestmark = pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
+pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not available")
 
 PRODUCTION_CHUNK = 1024          # beat::kChunk
 CHUNKS = (1, 2, 3, 31, 32, PRODUCTION_CHUNK)
@@ -20,11 +19,7 @@ CHUNKS = (1, 2, 3, 31, 32, PRODUCTION_CHUNK)
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    path = str(tmp_path_factory.mktemp("beat") / "beat_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "beat_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "beat_host.cu", "-O1")
 
 
 def _hex(values):

@@ -68,6 +68,54 @@ def test_counts(L):
     assert lib.b200aa_mid_windows(319, 40) == 8 and lib.b200aa_mid_windows(143999, 40) == 3600
 
 
+def _first_cuda_call_fails(L):
+    """One entry point of each kernel family's own .cu, with arguments that pass its checks: (name, call, the start of the
+    CUDA call its failure names).  Fake device pointers are never dereferenced: each call stops at its first CUDA call."""
+    lib, dev = L.lib(), ctypes.c_void_p(1 << 20)
+    clip = np.array([(0, 1, 1, 1)], dtype=[("offset", "<i8"), ("n_frames", "<i8"), ("format", "<i4"), ("channels", "<i4")])
+    off, idx, one = np.array([0, 1], np.int64), np.zeros(1, np.int64), np.ones(1, np.int64)
+    node, roots, values = np.array([[-1, 0, 0, 0]], np.int32), np.zeros(1, np.int32), np.full((1, 2), 0.5)
+    h = ctypes.c_void_p()
+
+    def ptr(a):
+        return ctypes.c_void_p(a.ctypes.data)
+    return [
+        ("mid.cu", lambda: lib.b200aa_frame_counts(dev, 1, 800, 400, 40, dev, dev, None), "frame_counts_kernel: "),
+        ("pcm.cu", lambda: lib.b200aa_decode_pcm(dev, 16, ptr(clip), 1, L.DTYPE_I16, dev, 1, 1, None), "cudaMallocAsync("),
+        ("beat.cu", lambda: lib.b200aa_beat_extraction(dev, 1, 68, 10, 10, None, 0.05, dev, None), "cudaMallocAsync("),
+        ("knn.cu", lambda: lib.b200aa_knn_classify(dev, dev, 1, 1, 1, 1, dev, L.DTYPE_F32, 1, 1, dev, dev, None),
+         "cudaMallocAsync("),
+        ("hmm.cu", lambda: lib.b200aa_hmm_statistics(dev, L.DTYPE_F32, 1, 1, 1, ptr(one), 1, ptr(off), ptr(idx), dev, None),
+         "cudaMallocAsync("),
+        ("trees.cu", lambda: lib.b200aa_trees_create(ctypes.byref(h), ptr(node), 1, ptr(roots), 1, ptr(values), 1, 2, 1, 0,
+                                                     None, 0), "cudaGetDevice("),
+    ]
+
+
+def test_error_state_is_shared_by_every_file(L):
+    """b200aa_last_cuda_error() and b200aa_launch_count() live in b200aa.cu and report the entry points of every .cu: each
+    call runs in a thread of its own, whose error text starts empty, and must leave the text of its own failed CUDA call."""
+    import threading
+    import torch
+    if torch.cuda.device_count() != 0:
+        pytest.skip("on a GPU host these calls would run")
+    lib = L.lib()
+    for name, call, what in _first_cuda_call_fails(L):
+        got = {}
+
+        def run():
+            before = lib.b200aa_launch_count()
+            got["rc"] = call()
+            got["launches"] = lib.b200aa_launch_count() - before
+            got["err"] = lib.b200aa_last_cuda_error().decode()
+        t = threading.Thread(target=run)
+        t.start()
+        t.join()
+        assert got["rc"] == L.ERR_CUDA, (name, got)
+        assert got["err"].startswith(what), (name, got["err"])
+        assert got["launches"] == (1 if what.endswith("_kernel: ") else 0), (name, got)
+
+
 def test_python_mirror_names():
     from pyaudioanalysis_b200 import ShortTermFeatures as S
     assert S.feature_names(True) == O.feature_names(True)

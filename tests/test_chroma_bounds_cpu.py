@@ -79,11 +79,11 @@ import pytest
 import scipy.fft
 
 from oracle import st_oracle as O
+from tests import host_exe
 from tests import signals as SG
 from tests.kernels import GENERIC_SWEEP
 from tests.parity import (DIV_REL, ROW_CLIPPED, ROW_EMPTY, ROW_FULL, _tables, check_chromagram_bounds, chromagram_bounds,
                           chromagram_rows, clip_norm, gamma, sum_depth)
-from tests.test_codelets_cpu import ROOT, _nvcc
 from tests.test_gpu_adversarial import ROW_CONFIGS
 
 CONFIGS = ROW_CONFIGS + [(16000, 800, 200)]
@@ -407,13 +407,9 @@ def test_chroma_tables_match_oracle(lib):
     assert negative >= 3 and raised >= 3, (negative, raised)
 
 
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
-def test_rows_rule_matches_library(tmp_path):
+def test_rows_rule_matches_library(tmp_path_factory):
     """parity.chromagram_rows is csrc/rows.cuh's rule (run on the host by tests/rows_host.cu) for every length 0 .. 3 w."""
-    exe = str(tmp_path / "rows_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "rows_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+    exe = host_exe.build(tmp_path_factory, "rows_host.cu", "-O1")
     configs = [(800, 400), (800, 200), (800, 100), (883, 300), (882, 441), (400, 160)]
     out = subprocess.run([exe], input="".join("%d %d %d\n" % (w, s, 3 * w) for w, s in configs), capture_output=True, text=True)
     assert out.returncode == 0, out.stderr
@@ -428,18 +424,15 @@ def test_rows_rule_matches_library(tmp_path):
                 assert (n_it, n_full) == (c_it, c_full), (w, s, n)
 
 
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
-def test_clipped_kernel_scratch_boundary(tmp_path):
+def test_clipped_kernel_scratch_boundary(tmp_path, tmp_path_factory):
     """clipped_chroma_kernel keeps its arrays (|X| row, w double2 twiddles, w double samples) in shared memory while
     clipped_bytes(w, w / 2) <= 226 KiB, else in global scratch: the last shared-memory window is 8 900, the first global one
     8 901 (tests/test_gpu_chroma_bounds.py runs both)."""
     src = tmp_path / "clipped_bytes.cu"
     src.write_text('#include <cstdio>\n#define B200AA_LAYOUT_ONLY 1\n#include "%s"\nint main() { for (int w = 2; w <= 20000; ++w) '
                    'printf("%%d %%zu\\n", w, b200aa::clipped_bytes(w, w / 2)); return 0; }\n'
-                   % os.path.join(ROOT, "pyaudioanalysis_b200", "csrc", "generic_kernel.cuh"))
-    exe = str(tmp_path / "clipped_bytes")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-arch=sm_90a", "-o", exe, str(src)], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+                   % os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc", "generic_kernel.cuh"))
+    exe = host_exe.build(tmp_path_factory, str(src))
     sizes = {int(a): int(b) for a, b in (ln.split() for ln in subprocess.run([exe], capture_output=True, text=True).stdout.splitlines())}
     fits = [w for w, b in sizes.items() if b <= SMEM_CAP]
     assert max(fits) == 8900 and fits == list(range(2, 8901)), max(fits)

@@ -1,27 +1,12 @@
 """CPU: the register FFT codelets of the fused kernel (csrc/dft_codelets.cuh are __host__ __device__ templates) and the
 R1 x R2 packed-real transform built from them, run on the host against a naive float64 DFT (tests/codelets_host.cu)."""
-import os
-import shutil
 import subprocess
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests import host_exe
 
 
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", shutil.which("nvcc")):
-        if cand and os.path.exists(cand):
-            return cand
-    return None
-
-
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
-def test_codelets_and_shapes_on_host(tmp_path):
-    exe = str(tmp_path / "codelets_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "codelets_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+def test_codelets_and_shapes_on_host(tmp_path_factory):
+    exe = host_exe.build(tmp_path_factory, "codelets_host.cu", "-O1")
     run = subprocess.run([exe], capture_output=True, text=True)
     assert run.returncode == 0, run.stdout
     lines = [ln.split() for ln in run.stdout.splitlines()]

@@ -4,25 +4,18 @@ NumPy on features.T, the Viterbi pass against tests/hmm_oracle.py and an exhaust
 the host helpers of audioSegmentation; and the C ABI's argument checks, which return before any CUDA call."""
 import ctypes
 import itertools
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 from tests import hmm_oracle as H
-from tests.test_codelets_cpu import ROOT, _nvcc
+from tests import host_exe
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    if _nvcc() is None:
-        pytest.skip("nvcc not available")
-    path = str(tmp_path_factory.mktemp("hmm") / "hmm_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "hmm_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "hmm_host.cu", "-O1")
 
 
 def _hex(values):

@@ -1,27 +1,22 @@
 """CPU: the pieces of the kNN kernel (csrc/knn.cuh, __host__ __device__) run on the host by tests/knn_host.cu -- the distance
 chain against scipy's cdist, the sort keys, and the radix selection, ordered pass and vote against the stable-sort oracle
 and the reference's Knn.classify (tests/golden/knn.npz), bit for bit."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 from scipy.spatial.distance import cdist
 
+from tests import host_exe
 from tests.conftest import load_golden
 from tests.knn_oracle import knn_oracle, slots_of
-from tests.test_codelets_cpu import ROOT, _nvcc
 
-pytestmark = pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
+pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not available")
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    path = str(tmp_path_factory.mktemp("knn") / "knn_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "knn_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "knn_host.cu", "-O1")
 
 
 def _hex(values):

@@ -6,7 +6,6 @@ the C ABI's argument checks."""
 import contextlib
 import ctypes
 import io
-import os
 import subprocess
 
 import numpy as np
@@ -14,22 +13,16 @@ import pytest
 from sklearn.preprocessing import StandardScaler
 
 from pyaudioanalysis_b200 import audioTrainTest as at
+from tests import host_exe
 from tests.conftest import load_golden
 from tests.knn_cv_oracle import reference_splits, scores, seeded_features
-from tests.test_codelets_cpu import ROOT, _nvcc
 
 INVALID = -1
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    if _nvcc() is None:
-        pytest.skip("nvcc not available")
-    path = str(tmp_path_factory.mktemp("knn_cv") / "knn_cv_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "knn_cv_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "knn_cv_host.cu", "-O1")
 
 
 def _hex(a):

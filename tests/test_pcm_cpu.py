@@ -8,7 +8,6 @@
   and a lazily opened ``_Clip`` has the sampling rate, length and staged format of today's host decode.
 * Every argument error of ``b200aa_decode_pcm`` returns B200AA_ERR_INVALID before any CUDA call.
 """
-import os
 import subprocess
 
 import numpy as np
@@ -17,8 +16,8 @@ import pytest
 from pyaudioanalysis_b200 import audioio
 from pyaudioanalysis_b200.MidTermFeatures import _open_clip
 from pyaudioanalysis_b200.ShortTermFeatures import _as_clip
+from tests import host_exe
 from tests import wavgen
-from tests.test_codelets_cpu import ROOT, _nvcc
 
 INVALID = -1
 
@@ -88,13 +87,7 @@ def flavour_samples(name, channels, seed):
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    if _nvcc() is None:
-        pytest.skip("nvcc not available")
-    path = str(tmp_path_factory.mktemp("pcm") / "pcm_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "pcm_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "pcm_host.cu", "-O1")
 
 
 def host_convert(exe, tmp_path, path):

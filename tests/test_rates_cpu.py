@@ -24,15 +24,14 @@ sweep points given): an empty filter that is not flushed (54), lane lists trunca
 truncated at CT = 8 (910), and the clamp moved one bin up (442: the last read lands one past the row) or down (204: the
 filter's last tap is dropped).
 """
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import st_oracle as O
+from tests import host_exe
 from tests.kernels import RATE_CONFIGS
-from tests.test_codelets_cpu import ROOT, _nvcc
 
 PAIR_WINDOWS = [320, 480, 512, 640, 800, 960, 1024]
 SOLO_WINDOWS = [400, 600, 882]
@@ -78,13 +77,7 @@ def run_tables(exe, points):
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    if _nvcc() is None:
-        pytest.skip("nvcc not available")
-    exe = str(tmp_path_factory.mktemp("tables") / "tables_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "tables_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return exe
+    return host_exe.build(tmp_path_factory, "tables_host.cu", "-O1")
 
 
 @pytest.fixture(scope="module")

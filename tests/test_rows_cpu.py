@@ -3,7 +3,6 @@ tests/rows_host.cu, for every clip length 0 .. 3 * window, against the oracle's 
 the single-clip entry points' refusals; and the argument checks of the ragged row entry points, which return before
 touching a device."""
 import ctypes
-import os
 import subprocess
 import warnings
 
@@ -11,7 +10,7 @@ import numpy as np
 import pytest
 
 from oracle import st_oracle as O
-from tests.test_codelets_cpu import ROOT, _nvcc
+from tests import host_exe
 
 CONFIGS = [(800, 400), (800, 200), (800, 333), (882, 441), (800, 800), (400, 160),
            (800, 1000), (600, 900), (882, 1323), (320, 400)]          # hops longer than the window: frames skip samples
@@ -20,12 +19,7 @@ FS = {882: 44100}
 
 @pytest.fixture(scope="module")
 def table(tmp_path_factory):
-    if _nvcc() is None:
-        pytest.skip("nvcc not available")
-    exe = str(tmp_path_factory.mktemp("rows") / "rows_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "rows_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+    exe = host_exe.build(tmp_path_factory, "rows_host.cu", "-O1")
     script = "".join("%d %d %d\n" % (w, s, 3 * w) for w, s in CONFIGS)
     out = subprocess.run([exe], input=script, capture_output=True, text=True)
     assert out.returncode == 0, out.stderr

@@ -5,35 +5,20 @@ n * (bytes + 1024) <= 233 472.  The CTA kernel (csrc/fast_kernel.cuh) is sized f
 the pair kernel (csrc/pair_kernel.cuh) runs one CTA of up to 20 autonomous warps per SM (9.6 KB of shared memory per warp on
 the headline shape, five warps per scheduler at 96 registers).  The generic kernel (csrc/generic_kernel.cuh) takes 8, 4,
 2 or 1 frames per CTA group by the same budget, or keeps its window-sized arrays in global scratch."""
-import os
-import shutil
 import subprocess
 
-import pytest
-
+from tests import host_exe
 from tests.kernels import GENERIC_SWEEP
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SM_BYTES, CTA_RESERVED = 233472, 1024
-
-
-def _nvcc():
-    for cand in (os.environ.get("NVCC"), "/usr/local/cuda/bin/nvcc", shutil.which("nvcc")):
-        if cand and os.path.exists(cand):
-            return cand
-    return None
 
 
 def ctas_per_sm(nbytes):
     return SM_BYTES // (nbytes + CTA_RESERVED)
 
 
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
-def test_shared_memory_budget(tmp_path):
-    exe = str(tmp_path / "smem_budget")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-arch=sm_90a", "-o", exe, os.path.join(ROOT, "tests", "smem_budget_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+def test_shared_memory_budget(tmp_path_factory):
+    exe = host_exe.build(tmp_path_factory, "smem_budget_host.cu")
     windows = ["%d:%d" % (fs, w) for fs, w, _, _ in GENERIC_SWEEP]
     lines = [ln.split() for ln in subprocess.run([exe] + windows, capture_output=True, text=True).stdout.splitlines()]
     # the generic kernel's spectrum sweep reaches the group size (and transform form) each window is listed for, with the

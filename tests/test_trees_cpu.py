@@ -3,25 +3,20 @@ over the arrays consumers.flatten_tree_ensemble makes, bit for bit scikit-learn'
 boosting's raw scores) on seeded forests and boosting models and adversarial query banks; the flattening against the
 tree_ attributes; the refusals; and the argument checks of b200aa_trees_create / b200aa_trees_classify."""
 import ctypes
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+from tests import host_exe
 from tests import tree_models as TM
-from tests.test_codelets_cpu import ROOT, _nvcc
 
-pytestmark = pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
+pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not available")
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    path = str(tmp_path_factory.mktemp("trees") / "trees_host")
-    res = subprocess.run([_nvcc(), "-std=c++17", "-O1", "-arch=sm_90a", "-o", path, os.path.join(ROOT, "tests", "trees_host.cu")],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return path
+    return host_exe.build(tmp_path_factory, "trees_host.cu", "-O1")
 
 
 @pytest.fixture(scope="module")
