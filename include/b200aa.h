@@ -313,6 +313,30 @@ int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feats, int64_t 
                       int n_states, const double *d_log_start, const double *d_log_trans, const double *d_means,
                       const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream);
 
+/* b200aa_hmm_decode_f64: b200aa_hmm_decode of float64 windows, the same model arguments, outputs and checks.  Clip b is
+ * d_mid + b * n_feats * m_stride: with window_major = 0 a [n_feats, m_stride] matrix (the layout b200aa_hmm_decode reads;
+ * predict(features.T) sums a window's density terms in sequence), with window_major = 1 a C-contiguous [m_stride, n_feats]
+ * matrix of one window per row (predict(X) of a C-contiguous X sums them pairwise, NumPy's order for a contiguous row).
+ * window_major other than 0 / 1 is B200AA_ERR_INVALID. */
+int b200aa_hmm_decode_f64(const double *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, int window_major,
+                          const int64_t *h_n_windows, int n_states, const double *d_log_start, const double *d_log_trans,
+                          const double *d_means, const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad,
+                          void *stream);
+
+/* Kernel 9 (csrc/cluster.cuh): the cluster distance means of speaker_diarization's silhouette (audioSegmentation.py:943-985)
+ * for one clustering of the n rows of d_X (float64, row r at d_X + r * x_stride, n_feats columns), h_labels [n] on the host,
+ * each in [0, n_clusters).  For every cluster c with h_want[c] != 0 (h_want NULL: every cluster), X_c its rows in ascending
+ * order, writes d_A[c] = np.mean(pdist(X_c.T)) and d_B[c * K + c2] = np.mean(cdist(X_c, X_c2)) for c2 != c, float64, bit
+ * for bit scipy's sequential euclidean chain and NumPy's pairwise sum of the condensed vector / the row-major block, then
+ * one division by the count.  A mean of no terms (n_feats < 2 for A, an empty X_c2 for B), a diagonal entry and the rows
+ * of clusters not wanted are NaN.  NULL pointers (h_want aside), n < 1, n_feats outside [1, 4096], x_stride < n_feats,
+ * n_clusters outside [1, B200AA_CLUSTER_MAX] and a label outside [0, n_clusters) are B200AA_ERR_INVALID, before any CUDA
+ * call.  Stream-ordered scratch: the gathered rows (n x n_feats doubles) and the distances of one pass (at most 128 MiB,
+ * or one segment of a mean's pairwise tree when that is larger). */
+#define B200AA_CLUSTER_MAX 1024
+int b200aa_cluster_distance_means(const double *d_X, int64_t n, int n_feats, int64_t x_stride, const int32_t *h_labels,
+                                  int n_clusters, const unsigned char *h_want, double *d_A, double *d_B, void *stream);
+
 /* Kernel 8 (csrc/trees.cuh): the tree classifiers of extract_features_and_train (audioTrainTest.py:52-93), bit for bit
  * scikit-learn 1.9's predict / predict_proba of RandomForestClassifier, ExtraTreesClassifier (mode 0, forest mean) and
  * GradientBoostingClassifier (mode 1, boosting sum).

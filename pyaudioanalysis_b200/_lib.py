@@ -68,6 +68,12 @@ SIGNATURES = {
     # (d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars, d_const, d_ids,
     #  d_bad, stream)
     "b200aa_hmm_decode": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (d_mid, n_clips, n_feats, m_stride, window_major, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars,
+    #  d_const, d_ids, d_bad, stream)
+    "b200aa_hmm_decode_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                      c_vp]),
+    # (d_X, n, n_feats, x_stride, h_labels, n_clusters, h_want, d_A, d_B, stream)
+    "b200aa_cluster_distance_means": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
     # (out, h_nodes, n_nodes, h_roots, n_trees, h_values, n_leaves, n_classes, n_feats, mode, h_init, allow_nan)
     "b200aa_trees_create": (c_int, [ctypes.POINTER(c_vp), c_vp, c_i64, c_vp, c_int, c_vp, c_i64, c_int, c_int, c_int, c_vp,
                                     c_int]),

@@ -17,11 +17,21 @@ The reference's behaviour is kept where it is visible to a caller:
 ``evaluate_segmentation_classification_dir`` decodes every file of the folder in one ragged batch and prints the
 reference's text.  Its classifier methods need the reference's own function (``install.install_segmentation`` keeps
 it); called here they raise ValueError.
+
+Speaker diarization (:815-1091): ``diarize`` runs the steps after the mid-term features.  The SVM posteriors, the
+StandardScaler, the feature-outlier rule, k-means and LDA stay on the host, as the reference makes them; the silhouette's
+cluster distance means run on the GPU (kernel 9, ``consumers.cluster_distance_means``) and the HMM smoothing on kernel 7
+(``train_hmm_compute_statistics`` and the float64 decode).  The reference's visible quirks are kept:
+- the "outliers" dropped are feature columns (dist_all is the pdist of the columns of the normalised matrix);
+- A[c] is the mean pdist over the transposed cluster, i.e. between its feature columns;
+- the labels smoothed by the HMM and the median filter are those of the LAST candidate speaker count, not of the best;
+- the speaker count reported (the class names, the plot) comes from the best silhouette.
 """
 import csv
 import glob
 import os
 import pickle
+import warnings
 
 import numpy as np
 
@@ -404,3 +414,294 @@ def dispatcher(original):
         return run(dir_name, model_name, method_name)
     evaluate_segmentation_classification_dir_dispatch.original = original
     return evaluate_segmentation_classification_dir_dispatch
+
+
+# ------------------------------------------------------------------ speaker diarization (:251-284, :815-1091)
+_DIARIZATION_MODELS = ("svm_rbf_speaker_10", "svm_rbf_speaker_male_female")
+
+
+def evaluate_speaker_diarization(labels, labels_gt):
+    """(cluster purity, speaker purity) of window labels against ground-truth labels over their common length."""
+    n = min(labels.shape[0], labels_gt.shape[0])
+    labels, labels_gt = labels[0:n], labels_gt[0:n]
+    flags, flags_gt = np.unique(labels), np.unique(labels_gt)
+    table = np.zeros((flags.shape[0], flags_gt.shape[0]))
+    np.add.at(table, (np.searchsorted(flags, labels), np.searchsorted(flags_gt, labels_gt)), 1.0)
+    row_sum, column_sum, total = np.sum(table, axis=0), np.sum(table, axis=1), np.sum(table)
+    purity_clust = np.array([np.max(table[i, :]) / column_sum[i] for i in range(table.shape[0])])
+    purity_speak = np.array([np.max(table[:, j]) / row_sum[j] for j in range(table.shape[1])])
+    return np.sum(purity_clust * column_sum) / total, np.sum(purity_speak * row_sum) / total
+
+
+def _posteriors(vectors, model):
+    """predict_proba of an SVM (classifier, mean, std) for the rows of `vectors`, normalised as the reference does per
+    window: one batched call, row-wise as the per-window loop."""
+    classifier, mean, std = model
+    return np.asarray(classifier.predict_proba((vectors - mean) / std))
+
+
+def _with_posteriors(feats, posteriors):
+    """[feats; p1 + 1e-4; p2 + 1e-4] (rows: features, columns: windows) as float64."""
+    return np.concatenate([np.asarray(feats, dtype=np.float64)] + [np.asarray(p, dtype=np.float64).T + 1e-4
+                                                                    for p in posteriors])
+
+
+def pool_frames(st, ratio):
+    """The LDA branch's pooling (:884-906): for every short-term frame i, the mean and population std of each feature row
+    over frames [i, min(i + ratio, T)), as [2F, T] float64 (means, then stds).  Each row's statistics are NumPy's of the
+    contiguous slice, as the reference's per-row loop takes them (np.mean / np.std along a row reduce it in the same
+    order as the 1-D slice)."""
+    st = np.ascontiguousarray(st, dtype=np.float64)
+    F, T = st.shape
+    out = np.zeros((2 * F, T))
+    for i in range(T):
+        w = st[:, i:min(i + ratio, T)]
+        out[:F, i] = np.mean(w, axis=1)
+        out[F:, i] = np.std(w, axis=1)
+    return out
+
+
+def _kmeans(x, k):
+    import sklearn.cluster
+    k_means = sklearn.cluster.KMeans(n_clusters=k)
+    k_means.fit(x)
+    return k_means.labels_
+
+
+def _silhouette(cls, k, A, B):
+    """The average silhouette of :949-985 from the cluster distance means (A [k], B [k, k], NumPy arrays)."""
+    sil_1, sil_2 = [], []
+    for c in range(k):
+        share = np.nonzero(cls == c)[0].shape[0] / float(len(cls))
+        if share < 0.020:
+            sil_1.append(0.0)
+            sil_2.append(0.0)
+        else:
+            sil_1.append(A[c] * share)
+            sil_temp = []
+            for c2 in range(k):
+                if c2 != c:
+                    share_2 = np.nonzero(cls == c2)[0].shape[0] / float(len(cls))
+                    sil_temp.append(B[c, c2] * (share + share_2) / 2.0)
+            sil_2.append(min(np.array(sil_temp)))
+    sil_1, sil_2 = np.array(sil_1), np.array(sil_2)
+    sil = [(sil_2[c] - sil_1[c]) / (max(sil_2[c], sil_1[c]) + 1e-5) for c in range(k)]
+    return np.mean(sil)
+
+
+def cluster_means_gpu(x, cls, k, rows):
+    """(A, B) of kernel 9 for one clustering, as NumPy arrays.  x: a CUDA float64 tensor (or host data, uploaded for this
+    call).  Every mean of no terms (pdist of fewer than two columns, cdist against an empty cluster) warns as np.mean of
+    an empty array does, in the reference's order, under the caller's np.errstate."""
+    import torch
+    from .consumers import cluster_distance_means
+    t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64)).cuda()
+    A, B = cluster_distance_means(t, cls, k, rows)
+    A, B = A.cpu().numpy(), B.cpu().numpy()
+    counts = np.bincount(np.asarray(cls, dtype=np.int64), minlength=k)
+    for c in sorted(rows):
+        if t.shape[1] < 2:
+            np.mean(np.empty(0))
+        for c2 in range(k):
+            if c2 != c and counts[c] * counts[c2] == 0:
+                np.mean(np.empty(0))
+    return A, B
+
+
+def _hmm_smooth(x, cls):
+    """The HMM post-processing of :1001-1010: statistics of x.T per label, then predict(x) of the C-contiguous x on the
+    GPU (kernel 7, float64 windows)."""
+    import torch
+    from .consumers import HmmModel, hmm_decode_batch
+    start_prob, transmat, means, cov = train_hmm_compute_statistics(x.T, cls)
+    hmm = DiagonalGaussianHMM(start_prob.shape[0], "diag")
+    hmm.startprob_, hmm.transmat_, hmm.means_, hmm.covars_ = start_prob, transmat, means, cov
+    t = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64)).cuda()
+    ids, bad = hmm_decode_batch(t.unsqueeze(0).transpose(1, 2), HmmModel(hmm, t.device))
+    if bool(bad[0]):
+        raise _nonfinite()
+    return ids[0].cpu().numpy().astype(np.int64)
+
+
+def diarize(mid, models, n_speakers, mid_step, short_window, lda_dim, st=None, mid_window=None, posteriors=None,
+            cluster=None, means=None, details=False):
+    """The steps of speaker_diarization after the mid-term features (:848-1012) for a mid-term matrix mid [F, M]:
+    returns cls [M] (float64, the median-filtered labels), or with ``details`` (cls, a dict of the intermediate arrays:
+    posteriors, i_non_outliers, labels per candidate count, sil_all, num_speakers).
+
+    models: the two (classifier, mean, std) SVM triples (svm_rbf_speaker_10, svm_rbf_speaker_male_female); posteriors:
+    their predict_proba matrices [M, C] instead.  lda_dim > 0 needs models (even with posteriors given: the posteriors of
+    the pooled short-term frames are computed here), st (the short-term features [68, T]) and mid_window: every
+    short-term frame is pooled as the reference pools it (``pool_frames``) and projected by LDA, and there is no HMM.  cluster(x, k) -> labels
+    (default: sklearn.cluster.KMeans(n_clusters=k), seeded by the global NumPy state as in the reference); means(x, cls,
+    k, rows) -> (A, B) (default: kernel 9)."""
+    from scipy.signal import medfilt
+    from scipy.spatial import distance
+    from sklearn.preprocessing import StandardScaler
+    cluster = _kmeans if cluster is None else cluster
+    means = cluster_means_gpu if means is None else means
+    mid = np.asarray(mid, dtype=np.float64)
+    if posteriors is None:
+        posteriors = [_posteriors(mid.T, m) for m in models]
+    mid_feats_norm = StandardScaler().fit_transform(_with_posteriors(mid, posteriors).T)
+    dist_all = np.sum(distance.squareform(distance.pdist(mid_feats_norm.T)), axis=0)
+    i_non_outliers = np.nonzero(dist_all < 1.1 * np.mean(dist_all))[0]
+    mt_feats_norm_or = mid_feats_norm
+    mid_feats_norm = mid_feats_norm[:, i_non_outliers]
+    if lda_dim > 0:
+        import sklearn.discriminant_analysis
+        if models is None or st is None or mid_window is None:
+            raise ValueError("lda_dim > 0 needs models (the posteriors of every short-term frame are computed here), st "
+                             "and mid_window")
+        pooled = pool_frames(st, int(round(mid_window / short_window)))
+        red = _with_posteriors(pooled, [_posteriors(pooled.T, m) for m in models])
+        red = StandardScaler().fit_transform(red.T).T
+        labels = np.zeros((red.shape[1],))
+        lda_step_ratio = 1.0 / short_window
+        for index in range(labels.shape[0]):
+            labels[index] = int(index * short_window / lda_step_ratio)
+        clf = sklearn.discriminant_analysis.LinearDiscriminantAnalysis(n_components=lda_dim)
+        mid_feats_norm = clf.fit_transform(red.T, labels)
+    s_range = range(2, 10) if n_speakers <= 0 else [n_speakers]
+    x = mid_feats_norm
+    if means is cluster_means_gpu:                  # one upload for every candidate count
+        import torch
+        x = torch.from_numpy(np.ascontiguousarray(mid_feats_norm, dtype=np.float64)).cuda()
+    cluster_labels, sil_all = [], []
+    cls = None
+    for speakers in s_range:
+        cls = cluster(mid_feats_norm, speakers)
+        cluster_labels.append(cls)
+        shares = np.bincount(np.asarray(cls, dtype=np.int64), minlength=speakers) / float(len(cls))
+        rows = [c for c in range(speakers) if not shares[c] < 0.020]
+        A, B = means(x, cls, speakers, rows)
+        sil_all.append(_silhouette(cls, speakers, A, B))
+    imax = int(np.argmax(sil_all))
+    num_speakers = s_range[imax]
+    if lda_dim <= 0:
+        cls = _hmm_smooth(mt_feats_norm_or, cls)
+    cls = medfilt(cls, 5)
+    if not details:
+        return cls
+    return cls, {"posteriors": posteriors, "i_non_outliers": i_non_outliers, "labels": cluster_labels,
+                 "sil_all": np.array(sil_all), "num_speakers": num_speakers}
+
+
+def _load_svm(path):
+    """(classifier, mean, std, class names) of a model file pair written by the reference's trainer."""
+    with open(path + "MEANS", "rb") as fo:
+        mean, std, class_names = pickle.load(fo), pickle.load(fo), pickle.load(fo)
+    with open(path, "rb") as fid:
+        classifier = pickle.load(fid)
+    return classifier, np.array(mean), np.array(std), class_names
+
+
+def _models_dir(models_dir):
+    if models_dir is None:
+        try:
+            import pyAudioAnalysis
+            models_dir = os.path.join(os.path.dirname(os.path.realpath(pyAudioAnalysis.__file__)), "data", "models")
+        except ImportError:
+            models_dir = None
+    paths = None if models_dir is None else [os.path.join(models_dir, m) for m in _DIARIZATION_MODELS]
+    if paths is None or not all(os.path.isfile(p) and os.path.isfile(p + "MEANS") for p in paths):
+        raise FileNotFoundError("speaker_diarization needs the SVM models %s and %s (with their MEANS files) in "
+                                "pyAudioAnalysis/data/models or models_dir" % _DIARIZATION_MODELS)
+    return paths
+
+
+def _diarization_features(filename, mid_window, mid_step):
+    """(mid [136, M], st [68, T], duration) of a file as speaker_diarization computes them (:828-846): the file read,
+    downmixed, and its mid-term features on the GPU (the drop-in mid_feature_extraction) at a 50 ms short-term window
+    and step."""
+    from . import audioio
+    from .MidTermFeatures import mid_feature_extraction
+    sampling_rate, signal = audioio.read_audio_file(filename)
+    signal = audioio.stereo_to_mono(signal)
+    duration = len(signal) / sampling_rate
+    mid, st, _ = mid_feature_extraction(signal, sampling_rate, mid_window * sampling_rate, mid_step * sampling_rate,
+                                        round(sampling_rate * 0.05), round(sampling_rate * 0.05))
+    return mid, st, duration
+
+
+def speaker_diarization(filename, n_speakers, mid_window=1.0, mid_step=0.1, short_window=0.1, lda_dim=0, plot_res=False,
+                        models_dir=None):
+    """The reference's speaker_diarization: (cls, cluster purity, speaker purity), the purities -1 without a .segments
+    file next to the WAV; prints them as the reference does.  Mid-term features on the GPU (the drop-in
+    mid_feature_extraction), then ``diarize``."""
+    paths = _models_dir(models_dir)
+    loaded = [_load_svm(p) for p in paths]
+    mid_feats, st_feats, duration = _diarization_features(filename, mid_window, mid_step)
+    return _diarize_file(filename, [m[:3] for m in loaded], mid_feats, st_feats, duration, n_speakers, mid_window,
+                         mid_step, short_window, lda_dim, plot_res)
+
+
+def _diarize_file(filename, models, mid_feats, st_feats, duration, n_speakers, mid_window, mid_step, short_window, lda_dim,
+                  plot_res):
+    """speaker_diarization after the features: diarize, the ground-truth lookup, the printed purities and the plot."""
+    cls, info = diarize(mid_feats, models, n_speakers, mid_step, short_window, lda_dim, st=st_feats,
+                        mid_window=mid_window, details=True)
+    num_speakers = info["num_speakers"]
+    class_names = ["speaker{0:d}".format(c) for c in range(num_speakers)]
+    gt_file = filename.replace(".wav", ".segments")
+    flags_gt = None
+    if os.path.isfile(gt_file):
+        seg_start, seg_end, seg_labs = read_segmentation_gt(gt_file)
+        flags_gt, _ = segments_to_labels(seg_start, seg_end, seg_labs, mid_step)
+    plt = None
+    if plot_res:
+        try:
+            import matplotlib.pyplot as plt
+        except ImportError:
+            plt = None
+    if plt is not None:
+        fig = plt.figure()
+        ax1 = fig.add_subplot(111) if n_speakers > 0 else fig.add_subplot(211)
+        ax1.set_yticks(np.array(range(len(class_names))))
+        ax1.axis((0, duration, -1, len(class_names)))
+        ax1.set_yticklabels(class_names)
+        ax1.plot(np.array(range(len(cls))) * mid_step + mid_step / 2.0, cls)
+    purity_cluster_m, purity_speaker_m = -1, -1
+    if flags_gt is not None:
+        if plt is not None:
+            ax1.plot(np.array(range(len(flags_gt))) * mid_step + mid_step / 2.0, flags_gt, "r")
+        purity_cluster_m, purity_speaker_m = evaluate_speaker_diarization(cls, flags_gt)
+        print("{0:.1f}\t{1:.1f}".format(100 * purity_cluster_m, 100 * purity_speaker_m))
+        if plt is not None:
+            plt.title("Cluster purity: {0:.1f}% - Speaker purity: {1:.1f}%".format(100 * purity_cluster_m,
+                                                                                   100 * purity_speaker_m))
+    if plt is not None:
+        plt.xlabel("time (seconds)")
+        if n_speakers <= 0:
+            plt.subplot(212)
+            plt.plot(list(range(2, 10)), info["sil_all"])
+            plt.xlabel("number of clusters")
+            plt.ylabel("average clustering's sillouette")
+        plt.show()
+    return cls, purity_cluster_m, purity_speaker_m
+
+
+def speaker_diarization_evaluation(folder_name, lda_dimensions, models_dir=None):
+    """Print the cluster and speaker purity of every WAV file of a folder with a .segments file, for each LDA dimension,
+    as the reference does by calling speaker_diarization(wav, n, 2.0, 0.2, 0.05, dim) per file; the speaker count of each
+    file comes from its ground truth (-1 without one).  Each file is read, downmixed and its features computed once, at
+    its first turn, and reused for every LDA dimension."""
+    wav_files = sorted(glob.glob(os.path.join(folder_name, "*.wav")))
+    num_speakers = []
+    for wav_file in wav_files:
+        gt_file = wav_file.replace(".wav", ".segments")
+        if os.path.isfile(gt_file):
+            _, _, seg_labs = read_segmentation_gt(gt_file)
+            num_speakers.append(len(list(set(seg_labs))))
+        else:
+            num_speakers.append(-1)
+    models, features = None, {}
+    for dim in lda_dimensions:
+        print("LDA = {0:d}".format(dim))
+        for i, wav_file in enumerate(wav_files):
+            if models is None:
+                models = [_load_svm(p)[:3] for p in _models_dir(models_dir)]
+            if i not in features:
+                features[i] = _diarization_features(wav_file, 2.0, 0.2)
+            mid, st, duration = features[i]
+            _diarize_file(wav_file, models, mid, st, duration, num_speakers[i], 2.0, 0.2, 0.05, dim, False)

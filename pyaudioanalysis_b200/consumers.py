@@ -247,14 +247,19 @@ def _host_counts(n_windows, B, M, lo):
 
 
 def hmm_decode_batch(mid, model, n_windows=None):
-    """GaussianHMM.predict (hmmlearn's Viterbi) of the windows of every clip of a CUDA float32 [B, F, M] mid-term batch, in
-    one launch pair on the current stream (DESIGN.md, kernel 7).  ``n_windows``: each clip's window count (>= 1), host
-    integers or a CUDA tensor; None: all M.  Returns CUDA (ids int32 [B, M], each clip's states and zeros past its count;
-    bad bool [B], True for a clip with a non-finite feature, whose ids are left unwritten -- hmmlearn raises ValueError
-    for it).  `model`: an HmmModel, or an HMM uploaded for this call."""
+    """GaussianHMM.predict (hmmlearn's Viterbi) of the windows of every clip of a CUDA float32 or float64 [B, F, M]
+    mid-term batch, in one launch pair on the current stream (DESIGN.md, kernel 7).  float32 is contiguous; float64 is
+    contiguous, or the transpose of a contiguous [B, M, F] batch of one window per row (``X.T`` of a C-contiguous X): a
+    window's density terms are then added pairwise, as predict(X) adds them, else in sequence, as predict(features.T)
+    does.  ``n_windows``: each clip's window count (>= 1), host integers or a CUDA tensor; None: all M.  Returns CUDA
+    (ids int32 [B, M], each clip's states and zeros past its count; bad bool [B], True for a clip with a non-finite
+    feature, whose ids are left unwritten -- hmmlearn raises ValueError for it).  `model`: an HmmModel, or an HMM
+    uploaded for this call."""
     _require_cuda(mid, "mid")
-    if mid.dim() != 3 or mid.dtype != torch.float32 or not mid.is_contiguous():
-        raise ValueError("mid must be contiguous float32 [B, F, M]")
+    window_major = (mid.dim() == 3 and mid.dtype == torch.float64 and not mid.is_contiguous()
+                    and mid.transpose(1, 2).is_contiguous())
+    if mid.dim() != 3 or mid.dtype not in (torch.float32, torch.float64) or not (mid.is_contiguous() or window_major):
+        raise ValueError("mid must be contiguous float32 / float64 [B, F, M], or float64 [B, M, F] transposed")
     if not isinstance(model, HmmModel):
         model = HmmModel(model, mid.device)
     B, F, M = mid.shape
@@ -266,7 +271,14 @@ def hmm_decode_batch(mid, model, n_windows=None):
     with torch.cuda.device(mid.device):
         ids = torch.zeros((B, M), dtype=torch.int32, device=mid.device)
         bad = torch.zeros((B,), dtype=torch.int32, device=mid.device)
-        if B:
+        if B and mid.dtype == torch.float64:
+            check(lib().b200aa_hmm_decode_f64(
+                ctypes.c_void_p(mid.data_ptr()), B, F, M, int(window_major), ctypes.c_void_p(counts.ctypes.data),
+                model.n_states, ctypes.c_void_p(model.log_start.data_ptr()), ctypes.c_void_p(model.log_trans.data_ptr()),
+                ctypes.c_void_p(model.means.data_ptr()), ctypes.c_void_p(model.vars.data_ptr()),
+                ctypes.c_void_p(model.const.data_ptr()), ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(bad.data_ptr()),
+                _stream()))
+        elif B:
             check(lib().b200aa_hmm_decode(
                 ctypes.c_void_p(mid.data_ptr()), B, F, M, ctypes.c_void_p(counts.ctypes.data), model.n_states,
                 ctypes.c_void_p(model.log_start.data_ptr()), ctypes.c_void_p(model.log_trans.data_ptr()),
@@ -297,6 +309,37 @@ def hmm_statistics_batch(mid, class_windows, n_windows=None):
             ctypes.c_void_p(counts.ctypes.data), len(lists), ctypes.c_void_p(off.ctypes.data),
             ctypes.c_void_p(idx.ctypes.data), ctypes.c_void_p(out.data_ptr()), _stream()))
     return out
+
+
+def cluster_distance_means(X, labels, K, rows=None):
+    """The cluster distance means of speaker_diarization's silhouette (audioSegmentation.py:958-972) for one clustering,
+    in one call on the current stream (``b200aa_cluster_distance_means``, DESIGN.md kernel 9).
+
+    X: CUDA float64 [n, D] (rows at any stride; a non-unit column stride is copied); labels: n host integers in [0, K);
+    rows: the clusters c to compute (None: all).  Returns CUDA float64 (A [K], B [K, K]): A[c] =
+    np.mean(pdist(X[labels == c].T)), B[c, c2] = np.mean(cdist(X[labels == c], X[labels == c2])), bit for bit; NaN on the
+    diagonal of B, for clusters not asked for and for a mean of no terms (D < 2, an empty cluster), where NumPy warns."""
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, D]")
+    n, D = X.shape
+    if D > 1 and X.stride(1) != 1:
+        X = X.contiguous()
+    labels = np.ascontiguousarray(labels.cpu().numpy() if isinstance(labels, torch.Tensor) else labels)
+    if labels.shape != (n,):
+        raise ValueError("labels must hold one cluster per row of X (%d)" % n)
+    labels = labels.astype(np.int32)
+    want = np.ones(K, dtype=np.uint8)
+    if rows is not None:
+        want[:] = 0
+        want[np.asarray(list(rows), dtype=np.int64)] = 1
+    with torch.cuda.device(X.device):
+        A = torch.empty(K, dtype=torch.float64, device=X.device)
+        B = torch.empty((K, K), dtype=torch.float64, device=X.device)
+        check(lib().b200aa_cluster_distance_means(
+            ctypes.c_void_p(X.data_ptr()), n, D, X.stride(0) if n > 1 else D, ctypes.c_void_p(labels.ctypes.data), int(K),
+            ctypes.c_void_p(want.ctypes.data), ctypes.c_void_p(A.data_ptr()), ctypes.c_void_p(B.data_ptr()), _stream()))
+    return A, B
 
 
 TREE_FOREST, TREE_BOOST = 0, 1

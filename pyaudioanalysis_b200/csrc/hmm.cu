@@ -35,8 +35,10 @@ __global__ void __launch_bounds__(128) hmm_stats_kernel(const T *__restrict__ mi
 
 // One thread per (clip, window, state), consecutive threads on consecutive windows of one (clip, state): e[row, state] of the
 // slice, row = the clip's first row + window.  clips[2b] = the clip's window count, clips[2b + 1] its first global row.
-// A non-finite feature of a valid window raises bad[b].
-__global__ void __launch_bounds__(128) hmm_emission_kernel(const float *__restrict__ mid, int F, int64_t m_stride,
+// A non-finite feature of a valid window raises bad[b].  kWindowMajor: clip b is a C-contiguous [m_stride, F] matrix whose
+// rows NumPy sums pairwise; else [F, m_stride], summed in sequence unless the clip has one window.
+template <class T, bool kWindowMajor>
+__global__ void __launch_bounds__(128) hmm_emission_kernel(const T *__restrict__ mid, int F, int64_t m_stride,
                                                            const int64_t *__restrict__ clips, int64_t b0, int64_t row_base,
                                                            int C, const double *__restrict__ mu, const double *__restrict__ var,
                                                            const double *__restrict__ konst, double *__restrict__ e,
@@ -47,15 +49,16 @@ __global__ void __launch_bounds__(128) hmm_emission_kernel(const float *__restri
     const int64_t t = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
     const int64_t n = clips[2 * b];
     if (t >= n) return;
-    const float *x = mid + size_t(b) * F * m_stride + t;
-    auto xf = [&](int64_t f) { return double(x[f * m_stride]); };
+    const int64_t f_stride = kWindowMajor ? 1 : m_stride;
+    const T *x = mid + size_t(b) * F * m_stride + (kWindowMajor ? t * F : t);
+    auto xf = [&](int64_t f) { return double(x[f * f_stride]); };
     if (j == 0) {
         bool finite = true;
-        for (int f = 0; f < F; ++f) finite &= isfinite(x[int64_t(f) * m_stride]);
+        for (int f = 0; f < F; ++f) finite &= isfinite(x[int64_t(f) * f_stride]);
         if (!finite) bad[b] = 1;
     }
     e[(clips[2 * b + 1] - row_base + t) * C + j] =
-        hmm::emission(xf, mu + size_t(j) * F, var + size_t(j) * F, F, konst[j], n == 1);
+        hmm::emission(xf, mu + size_t(j) * F, var + size_t(j) * F, F, konst[j], kWindowMajor || n == 1);
 }
 
 // One warp per clip: the forward pass serial in t, lanes on states j, j + 32, ...; delta_{t-1} and delta_t in shared memory,
@@ -149,15 +152,13 @@ extern "C" int b200aa_hmm_statistics(const void *d_mid, int dtype, int64_t n_cli
     return scratch.done(B200AA_OK);
 }
 
-extern "C" int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, const int64_t *h_n_windows,
-                                 int n_states, const double *d_log_start, const double *d_log_trans, const double *d_means,
-                                 const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
+namespace {
+// b200aa_hmm_decode / b200aa_hmm_decode_f64 after their argument checks
+template <class T, bool kWindowMajor>
+int hmm_decode(const T *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, const int64_t *h_n_windows, int n_states,
+               const double *d_log_start, const double *d_log_trans, const double *d_means, const double *d_vars,
+               const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
 {
-    NvtxRange nvtx_("b200aa_hmm_decode");
-    if (!d_mid || !h_n_windows || !d_log_start || !d_log_trans || !d_means || !d_vars || !d_const || !d_ids || !d_bad ||
-        n_clips < 1 || n_feats < 1 || m_stride < 1 || n_states < 1 || n_states > hmm::kMaxStates ||
-        !hmm_counts_ok(h_n_windows, n_clips, m_stride, 1))
-        return B200AA_ERR_INVALID;
     // per clip (window count, first global row); slices of whole clips whose e + backpointers stay under kScratchSliceBytes
     // (a clip larger than that on its own is a slice of its own), at most 65535 clips (grid z)
     const size_t row_bytes = size_t(n_states) * (sizeof(double) + sizeof(int32_t));
@@ -194,12 +195,50 @@ extern "C" int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feat
         int64_t max_n = 0;
         for (int64_t b = b0; b < b1; ++b) max_n = std::max(max_n, h_n_windows[b]);
         const int64_t row_base = clips[2 * b0 + 1];
-        hmm_emission_kernel<<<dim3(unsigned((max_n + 127) / 128), unsigned(n_states), unsigned(b1 - b0)), 128, 0, st>>>(
-            d_mid, n_feats, m_stride, d_clips, b0, row_base, n_states, d_means, d_vars, d_const, e, d_bad);
+        hmm_emission_kernel<T, kWindowMajor><<<dim3(unsigned((max_n + 127) / 128), unsigned(n_states), unsigned(b1 - b0)), 128, 0,
+                                               st>>>(d_mid, n_feats, m_stride, d_clips, b0, row_base, n_states, d_means, d_vars,
+                                                     d_const, e, d_bad);
         CK_LAUNCH("hmm_emission_kernel");
         hmm_viterbi_kernel<<<unsigned(b1 - b0), 32, smem, st>>>(d_clips, b0, row_base, n_states, m_stride, d_log_start,
                                                                d_log_trans, e, bp, d_bad, d_ids);
         CK_LAUNCH("hmm_viterbi_kernel");
     }
     return scratch.done(B200AA_OK);
+}
+
+bool hmm_decode_ok(const void *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, const int64_t *h_n_windows, int n_states,
+                   const double *d_log_start, const double *d_log_trans, const double *d_means, const double *d_vars,
+                   const double *d_const, int32_t *d_ids, int32_t *d_bad)
+{
+    return d_mid && h_n_windows && d_log_start && d_log_trans && d_means && d_vars && d_const && d_ids && d_bad && n_clips >= 1 &&
+           n_feats >= 1 && m_stride >= 1 && n_states >= 1 && n_states <= hmm::kMaxStates &&
+           hmm_counts_ok(h_n_windows, n_clips, m_stride, 1);
+}
+}  // namespace
+
+extern "C" int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, const int64_t *h_n_windows,
+                                 int n_states, const double *d_log_start, const double *d_log_trans, const double *d_means,
+                                 const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
+{
+    NvtxRange nvtx_("b200aa_hmm_decode");
+    if (!hmm_decode_ok(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars,
+                       d_const, d_ids, d_bad))
+        return B200AA_ERR_INVALID;
+    return hmm_decode<float, false>(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means,
+                                    d_vars, d_const, d_ids, d_bad, stream);
+}
+
+extern "C" int b200aa_hmm_decode_f64(const double *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, int window_major,
+                                     const int64_t *h_n_windows, int n_states, const double *d_log_start,
+                                     const double *d_log_trans, const double *d_means, const double *d_vars,
+                                     const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
+{
+    NvtxRange nvtx_("b200aa_hmm_decode_f64");
+    if ((window_major != 0 && window_major != 1) ||
+        !hmm_decode_ok(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars,
+                       d_const, d_ids, d_bad))
+        return B200AA_ERR_INVALID;
+    auto run = window_major ? hmm_decode<double, true> : hmm_decode<double, false>;
+    return run(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars, d_const,
+               d_ids, d_bad, stream);
 }

@@ -62,6 +62,22 @@ def install_segmentation(audio_segmentation=None):
     return done + ["%s.%s" % (audio_segmentation.__name__, n)]
 
 
+def install_diarization(audio_segmentation=None):
+    """Rebind an importable ``pyAudioAnalysis.audioSegmentation`` (or the module given) to the speaker diarization here
+    (``audioSegmentation.diarize``: the silhouette means on kernel 9, the HMM smoothing on kernel 7): speaker_diarization,
+    speaker_diarization_evaluation and evaluate_speaker_diarization.  Returns the attributes rebound."""
+    from . import audioSegmentation as ours
+    if audio_segmentation is None:
+        import importlib
+        audio_segmentation = importlib.import_module("pyAudioAnalysis.audioSegmentation")
+    done = []
+    for n in ("speaker_diarization", "speaker_diarization_evaluation", "evaluate_speaker_diarization"):
+        _saved.setdefault((audio_segmentation, n), getattr(audio_segmentation, n))
+        setattr(audio_segmentation, n, getattr(ours, n))
+        done.append("%s.%s" % (audio_segmentation.__name__, n))
+    return done
+
+
 def uninstall():
     for (mod, n), fn in list(_saved.items()):
         setattr(mod, n, fn)
