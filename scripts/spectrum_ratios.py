@@ -1,6 +1,6 @@
 """Worst measured err / bound of the spectrum check per kernel kind and window class (DESIGN section 6), and what the
 x - x[frame start] subtraction costs on the frames of edge_impulses_f32 at 800 / 200 (a loud first sample).  Runs the
-cases of tests/test_gpu_spectra.py through its helpers; any case outside the bound raises.
+cases of tests/test_gpu_spectra.py through the same helpers (tests/parity.py); any case outside the bound raises.
 
     python scripts/spectrum_ratios.py        (on a GPU machine)
 """
@@ -19,8 +19,7 @@ def main():
     from oracle import st_oracle as O
     from tests import parity as PA
     from tests import signals as SG
-    from tests import test_gpu_spectra as TS
-    from tests.kernels import CTA, GENERIC_SWEEP, KIND_NAMES, PAIR, SOLO, plans
+    from tests.kernels import CTA, CTA_CONFIGS, GENERIC_SWEEP, KIND_NAMES, PAIR, PAIR_CONFIGS, SOLO, SOLO_CONFIGS, plans
     from pyaudioanalysis_b200._lib import Plan
     import pyaudioanalysis_b200 as pkg
     worst = {}
@@ -29,16 +28,16 @@ def main():
         r = worst.get((kind, cls), (0.0, 0.0))
         worst[(kind, cls)] = (max([r[0]] + [q[0] for q in ratios]), max([r[1]] + [q[1] for q in ratios]))
 
-    for fs, w, s in TS.PAIR_CONFIGS:
-        note("pair", "hop N/2" if 2 * s == w else "other hops", TS.pair_spectra(pkg, fs, w, s))
-    for kind, configs in ((SOLO, TS.SOLO_CONFIGS), (CTA, TS.CTA_CONFIGS)):
+    for fs, w, s in PAIR_CONFIGS:
+        note("pair", "hop N/2" if 2 * s == w else "other hops", PA.pair_spectra(pkg, fs, w, s))
+    for kind, configs in ((SOLO, SOLO_CONFIGS), (CTA, CTA_CONFIGS)):
         for fs, w, s in configs:
-            for cls, ratios in TS.row_spectra(pkg, Plan(fs, w, s).prefer_kernel(kind), fs, w, s, KIND_NAMES[kind],
+            for cls, ratios in PA.row_spectra(pkg, Plan(fs, w, s).prefer_kernel(kind), fs, w, s, KIND_NAMES[kind],
                                               offset_view=kind == CTA).items():
                 note(KIND_NAMES[kind], cls, ratios)
     for fs, w, G, path in GENERIC_SWEEP:
         cls = "%s, %s" % ("even" if w % 2 == 0 else "odd", "global scratch" if G == 0 else "G = %d" % G)
-        note("generic", cls, TS.generic_spectra(pkg, fs, w, path))
+        note("generic", cls, PA.generic_spectra(pkg, fs, w, path))
     for (kind, cls), (r, rd) in sorted(worst.items()):
         print(json.dumps({"kernel": kind, "class": cls, "bins_err_over_bound": round(r, 4), "dc_err_over_bound": round(rd, 4)}))
     # edge_impulses_f32 at 800 / 200: err / bound with |z| (the check) and with |y_frame| in its place (a transform of

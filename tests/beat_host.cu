@@ -10,21 +10,9 @@
 #include <vector>
 
 #include "../pyaudioanalysis_b200/csrc/beat.cuh"
+#include "host_io.h"
 
 using namespace b200aa;
-
-static double rd()
-{
-    char buf[64];
-    if (scanf("%63s", buf) != 1) exit(2);
-    return strtod(buf, nullptr);
-}
-static long long rl() { return (long long)rd(); }
-static void pr(double x)
-{
-    if (x != x) printf(" nan");
-    else printf(" %a", x);
-}
 
 template <class G>
 static double lanes_sum(const G &get, int64_t n, int64_t nz, int levels)
@@ -67,8 +55,7 @@ int main()
     while (scanf("%15s", cmd) == 1) {
         if (!strcmp(cmd, "sum")) {
             const int64_t N = rl();
-            std::vector<double> v(N);
-            for (auto &x : v) x = rd();
+            const std::vector<double> v = rv(size_t(N));
             auto get = [&](int64_t i) { return v[i]; };
             const int64_t K = rl();
             for (int64_t j = 0; j < K; ++j) {
@@ -82,16 +69,14 @@ int main()
         } else if (!strcmp(cmd, "peaks")) {
             const int32_t C = int32_t(rl()), T = int32_t(rl());
             const double delta = rd();
-            std::vector<double> v(T);
-            for (auto &x : v) x = rd();
+            const std::vector<double> v = rv(size_t(T));
             printf("peaks");
             chunked_scan([&](int32_t i) { return v[i]; }, T, C, delta, [](int32_t p) { printf(" %d", p); });
             printf("\n");
         } else if (!strcmp(cmd, "beat")) {
             const int32_t C = int32_t(rl()), F = int32_t(rl()), T = int32_t(rl());
             const double w = rd();
-            std::vector<double> st(size_t(F) * T);
-            for (auto &x : st) x = rd();
+            const std::vector<double> st = rv(size_t(F) * T);
             const int64_t mbt = int64_t(std::nearbyint(2.0 / w));
             const int64_t nb = std::min<int64_t>(mbt, std::max(T - 1, 0));
             std::vector<unsigned> cnt(size_t(beat::kRows) * nb, 0u);

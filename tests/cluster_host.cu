@@ -12,21 +12,9 @@
 #include <vector>
 
 #include "../pyaudioanalysis_b200/csrc/cluster.cuh"
+#include "host_io.h"
 
 using namespace b200aa;
-
-static double rd()
-{
-    char buf[64];
-    if (scanf("%63s", buf) != 1) exit(2);
-    return strtod(buf, nullptr);
-}
-static long long rl() { return (long long)rd(); }
-static void pr(double x)
-{
-    if (x != x) printf(" nan");
-    else printf(" %a", x);
-}
 
 // the distance of items u, v of segment s: the kernel's chain
 static double chain(const cluster::Segment &s, const double *G, int D, int64_t u, int64_t v)
@@ -56,8 +44,7 @@ int main()
             for (auto &l : labels) l = int(rl());
             std::vector<unsigned char> want(K);
             for (auto &w : want) w = (unsigned char)rl();
-            std::vector<double> X(size_t(n) * D);
-            for (auto &x : X) x = rd();
+            const std::vector<double> X = rv(size_t(n) * D);
             // G: the rows of each cluster together, in ascending order (cluster_gather_kernel)
             std::vector<int64_t> off(K + 1, 0);
             for (int l : labels) ++off[l + 1];
@@ -104,8 +91,7 @@ int main()
             const int kind = int(rl());
             const int64_t n = rl();
             const int D = int(rl());
-            std::vector<double> X(size_t(n) * D);
-            for (auto &x : X) x = rd();
+            const std::vector<double> X = rv(size_t(n) * D);
             cluster::Segment s{};
             s.kind = kind;
             if (kind == cluster::kBlock) {

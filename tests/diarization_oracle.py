@@ -14,6 +14,22 @@ from sklearn.preprocessing import StandardScaler
 from tests import hmm_oracle as H
 
 
+def reference(X, labels, K, want=None):
+    """(A [K], B [K, K]) as speaker_diarization computes them (audioSegmentation.py:958-972), NaN where not computed."""
+    A, B = np.full(K, np.nan), np.full((K, K), np.nan)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)
+        for c in range(K):
+            if want is not None and not want[c]:
+                continue
+            xc = X[labels == c, :]
+            A[c] = np.mean(distance.pdist(xc.T))
+            for c2 in range(K):
+                if c2 != c:
+                    B[c, c2] = np.mean(distance.cdist(xc, X[labels == c2, :]))
+    return A, B
+
+
 def statistics(features, labels):
     """train_hmm_compute_statistics (:287-344) in NumPy: priors, transitions, means, std of features [F, n]."""
     u_label = np.unique(labels)

@@ -11,27 +11,9 @@
 #include <vector>
 
 #include "../pyaudioanalysis_b200/csrc/hmm.cuh"
+#include "host_io.h"
 
 using namespace b200aa;
-
-static double rd()
-{
-    char buf[64];
-    if (scanf("%63s", buf) != 1) exit(2);
-    return strtod(buf, nullptr);
-}
-static long long rl() { return (long long)rd(); }
-static void pr(double x)
-{
-    if (x != x) printf(" nan");
-    else printf(" %a", x);
-}
-static std::vector<double> rv(size_t n)
-{
-    std::vector<double> v(n);
-    for (auto &x : v) x = rd();
-    return v;
-}
 
 int main()
 {

@@ -1,8 +1,32 @@
-"""Helpers shared by the GPU test modules: the kernel kinds a plan reaches and ragged batches on the device."""
+"""Kernel kinds and the configurations the tests run them at, shared by the test modules and the golden generators: the
+kernel kinds a plan reaches, the (fs, window, hop) lists of each sweep, the specialised windows and sample rates, and
+ragged batches on the device."""
 import numpy as np
 
 PAIR, SOLO, CTA, GENERIC = 2, 3, 1, 0
 KIND_NAMES = {PAIR: "pair", SOLO: "solo", CTA: "CTA", GENERIC: "generic"}
+
+# Feature configs of the adversarial bank (tests/test_gpu_adversarial.py, tests/test_gpu_feature_bounds.py): (fs, window,
+# hop) and the kernel kinds a plan reaches through prefer_kernel / force_generic
+FEATURE_CONFIGS = [
+    (16000, 320, 160, {PAIR, CTA, GENERIC}), (16000, 480, 240, {PAIR, CTA, GENERIC}), (16000, 512, 256, {PAIR, GENERIC}),
+    (16000, 640, 320, {PAIR, CTA, GENERIC}), (16000, 800, 400, {PAIR, CTA, GENERIC}), (48000, 960, 480, {PAIR, GENERIC}),
+    (16000, 1024, 512, {PAIR, GENERIC}), (16000, 800, 800, {PAIR, CTA, GENERIC}), (16000, 800, 200, {PAIR, CTA, GENERIC}),
+    (16000, 800, 333, {PAIR, CTA, GENERIC}), (16000, 1024, 300, {PAIR, GENERIC}),
+    (44100, 882, 441, {SOLO, CTA, GENERIC}), (44100, 882, 300, {SOLO, CTA, GENERIC}), (16000, 400, 160, {SOLO, CTA, GENERIC}),
+    (16000, 400, 200, {SOLO, CTA, GENERIC}), (8000, 600, 300, {SOLO, CTA, GENERIC}),
+    (22050, 551, 200, {GENERIC}), (16000, 883, 300, {GENERIC}), (16000, 2048, 1024, {GENERIC}),
+]
+# Row configs (spectrogram / chromagram) of the adversarial bank and the chromagram bounds
+ROW_CONFIGS = [(16000, 800, 400), (16000, 800, 333), (44100, 882, 441), (16000, 400, 160), (8000, 600, 300)]
+# Spectrum checks per kernel kind (tests/test_gpu_spectra.py, scripts/spectrum_ratios.py).
+# pair kernel: every window at hop N / 2 (shared halves), and the independent-frame path at other hops
+PAIR_CONFIGS = [(16000, 320, 160), (16000, 480, 240), (16000, 512, 256), (16000, 640, 320), (16000, 800, 400),
+                (48000, 960, 480), (16000, 1024, 512), (16000, 800, 200), (16000, 800, 333), (16000, 800, 800),
+                (16000, 1024, 300)]
+SOLO_CONFIGS = [(44100, 882, 441), (44100, 882, 300), (16000, 400, 200), (16000, 400, 160), (8000, 600, 300)]
+CTA_CONFIGS = [(16000, 320, 160), (16000, 400, 200), (16000, 480, 240), (8000, 600, 300), (16000, 640, 320),
+               (16000, 800, 400), (16000, 800, 200), (16000, 800, 333), (44100, 882, 441)]
 
 # Windows of the generic kernel's spectrum sweep (tests/test_gpu_spectra.py), each chosen for the code path it reaches:
 # (fs, window, frames per CTA group, path).  The group size G (8, 4, 2, 1; 0 = global scratch) is what launch_generic
@@ -79,6 +103,19 @@ RATE_CONFIGS = [
     (44100, 882, 1323, {SOLO, CTA, GENERIC}, "hop longer than the window"),
     (16000, 600, 900, {SOLO, CTA, GENERIC}, "hop longer than the window"),
 ]
+
+
+# The (fs, window) sweep of the specialised kernels' tables (tests/test_rates_cpu.py, tests/golden/rates.npz): every
+# specialised window at every rate of FINE and RATES.
+PAIR_WINDOWS = [320, 480, 512, 640, 800, 960, 1024]
+SOLO_WINDOWS = [400, 600, 882]
+CTA_WINDOWS = [320, 400, 480, 600, 640, 800, 882]
+WINDOWS = sorted(set(PAIR_WINDOWS + SOLO_WINDOWS + CTA_WINDOWS))
+FINE = list(range(6300, 7101))               # the mel bank's refusal boundary at every specialised window
+RATES = [8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 48000, 88200, 96000, 176400, 192000]
+# (window, hop) whose CTA staging exceeds its cap: the launcher returns unsupported and the generic kernel runs instead.
+# With run staging (hop a multiple of 8) the 800-sample window crosses the cap from hop 1 200 (6 854 Hz) .. 1 232 (16 kHz).
+CTA_FALLBACK = {(800, 1600)}
 
 
 def plans(fs, w, s):

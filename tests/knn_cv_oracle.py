@@ -47,3 +47,19 @@ def scores(y_test, y_pred):
     """The reference's per-experiment confusion_matrix and macro f1_score (:682-683)."""
     return (sklearn.metrics.confusion_matrix(y_test, y_pred),
             sklearn.metrics.f1_score(y_test, y_pred, average='macro'))
+
+
+def golden_features(g, c):
+    sizes = g[c + "_sizes"]
+    if c + "_gen" in g.files:
+        seed, F = (int(v) for v in g[c + "_gen"])
+        feats = seeded_features(seed, tuple(int(s) for s in sizes), F)
+        assert np.vstack(feats).sum() == g[c + "_X_sum"], c
+        return feats
+    return np.split(g[c + "_X"], np.cumsum(sizes)[:-1])
+
+
+def golden_args(g, c):
+    ids = g[c + "_ids"].tolist() or None
+    return (list(g[c + "_class_names"]), g[c + "_params"], int(g[c + "_mode"]), ids, int(g[c + "_n_exp"]),
+            float(g[c + "_train_percentage"]))

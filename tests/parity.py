@@ -20,11 +20,21 @@ float64 DFT under a bound derived from float32 FFT arithmetic (derivation: tests
 bound on every entry of the 68 rows (derivation: tests/test_feature_bounds_cpu.py).
 ``chromagram_bounds`` / ``check_chromagram_bounds`` do the same for chromagram rows: full rows from the spectrum bound,
 clipped rows from a per-bin model of the clipped-frame kernel's fp64 DFT (derivation: tests/test_chroma_bounds_cpu.py).
+
+The GPU tests share the runs behind these checks: every clip of a batch under its spectrum bound for each kernel kind
+(``pair_spectra``, ``row_spectra``, ``generic_spectra``), under its feature or chromagram bound (``batch_bounds``,
+``ragged_bounds``, ``check_rows``, accumulated by ``note`` and printed by ``report``), the clips that end in clipped
+chromagram frames (``clipped_clips``) and the exact check of a float32 clip record (``check_f32_clip``).
 """
+import contextlib
+import ctypes
+import json
 import math
 from fractions import Fraction
 
 import numpy as np
+
+from tests.kernels import PAIR, ragged
 
 RTOL, ATOL = 1e-4, 1e-5
 ZCR_ROW, ENERGY_ROW, ROLLOFF_ROW = 0, 1, 7
@@ -720,3 +730,242 @@ def check_chromagram_bounds(got, cb, what=""):
         if sel.any():
             worst[name] = float(ratio[sel].max())
     return worst, dict(cb.unbounded)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Every clip of a batch under its spectrum bound, through each kernel kind
+ODD = 3                 # sample offset of the unaligned view
+
+
+@contextlib.contextmanager
+def pair_dump(B, T, K):
+    """A NaN-filled float32 [B, T, K] buffer the pair kernel writes its |X| rows into while the block runs.  The dump
+    pointer is process-wide: it is cleared once the launches that may write through it are done, before the buffer is
+    freed, however the block ends."""
+    import torch
+    from pyaudioanalysis_b200._lib import lib
+    buf = torch.full((B, T, K), float("nan"), dtype=torch.float32, device="cuda")
+    assert lib().b200aa_debug_set_dump(ctypes.c_void_p(buf.data_ptr())) == 0
+    try:
+        yield buf
+    finally:
+        torch.cuda.synchronize()
+        lib().b200aa_debug_set_dump(None)
+
+
+def pair_spectra(P, fs, w, s):
+    """The bank plus odd_tail (int16 and float32) as ragged feature batches through the pair kernel, every frame's dumped
+    |X| row under the spectrum bound, exactly the frames below each clip's frame count written.  Returns the
+    (bins, DC) err / bound of every clip."""
+    from oracle import st_oracle as O
+    from pyaudioanalysis_b200._lib import Plan
+    from tests import signals as SG
+    pl = Plan(fs, w, s).prefer_kernel(PAIR)
+    assert pl.kernel_kind() == PAIR
+    K = w // 2
+    ints = dict(SG.bank(fs, w, s), odd_tail=SG.odd_tail(fs, w, s))
+    flts = dict(SG.float_bank(fs, w, s), odd_tail_f32=ints["odd_tail"].astype(np.float32) * np.float32(0.37) + np.float32(11.5))
+    ratios = []
+    for bank, dtype in ((ints, np.int16), (flts, np.float32)):
+        names, clips = list(bank), list(bank.values())
+        d, lens = ragged(clips, dtype)
+        with pair_dump(len(clips), O.frame_count(d.shape[1], w, s), K) as buf:
+            P.feature_extraction_batch(d, fs, w, s, lengths=lens, plan=pl)
+        got = buf.cpu().numpy()
+        for i, name in enumerate(names):
+            Tb = O.frame_count(clips[i].size, w, s)
+            what = "pair kernel |X| rows, fs=%d w=%d s=%d: %s (%d frames)" % (fs, w, s, name, Tb)
+            assert not np.isnan(got[i, :Tb]).any(), what + ": a frame below T_b was not written"
+            assert np.isnan(got[i, Tb:]).all(), what + ": a frame at or past T_b was written"
+            ratios.append(check_spectrum(got[i, :Tb], clips[i], s * np.arange(Tb), w, what))
+    return ratios
+
+
+def row_spectra(P, pl, fs, w, s, kind_name, offset_view=False):
+    """The bank (int16 and float32) as ragged batches through spectrogram_batch on plan pl, every clip's rows under the
+    spectrum bound; with offset_view also the int16 batch as a view at an odd sample offset.  Returns
+    {"int16" | "float32" | "odd offset": [(bins, DC) err / bound of every clip]}."""
+    from tests import signals as SG
+    ints, flts = SG.bank(fs, w, s), SG.float_bank(fs, w, s)
+    ratios = {}
+    for bank, dtype, offsets in ((ints, np.int16, (0, ODD) if offset_view else (0,)), (flts, np.float32, (0,))):
+        names, clips = list(bank), list(bank.values())
+        for off in offsets:
+            d, lens = ragged(clips, dtype, offset=off)
+            sp = P.spectrogram_batch(d, fs, w, s, plan=pl, lengths=lens).cpu().numpy()
+            for i, name in enumerate(names):
+                R = int((clips[i].size - w) / s) + 1
+                what = "%s rows, fs=%d w=%d s=%d%s: %s" % (kind_name, fs, w, s, ", odd offset" if off else "", name)
+                cls = "odd offset" if off else ("float32" if dtype == np.float32 else "int16")
+                ratios.setdefault(cls, []).append(check_spectrogram_rows(sp[i, :R], clips[i], w, s, what))
+    return ratios
+
+
+def generic_spectra(P, fs, w, path):
+    """sweep_clips through a force_generic plan (the int16 clips as a ragged batch, the float32 clip alone), every row
+    under the spectrum bound.  Returns the (bins, DC) err / bound of every clip."""
+    import torch
+    from pyaudioanalysis_b200._lib import Plan
+    from tests.signals import sweep_clips
+    s, ints, flt = sweep_clips(w)
+    pl = Plan(fs, w, s)
+    pl.force_generic(True)
+    d, lens = ragged(ints, np.int16)              # ragged row kernel
+    sp = P.spectrogram_batch(d, fs, w, s, plan=pl, lengths=lens).cpu().numpy()
+    ratios = [check_spectrogram_rows(sp[i], x, w, s, "generic rows, w=%d s=%d (%s): int16 clip %d" % (w, s, path, i))
+              for i, x in enumerate(ints)]
+    spf = P.spectrogram_batch(torch.from_numpy(flt).cuda()[None], fs, w, s, plan=pl).cpu().numpy()   # equal-length row kernel
+    ratios.append(check_spectrogram_rows(spf[0], flt, w, s, "generic rows, w=%d s=%d (%s): float32 chirp" % (w, s, path)))
+    return ratios
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Clips that end in clipped chromagram frames
+def prime_between(lo, hi):
+    for n in range((lo + hi) // 2, hi):
+        if n > 1 and all(n % d for d in range(2, int(n ** 0.5) + 1)):
+            return n
+    return None
+
+
+def clipped_targets(w, s):
+    """Lengths the last clipped frame of an accepted clip can have, picked at K, K + 1, a prime and w - 1 where each is
+    reachable.  The loop's last start p < len - s leaves n = len - p in (s, 2 s], and the reference needs n >= K; the
+    clipped frames before it have n + s, n + 2 s, ... < w samples."""
+    lo, hi = max(w // 2, s + 1), min(2 * s, w - 1)
+    out = [n for n in (w // 2, w // 2 + 1, prime_between(lo, hi + 1), w - 1, hi) if n is not None and lo <= n <= hi]
+    return sorted(set(out))
+
+
+def clipped_clips(fs, w, s, n_last):
+    """{name: clip} whose last chromagram row transforms a clipped frame of n_last samples, after a few full rows and the
+    other clipped rows of its chain.  Signals: noise; DC 20000 +- 3 LSB (the record's bp and the DC rebuild); quiet noise
+    with a loud first sample in every clipped frame (x - x0); a tone with a whole number of cycles in the last clipped
+    frame, off the w-point bins (its other classes are ~1e-10 of the total, where only an fp64 transform keeps them); +-1
+    LSB dither; a last clipped frame that is a run at the clip's exact integer mean (exact zeros); float32 noise at offset
+    11.5 and a float32 tone with noise at 1e-3 full scale."""
+    L = w + (-(-w // s) + 2) * s + n_last
+    _, n_it, n_full, refused = chromagram_rows(L, w, s)
+    assert not refused and n_full >= 2 and L - (w + (n_it - 1) * s) == n_last, (w, s, n_last)
+    rng = np.random.default_rng(w * 31 + s * 7 + n_last)
+    p_last = L - n_last
+    firsts = [w + i * s for i in range(n_full, n_it)]
+    t = np.arange(L)
+    cyc = max(3, round(n_last * 523.25 / fs))          # C5-ish, whole cycles over n_last samples
+    out = {"noise": np.round(rng.normal(0, 3000.0, L)).astype(np.int16),
+           "dc": (20000 + rng.integers(-3, 4, L)).astype(np.int16)}
+    x = np.round(rng.normal(0, 30.0, L))
+    x[firsts] = 30000.0
+    out["loud_first"] = x.astype(np.int16)
+    out["tone"] = np.round(20000.0 * np.sin(2 * np.pi * cyc * t / n_last + 0.3)).astype(np.int16)
+    out["dither"] = rng.integers(-1, 2, L).astype(np.int16)
+    x = rng.integers(-3000, 3001, L).astype(np.int64) + 7
+    x[p_last:] = 7
+    q, r = divmod(int(x.sum()) - 7 * L, w)
+    x[:w] -= q                                          # samples in no row: the clip mean becomes exactly 7
+    x[0] -= r
+    assert x.sum() == 7 * L
+    out["mean_run"] = x.astype(np.int16)
+    F = np.float32
+    out["noise_f32"] = (out["noise"].astype(F) * F(0.37) + F(11.5)).astype(F)
+    out["small_f32"] = (rng.normal(0, 1e-3 / 3, L) + 1e-3 * np.sin(2 * np.pi * cyc * t / n_last)).astype(F)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Batches under the per-entry bounds: worst err / bound and unbounded counts per (kernel, input), printed as JSON
+def note(acc, worst, unb):
+    for k, v in worst.items():
+        acc["worst"][k] = max(acc["worst"].get(k, 0.0), v)
+    for k, v in unb.items():
+        acc["unbounded"][k] = acc["unbounded"].get(k, 0) + v
+
+
+def report(tag, accs):
+    for key, acc in accs.items():
+        print(json.dumps(dict(config=tag, kernel=key[0], input=key[1],
+                              worst={k: round(v, 4) for k, v in acc["worst"].items()}, unbounded=acc["unbounded"])))
+
+
+def check_rows(out, cbs, what, accs, key):
+    """out [B, R, 12] of a ragged batch (or an equal-length one): clip i's rows under its bound, the rows past them
+    zero; a refused clip has none."""
+    for i, cb in enumerate(cbs):
+        R = cb.ref.shape[0]
+        assert not out[i, R:].any(), what[i] + ": rows past the clip's own"
+        if cb.refused:
+            continue
+        note(accs.setdefault(key, {"worst": {}, "unbounded": {}}), *check_chromagram_bounds(out[i, :R], cb, what[i]))
+
+
+def ragged_bounds(P, pl, clips, names, dtype, fs, w, s, tag, accs, key, cbs=None):
+    """clips as one ragged chromagram batch through plan pl, every clip under its bound.  Returns the bounds."""
+    d, lens = ragged(clips, dtype)
+    cbs = cbs or [chromagram_bounds(x, fs, w, s) for x in clips]
+    out = P.chromagram_batch(d, fs, w, s, plan=pl, lengths=lens).cpu().numpy()
+    assert P.row_counts(lens, w, s, 1).cpu().tolist() == [0 if cb.refused else cb.ref.shape[0] for cb in cbs], tag
+    check_rows(out, cbs, ["%s: %s" % (tag, n) for n in names], accs, key)
+    return cbs
+
+
+def batch_bounds(P, pl, clips, dtype, fs, w, s, what, acc):
+    """clips as one ragged batch through plan pl, deltas on and off, every clip under its bound; rows past a clip's
+    frame count stay zero."""
+    d, lens = ragged(clips, dtype)
+    fbs = [feature_bounds(x, fs, w, s, deltas=True) for x in clips]
+    for deltas in (True, False):
+        out = P.feature_extraction_batch(d, fs, w, s, lengths=lens, plan=pl, deltas=deltas).cpu().numpy()
+        for i, fb in enumerate(fbs):
+            T = fb.ref.shape[1]
+            F = 68 if deltas else 34
+            assert not out[i, :, T:].any(), what[i] + ": output past the clip's frames"
+            if not deltas:
+                fb = type(fb)(fb.ref[:34], fb.bound[:34], fb.roll, {k: v for k, v in fb.unbounded.items()
+                                                                    if not k.startswith("delta")}, fb.K)
+            note(acc, *check_feature_bounds(out[i, :F, :T], fb, what[i] + (", deltas" if deltas else ", no deltas")))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Kernel 0's clip record against exact arithmetic
+A_EMPTY = np.float32(1.0 / (32768.0 * 1e-10))      # a of a clip without samples (max deviation 0)
+
+
+def check_f32_clip(rec, x, what):
+    a, bp, m, lo, hi = (float(v) for v in rec[:5])
+    assert not rec[5:].any(), what + ": reserved words not cleared"
+    L = x.size
+    if L == 0:
+        assert rec[0] == A_EMPTY and not rec[1:5].any(), what + ": record of an empty clip"
+        return
+    xd = x.astype(np.float64)
+    total = math.fsum(xd.tolist())
+    mean = total / L
+    assert abs(m - mean) <= float(np.spacing(np.float32(abs(mean)))), "%s: m = %r, mean %r" % (what, m, mean)
+    if m == mean:
+        assert lo == hi == 0.0, "%s: mean %r is a float32 but lo / hi = %r / %r" % (what, mean, lo, hi)
+    else:
+        lo_abs, hi_abs = np.float32(m + lo), np.float32(m + hi)
+        assert float(lo_abs) < mean < float(hi_abs) and np.nextafter(lo_abs, np.float32(np.inf)) == hi_abs, \
+            "%s: [%r, %r] does not bracket the mean %r between neighbouring floats" % (what, m + lo, m + hi, mean)
+    ra = 1.0 / (max(xd.max() - mean, mean - xd.min()) + 32768.0 * 1e-10)
+    assert abs(a - ra) <= float(np.spacing(np.float32(ra))), "%s: a = %r, expected %r" % (what, a, ra)
+    rbp = ra * (m - mean)
+    assert abs(bp - rbp) <= 2.0 ** -24 * abs(rbp) + 2.0 ** -149 + ra * 2.0 ** -50 * float(np.abs(xd).sum()), \
+        "%s: bp = %r, expected %r" % (what, bp, rbp)
+    check_samples(rec, x, np.sign(xd - mean), what)
+
+
+def check_samples(rec, x, sign, what):
+    """lo / hi classify d = x - m (float32, as the kernels form it) exactly as sign(x - mean); fma(a, d, bp) is the
+    reference's normalised sample to float32 resolution of the clip's full scale."""
+    from oracle import st_oracle as O
+    a, bp, m, lo, hi = (np.float32(v) for v in rec[:5])
+    d = x.astype(np.float32) - m
+    cls = (d > lo).astype(np.int64) - (d < hi).astype(np.int64)
+    bad = cls != sign
+    assert not bad.any(), "%s: sign(x - mean) wrong for %d samples, first at %d" % (what, int(bad.sum()), int(np.argmax(bad)))
+    y = (np.float64(a) * d.astype(np.float64) + np.float64(bp)).astype(np.float32).astype(np.float64)
+    ref = O.normalize_clip(x.astype(np.float64))
+    tol = 8 * 2.0 ** -24 * np.abs(ref).max() + 1e-30
+    err = np.abs(y - ref)
+    assert err.max() <= tol, "%s: a (x - m) + bp off by %.3g (tolerance %.3g) at sample %d" % (what, err.max(), tol, int(np.argmax(err)))

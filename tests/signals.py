@@ -11,6 +11,9 @@ zero spectrum beyond DC, its mel bands become ``log10(round-off + eps)`` and its
 those rows of a reference matrix, and every row is then compared as usual.  The bank
 avoids the other inputs of that kind (tones exactly on a bin, periods that divide the window, Nyquist alternation)
 and keeps the spectral range inside each frame to about 60 dB; the range between frames is large on purpose.
+
+The other seeded inputs the tests share follow the bank: the short clips of the generic kernel's sweep, ``odd_tail``
+for the pair kernel, float32 short-term rows for mid-term pooling, and the peak-picking walks.
 """
 import math
 
@@ -202,3 +205,79 @@ def patch_noise_defined(F, x, window, hop):
             F[O.N_BASE:, 1:] = F[:O.N_BASE, 1:] - F[:O.N_BASE, :-1]
             F[O.N_BASE:, 0] = 0.0
     return F, bad
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Clips of the spectrum, feature and chromagram checks of the generic kernel's sweep and of the pair kernel
+def sweep_clips(w):
+    """Two int16 clips (noise; noise with a loud first sample in every other frame) and one float32 clip (a chirp),
+    long enough for five full spectrogram rows and a few rows past them."""
+    s = max(1, w // 2)
+    n = 2 * w + 5 * s + 3
+    rng = np.random.default_rng(w)
+    noise = np.round(rng.normal(0, 3000.0, n)).astype(np.int16)
+    edges = np.round(rng.normal(0, 30.0, n))
+    edges[w::2 * s] = 20000.0
+    t = np.arange(n)
+    chirp = (0.3 * np.sin(2 * np.pi * (0.01 + 0.4 * t / n) * t) + rng.normal(0, 0.01, n)).astype(np.float32)
+    return s, [noise, edges.astype(np.int16)], chirp
+
+
+def odd_tail(fs, w, s):
+    """A clip with an odd frame count whose last frame (paired with itself) is loud in its first half and 80 dB quieter in
+    its second: with shared halves the partner's energy is not the frame's own, and a scale taken from it buries the
+    frame under its copy."""
+    rng = np.random.default_rng(w + s)
+    T = 2 * (fs // (2 * s)) + 1
+    n = w + (T - 1) * s
+    x = rng.normal(0, 2.0, n)
+    a = (T - 1) * s
+    t = np.arange(w // 2)
+    x[a:a + w // 2] = 20000.0 * np.sin(2 * np.pi * 37.37 * t / w) + rng.normal(0, 300.0, w // 2)
+    x = np.round(x).astype(np.int16)
+    assert O.frame_count(n, w, s) == T and T % 2 == 1
+    return x
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Mid-term pooling: float32 short-term rows of every kind and the oracle's short-term matrix of a clip
+ROW_KINDS = 6
+
+
+def rows(rng, F, T, first_kind):
+    """float32 [F, T]: row f is of kind (first_kind + f) % 6."""
+    out = np.empty((F, T), dtype=np.float32)
+    for f in range(F):
+        k = (first_kind + f) % ROW_KINDS
+        n = rng.standard_normal(T)
+        if k == 0:
+            out[f] = n
+        elif k == 1:
+            out[f] = 3.25
+        elif k == 2:
+            out[f] = 1e4 + 1e-3 * n
+        elif k == 3:
+            out[f] = -99.00180475 + 1e-3 * n
+        elif k == 4:
+            out[f] = np.where(np.arange(T) % 2 == 0, 1.0, -1.0) * (1.0 + 0.1 * np.abs(n))
+        else:
+            out[f] = n
+            out[f, T // 2] = np.nan
+    return out
+
+
+def oracle_st(x, fs, w, s):
+    return patch_noise_defined(O.feature_extraction(x, fs, w, s)[0], x, w, s)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Peak picking and beat extraction (tests/golden/reference_checks.npz)
+def peak_inputs():
+    """(signal, delta, feature matrix) of the peak-picking comparison, seeded."""
+    rng = np.random.default_rng(3)
+    out = []
+    for k in range(6):
+        v = np.cumsum(rng.standard_normal(400)) * (0.1 + k)
+        delta = 2.0 * np.abs(np.diff(v)).mean()
+        out.append((v, delta, np.cumsum(rng.standard_normal((34, 200 + 30 * k)), axis=1)))
+    return out

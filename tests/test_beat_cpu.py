@@ -1,15 +1,15 @@
 """CPU: the pieces of the beat-extraction kernel (csrc/beat.cuh, __host__ __device__) run on the host by tests/beat_host.cu --
 NumPy's pairwise summation order, the chunked three-phase peak scan, and the whole per-clip computation -- against NumPy and
 the host MidTermFeatures.beat_extraction, bit for bit."""
-import subprocess
 
 import numpy as np
 import pytest
 
 from pyaudioanalysis_b200.MidTermFeatures import _peak_positions, beat_extraction
 from tests import host_exe
+from tests.host_exe import hexes, run
 from tests.conftest import load_golden
-from tests.test_host_cpu import peak_inputs
+from tests.signals import peak_inputs
 
 pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not available")
 
@@ -22,16 +22,6 @@ def exe(tmp_path_factory):
     return host_exe.build(tmp_path_factory, "beat_host.cu", "-O1")
 
 
-def _hex(values):
-    return " ".join(float(x).hex() for x in np.asarray(values, dtype=np.float64).ravel())
-
-
-def _run(exe, script):
-    res = subprocess.run([exe], input=script, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return [ln.split() for ln in res.stdout.splitlines()]
-
-
 def _same(a, b):
     """Bit-for-bit equality, NaN equal to NaN."""
     a, b = float(a), float(b)
@@ -42,7 +32,7 @@ def test_pairwise_sum_matches_numpy(exe):
     rng = np.random.default_rng(1)
     d = np.abs(np.diff(rng.standard_normal(200001).astype(np.float32).astype(np.float64)))
     lengths = list(range(0, 301)) + [1000, 8191, 8192, 8193, 16384, 143998, 200000]
-    out = _run(exe, "sum %d %s %d %s\n" % (d.size, _hex(d), len(lengths), " ".join(map(str, lengths))))
+    out = run(exe, "sum %d %s %d %s\n" % (d.size, hexes(d), len(lengths), " ".join(map(str, lengths))))
     assert len(out) == len(lengths)
     for n, line in zip(lengths, out):
         ref = float(np.add.reduce(d[:n]))
@@ -89,8 +79,8 @@ def test_chunked_scan_matches_peakdet(exe):
     script = []
     for v, delta in cases:
         for C in CHUNKS:
-            script.append("peaks %d %d %s %s" % (C, v.size, float(delta).hex(), _hex(v)))
-    out = _run(exe, "\n".join(script) + "\n")
+            script.append("peaks %d %d %s %s" % (C, v.size, float(delta).hex(), hexes(v)))
+    out = run(exe, "\n".join(script) + "\n")
     i = 0
     for v, delta in cases:
         ref = _peak_positions(v, delta)
@@ -112,9 +102,9 @@ def _beat_cases():
 
 def test_whole_clip_matches_host_beat_extraction(exe):
     cases = _beat_cases()
-    script = ["beat %d %d %d %s %s" % (C, st.shape[0], st.shape[1], float(w).hex(), _hex(st)) for st, w in cases
+    script = ["beat %d %d %d %s %s" % (C, st.shape[0], st.shape[1], float(w).hex(), hexes(st)) for st, w in cases
               for C in (3, 32, PRODUCTION_CHUNK)]
-    out = _run(exe, "\n".join(script) + "\n")
+    out = run(exe, "\n".join(script) + "\n")
     i = 0
     for st, w in cases:
         bpm, ratio = beat_extraction(st, w)

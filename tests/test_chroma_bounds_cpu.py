@@ -81,10 +81,9 @@ import scipy.fft
 from oracle import st_oracle as O
 from tests import host_exe
 from tests import signals as SG
-from tests.kernels import GENERIC_SWEEP
+from tests.kernels import GENERIC_SWEEP, ROW_CONFIGS
 from tests.parity import (DIV_REL, ROW_CLIPPED, ROW_EMPTY, ROW_FULL, _tables, check_chromagram_bounds, chromagram_bounds,
-                          chromagram_rows, clip_norm, gamma, sum_depth)
-from tests.test_gpu_adversarial import ROW_CONFIGS
+                          chromagram_rows, clip_norm, clipped_clips, clipped_targets, gamma, sum_depth)
 
 CONFIGS = ROW_CONFIGS + [(16000, 800, 200)]
 F = np.float32
@@ -194,56 +193,6 @@ def emulate(x, fs, w, s):
 
 def bank_clips(fs, w, s):
     return list(SG.bank(fs, w, s).items()) + list(SG.float_bank(fs, w, s).items())
-
-
-def _prime_between(lo, hi):
-    for n in range((lo + hi) // 2, hi):
-        if n > 1 and all(n % d for d in range(2, int(n ** 0.5) + 1)):
-            return n
-    return None
-
-
-def clipped_targets(w, s):
-    """Lengths the last clipped frame of an accepted clip can have, picked at K, K + 1, a prime and w - 1 where each is
-    reachable.  The loop's last start p < len - s leaves n = len - p in (s, 2 s], and the reference needs n >= K; the
-    clipped frames before it have n + s, n + 2 s, ... < w samples."""
-    lo, hi = max(w // 2, s + 1), min(2 * s, w - 1)
-    out = [n for n in (w // 2, w // 2 + 1, _prime_between(lo, hi + 1), w - 1, hi) if n is not None and lo <= n <= hi]
-    return sorted(set(out))
-
-
-def clipped_clips(fs, w, s, n_last):
-    """{name: clip} whose last chromagram row transforms a clipped frame of n_last samples, after a few full rows and the
-    other clipped rows of its chain.  Signals: noise; DC 20000 +- 3 LSB (the record's bp and the DC rebuild); quiet noise
-    with a loud first sample in every clipped frame (x - x0); a tone with a whole number of cycles in the last clipped
-    frame, off the w-point bins (its other classes are ~1e-10 of the total, where only an fp64 transform keeps them); +-1
-    LSB dither; a last clipped frame that is a run at the clip's exact integer mean (exact zeros); float32 noise at offset
-    11.5 and a float32 tone with noise at 1e-3 full scale."""
-    L = w + (-(-w // s) + 2) * s + n_last
-    _, n_it, n_full, refused = chromagram_rows(L, w, s)
-    assert not refused and n_full >= 2 and L - (w + (n_it - 1) * s) == n_last, (w, s, n_last)
-    rng = np.random.default_rng(w * 31 + s * 7 + n_last)
-    p_last = L - n_last
-    firsts = [w + i * s for i in range(n_full, n_it)]
-    t = np.arange(L)
-    cyc = max(3, round(n_last * 523.25 / fs))          # C5-ish, whole cycles over n_last samples
-    out = {"noise": np.round(rng.normal(0, 3000.0, L)).astype(np.int16),
-           "dc": (20000 + rng.integers(-3, 4, L)).astype(np.int16)}
-    x = np.round(rng.normal(0, 30.0, L))
-    x[firsts] = 30000.0
-    out["loud_first"] = x.astype(np.int16)
-    out["tone"] = np.round(20000.0 * np.sin(2 * np.pi * cyc * t / n_last + 0.3)).astype(np.int16)
-    out["dither"] = rng.integers(-1, 2, L).astype(np.int16)
-    x = rng.integers(-3000, 3001, L).astype(np.int64) + 7
-    x[p_last:] = 7
-    q, r = divmod(int(x.sum()) - 7 * L, w)
-    x[:w] -= q                                          # samples in no row: the clip mean becomes exactly 7
-    x[0] -= r
-    assert x.sum() == 7 * L
-    out["mean_run"] = x.astype(np.int16)
-    out["noise_f32"] = (out["noise"].astype(F) * F(0.37) + F(11.5)).astype(F)
-    out["small_f32"] = (rng.normal(0, 1e-3 / 3, L) + 1e-3 * np.sin(2 * np.pi * cyc * t / n_last)).astype(F)
-    return out
 
 
 CLIPPED_CPU = [(16000, 800, 200), (16000, 800, 400), (16000, 883, 300), (44100, 882, 441)]

@@ -2,14 +2,14 @@
 against np.mean of scipy's pdist / cdist, compared as float64 bit patterns; NumPy's reduction order that the kernel
 relies on; and the C ABI's argument checks, which return before any CUDA call."""
 import ctypes
-import subprocess
-import warnings
 
 import numpy as np
 import pytest
 from scipy.spatial import distance
 
 from tests import host_exe
+from tests.diarization_oracle import reference
+from tests.host_exe import bits, floats, hexes, run
 
 
 @pytest.fixture(scope="module")
@@ -17,58 +17,20 @@ def exe(tmp_path_factory):
     return host_exe.build(tmp_path_factory, "cluster_host.cu", "-O2")
 
 
-def _hex(values):
-    return " ".join(float(x).hex() if np.isfinite(x) or np.isinf(x) else "nan"
-                    for x in np.asarray(values, dtype=np.float64).ravel())
-
-
-def _run(exe, script):
-    res = subprocess.run([exe], input=script, capture_output=True, text=True)
-    assert res.returncode == 0, (res.returncode, res.stderr)
-    return [ln.split() for ln in res.stdout.splitlines()]
-
-
-def _floats(tokens):
-    return np.array([float.fromhex(t) if t != "nan" else np.nan for t in tokens])
-
-
-def _bits(a):
-    a = np.asarray(a, dtype=np.float64)
-    b = a.view(np.uint64).copy()
-    b[np.isnan(a)] = 0x7ff8000000000000
-    return b
-
-
-def reference(X, labels, K, want=None):
-    """(A [K], B [K, K]) as speaker_diarization computes them (audioSegmentation.py:958-972), NaN where not computed."""
-    A, B = np.full(K, np.nan), np.full((K, K), np.nan)
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore", RuntimeWarning)
-        for c in range(K):
-            if want is not None and not want[c]:
-                continue
-            xc = X[labels == c, :]
-            A[c] = np.mean(distance.pdist(xc.T))
-            for c2 in range(K):
-                if c2 != c:
-                    B[c, c2] = np.mean(distance.cdist(xc, X[labels == c2, :]))
-    return A, B
-
-
 def host_means(exe, X, labels, K, want=None, seg_terms=1 << 22, pass_terms=1 << 24):
     n, D = X.shape
     want = np.ones(K, dtype=np.int64) if want is None else np.asarray(want, dtype=np.int64)
     script = "means %d %d %d %d %d %s %s %s\n" % (K, D, n, seg_terms, pass_terms, " ".join(map(str, labels)),
-                                                 " ".join(map(str, want)), _hex(X))
-    out = _floats(_run(exe, script)[0][1:])
+                                                 " ".join(map(str, want)), hexes(X))
+    out = floats(run(exe, script)[0][1:])
     return out[:K], out[K:].reshape(K, K)
 
 
 def _check(exe, X, labels, K, want=None, **plan):
     A, B = host_means(exe, X, labels, K, want, **plan)
     rA, rB = reference(X, labels, K, want)
-    assert np.array_equal(_bits(A), _bits(rA)), (A, rA)
-    assert np.array_equal(_bits(B), _bits(rB)), (B, rB)
+    assert np.array_equal(bits(A), bits(rA)), (A, rA)
+    assert np.array_equal(bits(B), bits(rB)), (B, rB)
 
 
 def _adversarial(rng, n, D):
@@ -89,12 +51,12 @@ def test_pdist_adds_like_cdist(exe, kind):
         X = _adversarial(rng, n, D)
         if n * D > 4:
             X.flat[rng.integers(0, n * D, size=2)] = [np.nan, np.inf]
-        got = _floats(_run(exe, "dist %d %d %d %s\n" % (kind, n, D, _hex(X)))[0][1:])
+        got = floats(run(exe, "dist %d %d %d %s\n" % (kind, n, D, hexes(X)))[0][1:])
         want = (distance.cdist(X, X) if kind == 0 else distance.pdist(X.T)).ravel()
-        assert np.array_equal(_bits(got), _bits(want)), (kind, n, D)
+        assert np.array_equal(bits(got), bits(want)), (kind, n, D)
     # the two scipy functions agree with each other on the same pairs
     X = _adversarial(rng, 30, 6)
-    assert np.array_equal(_bits(distance.pdist(X.T)), _bits(distance.cdist(X.T, X.T)[np.triu_indices(6, 1)]))
+    assert np.array_equal(bits(distance.pdist(X.T)), bits(distance.cdist(X.T, X.T)[np.triu_indices(6, 1)]))
 
 
 @pytest.mark.parametrize("sizes", [(1, 1), (1, 7), (8, 16), (13, 10), (128, 1), (64, 3), (129, 2), (100, 83), (91, 91)])
@@ -186,7 +148,7 @@ def test_numpy_mean_is_one_pairwise_sum():
 def test_sum_past_2_31_terms(exe):
     """A pairwise sum of more than 2^31 terms (64-bit offsets), cut into segments and leaves, equals the direct
     pairwise sum; the segments tile the terms and no leaf exceeds 128 (the harness checks both)."""
-    got = _floats(_run(exe, "bigsum %d %d\n" % ((1 << 31) + 1000, 1 << 22))[0][1:])
+    got = floats(run(exe, "bigsum %d %d\n" % ((1 << 31) + 1000, 1 << 22))[0][1:])
     assert got[0].view(np.uint64) == got[1].view(np.uint64)
 
 

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 from tests import diarization_oracle as O
-from tests.test_cluster_cpu import reference
+from tests.diarization_cases import fixed, lda_case
+from tests.diarization_oracle import reference
 from pyaudioanalysis_b200 import audioSegmentation as S
 
 
@@ -112,47 +113,20 @@ def test_pool_frames_matches_reference_loop():
         assert np.array_equal(got.view(np.uint64), want.view(np.uint64)), ratio
 
 
-def _svm_models(rng, F=136):
-    from sklearn.svm import SVC
-    models = []
-    for C in (4, 2):
-        X = rng.normal(size=(60 * C, F)) + (np.arange(60 * C) % C)[:, None] * 0.4
-        y = np.arange(60 * C) % C
-        mean, std = X.mean(axis=0), X.std(axis=0)
-        models.append((SVC(probability=True, random_state=0).fit((X - mean) / std, y), mean, std))
-    return models
-
-
-def _lda_case(rng, T=450):
-    models = _svm_models(rng)
-    st = (rng.normal(size=(68, T)) + np.repeat(rng.normal(size=(68, T // 50 + 1)), 50, axis=1)[:, :T]).astype(np.float32)
-    mid = rng.normal(size=(136, T // 10))
-    post = [S._posteriors(mid.T, m) for m in models]
-    return models, st.astype(np.float64), mid, post
-
-
-def _fixed(x, k):
-    lab = (np.arange(x.shape[0]) // 20) % k
-    if k > 3:
-        lab[lab == k - 1] = 0
-        lab[:5] = k - 1                                          # a cluster below the 2 % share
-    return lab
-
-
 @pytest.mark.parametrize("n_speakers,lda_dim", [(3, 2), (0, 3)])
 def test_diarize_lda_host_steps(n_speakers, lda_dim):
     """diarize with lda_dim > 0 (no HMM, so every step runs on the host once kernel 9 is replaced by its NumPy statement)
     against the restatement of the reference's LDA branch: sil_all, the chosen count and cls, in bits."""
     rng = np.random.default_rng(21 + n_speakers)
-    models, st, mid, post = _lda_case(rng)
+    models, st, mid, post = lda_case(rng)
 
     def means(x, cls, k, rows):
         want = np.zeros(k, dtype=bool)
         want[list(rows)] = True
         return reference(np.asarray(x), cls, k, want)
     cls, info = S.diarize(mid, models, n_speakers, 0.1, 0.1, lda_dim, st=st, mid_window=1.0, posteriors=post,
-                          cluster=_fixed, means=means, details=True)
-    want_cls, sil_all, num, _ = O.diarize(mid, post, n_speakers, _fixed, lda=(st, models, 1.0, 0.1, lda_dim))
+                          cluster=fixed, means=means, details=True)
+    want_cls, sil_all, num, _ = O.diarize(mid, post, n_speakers, fixed, lda=(st, models, 1.0, 0.1, lda_dim))
     assert cls.shape == (st.shape[1],)
     assert np.array_equal(info["sil_all"].view(np.uint64), sil_all.view(np.uint64))
     assert info["num_speakers"] == num
@@ -161,6 +135,6 @@ def test_diarize_lda_host_steps(n_speakers, lda_dim):
 
 def test_diarize_lda_needs_models():
     rng = np.random.default_rng(22)
-    _, st, mid, post = _lda_case(rng)
+    _, st, mid, post = lda_case(rng)
     with pytest.raises(ValueError, match="lda_dim > 0 needs models"):
-        S.diarize(mid, None, 3, 0.1, 0.1, 2, st=st, mid_window=1.0, posteriors=post, cluster=_fixed)
+        S.diarize(mid, None, 3, 0.1, 0.1, 2, st=st, mid_window=1.0, posteriors=post, cluster=fixed)

@@ -81,7 +81,7 @@ from oracle import st_oracle as O
 from tests import signals as SG
 from tests.parity import check_feature_bounds, clip_norm, feature_bounds
 
-# the (fs, window, hop) of tests/test_gpu_adversarial.py FEATURE_CONFIGS
+# the (fs, window, hop) of tests.kernels.FEATURE_CONFIGS
 FEATURE_WINDOWS = [(16000, 320, 160), (16000, 480, 240), (16000, 512, 256), (16000, 640, 320), (16000, 800, 400),
                    (48000, 960, 480), (16000, 1024, 512), (16000, 800, 800), (16000, 800, 200), (16000, 800, 333),
                    (16000, 1024, 300), (44100, 882, 441), (44100, 882, 300), (16000, 400, 160), (16000, 400, 200),

@@ -14,23 +14,12 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
-from tests.kernels import CTA, GENERIC, KIND_NAMES, PAIR, SOLO, plans, ragged
+from tests.kernels import CTA, FEATURE_CONFIGS, KIND_NAMES, PAIR, ROW_CONFIGS, plans, ragged
 from tests.parity import (check_close, check_energy_relative, check_features, check_spectrogram_rows, check_zcr_exact,
                           exception_bounds)
 
 pytestmark = pytest.mark.gpu
 
-# (fs, window, hop): the kernel kinds a plan reaches through prefer_kernel / force_generic
-FEATURE_CONFIGS = [
-    (16000, 320, 160, {PAIR, CTA, GENERIC}), (16000, 480, 240, {PAIR, CTA, GENERIC}), (16000, 512, 256, {PAIR, GENERIC}),
-    (16000, 640, 320, {PAIR, CTA, GENERIC}), (16000, 800, 400, {PAIR, CTA, GENERIC}), (48000, 960, 480, {PAIR, GENERIC}),
-    (16000, 1024, 512, {PAIR, GENERIC}), (16000, 800, 800, {PAIR, CTA, GENERIC}), (16000, 800, 200, {PAIR, CTA, GENERIC}),
-    (16000, 800, 333, {PAIR, CTA, GENERIC}), (16000, 1024, 300, {PAIR, GENERIC}),
-    (44100, 882, 441, {SOLO, CTA, GENERIC}), (44100, 882, 300, {SOLO, CTA, GENERIC}), (16000, 400, 160, {SOLO, CTA, GENERIC}),
-    (16000, 400, 200, {SOLO, CTA, GENERIC}), (8000, 600, 300, {SOLO, CTA, GENERIC}),
-    (22050, 551, 200, {GENERIC}), (16000, 883, 300, {GENERIC}), (16000, 2048, 1024, {GENERIC}),
-]
-ROW_CONFIGS = [(16000, 800, 400), (16000, 800, 333), (44100, 882, 441), (16000, 400, 160), (8000, 600, 300)]
 ODD = 3                 # sample offset of the unaligned view
 
 

@@ -23,11 +23,10 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
-from tests.kernels import GENERIC_SWEEP, KIND_NAMES, PAIR, plans, ragged
-from tests.parity import check_chromagram_bounds, chromagram_bounds, chromagram_rows
-from tests.test_chroma_bounds_cpu import clipped_clips, clipped_targets
-from tests.test_gpu_adversarial import ROW_CONFIGS
-from tests.test_gpu_spectra import sweep_clips
+from tests.kernels import GENERIC_SWEEP, KIND_NAMES, PAIR, ROW_CONFIGS, plans, ragged
+from tests.parity import (check_rows, chromagram_bounds, chromagram_rows, clipped_clips, clipped_targets, ragged_bounds,
+                          report)
+from tests.signals import sweep_clips
 
 pytestmark = pytest.mark.gpu
 
@@ -42,41 +41,6 @@ def P():
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     import pyaudioanalysis_b200 as pkg
     return pkg
-
-
-def note(accs, key, worst, unb):
-    acc = accs.setdefault(key, {"worst": {}, "unbounded": {}})
-    for k, v in worst.items():
-        acc["worst"][k] = max(acc["worst"].get(k, 0.0), v)
-    for k, v in unb.items():
-        acc["unbounded"][k] = acc["unbounded"].get(k, 0) + v
-
-
-def report(tag, accs):
-    for key, acc in accs.items():
-        print(json.dumps(dict(config=tag, kernel=key[0], input=key[1],
-                              worst={k: round(v, 4) for k, v in acc["worst"].items()}, unbounded=acc["unbounded"])))
-
-
-def check_rows(out, cbs, what, accs, key):
-    """out [B, R, 12] of a ragged batch (or an equal-length one): clip i's rows under its bound, the rows past them
-    zero; a refused clip has none."""
-    for i, cb in enumerate(cbs):
-        R = cb.ref.shape[0]
-        assert not out[i, R:].any(), what[i] + ": rows past the clip's own"
-        if cb.refused:
-            continue
-        note(accs, key, *check_chromagram_bounds(out[i, :R], cb, what[i]))
-
-
-def ragged_bounds(P, pl, clips, names, dtype, fs, w, s, tag, accs, key, cbs=None):
-    """clips as one ragged chromagram batch through plan pl, every clip under its bound.  Returns the bounds."""
-    d, lens = ragged(clips, dtype)
-    cbs = cbs or [chromagram_bounds(x, fs, w, s) for x in clips]
-    out = P.chromagram_batch(d, fs, w, s, plan=pl, lengths=lens).cpu().numpy()
-    assert P.row_counts(lens, w, s, 1).cpu().tolist() == [0 if cb.refused else cb.ref.shape[0] for cb in cbs], tag
-    check_rows(out, cbs, ["%s: %s" % (tag, n) for n in names], accs, key)
-    return cbs
 
 
 @pytest.mark.parametrize("fs,w,s", CONFIGS, ids=["%d-%d-%d" % c for c in CONFIGS])

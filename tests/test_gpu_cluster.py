@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 from scipy.spatial import distance
 
-from tests.test_cluster_cpu import _bits, reference
+from tests.diarization_oracle import reference
+from tests.host_exe import bits
 
 pytestmark = pytest.mark.gpu
 
@@ -27,8 +28,8 @@ def _run(C, X, labels, K, rows=None):
 
 
 def _same(got, want):
-    assert np.array_equal(_bits(got[0]), _bits(want[0])), (got[0], want[0])
-    assert np.array_equal(_bits(got[1]), _bits(want[1])), (got[1], want[1])
+    assert np.array_equal(bits(got[0]), bits(want[0])), (got[0], want[0])
+    assert np.array_equal(bits(got[1]), bits(want[1])), (got[1], want[1])
 
 
 @pytest.mark.parametrize("M,D,K", [(50, 7, 2), (600, 146, 4), (3600, 146, 9), (3600, 1, 3), (36000, 3, 3)])

@@ -22,7 +22,7 @@ kernel holds SMs) still finishes.
   its float64 bound (``parity.feature_bounds``, ``check_spectrogram_rows``, ``chromagram_bounds``).
 * Bit-equal results are promised for int16 input.  Float32 clip statistics add doubles with atomics in no fixed order:
   the float32 feature jobs take the baseline's records as ``norm=``, and the concurrent float32 ``clip_stats`` are held
-  to the exact-arithmetic check of ``test_gpu_stats.check_f32_clip``.
+  to the exact-arithmetic check of ``parity.check_f32_clip``.
 
 Inputs are made before a phase on the default stream, which every stream waits on; outputs passed as ``out=`` are
 allocated there too, the others by the entry point on the job's stream.  Every tensor is held until the final
@@ -37,9 +37,8 @@ import pytest
 from oracle import st_oracle as O
 from tests import wavgen
 from tests.kernels import CTA, GENERIC, PAIR, SOLO, ragged
-from tests.parity import check_feature_bounds, check_spectrogram_rows, chromagram_bounds, feature_bounds
-from tests.test_gpu_chroma_bounds import check_rows
-from tests.test_gpu_stats import check_f32_clip
+from tests.parity import (check_f32_clip, check_feature_bounds, check_rows, check_spectrogram_rows, chromagram_bounds,
+                          feature_bounds)
 
 pytestmark = pytest.mark.gpu
 

@@ -146,12 +146,12 @@ def test_speaker_diarization_end_to_end(S, tmp_path):
 @pytest.mark.parametrize("n_speakers,lda_dim", [(3, 2), (0, 3)])
 def test_diarize_lda_on_kernel9(S, n_speakers, lda_dim):
     """The LDA branch with the silhouette means on kernel 9, against the restatement of the reference's branch."""
-    from tests.test_diarization_cpu import _fixed, _lda_case
+    from tests.diarization_cases import fixed, lda_case
     rng = np.random.default_rng(21 + n_speakers)
-    models, st, mid, post = _lda_case(rng)
+    models, st, mid, post = lda_case(rng)
     cls, info = S.diarize(mid, models, n_speakers, 0.1, 0.1, lda_dim, st=st, mid_window=1.0, posteriors=post,
-                          cluster=_fixed, details=True)
-    want_cls, sil_all, num, _ = O.diarize(mid, post, n_speakers, _fixed, lda=(st, models, 1.0, 0.1, lda_dim))
+                          cluster=fixed, details=True)
+    want_cls, sil_all, num, _ = O.diarize(mid, post, n_speakers, fixed, lda=(st, models, 1.0, 0.1, lda_dim))
     assert np.array_equal(info["sil_all"].view(np.uint64), sil_all.view(np.uint64))
     assert info["num_speakers"] == num
     assert np.array_equal(cls, want_cls)

@@ -18,10 +18,9 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
-from tests.kernels import GENERIC_SWEEP, KIND_NAMES, plans, ragged
-from tests.parity import check_feature_bounds, feature_bounds
-from tests.test_gpu_adversarial import FEATURE_CONFIGS
-from tests.test_gpu_spectra import odd_tail, sweep_clips
+from tests.kernels import FEATURE_CONFIGS, GENERIC_SWEEP, KIND_NAMES, plans, ragged
+from tests.parity import batch_bounds, check_feature_bounds, feature_bounds, note, report
+from tests.signals import odd_tail, sweep_clips
 
 pytestmark = pytest.mark.gpu
 
@@ -32,36 +31,6 @@ def P():
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     import pyaudioanalysis_b200 as pkg
     return pkg
-
-
-def note(acc, worst, unb):
-    for k, v in worst.items():
-        acc["worst"][k] = max(acc["worst"].get(k, 0.0), v)
-    for k, v in unb.items():
-        acc["unbounded"][k] = acc["unbounded"].get(k, 0) + v
-
-
-def report(tag, accs):
-    for key, acc in accs.items():
-        print(json.dumps(dict(config=tag, kernel=key[0], input=key[1],
-                              worst={k: round(v, 4) for k, v in acc["worst"].items()}, unbounded=acc["unbounded"])))
-
-
-def batch_bounds(P, pl, clips, dtype, fs, w, s, what, acc):
-    """clips as one ragged batch through plan pl, deltas on and off, every clip under its bound; rows past a clip's
-    frame count stay zero."""
-    d, lens = ragged(clips, dtype)
-    fbs = [feature_bounds(x, fs, w, s, deltas=True) for x in clips]
-    for deltas in (True, False):
-        out = P.feature_extraction_batch(d, fs, w, s, lengths=lens, plan=pl, deltas=deltas).cpu().numpy()
-        for i, fb in enumerate(fbs):
-            T = fb.ref.shape[1]
-            F = 68 if deltas else 34
-            assert not out[i, :, T:].any(), what[i] + ": output past the clip's frames"
-            if not deltas:
-                fb = type(fb)(fb.ref[:34], fb.bound[:34], fb.roll, {k: v for k, v in fb.unbounded.items()
-                                                                    if not k.startswith("delta")}, fb.K)
-            note(acc, *check_feature_bounds(out[i, :F, :T], fb, what[i] + (", deltas" if deltas else ", no deltas")))
 
 
 @pytest.mark.parametrize("fs,w,s,kinds", FEATURE_CONFIGS, ids=["%d-%d-%d" % c[:3] for c in FEATURE_CONFIGS])

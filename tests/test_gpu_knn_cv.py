@@ -13,7 +13,7 @@ from sklearn.preprocessing import StandardScaler
 
 from tests import knn_cv_oracle as oracle
 from tests.conftest import load_golden
-from tests.test_knn_cv_cpu import golden_args, golden_features
+from tests.knn_cv_oracle import golden_args, golden_features
 
 pytestmark = pytest.mark.gpu
 

@@ -10,7 +10,7 @@ Path level: the adversarial bank (tests/signals.py) through MidTermFeatures.mid_
 and mid_feature_extraction_batch (device path): both bit-equal, the mid-term matrix equal to float64 pooling of the
 returned short-term matrix, and within the propagated tolerance (tests/parity.check_mid_propagated) of pooling of the
 oracle's short-term matrix.  The reference's own mid-term matrices at ratio 0 / -1 and the other unusual ratios of
-tests/test_oracle_mid.CASES (tests/golden/mid_edges.npz) are held to the same propagated tolerance.
+tests/golden_cases.MID_CASES (tests/golden/mid_edges.npz) are held to the same propagated tolerance.
 """
 import warnings
 
@@ -19,16 +19,16 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
-from tests import test_oracle_mid as EDGES
+from tests import golden_cases as EDGES
 from tests.conftest import load_golden
 from tests.parity import check_features, check_mid_propagated, exception_bounds, mid_slices
+from tests.signals import ROW_KINDS, oracle_st, rows
 
 pytestmark = pytest.mark.gpu
 
 T_VALUES = [1, 2, 31, 32, 33, 65, 399, 143999]
 LONG = 143999            # one hour at 50 / 25 ms
 SHAPES = [(1, 1), (34, 3), (68, 1), (1, 3), (34, 1), (68, 3)]       # (F, B), taken in turn
-ROW_KINDS = 6
 
 
 @pytest.fixture(scope="module")
@@ -44,28 +44,6 @@ def pool64(st, ratio, stepr):
     with warnings.catch_warnings():
         warnings.simplefilter("ignore", RuntimeWarning)         # mean of an empty slice, NaN rows
         return O.mid_pool(np.asarray(st, dtype=np.float64), ratio, stepr)
-
-
-def rows(rng, F, T, first_kind):
-    """float32 [F, T]: row f is of kind (first_kind + f) % 6."""
-    out = np.empty((F, T), dtype=np.float32)
-    for f in range(F):
-        k = (first_kind + f) % ROW_KINDS
-        n = rng.standard_normal(T)
-        if k == 0:
-            out[f] = n
-        elif k == 1:
-            out[f] = 3.25
-        elif k == 2:
-            out[f] = 1e4 + 1e-3 * n
-        elif k == 3:
-            out[f] = -99.00180475 + 1e-3 * n
-        elif k == 4:
-            out[f] = np.where(np.arange(T) % 2 == 0, 1.0, -1.0) * (1.0 + 0.1 * np.abs(n))
-        else:
-            out[f] = n
-            out[f, T // 2] = np.nan
-    return out
 
 
 def st_batch(T, F, B, seed):
@@ -161,10 +139,6 @@ PATH_CONFIGS = [
 ]
 
 
-def oracle_st(x, fs, w, s):
-    return SG.patch_noise_defined(O.feature_extraction(x, fs, w, s)[0], x, w, s)[0]
-
-
 @pytest.mark.parametrize("fs,w,s,mw,ms", PATH_CONFIGS, ids=["%d-%d-%d-%d-%d" % c for c in PATH_CONFIGS])
 def test_mid_path_on_bank(P, fs, w, s, mw, ms):
     import torch
@@ -192,10 +166,10 @@ def test_mid_edges_against_reference(P, signal):
     x = EDGES.clip(signal)
     fs, w, s = EDGES.FS, EDGES.W, EDGES.S
     ref_st = oracle_st(x, fs, w, s)
-    for name, (mw, ms, ratio, stepr) in EDGES.CASES.items():
+    for name, (mw, ms, ratio, stepr) in EDGES.MID_CASES.items():
         what = "%s, %s" % (signal, name)
         mid, st, _ = P.MidTermFeatures.mid_feature_extraction(x, fs, mw, ms, w, s)
-        ref = g[EDGES.key(signal, name, "mid")]
+        ref = g[EDGES.mid_key(signal, name, "mid")]
         assert mid.shape == ref.shape, what
         check_mid_propagated(mid, st, ref_st, ratio, stepr, w // 2, what, ref_mid=ref)
         if ratio <= 0:

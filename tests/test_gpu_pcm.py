@@ -78,12 +78,11 @@ def arena_of(payloads):
 
 def test_one_ragged_launch_all_flavours(P, tmp_path):
     from pyaudioanalysis_b200 import audioio
-    from tests.test_pcm_cpu import flavour_samples
     # 0 and 1 frames; 24-bit payloads of 9003 and 17 970 bytes, not a multiple of 4 or 16
     frames = [0, 1, 3000, 2999, 3001, 2995, 2998, 2500, 3000, 2997, 3001, 4000]
     lens, files = {}, []
     for k, (name, ch) in enumerate(wavgen.FLAVOURS):
-        x = flavour_samples(name, ch, 30 + k)
+        x = wavgen.flavour_samples(name, ch, 30 + k)
         assert x.shape[0] >= frames[k]
         p = str(tmp_path / ("%02d_%s_%d.wav" % (k, name, ch)))
         wavgen.write(p, 16000, x[:frames[k]], name)

@@ -19,7 +19,7 @@ from oracle import st_oracle as O
 from tests import signals as SG
 from tests.kernels import ragged
 from tests.parity import check_close, check_mid_propagated, exception_bounds
-from tests.test_gpu_mid import oracle_st, rows
+from tests.signals import oracle_st, rows
 
 pytestmark = pytest.mark.gpu
 

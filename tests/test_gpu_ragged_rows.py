@@ -14,9 +14,8 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
-from tests.kernels import PAIR, KIND_NAMES, plans, ragged
+from tests.kernels import PAIR, KIND_NAMES, ROW_CONFIGS, plans, ragged
 from tests.parity import check_close, check_spectrogram_rows
-from tests.test_gpu_adversarial import ROW_CONFIGS
 
 pytestmark = pytest.mark.gpu
 

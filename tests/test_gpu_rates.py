@@ -13,7 +13,7 @@ float32 batches:
 * the kernel that ran is the one asked for: with ``B200AA_DEBUG`` set the pair, solo and CTA launchers print one line per
   launch and the generic kernel none.  A launcher that declines a shape falls through to the next kernel silently, and
   the values would still be right: this is what tells the two apart.  At 800 / 1600 the CTA kernel's staging is over its
-  cap by design (tests/test_rates_cpu.CTA_FALLBACK) and the generic kernel runs: that is asserted too.
+  cap by design (tests.kernels.CTA_FALLBACK) and the generic kernel runs: that is asserted too.
 
 Entries with an unbounded bound are counted per reason and printed with the worst err / bound per kernel and input.
 
@@ -32,12 +32,9 @@ import numpy as np
 import pytest
 
 from tests import signals as SG
-from tests.kernels import CTA, GENERIC, KIND_NAMES, PAIR, RATE_CONFIGS, SOLO, plans, ragged
-from tests.parity import check_spectrogram_rows
-from tests.test_gpu_chroma_bounds import ragged_bounds
-from tests.test_gpu_feature_bounds import batch_bounds
-from tests.test_gpu_spectra import odd_tail
-from tests.test_rates_cpu import CTA_FALLBACK
+from tests.kernels import CTA, CTA_FALLBACK, GENERIC, KIND_NAMES, PAIR, RATE_CONFIGS, SOLO, plans, ragged
+from tests.parity import batch_bounds, check_spectrogram_rows, note, ragged_bounds
+from tests.signals import odd_tail
 
 pytestmark = pytest.mark.gpu
 
@@ -66,14 +63,6 @@ def ran(capfd, expect, what):
     names = {name for name in LAUNCHERS.values() if any(ln.startswith("[b200aa] " + name) for ln in lines)}
     want = set() if expect is None else {expect}
     assert names == want, "%s: launched %s, expected %s" % (what, sorted(names) or "the generic kernel", expect or "the generic kernel")
-
-
-def accumulate(accs, key, worst, unb):
-    acc = accs.setdefault(key, {"worst": {}, "unbounded": {}})
-    for k, v in worst.items():
-        acc["worst"][k] = max(acc["worst"].get(k, 0.0), v)
-    for k, v in unb.items():
-        acc["unbounded"][k] = acc["unbounded"].get(k, 0) + v
 
 
 @pytest.mark.parametrize("fs,w,s,kinds,layout", RATE_CONFIGS, ids=["%d-%d-%d" % c[:3] for c in RATE_CONFIGS])
@@ -107,7 +96,7 @@ def test_kernels_across_rates(P, debug, capfd, fs, w, s, kinds, layout):
                 R = int((x.size - w) / s) + 1
                 assert not sp[i, R:].any(), "%s: %s: rows past the clip's own" % (rtag, n)
                 bins, dc = check_spectrogram_rows(sp[i, :R], x, w, s, "%s: %s spectrogram" % (rtag, n))
-                accumulate(accs, ("spectrogram", name, cls), {"bins": bins, "dc": dc}, {})
+                note(accs.setdefault(("spectrogram", name, cls), {"worst": {}, "unbounded": {}}), {"bins": bins, "dc": dc}, {})
     assert seen == kinds, (seen, kinds)
     assert GENERIC in seen
     for (what, kernel, cls), acc in accs.items():

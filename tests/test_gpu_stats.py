@@ -13,22 +13,19 @@ those of each clip alone, and every feature kernel must give what it gives on th
 The output contract: feature_extraction_batch writes exactly the columns below each clip's own frame count of an ``out``
 wider than T (odd row stride), and nothing else; spectrogram_batch writes every element of ``out``.
 """
-import math
-
 import numpy as np
 import pytest
 
 from oracle import st_oracle as O
 from tests import signals as SG
 from tests.kernels import KIND_NAMES, plans, ragged
-from tests.parity import check_features
+from tests.parity import A_EMPTY, check_f32_clip, check_features, check_samples
 
 pytestmark = pytest.mark.gpu
 
 LENGTHS = [0, 1, 7, 8, 9, 31, 33, 4095, 4097, 32767, 32769, 160000]
 ODD_LENGTH = 160001          # per = ceil(L / chunks) is odd: chunk starts fall off the 16-byte boundary
 RAILS = np.array([32767, -32768], dtype=np.int16)
-A_EMPTY = np.float32(1.0 / (32768.0 * 1e-10))      # a of a clip without samples (max deviation 0)
 
 
 @pytest.fixture(scope="module")
@@ -115,46 +112,6 @@ def check_i16_clip(rec, x, what):
     check_i16_records(rec[None], [x64.sum()], [L], [x64.min() if L else 0], [x64.max() if L else 0], what)
     if L:
         check_samples(rec, x, np.sign(x64 * L - x64.sum()), what)
-
-
-def check_f32_clip(rec, x, what):
-    a, bp, m, lo, hi = (float(v) for v in rec[:5])
-    assert not rec[5:].any(), what + ": reserved words not cleared"
-    L = x.size
-    if L == 0:
-        assert rec[0] == A_EMPTY and not rec[1:5].any(), what + ": record of an empty clip"
-        return
-    xd = x.astype(np.float64)
-    total = math.fsum(xd.tolist())
-    mean = total / L
-    assert abs(m - mean) <= float(np.spacing(np.float32(abs(mean)))), "%s: m = %r, mean %r" % (what, m, mean)
-    if m == mean:
-        assert lo == hi == 0.0, "%s: mean %r is a float32 but lo / hi = %r / %r" % (what, mean, lo, hi)
-    else:
-        lo_abs, hi_abs = np.float32(m + lo), np.float32(m + hi)
-        assert float(lo_abs) < mean < float(hi_abs) and np.nextafter(lo_abs, np.float32(np.inf)) == hi_abs, \
-            "%s: [%r, %r] does not bracket the mean %r between neighbouring floats" % (what, m + lo, m + hi, mean)
-    ra = 1.0 / (max(xd.max() - mean, mean - xd.min()) + 32768.0 * 1e-10)
-    assert abs(a - ra) <= float(np.spacing(np.float32(ra))), "%s: a = %r, expected %r" % (what, a, ra)
-    rbp = ra * (m - mean)
-    assert abs(bp - rbp) <= 2.0 ** -24 * abs(rbp) + 2.0 ** -149 + ra * 2.0 ** -50 * float(np.abs(xd).sum()), \
-        "%s: bp = %r, expected %r" % (what, bp, rbp)
-    check_samples(rec, x, np.sign(xd - mean), what)
-
-
-def check_samples(rec, x, sign, what):
-    """lo / hi classify d = x - m (float32, as the kernels form it) exactly as sign(x - mean); fma(a, d, bp) is the
-    reference's normalised sample to float32 resolution of the clip's full scale."""
-    a, bp, m, lo, hi = (np.float32(v) for v in rec[:5])
-    d = x.astype(np.float32) - m
-    cls = (d > lo).astype(np.int64) - (d < hi).astype(np.int64)
-    bad = cls != sign
-    assert not bad.any(), "%s: sign(x - mean) wrong for %d samples, first at %d" % (what, int(bad.sum()), int(np.argmax(bad)))
-    y = (np.float64(a) * d.astype(np.float64) + np.float64(bp)).astype(np.float32).astype(np.float64)
-    ref = O.normalize_clip(x.astype(np.float64))
-    tol = 8 * 2.0 ** -24 * np.abs(ref).max() + 1e-30
-    err = np.abs(y - ref)
-    assert err.max() <= tol, "%s: a (x - m) + bp off by %.3g (tolerance %.3g) at sample %d" % (what, err.max(), tol, int(np.argmax(err)))
 
 
 def stats(P, d, lens=None):

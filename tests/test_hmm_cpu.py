@@ -4,39 +4,18 @@ NumPy on features.T, the Viterbi pass against tests/hmm_oracle.py and an exhaust
 the host helpers of audioSegmentation; and the C ABI's argument checks, which return before any CUDA call."""
 import ctypes
 import itertools
-import subprocess
 
 import numpy as np
 import pytest
 
 from tests import hmm_oracle as H
 from tests import host_exe
+from tests.host_exe import bits, floats, hexes, run
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
     return host_exe.build(tmp_path_factory, "hmm_host.cu", "-O1")
-
-
-def _hex(values):
-    return " ".join(float(x).hex() for x in np.asarray(values, dtype=np.float64).ravel())
-
-
-def _run(exe, script):
-    res = subprocess.run([exe], input=script, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return [ln.split() for ln in res.stdout.splitlines()]
-
-
-def _floats(tokens):
-    return np.array([float.fromhex(t) if t != "nan" else np.nan for t in tokens])
-
-
-def _bits(a):
-    a = np.asarray(a, dtype=np.float64)
-    b = a.view(np.uint64).copy()
-    b[np.isnan(a)] = 0x7ff8000000000000
-    return b
 
 
 def _features(rng, F, M):
@@ -54,21 +33,21 @@ def test_class_stats_match_numpy(exe, F, M):
         idx = np.nonzero(labels == u)[0]
         mean = feats[:, idx].mean(axis=1)
         std = np.std(feats[:, idx], axis=1)
-        script = "".join("stats %d %d %s\n" % (idx.size, F == 1, _hex(feats[f, idx])) for f in range(F))
-        got = np.array([_floats(ln[1:]) for ln in _run(exe, script)])
-        assert np.array_equal(_bits(got[:, 1]), _bits(mean)), (F, M, u)
-        assert np.array_equal(_bits(got[:, 3]), _bits(std)), (F, M, u)
+        script = "".join("stats %d %d %s\n" % (idx.size, F == 1, hexes(feats[f, idx])) for f in range(F))
+        got = np.array([floats(ln[1:]) for ln in run(exe, script)])
+        assert np.array_equal(bits(got[:, 1]), bits(mean)), (F, M, u)
+        assert np.array_equal(bits(got[:, 3]), bits(std)), (F, M, u)
 
 
 def test_class_stats_edges(exe):
     """A constant feature (std 0), one window, -0.0 values, an empty class (NaN)."""
     feats = np.array([[2.5, 2.5, 2.5, 2.5], [-0.0, -0.0, -0.0, -0.0], [1.0, -1.0, 3.0, 1e300]])
     for idx in (np.arange(4), np.array([2]), np.array([0, 1])):
-        script = "".join("stats %d 0 %s\n" % (idx.size, _hex(feats[f, idx])) for f in range(3))
-        got = np.array([_floats(ln[1:]) for ln in _run(exe, script)])
-        assert np.array_equal(_bits(got[:, 1]), _bits(feats[:, idx].mean(axis=1)))
-        assert np.array_equal(_bits(got[:, 3]), _bits(np.std(feats[:, idx], axis=1)))
-    got = _floats(_run(exe, "stats 0 0\n")[0][1:])
+        script = "".join("stats %d 0 %s\n" % (idx.size, hexes(feats[f, idx])) for f in range(3))
+        got = np.array([floats(ln[1:]) for ln in run(exe, script)])
+        assert np.array_equal(bits(got[:, 1]), bits(feats[:, idx].mean(axis=1)))
+        assert np.array_equal(bits(got[:, 3]), bits(np.std(feats[:, idx], axis=1)))
+    got = floats(run(exe, "stats 0 0\n")[0][1:])
     assert np.isnan(got[1]) and np.isnan(got[3])
 
 
@@ -77,9 +56,9 @@ def _emissions(exe, feats, means, var):
     konst = F * np.log(2 * np.pi) + np.log(var).sum(axis=-1)
     out = []
     for j in range(means.shape[0]):
-        ln = _run(exe, "emission %d %d %d %s %s %s %s\n" % (F, M, M == 1, float(konst[j]).hex(), _hex(means[j]), _hex(var[j]),
-                                                            _hex(feats.T)))[0]
-        out.append(_floats(ln[1:]))
+        ln = run(exe, "emission %d %d %d %s %s %s %s\n" % (F, M, M == 1, float(konst[j]).hex(), hexes(means[j]), hexes(var[j]),
+                                                            hexes(feats.T)))[0]
+        out.append(floats(ln[1:]))
     return np.stack(out, axis=1)
 
 
@@ -91,12 +70,12 @@ def test_emission_matches_numpy_density(exe, F, M, C):
     var = rng.random((C, F)) * rng.choice([1e-6, 1.0, 1e4], size=(C, 1)) + 1e-9
     got = _emissions(exe, feats, means, var)
     ref = H.log_density(feats.T, means, var)
-    assert np.array_equal(_bits(got), _bits(ref)), (F, M, C)
+    assert np.array_equal(bits(got), bits(ref)), (F, M, C)
 
 
 def _viterbi(exe, log_start, log_trans, frame):
     n, C = frame.shape
-    ln = _run(exe, "viterbi %d %d %s %s %s\n" % (C, n, _hex(log_start), _hex(log_trans), _hex(frame)))[0]
+    ln = run(exe, "viterbi %d %d %s %s %s\n" % (C, n, hexes(log_start), hexes(log_trans), hexes(frame)))[0]
     return np.array([int(t) for t in ln[1:]], dtype=np.int64)
 
 

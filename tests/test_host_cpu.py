@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from tests.conftest import load_golden
+from tests.signals import peak_inputs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -22,17 +23,6 @@ def test_beat_extraction_matches_reference_golden():
         bpm, ratio = beat_extraction(g["st_%d" % i], float(g["win_%d" % i]))
         assert bpm == pytest.approx(float(g["bpm_%d" % i]), rel=1e-12), i
         assert ratio == pytest.approx(float(g["ratio_%d" % i]), rel=1e-12, abs=1e-15), i
-
-
-def peak_inputs():
-    """(signal, delta, feature matrix) of the peak-picking comparison, seeded."""
-    rng = np.random.default_rng(3)
-    out = []
-    for k in range(6):
-        v = np.cumsum(rng.standard_normal(400)) * (0.1 + k)
-        delta = 2.0 * np.abs(np.diff(v)).mean()
-        out.append((v, delta, np.cumsum(rng.standard_normal((34, 200 + 30 * k)), axis=1)))
-    return out
 
 
 def test_beat_extraction_against_imported_reference():

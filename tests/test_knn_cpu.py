@@ -1,13 +1,13 @@
 """CPU: the pieces of the kNN kernel (csrc/knn.cuh, __host__ __device__) run on the host by tests/knn_host.cu -- the distance
 chain against scipy's cdist, the sort keys, and the radix selection, ordered pass and vote against the stable-sort oracle
 and the reference's Knn.classify (tests/golden/knn.npz), bit for bit."""
-import subprocess
 
 import numpy as np
 import pytest
 from scipy.spatial.distance import cdist
 
 from tests import host_exe
+from tests.host_exe import bits, floats, hexes, run
 from tests.conftest import load_golden
 from tests.knn_oracle import knn_oracle, slots_of
 
@@ -19,36 +19,18 @@ def exe(tmp_path_factory):
     return host_exe.build(tmp_path_factory, "knn_host.cu", "-O1")
 
 
-def _hex(values):
-    return " ".join(float(x).hex() for x in np.asarray(values, dtype=np.float64).ravel())
-
-
-def _run(exe, script):
-    res = subprocess.run([exe], input=script, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    return [ln.split() for ln in res.stdout.splitlines()]
-
-
-def _bits(a):
-    """Bit patterns, every NaN mapped to one value."""
-    a = np.asarray(a, dtype=np.float64)
-    b = a.view(np.uint64).copy()
-    b[np.isnan(a)] = 0x7ff8000000000000
-    return b
-
-
 def _dist(exe, v, x):
-    out = _run(exe, "dist %d %d %d %s %s\n" % (v.shape[0], v.shape[1], x.shape[0], _hex(v), _hex(x)))
-    return np.array([[float.fromhex(t) if t != "nan" else np.nan for t in ln[1:]] for ln in out])
+    out = run(exe, "dist %d %d %d %s %s\n" % (v.shape[0], v.shape[1], x.shape[0], hexes(v), hexes(x)))
+    return np.array([floats(ln[1:]) for ln in out])
 
 
 def _classify(exe, feats, labels, k, x):
     slots, C = slots_of(labels)
     N, F = feats.shape
-    script = "classify %d %d %d %d %s %s %d %s\n" % (N, F, C, k, " ".join(map(str, slots)), _hex(feats), x.shape[0], _hex(x))
-    out = _run(exe, script)
+    script = "classify %d %d %d %d %s %s %d %s\n" % (N, F, C, k, " ".join(map(str, slots)), hexes(feats), x.shape[0], hexes(x))
+    out = run(exe, script)
     ids = np.array([int(ln[1]) for ln in out], dtype=np.int64)
-    P = np.array([[float.fromhex(t) for t in ln[2:]] for ln in out]).reshape(len(out), C)
+    P = np.array([floats(ln[2:]) for ln in out]).reshape(len(out), C)
     return ids, P
 
 
@@ -58,8 +40,8 @@ def test_distance_matches_cdist(exe):
         v = rng.normal(size=(23, F)) * rng.choice([1e-3, 1.0, 1e3], size=(23, 1))
         x = rng.normal(size=(9, F))
         got = _dist(exe, v, x)
-        assert np.array_equal(_bits(got), _bits(cdist(x, v))), F
-        assert np.array_equal(_bits(got), _bits(cdist(v, x).T)), F          # the reference's argument order
+        assert np.array_equal(bits(got), bits(cdist(x, v))), F
+        assert np.array_equal(bits(got), bits(cdist(v, x).T)), F          # the reference's argument order
 
 
 def test_distance_hard_values(exe):
@@ -74,13 +56,13 @@ def test_distance_hard_values(exe):
             a[mask] = rng.choice(specials, size=mask.sum())
         v[0] = x[0]                                       # a zero distance
         got = _dist(exe, v, x)
-        assert np.array_equal(_bits(got), _bits(cdist(x, v))), F
+        assert np.array_equal(bits(got), bits(cdist(x, v))), F
 
 
 def test_key_order(exe):
     d = np.array([0.0, 5e-324, 1e-300, 0.5, 1.0, 1.0000000000000002, 1e300, np.inf, np.nan, -np.nan,
                   np.frombuffer(np.uint64(0x7ff0000000000001).tobytes(), dtype=np.float64)[0], -0.0])
-    out = _run(exe, "key %d %s\n" % (d.size, _hex(d).replace("-nan", "nan")))
+    out = run(exe, "key %d %s\n" % (d.size, hexes(d).replace("-nan", "nan")))
     keys = [int(t, 16) for t in out[0][1:]]
     assert keys[:8] == sorted(keys[:8]) and len(set(keys[:8])) == 8          # finite ascending, then +inf
     assert keys[8] == keys[9] == keys[10] == 0x7ff8000000000000 > keys[7]  # every NaN one key, above +inf

@@ -6,7 +6,6 @@ the C ABI's argument checks."""
 import contextlib
 import ctypes
 import io
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,8 +13,9 @@ from sklearn.preprocessing import StandardScaler
 
 from pyaudioanalysis_b200 import audioTrainTest as at
 from tests import host_exe
+from tests.host_exe import floats, hexes, run
 from tests.conftest import load_golden
-from tests.knn_cv_oracle import reference_splits, scores, seeded_features
+from tests.knn_cv_oracle import golden_args, golden_features, reference_splits, scores, seeded_features
 
 INVALID = -1
 
@@ -25,19 +25,10 @@ def exe(tmp_path_factory):
     return host_exe.build(tmp_path_factory, "knn_cv_host.cu", "-O1")
 
 
-def _hex(a):
-    return " ".join(float(x).hex() for x in np.asarray(a, dtype=np.float64).ravel())
-
-
 def _fit(exe, train, test):
     n, F = train.shape
-    res = subprocess.run([exe], input="fit %d %d %d %s %s\n" % (n, test.shape[0], F, _hex(train), _hex(test)),
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
-    out = {}
-    for ln in res.stdout.splitlines():
-        t = ln.split()
-        out[t[0]] = np.array([float.fromhex(v) for v in t[1:]])
+    lines = run(exe, "fit %d %d %d %s %s\n" % (n, test.shape[0], F, hexes(train), hexes(test)))
+    out = {t[0]: floats(t[1:]) for t in lines}
     return out["mean"], out["scale"], out["train"].reshape(n, F), out["test"].reshape(test.shape)
 
 
@@ -117,22 +108,6 @@ def test_scores_match_sklearn():
         assert np.array_equal(cmt[np.ix_(labels, labels)], ref_cmt), trial
         if labels.size == C:
             assert np.array_equal(cmt, counts), trial
-
-
-def golden_features(g, c):
-    sizes = g[c + "_sizes"]
-    if c + "_gen" in g.files:
-        seed, F = (int(v) for v in g[c + "_gen"])
-        feats = seeded_features(seed, tuple(int(s) for s in sizes), F)
-        assert np.vstack(feats).sum() == g[c + "_X_sum"], c
-        return feats
-    return np.split(g[c + "_X"], np.cumsum(sizes)[:-1])
-
-
-def golden_args(g, c):
-    ids = g[c + "_ids"].tolist() or None
-    return (list(g[c + "_class_names"]), g[c + "_params"], int(g[c + "_mode"]), ids, int(g[c + "_n_exp"]),
-            float(g[c + "_train_percentage"]))
 
 
 def test_report_reproduces_reference_output():

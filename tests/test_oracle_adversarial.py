@@ -1,6 +1,6 @@
 """CPU: the oracle against the UNMODIFIED reference on the adversarial signal bank (tests/signals.py).
 
-The reference's outputs are stored as fingerprints (tests/test_oracle_vs_reference.fingerprint) in
+The reference's outputs are stored as fingerprints (tests/golden_cases.fingerprint) in
 tests/golden/adversarial.npz; oracle/make_golden_adversarial.py regenerates them where the reference tree exists.
 Constant frames are noise-defined in the reference (float64 round-off through log10(. + eps)): both sides get the exact
 DC-only values in those rows (signals.patch_noise_defined) before the fingerprint is taken.
@@ -11,28 +11,7 @@ import pytest
 from oracle import st_oracle as O
 from tests import signals as SG
 from tests.conftest import load_golden
-from tests.test_oracle_vs_reference import check_fingerprint
-
-# (fs, window, hop, deltas, with spectrogram / chromagram, with the float32 variants)
-CONFIGS = [(16000, 800, 400, True, True, True), (44100, 882, 441, False, True, False),
-           (16000, 400, 160, True, False, False), (16000, 800, 333, False, False, False)]
-
-
-def config_inputs(fs, w, s, floats):
-    b = dict(SG.bank(fs, w, s))
-    if floats:
-        b.update(SG.float_bank(fs, w, s))
-    return b
-
-
-def as_reference_input(x):
-    """float32 clips reach the reference as float64 (the values are exact)."""
-    return x.astype(np.float64) if x.dtype == np.float32 else x
-
-
-def key(fs, w, s, name, what):
-    return "%d_%d_%d_%s_%s" % (fs, w, s, name, what)
-
+from tests.golden_cases import CONFIGS, adv_key, as_reference_input, check_fingerprint, config_inputs
 
 @pytest.fixture(scope="module")
 def ADV():
@@ -45,10 +24,10 @@ def test_oracle_matches_reference_on_bank(ADV, fs, w, s, deltas, rows, floats):
         xx = as_reference_input(x)
         F, _ = O.feature_extraction(xx, fs, w, s, deltas=deltas)
         F, _ = SG.patch_noise_defined(F, x, w, s)
-        check_fingerprint(F, ADV, key(fs, w, s, name, "st"), rtol=1e-9, atol=1e-12)
+        check_fingerprint(F, ADV, adv_key(fs, w, s, name, "st"), rtol=1e-9, atol=1e-12)
         if rows:
-            check_fingerprint(O.spectrogram(xx, fs, w, s)[0], ADV, key(fs, w, s, name, "sp"), rtol=1e-9, atol=1e-12)
-            check_fingerprint(O.chromagram(xx, fs, w, s)[0], ADV, key(fs, w, s, name, "ch"), rtol=1e-9, atol=1e-12)
+            check_fingerprint(O.spectrogram(xx, fs, w, s)[0], ADV, adv_key(fs, w, s, name, "sp"), rtol=1e-9, atol=1e-12)
+            check_fingerprint(O.chromagram(xx, fs, w, s)[0], ADV, adv_key(fs, w, s, name, "ch"), rtol=1e-9, atol=1e-12)
 
 
 def test_bank_properties():

@@ -14,27 +14,7 @@ import pytest
 from oracle import st_oracle as O
 from tests import signals as SG
 from tests.conftest import load_golden
-
-FS, W, S = 16000, 800, 400
-SIGNALS = ("loud_quiet", "chirp")
-# name -> (mid_window, mid_step) in samples, with the (ratio, step ratio) the reference derives from them
-CASES = {
-    "ratio_0": (400, 800, 0, 2),
-    "ratio_minus_1": (0, 800, -1, 2),
-    "tie_half_to_0": (600, 800, 0, 2),          # 0.5 rounds to even: 0
-    "tie_3_halves_to_2": (1000, 800, 2, 2),     # 1.5 rounds to even: 2
-    "longer_than_clip": (32000, 16000, 79, 40),
-    "step_above_ratio": (1200, 2000, 2, 5),
-}
-
-
-def key(signal, case, what):
-    return "%s_%s_%s" % (signal, case, what)
-
-
-def clip(signal):
-    return SG.bank(FS, W, S)[signal]
-
+from tests.golden_cases import FS, MID_CASES, S, SIGNALS, W, clip, mid_key
 
 @pytest.fixture(scope="module")
 def MID():
@@ -42,7 +22,7 @@ def MID():
 
 
 def test_case_ratios():
-    for name, (mw, ms, ratio, stepr) in CASES.items():
+    for name, (mw, ms, ratio, stepr) in MID_CASES.items():
         assert O.mid_ratios(mw, ms, W, S) == (ratio, stepr), name
 
 
@@ -51,11 +31,11 @@ def test_oracle_matches_reference_mid_edges(MID, signal):
     x = clip(signal)
     assert not SG.noise_defined_frames(x, W, S).any()          # no round-off-defined reference values
     T = O.frame_count(x.size, W, S)
-    for name, (mw, ms, ratio, stepr) in CASES.items():
+    for name, (mw, ms, ratio, stepr) in MID_CASES.items():
         with warnings.catch_warnings():
             warnings.simplefilter("ignore", RuntimeWarning)       # mean of an empty slice
             mid, st, _ = O.mid_feature_extraction(x, FS, mw, ms, W, S)
-        ref = MID[key(signal, name, "mid")]
+        ref = MID[mid_key(signal, name, "mid")]
         assert mid.shape == ref.shape == (136, -(-T // stepr)), name
         np.testing.assert_allclose(mid, ref, rtol=1e-9, atol=1e-12, err_msg="%s %s" % (signal, name))
         if ratio <= 0:

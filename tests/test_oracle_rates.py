@@ -7,7 +7,7 @@
 * At the common rates and the lowest accepted ones, the mel bank and the chroma operator are the reference's.
 * At every GPU rate config (tests.kernels.RATE_CONFIGS, hops longer than the window among them), the oracle's
   feature_extraction and chromagram of a seeded clip are the reference's, as fingerprints
-  (tests/test_oracle_vs_reference.fingerprint).
+  (tests/golden_cases.fingerprint).
 """
 import warnings
 
@@ -16,30 +16,15 @@ import pytest
 
 from oracle import st_oracle as O
 from tests.conftest import load_golden
-from tests.kernels import RATE_CONFIGS
-from tests.test_oracle_vs_reference import check_fingerprint
-from tests.test_rates_cpu import RATES
+from tests.golden_cases import TABLE_RATES, check_fingerprint, chroma_input, mel_probe, rate_input
+from tests.kernels import RATE_CONFIGS, RATES
 
-TABLE_RATES = set(RATES) | set(range(6854, 6871))
 EXC = {0: None, 1: IndexError, 2: ValueError}
 
 
 @pytest.fixture(scope="module")
 def REF():
     return load_golden("rates.npz")
-
-
-def mel_probe(K):
-    return np.random.default_rng(K).uniform(0.5, 1.5, K)
-
-
-def chroma_input(K):
-    return np.random.default_rng(K + 1).uniform(0.1, 1.0, K)
-
-
-def rate_input(fs, w, s):
-    """Half a second of the oracle's synthetic clip plus a few frames, the seed from the config."""
-    return O.synth_clip(fs + w + s, fs // 2 + 3 * w + s // 3, fs)
 
 
 def raised(fn, *a):

@@ -10,6 +10,7 @@ import pytest
 
 from oracle import st_oracle as O
 from tests.conftest import load_golden
+from tests.golden_cases import ERROR_CASES, REF_CASES, TABLE_CASES, case_input, check_fingerprint, mid_params
 
 
 @pytest.fixture(scope="module")
@@ -17,68 +18,9 @@ def REF():
     return load_golden("reference_checks.npz")
 
 
-CASES = []
-_rng = np.random.default_rng(20260922)
-for _ in range(14):
-    fs = int(_rng.choice([8000, 16000, 22050, 32000, 44100, 48000]))
-    w = int(_rng.integers(max(240, fs // 70), fs // 12))
-    s = int(_rng.integers(max(1, w // 8), w + 1))
-    n = int(_rng.integers(3 * w, 12 * w))
-    CASES.append((fs, w, s, n, int(_rng.integers(0, 10 ** 6))))
-TABLE_CASES = [(16000, 400), (44100, 441), (8000, 200), (22050, 551), (48000, 1200)]
-ERROR_CASES = [(4000, 100, 50, 50), (4000, 100, 50, 1000), (8000, 160, 80, 100),
-               (8000, 160, 80, 1000), (4000, 400, 200, 100), (16000, 800, 400, 799)]
-
-
-def case_input(fs, n, seed):
-    x = O.synth_clip(seed, n, fs)
-    if seed % 3 == 0:                       # float-valued input with a DC offset
-        rng = np.random.default_rng(seed)
-        x = x.astype(np.float64) * float(rng.uniform(0.01, 3.0)) + float(rng.uniform(-500, 500))
-    return x
-
-
-PROJ = 4          # signed row sums per row: all +1, then seeded random +-1
-
-
-def fingerprint(key, a, picks=16):
-    """One float64 vector for a 2-D array: its shape, per-row sums of |a|, PROJ per-row sums under +-1 signs seeded by `key`
-    (the first all +1: the plain row sum), and `picks` entries at positions seeded by `key`.  A sign error or compensating
-    errors inside a row change a signed sum unless they are within the tolerance."""
-    rng = np.random.default_rng(sum(key.encode()))
-    signs = rng.choice([-1.0, 1.0], size=(a.shape[1], PROJ))
-    signs[:, 0] = 1.0
-    idx = rng.choice(a.size, size=min(picks, a.size), replace=False)
-    return np.concatenate([np.array(a.shape, dtype=np.float64), np.abs(a).sum(axis=1), (a @ signs).ravel(), a.ravel()[idx]])
-
-
-def check_fingerprint(got, REF, key, rtol, atol):
-    """`got` against the stored fingerprint of the reference's matrix.  Every element within rtol / atol of the reference
-    bounds each row's sum of |values| and each signed row sum by rtol x the reference's sum of |values| plus atol per
-    element; the sampled entries are held to rtol / atol themselves."""
-    got = np.asarray(got, dtype=np.float64)
-    ref = REF[key]
-    assert got.shape == tuple(int(v) for v in ref[:2]), key
-    R, C = got.shape
-    fp = fingerprint(key, got)
-    a0, p0, s0 = 2, 2 + R, 2 + R + R * PROJ
-    bound = rtol * ref[a0:p0] + atol * C
-    np.testing.assert_array_less(np.abs(fp[a0:p0] - ref[a0:p0]), bound + 1e-300, err_msg=key + " |row| sums")
-    np.testing.assert_array_less(np.abs(fp[p0:s0] - ref[p0:s0]).reshape(R, PROJ), np.repeat(bound[:, None], PROJ, axis=1) + 1e-300,
-                                 err_msg=key + " signed row sums")
-    np.testing.assert_allclose(fp[s0:], ref[s0:], rtol=rtol, atol=atol, err_msg=key)
-
-
-def mid_params(w, s, seed):
-    rng = np.random.default_rng(seed)
-    if seed % 3 == 0:                       # the draws case_input made from the same generator
-        rng.uniform(0.01, 3.0), rng.uniform(-500, 500)
-    return int(rng.integers(2, 9)) * s + w, int(rng.integers(1, 9)) * s
-
-
-@pytest.mark.parametrize("fs,w,s,n,seed", CASES)
+@pytest.mark.parametrize("fs,w,s,n,seed", REF_CASES)
 def test_random_configurations(REF, fs, w, s, n, seed):
-    i = CASES.index((fs, w, s, n, seed))
+    i = REF_CASES.index((fs, w, s, n, seed))
     x = case_input(fs, n, seed)
     err = str(REF["c%d_error" % i])
     if err:

@@ -31,19 +31,10 @@ import pytest
 
 from oracle import st_oracle as O
 from tests import host_exe
-from tests.kernels import RATE_CONFIGS
+from tests.kernels import CTA_FALLBACK, CTA_WINDOWS, FINE, PAIR_WINDOWS, RATE_CONFIGS, RATES, SOLO_WINDOWS, WINDOWS
 
-PAIR_WINDOWS = [320, 480, 512, 640, 800, 960, 1024]
-SOLO_WINDOWS = [400, 600, 882]
-CTA_WINDOWS = [320, 400, 480, 600, 640, 800, 882]
-WINDOWS = sorted(set(PAIR_WINDOWS + SOLO_WINDOWS + CTA_WINDOWS))
-FINE = list(range(6300, 7101))               # the mel bank's refusal boundary at every specialised window
-RATES = [8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 48000, 88200, 96000, 176400, 192000]
 SWEEP = [(fs, w) for fs in FINE + RATES for w in WINDOWS]
 CTA_CAP = 110 * 1024
-# (window, hop) whose CTA staging exceeds its cap: the launcher returns unsupported and the generic kernel runs instead.
-# With run staging (hop a multiple of 8) the 800-sample window crosses the cap from hop 1 200 (6 854 Hz) .. 1 232 (16 kHz).
-CTA_FALLBACK = {(800, 1600)}
 ST_OK, ST_CHROMA, ST_MEL = 0, -3, -4
 EXC = {ST_OK: None, ST_CHROMA: "ValueError", ST_MEL: "IndexError"}
 

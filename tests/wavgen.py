@@ -73,3 +73,46 @@ def signal(name, channels, n, seed, fs=16000):
     lo, hi = _RANGE[name]
     mid, half = (lo + hi + 1) / 2, (hi - lo + 1) / 2
     return np.clip(np.round(mid + half * y), lo, hi).astype(np.int64)
+
+
+def _f32_bits(u):
+    return np.asarray(u, dtype=np.uint32).view(np.float32)
+
+
+def special_values(name, rng):
+    """1-D samples of a format: its edge cases followed by random ones."""
+    if name in _RANGE:
+        lo, hi = _RANGE[name]
+        edges = [lo, lo + 1, -1, 0, 1, hi - 1, hi, (lo + hi) // 2, (lo + hi + 1) // 2]
+        if name == "s32":               # odd values above 2^24: float32 rounding, ties included
+            edges += [2 ** 24 + 1, 2 ** 24 + 3, -(2 ** 24 + 1), 2 ** 25 + 2, 2 ** 25 + 6, 2 ** 30 + 65, -(2 ** 31 - 65),
+                      2 ** 31 - 64, 2 ** 31 - 128]
+        edges = [v for v in edges if lo <= v <= hi]
+        return np.concatenate([np.array(edges, dtype=np.int64), rng.integers(lo, hi + 1, size=3000)])
+    f32 = np.finfo(np.float32)
+    sub = _f32_bits([1, 2, 3, 5, 0x7FFFFF, 0x7FFFFE, 0x400001, 0x80000001, 0x80000003, 0x807FFFFF])
+    edges32 = np.concatenate([np.array([0.0, -0.0, np.inf, -np.inf, np.nan, 1.0, -1.0, 0.5, 3.0, f32.max, -f32.max,
+                                        f32.tiny, -f32.tiny, f32.tiny * 3], dtype=np.float32), sub])
+    if name == "f32":
+        rand = np.concatenate([rng.standard_normal(1500).astype(np.float32),
+                               _f32_bits(rng.integers(1, 2 ** 23, size=500)),                    # subnormals
+                               _f32_bits(rng.integers(0, 2 ** 32, size=1000, dtype=np.uint64))])  # any bits, NaNs too
+        return np.concatenate([edges32, rand])
+    edges64 = np.array([1e39, -1e39, 3.4028235677973366e38, 3.4028235677973362e38, 3.4028236e38, float(f32.max) * 1.5,
+                        1 + 2.0 ** -24, 1 + 3 * 2.0 ** -24, -(1 + 2.0 ** -24), 5e-324, -5e-324, 1e-300, 7e-46, 7.006e-46,
+                        2.0 ** -150, 2.0 ** -149 * 1.5, 1e-45, -1e-45, 1e308, -np.inf], dtype=np.float64)
+    rand = np.concatenate([rng.standard_normal(1500), rng.standard_normal(500) * 1e-40, rng.standard_normal(300) * 1e38,
+                           rng.integers(0, 2 ** 63, size=700, dtype=np.uint64).view(np.float64)])
+    return np.concatenate([edges32.astype(np.float64), edges64, rand])
+
+
+def flavour_samples(name, channels, seed):
+    rng = np.random.default_rng(seed)
+    v = special_values(name, rng)
+    if channels == 1:
+        return v
+    m = 40                                      # every pair of the first 40 values, then random pairs
+    head = v[:m]
+    left = np.concatenate([np.tile(head, m), v[m:]])
+    right = np.concatenate([np.concatenate([np.roll(head, k) for k in range(m)]), rng.permutation(v[m:])])
+    return np.stack([left, right], axis=1)
