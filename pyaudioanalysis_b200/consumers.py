@@ -311,12 +311,24 @@ def hmm_statistics_batch(mid, class_windows, n_windows=None):
     return out
 
 
+def _cluster_ids(values, K, what):
+    """values as int32 cluster ids, or ValueError unless each is an integer in [0, K).  Checked before any conversion:
+    a cast would silently move 2**32, -0.5 or 1.7 into a cluster that NumPy's ``labels == c`` leaves them out of, and
+    a negative index would mark a cluster from the end."""
+    if values.dtype.kind not in "biuf" or (values.dtype.kind == "f" and not np.all(np.floor(values) == values)):
+        raise ValueError("%s must be integer cluster ids" % what)
+    if values.size and (values.min() < 0 or values.max() >= K):
+        raise ValueError("%s must lie in [0, %d)" % (what, K))
+    return values.astype(np.int32)
+
+
 def cluster_distance_means(X, labels, K, rows=None):
     """The cluster distance means of speaker_diarization's silhouette (audioSegmentation.py:958-972) for one clustering,
     in one call on the current stream (``b200aa_cluster_distance_means``, DESIGN.md kernel 9).
 
-    X: CUDA float64 [n, D] (rows at any stride; a non-unit column stride is copied); labels: n host integers in [0, K);
-    rows: the clusters c to compute (None: all).  Returns CUDA float64 (A [K], B [K, K]): A[c] =
+    X: CUDA float64 [n, D] (rows at any stride; a non-unit column stride is copied); labels: n integers in [0, K), host
+    or a tensor; rows: the clusters c to compute (None: all).  A label or row that is not an integer in [0, K) raises
+    ValueError.  Returns CUDA float64 (A [K], B [K, K]): A[c] =
     np.mean(pdist(X[labels == c].T)), B[c, c2] = np.mean(cdist(X[labels == c], X[labels == c2])), bit for bit; NaN on the
     diagonal of B, for clusters not asked for and for a mean of no terms (D < 2, an empty cluster), where NumPy warns."""
     _require_cuda(X, "X")
@@ -328,11 +340,11 @@ def cluster_distance_means(X, labels, K, rows=None):
     labels = np.ascontiguousarray(labels.cpu().numpy() if isinstance(labels, torch.Tensor) else labels)
     if labels.shape != (n,):
         raise ValueError("labels must hold one cluster per row of X (%d)" % n)
-    labels = labels.astype(np.int32)
+    labels = _cluster_ids(labels, K, "labels")
     want = np.ones(K, dtype=np.uint8)
     if rows is not None:
         want[:] = 0
-        want[np.asarray(list(rows), dtype=np.int64)] = 1
+        want[_cluster_ids(np.asarray(list(rows)), K, "rows")] = 1
     with torch.cuda.device(X.device):
         A = torch.empty(K, dtype=torch.float64, device=X.device)
         B = torch.empty((K, K), dtype=torch.float64, device=X.device)

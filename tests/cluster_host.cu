@@ -6,6 +6,8 @@
 //   dist kind n D X (n x D)     kind 0: cdist(X, X) (n x n); kind 1: pdist(X.T) (D (D - 1) / 2)
 //   bigsum N seg_terms          a pairwise sum of N generated terms, by segments and leaves, then npy::pairwise_sum;
 //                               also checks that the segments tile [0, N) and every leaf holds at most 128 terms
+//   plan K D sizes (K)          make_plan at the library's kSegTerms / kPassTerms for every cluster of the given sizes:
+//                               seg_terms pass_terms n_passes, then per segment in plan order: kind, mean slot, len, pass
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -142,6 +144,23 @@ int main()
             printf("bigsum");
             pr(cluster::combine(seg.data(), L));
             pr(npy::pairwise_sum(term, 0, N, N));
+            printf("\n");
+        } else if (!strcmp(cmd, "plan")) {
+            const int K = int(rl()), D = int(rl());
+            std::vector<int64_t> off(K + 1, 0);
+            for (int c = 0; c < K; ++c) off[c + 1] = off[c] + rl();
+            const std::vector<unsigned char> want(K, 1);
+            cluster::Plan plan;
+            cluster::make_plan(off.data(), K, D, want.data(), cluster::kSegTerms, cluster::kPassTerms, plan);
+            std::vector<int> slot(plan.segs.size()), pass(plan.segs.size());
+            for (const cluster::Mean &m : plan.means)
+                for (int k = 0; k < (1 << m.levels); ++k) slot[size_t(m.seg0 + k)] = m.slot;
+            for (size_t p = 0; p + 1 < plan.pass_seg.size(); ++p)
+                for (int64_t g = plan.pass_seg[p]; g < plan.pass_seg[p + 1]; ++g) pass[size_t(g)] = int(p);
+            printf("plan %lld %lld %d", (long long)cluster::kSegTerms, (long long)cluster::kPassTerms,
+                   int(plan.pass_seg.size()) - 1);
+            for (size_t g = 0; g < plan.segs.size(); ++g)
+                printf(" %d %d %lld %d", plan.segs[g].kind, slot[g], (long long)plan.segs[g].len, pass[g]);
             printf("\n");
         } else {
             return 2;

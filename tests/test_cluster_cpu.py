@@ -8,6 +8,7 @@ import pytest
 from scipy.spatial import distance
 
 from tests import host_exe
+from tests.cluster_cases import PLAN_CASES, Plan, adversarial
 from tests.diarization_oracle import reference
 from tests.host_exe import bits, floats, hexes, run
 
@@ -33,29 +34,20 @@ def _check(exe, X, labels, K, want=None, **plan):
     assert np.array_equal(bits(B), bits(rB)), (B, rB)
 
 
-def _adversarial(rng, n, D):
-    x = rng.normal(size=(n, D)) * np.exp(rng.uniform(-40, 40, size=(n, D)))
-    x[rng.random((n, D)) < 0.05] = -0.0
-    x[rng.random((n, D)) < 0.05] = 0.0
-    x[rng.random((n, D)) < 0.05] = 5e-324 * rng.integers(1, 1000)
-    x[rng.random((n, D)) < 0.03] = 1e300 * rng.choice([-1, 1])
-    return x
-
-
 @pytest.mark.parametrize("kind", [0, 1])
 def test_pdist_adds_like_cdist(exe, kind):
     """Both kinds of distance run the same chain and equal scipy's, element by element, on adversarial values (the
     chain's order shows at huge and tiny scales)."""
     rng = np.random.default_rng(3 + kind)
     for n, D in ((1, 1), (1, 5), (7, 1), (9, 13), (40, 24), (3, 150)):
-        X = _adversarial(rng, n, D)
+        X = adversarial(rng, n, D)
         if n * D > 4:
             X.flat[rng.integers(0, n * D, size=2)] = [np.nan, np.inf]
         got = floats(run(exe, "dist %d %d %d %s\n" % (kind, n, D, hexes(X)))[0][1:])
         want = (distance.cdist(X, X) if kind == 0 else distance.pdist(X.T)).ravel()
         assert np.array_equal(bits(got), bits(want)), (kind, n, D)
     # the two scipy functions agree with each other on the same pairs
-    X = _adversarial(rng, 30, 6)
+    X = adversarial(rng, 30, 6)
     assert np.array_equal(bits(distance.pdist(X.T)), bits(distance.cdist(X.T, X.T)[np.triu_indices(6, 1)]))
 
 
@@ -74,7 +66,7 @@ def test_block_sizes(exe, sizes):
 def test_adversarial_values(exe):
     """+-0, subnormals, huge and tiny scales, NaN and inf in the rows; a one-row cluster; one feature (A is NaN)."""
     rng = np.random.default_rng(5)
-    X = _adversarial(rng, 60, 9)
+    X = adversarial(rng, 60, 9)
     labels = rng.integers(0, 4, size=60)
     labels[17] = 4                                                  # cluster 4 has one row
     _check(exe, X, labels, 5)
@@ -150,6 +142,14 @@ def test_sum_past_2_31_terms(exe):
     pairwise sum; the segments tile the terms and no leaf exceeds 128 (the harness checks both)."""
     got = floats(run(exe, "bigsum %d %d\n" % ((1 << 31) + 1000, 1 << 22))[0][1:])
     assert got[0].view(np.uint64) == got[1].view(np.uint64)
+
+
+@pytest.mark.parametrize("case", PLAN_CASES, ids=lambda c: c.name)
+def test_plan_cases_take_their_path(exe, case):
+    """Each clustering that tests/test_gpu_cluster.py runs to reach a path of make_plan still takes it at the library's
+    kSegTerms and kPassTerms, so a change of either limit cannot quietly turn the case into an easy one."""
+    plan = Plan.parse(run(exe, "plan %d %d %s\n" % (len(case.sizes), case.D, " ".join(map(str, case.sizes))))[0])
+    assert case.check(plan, case.D), (case.hits, plan.passes, plan.kind, plan.len, plan.pass_of)
 
 
 # ------------------------------------------------------------------ C ABI argument checks (no CUDA call is made)
