@@ -337,6 +337,24 @@ int b200aa_hmm_decode_f64(const double *d_mid, int64_t n_clips, int n_feats, int
 int b200aa_cluster_distance_means(const double *d_X, int64_t n, int n_feats, int64_t x_stride, const int32_t *h_labels,
                                   int n_clusters, const unsigned char *h_want, double *d_A, double *d_B, void *stream);
 
+/* Kernel 10 (csrc/thumb.cuh): music_thumbnailing's self-similarity matrix, diagonal filter, masked argmax and walk
+ * (audioSegmentation.py:40-55, :1093-1180) for a ragged batch of n_tracks standardised tracks.  Track b is h_frames[b]
+ * consecutive rows of d_X (float64, row r at d_X + r * x_stride, n_feats columns, one frame per row), after the rows of the
+ * tracks before it.  Bit for bit scipy and NumPy:
+ *   S = 1 - squareform(pdist(X_b, 'cosine'))       scipy's two-accumulator dot product, no FMA; 1.0 on the diagonal
+ *   C = convolve2d(S, eye(filter_len), 'valid')    R_b = T_b - filter_len + 1; NaN when any entry of the box is NaN
+ *   entries with |i - j| < diag_gap, i > j, or a row or column outside [h_limits[2b], h_limits[2b + 1]) set to np.min(C)
+ *   the first maximum in row-major order (the first NaN when there is one), then the reference's walk.
+ * Two modes.  d_sim non-NULL (d_out and d_idx NULL): only S, track b's [T_b, T_b] at d_sim + sum_{c<b} T_c^2.  Otherwise
+ * d_out receives the masked C, track b's [R_b, R_b] at d_out + sum_{c<b} R_c^2, and d_idx[4b ..] (i1, i2, j1, j2), frame
+ * indices (the reference returns short_step times these).  NULL pointers, n_feats < 1, x_stride < n_feats, n_tracks < 1,
+ * T_b < 1 or above 2^28, and for the filter filter_len < 1, T_b < filter_len or limits outside [0, R_b] are
+ * B200AA_ERR_INVALID, before any CUDA call.  Stream-ordered scratch: the row norms, and S plus T_b x R_b bytes of NaN
+ * windows for a slice of tracks of at most 256 MiB (a larger track is a slice of its own). */
+int b200aa_music_thumbnail(const double *d_X, int n_feats, int64_t x_stride, const int64_t *h_frames, int64_t n_tracks,
+                           int filter_len, double diag_gap, const int64_t *h_limits, double *d_sim, double *d_out,
+                           int64_t *d_idx, void *stream);
+
 /* Kernel 8 (csrc/trees.cuh): the tree classifiers of extract_features_and_train (audioTrainTest.py:52-93), bit for bit
  * scikit-learn 1.9's predict / predict_proba of RandomForestClassifier, ExtraTreesClassifier (mode 0, forest mean) and
  * GradientBoostingClassifier (mode 1, boosting sum).

@@ -74,6 +74,8 @@ SIGNATURES = {
                                       c_vp]),
     # (d_X, n, n_feats, x_stride, h_labels, n_clusters, h_want, d_A, d_B, stream)
     "b200aa_cluster_distance_means": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    # (d_X, n_feats, x_stride, h_frames, n_tracks, filter_len, diag_gap, h_limits, d_sim, d_out, d_idx, stream)
+    "b200aa_music_thumbnail": (c_int, [c_vp, c_int, c_i64, c_vp, c_i64, c_int, ctypes.c_double, c_vp, c_vp, c_vp, c_vp, c_vp]),
     # (out, h_nodes, n_nodes, h_roots, n_trees, h_values, n_leaves, n_classes, n_feats, mode, h_init, allow_nan)
     "b200aa_trees_create": (c_int, [ctypes.POINTER(c_vp), c_vp, c_i64, c_vp, c_int, c_vp, c_i64, c_int, c_int, c_int, c_vp,
                                     c_int]),

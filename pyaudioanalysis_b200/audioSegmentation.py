@@ -705,3 +705,37 @@ def speaker_diarization_evaluation(folder_name, lda_dimensions, models_dir=None)
                 features[i] = _diarization_features(wav_file, 2.0, 0.2)
             mid, st, duration = features[i]
             _diarize_file(wav_file, models, mid, st, duration, num_speakers[i], 2.0, 0.2, 0.05, dim, False)
+
+
+def standardise(st_feats):
+    """StandardScaler().fit_transform(st_feats.T) (audioSegmentation.py:51-52) on the host, as a C-contiguous float64
+    [T, F] matrix of one frame per row: the rows self_similarity_matrix compares."""
+    from sklearn.preprocessing import StandardScaler
+    return np.ascontiguousarray(StandardScaler().fit_transform(np.asarray(st_feats).T), dtype=np.float64)
+
+
+def self_similarity_matrix(feature_vectors):
+    """The reference's self_similarity_matrix (:40-55): the scaler on the host, the cosine similarities on the GPU
+    (kernel 10, ``consumers.self_similarity_batch``), bit for bit.  Returns a NumPy float64 [n_vectors, n_vectors]."""
+    import torch
+    from .consumers import self_similarity_batch
+    X = standardise(feature_vectors)
+    return self_similarity_batch(torch.from_numpy(X).cuda(), [X.shape[0]])[0].cpu().numpy()
+
+
+def music_thumbnailing(signal, sampling_rate, short_window=1.0, short_step=0.5, thumb_size=10.0, limit_1=0, limit_2=1):
+    """The reference's music_thumbnailing (:1093-1180): (A1, A2, B1, B2, the masked filtered matrix), the times NumPy
+    float64 as the reference returns them.  The signal is downmixed, its short-term features come from the drop-in
+    feature_extraction, the scaler runs on the host, and the similarity matrix, diagonal filter, masks, argmax and walk
+    run on the GPU (kernel 10, ``consumers.thumbnail_batch``), bit for bit the reference's steps on the same features."""
+    import torch
+    from .audioio import stereo_to_mono
+    from .consumers import thumbnail_batch
+    from .ShortTermFeatures import feature_extraction
+    signal = stereo_to_mono(signal)
+    st_feats, _ = feature_extraction(signal, sampling_rate, sampling_rate * short_window, sampling_rate * short_step)
+    X = standardise(st_feats)
+    idx, C = thumbnail_batch(torch.from_numpy(X).cuda(), [X.shape[0]], int(round(thumb_size / short_step)),
+                             5.0 / short_step, limit_1, limit_2)
+    i1, i2, j1, j2 = idx[0]
+    return short_step * i1, short_step * i2, short_step * j1, short_step * j2, C[0].cpu().numpy()

@@ -354,6 +354,116 @@ def cluster_distance_means(X, labels, K, rows=None):
     return A, B
 
 
+def _track_rows(X, frames):
+    """A CUDA float64 [sum T_b, F] matrix of tracks and its per-track frame counts: (X, made contiguous where the kernel
+    cannot read its strides; its row stride; frames as int64)."""
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [frames, F]")
+    n, F = X.shape
+    frames = np.ascontiguousarray(np.asarray(frames).ravel())
+    if frames.dtype.kind not in "iu" or frames.size < 1 or frames.min() < 1 or int(frames.sum()) != n or F < 1:
+        raise ValueError("frames must be positive per-track row counts of X, summing to %d" % n)
+    if F > 1 and X.stride(1) != 1:
+        X = X.contiguous()
+    return X, frames.astype(np.int64), X.stride(0) if n > 1 else F
+
+
+def _packed(buf, sides):
+    """Square [s, s] views of one packed buffer, one per side, in order."""
+    off = np.concatenate([[0], np.cumsum(sides.astype(np.int64) ** 2)])
+    return [buf[int(off[b]):int(off[b + 1])].view(int(s), int(s)) for b, s in enumerate(sides)]
+
+
+def self_similarity_batch(X, frames):
+    """The self-similarity matrices of a ragged batch of standardised tracks, in one call on the current stream
+    (``b200aa_music_thumbnail``, DESIGN.md kernel 10).  X: CUDA float64 [sum T_b, F], track b the frames[b] rows after the
+    tracks before it, one frame per row.  Returns a list of CUDA float64 [T_b, T_b]: 1 - squareform(pdist(X_b, 'cosine')),
+    bit for bit scipy's (NaN for a zero-norm or NaN frame, 1.0 on the diagonal)."""
+    X, frames, stride = _track_rows(X, frames)
+    with torch.cuda.device(X.device):
+        S = torch.empty(int((frames ** 2).sum()), dtype=torch.float64, device=X.device)
+        check(lib().b200aa_music_thumbnail(ctypes.c_void_p(X.data_ptr()), X.shape[1], stride,
+                                           ctypes.c_void_p(frames.ctypes.data), frames.size, 0, 0.0, None,
+                                           ctypes.c_void_p(S.data_ptr()), None, None, _stream()))
+    return _packed(S, frames)
+
+
+def _limit_bounds(R, limit_1, limit_2):
+    """The rows and columns [lo, hi) the reference's limit slices leave alone (audioSegmentation.py:1158-1161): ``0:int(limit_1
+    * R)`` and ``int(limit_2 * R)::`` resolved by Python's slice rules."""
+    return slice(0, int(limit_1 * R)).indices(R)[1], slice(int(limit_2 * R), None).indices(R)[0]
+
+
+def thumbnail_host(S, filter_len, diag_gap, limit_1, limit_2):
+    """The reference's steps after the similarity matrix (audioSegmentation.py:1145-1177) on the host, for the sizes the
+    kernel does not take: filter_len < 1 (np.eye raises for a negative size; eye(0) gives a (T + 1)^2 matrix of zeros) and
+    T < filter_len (convolve2d swaps its inputs in 'valid' mode).  Those matrices hold at most max(T + 1, filter_len)^2
+    entries.  Returns ((i1, i2, j1, j2), the masked matrix)."""
+    import scipy.signal
+    C = scipy.signal.convolve2d(S, np.eye(filter_len, filter_len), "valid")
+    min_sm = np.min(C)
+    i, j = np.indices(C.shape)
+    C[(np.abs(i - j) < diag_gap) | (i > j)] = min_sm
+    R = C.shape[0]
+    lo, hi = _limit_bounds(R, limit_1, limit_2)
+    C[0:lo, :] = min_sm
+    C[:, 0:lo] = min_sm
+    C[hi:, :] = min_sm
+    C[:, hi:] = min_sm
+    r, c = np.unravel_index(C.argmax(), C.shape)
+    i1, i2, j1, j2 = r, r, c, c
+    while i2 - i1 < filter_len:
+        if i1 <= 0 or j1 <= 0 or i2 >= C.shape[0] - 2 or j2 >= C.shape[1] - 2:
+            break
+        if C[i1 - 1, j1 - 1] > C[i2 + 1, j2 + 1]:
+            i1, j1 = i1 - 1, j1 - 1
+        else:
+            i2, j2 = i2 + 1, j2 + 1
+    return (i1, i2, j1, j2), C
+
+
+def thumbnail_batch(X, frames, filter_len, diag_gap, limit_1=0, limit_2=1):
+    """music_thumbnailing's steps after the scaler (audioSegmentation.py:1140-1177) for a ragged batch of standardised
+    tracks, in one call on the current stream (``b200aa_music_thumbnail``, DESIGN.md kernel 10).  X and frames as for
+    ``self_similarity_batch``; filter_len = int(round(thumb_size / short_step)); diag_gap = 5.0 / short_step.  Returns
+    (idx int64 [B, 4]: i1, i2, j1, j2 of each track, frame indices; a list of CUDA float64 [R_b, R_b], the masked filtered
+    matrices), bit for bit the reference's.  A track shorter than filter_len, and every track when filter_len < 1, runs
+    its filter, mask and walk on the host (``thumbnail_host``) from the kernel's similarity matrix."""
+    X, frames, stride = _track_rows(X, frames)
+    m = int(filter_len)
+    device = (frames >= m) & (m >= 1)
+    B = frames.size
+    idx = np.zeros((B, 4), dtype=np.int64)
+    out = [None] * B
+    with torch.cuda.device(X.device):
+        if device.any():
+            row0 = np.concatenate([[0], np.cumsum(frames)])
+            rows = np.concatenate([np.arange(row0[b], row0[b + 1]) for b in np.flatnonzero(device)])
+            Xd = X if device.all() else X[torch.as_tensor(rows, device=X.device)]
+            fd = frames[device]
+            R = fd - m + 1
+            limits = np.ascontiguousarray([_limit_bounds(int(r), limit_1, limit_2) for r in R], dtype=np.int64)
+            C = torch.empty(int((R ** 2).sum()), dtype=torch.float64, device=X.device)
+            d_idx = torch.empty((fd.size, 4), dtype=torch.int64, device=X.device)
+            check(lib().b200aa_music_thumbnail(
+                ctypes.c_void_p(Xd.data_ptr()), X.shape[1], Xd.stride(0) if Xd is not X else stride,
+                ctypes.c_void_p(fd.ctypes.data), fd.size, m, float(diag_gap), ctypes.c_void_p(limits.ctypes.data), None,
+                ctypes.c_void_p(C.data_ptr()), ctypes.c_void_p(d_idx.data_ptr()), _stream()))
+            idx[device] = d_idx.cpu().numpy()
+            for b, c in zip(np.flatnonzero(device), _packed(C, R)):
+                out[b] = c
+        if not device.all():
+            host = np.flatnonzero(~device)
+            row0 = np.concatenate([[0], np.cumsum(frames)])
+            Xh = X[torch.as_tensor(np.concatenate([np.arange(row0[b], row0[b + 1]) for b in host]), device=X.device)]
+            for b, S in zip(host, self_similarity_batch(Xh, frames[host])):
+                (i1, i2, j1, j2), C = thumbnail_host(S.cpu().numpy(), m, diag_gap, limit_1, limit_2)
+                idx[b] = (i1, i2, j1, j2)
+                out[b] = torch.from_numpy(C).to(X.device)
+    return idx, out
+
+
 TREE_FOREST, TREE_BOOST = 0, 1
 _TREE_TYPES = ("randomforest", "extratrees", "gradientboosting")
 

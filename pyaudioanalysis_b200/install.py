@@ -78,6 +78,22 @@ def install_diarization(audio_segmentation=None):
     return done
 
 
+def install_thumbnailing(audio_segmentation=None):
+    """Rebind an importable ``pyAudioAnalysis.audioSegmentation`` (or the module given) to the music thumbnails here
+    (``audioSegmentation.music_thumbnailing``: the similarity matrix, filter, masks, argmax and walk on kernel 10):
+    music_thumbnailing and self_similarity_matrix.  Returns the attributes rebound."""
+    from . import audioSegmentation as ours
+    if audio_segmentation is None:
+        import importlib
+        audio_segmentation = importlib.import_module("pyAudioAnalysis.audioSegmentation")
+    done = []
+    for n in ("music_thumbnailing", "self_similarity_matrix"):
+        _saved.setdefault((audio_segmentation, n), getattr(audio_segmentation, n))
+        setattr(audio_segmentation, n, getattr(ours, n))
+        done.append("%s.%s" % (audio_segmentation.__name__, n))
+    return done
+
+
 def uninstall():
     for (mod, n), fn in list(_saved.items()):
         setattr(mod, n, fn)
