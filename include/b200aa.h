@@ -355,6 +355,40 @@ int b200aa_music_thumbnail(const double *d_X, int n_feats, int64_t x_stride, con
                            int filter_len, double diag_gap, const int64_t *h_limits, double *d_sim, double *d_out,
                            int64_t *d_idx, void *stream);
 
+/* Kernel 11 (csrc/front.cuh): the host steps of speaker_diarization and music_thumbnailing between the features and
+ * kernels 9 and 10, bit for bit scikit-learn 1.9, scipy and NumPy.
+ *
+ * b200aa_standard_scale: StandardScaler().fit_transform of each of n_mats matrices.  Matrix b has h_rows[b] rows and n_feats
+ * columns, entry (i, j) at d_X + b * mat_stride + i * row_stride + j * col_stride, float32 (widened) or float64
+ * (B200AA_DTYPE_F32 / F64).  Its columns are summed as np.sum / np.nansum over axis 0 sums them: pairwise down each column
+ * when row_stride < col_stride or n_feats == 1, else row by row.  NaN is left out of the sums and the counts and passes
+ * through.  Writes entry (i, j) of the result at d_out + h_out_off[b] + i * out_row_stride + j * out_col_stride, and
+ * d_mean / d_scale [n_mats, n_feats] (scikit-learn's mean_ and scale_), and d_bad int32 [n_mats]: 1 for a matrix holding
+ * +-inf, which scikit-learn refuses and whose outputs are meaningless.  NULL pointers, n_mats < 1, n_feats < 1, a row count
+ * below 1, a negative offset or mat_stride, strides below 1 and an unknown dtype are B200AA_ERR_INVALID, before any CUDA
+ * call.  Stream-ordered scratch: the row counts and offsets.
+ *
+ * b200aa_outlier_columns: the feature-outlier rule of speaker_diarization (audioSegmentation.py:861-865) for the
+ * normalised [n_rows, n_feats] matrix X, column u at d_X + u * col_stride (its n_rows values contiguous): d_dist_all
+ * [n_feats] = np.sum(squareform(pdist(X.T)), axis=0), *d_mean = np.mean(dist_all), d_keep [n_feats] = dist_all < 1.1 *
+ * mean (1 / 0).  NULL pointers, n_rows < 1, n_feats outside [1, 4096] and col_stride outside [n_rows, INT_MAX] are
+ * B200AA_ERR_INVALID, before any CUDA call.  Stream-ordered scratch: the n_feats^2 distances.
+ *
+ * b200aa_pool_frames: the LDA branch's pooling (audioSegmentation.py:884-906) of n_clips [n_feats, T_b] matrices, entry
+ * (f, i) of clip b at d_st + b * clip_stride + f * row_stride + i, float32 (widened) or float64, T_b = h_frames[b]:
+ * d_out [n_clips, 2 n_feats, out_stride] float64, row f of clip b at frame i the np.mean and row n_feats + f the np.std of
+ * frames [i, min(i + ratio, T_b)) of row f; entries past T_b are not written.  NULL pointers, n_clips < 1, n_feats < 1,
+ * ratio < 1, negative strides, a frame count outside [1, out_stride] and an unknown dtype are B200AA_ERR_INVALID, before
+ * any CUDA call. */
+int b200aa_standard_scale(const void *d_X, int dtype, int64_t n_mats, int n_feats, const int64_t *h_rows, int64_t mat_stride,
+                          int64_t row_stride, int64_t col_stride, double *d_out, const int64_t *h_out_off,
+                          int64_t out_row_stride, int64_t out_col_stride, double *d_mean, double *d_scale, int32_t *d_bad,
+                          void *stream);
+int b200aa_outlier_columns(const double *d_X, int64_t n_rows, int n_feats, int64_t col_stride, double *d_dist_all,
+                           double *d_mean, unsigned char *d_keep, void *stream);
+int b200aa_pool_frames(const void *d_st, int dtype, int64_t n_clips, int n_feats, int64_t clip_stride, int64_t row_stride,
+                       const int64_t *h_frames, int64_t ratio, double *d_out, int64_t out_stride, void *stream);
+
 /* Kernel 8 (csrc/trees.cuh): the tree classifiers of extract_features_and_train (audioTrainTest.py:52-93), bit for bit
  * scikit-learn 1.9's predict / predict_proba of RandomForestClassifier, ExtraTreesClassifier (mode 0, forest mean) and
  * GradientBoostingClassifier (mode 1, boosting sum).

@@ -76,6 +76,14 @@ SIGNATURES = {
     "b200aa_cluster_distance_means": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
     # (d_X, n_feats, x_stride, h_frames, n_tracks, filter_len, diag_gap, h_limits, d_sim, d_out, d_idx, stream)
     "b200aa_music_thumbnail": (c_int, [c_vp, c_int, c_i64, c_vp, c_i64, c_int, ctypes.c_double, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (d_X, dtype, n_mats, n_feats, h_rows, mat_stride, row_stride, col_stride, d_out, h_out_off, out_row_stride,
+    #  out_col_stride, d_mean, d_scale, d_bad, stream)
+    "b200aa_standard_scale": (c_int, [c_vp, c_int, c_i64, c_int, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_vp, c_vp,
+                                      c_vp, c_vp]),
+    # (d_X, n_rows, n_feats, col_stride, d_dist_all, d_mean, d_keep, stream)
+    "b200aa_outlier_columns": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    # (d_st, dtype, n_clips, n_feats, clip_stride, row_stride, h_frames, ratio, d_out, out_stride, stream)
+    "b200aa_pool_frames": (c_int, [c_vp, c_int, c_i64, c_int, c_i64, c_i64, c_vp, c_i64, c_vp, c_i64, c_vp]),
     # (out, h_nodes, n_nodes, h_roots, n_trees, h_values, n_leaves, n_classes, n_feats, mode, h_init, allow_nan)
     "b200aa_trees_create": (c_int, [ctypes.POINTER(c_vp), c_vp, c_i64, c_vp, c_int, c_vp, c_i64, c_int, c_int, c_int, c_vp,
                                     c_int]),

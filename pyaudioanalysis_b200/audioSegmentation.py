@@ -18,10 +18,12 @@ The reference's behaviour is kept where it is visible to a caller:
 reference's text.  Its classifier methods need the reference's own function (``install.install_segmentation`` keeps
 it); called here they raise ValueError.
 
-Speaker diarization (:815-1091): ``diarize`` runs the steps after the mid-term features.  The SVM posteriors, the
-StandardScaler, the feature-outlier rule, k-means and LDA stay on the host, as the reference makes them; the silhouette's
-cluster distance means run on the GPU (kernel 9, ``consumers.cluster_distance_means``) and the HMM smoothing on kernel 7
-(``train_hmm_compute_statistics`` and the float64 decode).  The reference's visible quirks are kept:
+Speaker diarization (:815-1091): ``diarize`` runs the steps after the mid-term features.  The SVM posteriors, k-means
+and LDA stay on the host, as the reference makes them; the StandardScalers, the feature-outlier rule and the LDA branch's
+pooling run on the GPU (kernel 11, ``consumers.standard_scale_batch`` / ``outlier_columns`` / ``pool_frames_batch``), the
+silhouette's cluster distance means on kernel 9 (``consumers.cluster_distance_means``) and the HMM smoothing on kernel 7
+(``hmm_statistics_batch`` and the float64 decode), all from one upload of the matrix.  The reference's visible quirks are
+kept:
 - the "outliers" dropped are feature columns (dist_all is the pdist of the columns of the normalised matrix);
 - A[c] is the mean pdist over the transposed cluster, i.e. between its feature columns;
 - the labels smoothed by the HMM and the median filter are those of the LAST candidate speaker count, not of the best;
@@ -509,14 +511,18 @@ def cluster_means_gpu(x, cls, k, rows):
 
 
 def _hmm_smooth(x, cls):
-    """The HMM post-processing of :1001-1010: statistics of x.T per label, then predict(x) of the C-contiguous x on the
-    GPU (kernel 7, float64 windows)."""
+    """The HMM post-processing of :1001-1010 for the normalised matrix x [M, D] (a CUDA float64 tensor, or host data,
+    uploaded here): statistics of x.T per label, then predict(x) of the C-contiguous x on the GPU (kernel 7, float64
+    windows)."""
     import torch
-    from .consumers import HmmModel, hmm_decode_batch
-    start_prob, transmat, means, cov = train_hmm_compute_statistics(x.T, cls)
+    from .consumers import HmmModel, hmm_decode_batch, hmm_statistics_batch
+    if not isinstance(x, torch.Tensor):
+        x = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64)).cuda()
+    features = x.t().contiguous().unsqueeze(0)
+    start_prob, transmat, means, cov = _statistics(cls, x.shape[0], lambda windows: hmm_statistics_batch(features, windows))
     hmm = DiagonalGaussianHMM(start_prob.shape[0], "diag")
     hmm.startprob_, hmm.transmat_, hmm.means_, hmm.covars_ = start_prob, transmat, means, cov
-    t = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float64)).cuda()
+    t = x.contiguous()
     ids, bad = hmm_decode_batch(t.unsqueeze(0).transpose(1, 2), HmmModel(hmm, t.device))
     if bool(bad[0]):
         raise _nonfinite()
@@ -535,27 +541,48 @@ def diarize(mid, models, n_speakers, mid_step, short_window, lda_dim, st=None, m
     short-term frame is pooled as the reference pools it (``pool_frames``) and projected by LDA, and there is no HMM.  cluster(x, k) -> labels
     (default: sklearn.cluster.KMeans(n_clusters=k), seeded by the global NumPy state as in the reference); means(x, cls,
     k, rows) -> (A, B) (default: kernel 9)."""
+    import torch
     from scipy.signal import medfilt
-    from scipy.spatial import distance
-    from sklearn.preprocessing import StandardScaler
+    from .consumers import outlier_columns, pool_frames_batch, standard_scale_batch
     cluster = _kmeans if cluster is None else cluster
     means = cluster_means_gpu if means is None else means
     mid = np.asarray(mid, dtype=np.float64)
+    if lda_dim > 0 and (models is None or st is None or mid_window is None):
+        raise ValueError("lda_dim > 0 needs models (the posteriors of every short-term frame are computed here), st "
+                         "and mid_window")
     if posteriors is None:
         posteriors = [_posteriors(mid.T, m) for m in models]
-    mid_feats_norm = StandardScaler().fit_transform(_with_posteriors(mid, posteriors).T)
-    dist_all = np.sum(distance.squareform(distance.pdist(mid_feats_norm.T)), axis=0)
-    i_non_outliers = np.nonzero(dist_all < 1.1 * np.mean(dist_all))[0]
-    mt_feats_norm_or = mid_feats_norm
-    mid_feats_norm = mid_feats_norm[:, i_non_outliers]
+    feats = _with_posteriors(mid, posteriors)
+    on_device = means is cluster_means_gpu          # a caller's own host means keeps the matrix on the host
+    if on_device:
+        # StandardScaler().fit_transform(feats.T) of the C-contiguous [D, M] feats: a column-major [M, D] on the device
+        norm_dev = standard_scale_batch(torch.from_numpy(feats).cuda().t())[0]
+        i_non_outliers = outlier_columns(norm_dev)[0]
+        mt_feats_norm_or = norm_dev.t().cpu().numpy().T
+    else:
+        from scipy.spatial import distance
+        from sklearn.preprocessing import StandardScaler
+        mt_feats_norm_or = StandardScaler().fit_transform(feats.T)
+        dist_all = np.sum(distance.squareform(distance.pdist(mt_feats_norm_or.T)), axis=0)
+        i_non_outliers = np.nonzero(dist_all < 1.1 * np.mean(dist_all))[0]
+        norm_dev = None
+    mid_feats_norm = mt_feats_norm_or[:, i_non_outliers]
     if lda_dim > 0:
         import sklearn.discriminant_analysis
-        if models is None or st is None or mid_window is None:
-            raise ValueError("lda_dim > 0 needs models (the posteriors of every short-term frame are computed here), st "
-                             "and mid_window")
-        pooled = pool_frames(st, int(round(mid_window / short_window)))
-        red = _with_posteriors(pooled, [_posteriors(pooled.T, m) for m in models])
-        red = StandardScaler().fit_transform(red.T).T
+        ratio = int(round(mid_window / short_window))
+        if on_device:
+            st = np.asarray(st)
+            st_dev = torch.from_numpy(np.ascontiguousarray(st, dtype=np.float32 if st.dtype == np.float32 else np.float64))
+            pooled_dev = pool_frames_batch(st_dev.cuda(), ratio)
+            pooled = pooled_dev.cpu().numpy()
+            post = _with_posteriors(np.zeros((0, pooled.shape[1])), [_posteriors(pooled.T, m) for m in models])
+            red_dev = torch.cat([pooled_dev, torch.from_numpy(post).to(pooled_dev.device)])
+            red = standard_scale_batch(red_dev.t())[0].t().cpu().numpy()
+        else:
+            from sklearn.preprocessing import StandardScaler
+            pooled = pool_frames(st, ratio)
+            red = _with_posteriors(pooled, [_posteriors(pooled.T, m) for m in models])
+            red = StandardScaler().fit_transform(red.T).T
         labels = np.zeros((red.shape[1],))
         lda_step_ratio = 1.0 / short_window
         for index in range(labels.shape[0]):
@@ -564,8 +591,9 @@ def diarize(mid, models, n_speakers, mid_step, short_window, lda_dim, st=None, m
         mid_feats_norm = clf.fit_transform(red.T, labels)
     s_range = range(2, 10) if n_speakers <= 0 else [n_speakers]
     x = mid_feats_norm
-    if means is cluster_means_gpu:                  # one upload for every candidate count
-        import torch
+    if on_device and lda_dim <= 0:                  # the device copy, for every candidate count
+        x = norm_dev[:, torch.from_numpy(i_non_outliers).to(norm_dev.device)].contiguous()
+    elif on_device:
         x = torch.from_numpy(np.ascontiguousarray(mid_feats_norm, dtype=np.float64)).cuda()
     cluster_labels, sil_all = [], []
     cls = None
@@ -579,7 +607,7 @@ def diarize(mid, models, n_speakers, mid_step, short_window, lda_dim, st=None, m
     imax = int(np.argmax(sil_all))
     num_speakers = s_range[imax]
     if lda_dim <= 0:
-        cls = _hmm_smooth(mt_feats_norm_or, cls)
+        cls = _hmm_smooth(mt_feats_norm_or if norm_dev is None else norm_dev, cls)
     cls = medfilt(cls, 5)
     if not details:
         return cls
@@ -714,28 +742,36 @@ def standardise(st_feats):
     return np.ascontiguousarray(StandardScaler().fit_transform(np.asarray(st_feats).T), dtype=np.float64)
 
 
-def self_similarity_matrix(feature_vectors):
-    """The reference's self_similarity_matrix (:40-55): the scaler on the host, the cosine similarities on the GPU
-    (kernel 10, ``consumers.self_similarity_batch``), bit for bit.  Returns a NumPy float64 [n_vectors, n_vectors]."""
+def _standardise_device(st_feats):
+    """``standardise`` on the GPU (kernel 11): StandardScaler().fit_transform(st_feats.T) of the float64 features,
+    as a CUDA C-contiguous float64 [T, F] matrix, bit for bit."""
     import torch
+    from .consumers import standard_scale_batch
+    st = torch.from_numpy(np.ascontiguousarray(st_feats, dtype=np.float64)).cuda()
+    return standard_scale_batch(st.t())[0].contiguous()
+
+
+def self_similarity_matrix(feature_vectors):
+    """The reference's self_similarity_matrix (:40-55): the scaler and the cosine similarities on the GPU (kernels 11 and
+    10, ``consumers.standard_scale_batch`` and ``consumers.self_similarity_batch``), bit for bit.  Returns a NumPy float64
+    [n_vectors, n_vectors]."""
     from .consumers import self_similarity_batch
-    X = standardise(feature_vectors)
-    return self_similarity_batch(torch.from_numpy(X).cuda(), [X.shape[0]])[0].cpu().numpy()
+    X = _standardise_device(feature_vectors)
+    return self_similarity_batch(X, [X.shape[0]])[0].cpu().numpy()
 
 
 def music_thumbnailing(signal, sampling_rate, short_window=1.0, short_step=0.5, thumb_size=10.0, limit_1=0, limit_2=1):
     """The reference's music_thumbnailing (:1093-1180): (A1, A2, B1, B2, the masked filtered matrix), the times NumPy
     float64 as the reference returns them.  The signal is downmixed, its short-term features come from the drop-in
-    feature_extraction, the scaler runs on the host, and the similarity matrix, diagonal filter, masks, argmax and walk
-    run on the GPU (kernel 10, ``consumers.thumbnail_batch``), bit for bit the reference's steps on the same features."""
-    import torch
+    feature_extraction, the scaler runs on the GPU (kernel 11), and the similarity matrix, diagonal filter, masks, argmax
+    and walk on kernel 10 (``consumers.thumbnail_batch``), bit for bit the reference's steps on the same features."""
     from .audioio import stereo_to_mono
     from .consumers import thumbnail_batch
     from .ShortTermFeatures import feature_extraction
     signal = stereo_to_mono(signal)
     st_feats, _ = feature_extraction(signal, sampling_rate, sampling_rate * short_window, sampling_rate * short_step)
-    X = standardise(st_feats)
-    idx, C = thumbnail_batch(torch.from_numpy(X).cuda(), [X.shape[0]], int(round(thumb_size / short_step)),
+    X = _standardise_device(st_feats)
+    idx, C = thumbnail_batch(X, [X.shape[0]], int(round(thumb_size / short_step)),
                              5.0 / short_step, limit_1, limit_2)
     i1, i2, j1, j2 = idx[0]
     return short_step * i1, short_step * i2, short_step * j1, short_step * j2, C[0].cpu().numpy()

@@ -316,21 +316,23 @@ def music_thumbnailing_batch(signals, sampling_rate, short_window=1.0, short_ste
                              limit_2=1, lengths=None):
     """Batched audioSegmentation.music_thumbnailing for mono clips (what audioio.load_batch returns): (times float64
     [B, 4]: A1, A2, B1, B2 of each clip; a list of CUDA float64 [R_b, R_b], the masked filtered matrices).  Clip b's results
-    are bit for bit the one-clip call on ``signals[b, :lengths[b]]``.  The short-term features and kernel 10 run on the
-    GPU; each clip's StandardScaler runs on the host, as in the one-clip call.  A clip shorter than one window raises the
-    feature path's ValueError."""
+    are bit for bit the one-clip call on ``signals[b, :lengths[b]]``.  Everything runs on the GPU: the short-term
+    features, every clip's StandardScaler in one launch (kernel 11) read straight from the feature tensor, and kernel 10.
+    A clip shorter than one window raises the feature path's ValueError."""
     import numpy as np
 
-    from .audioSegmentation import standardise
-    from .consumers import thumbnail_batch
+    from .consumers import _scale_input, _scale_into, thumbnail_batch
     window, step = int(sampling_rate * short_window), int(sampling_rate * short_step)
     feats = feature_extraction_batch(signals, sampling_rate, window, step, lengths=lengths)
     B, _, T = feats.shape
     frames = np.full(B, T, dtype=np.int64) if lengths is None else frame_counts(lengths, window, step).cpu().numpy()
     if (frames < 1).any():
         check(_lib.ERR_TOO_SHORT)
-    host = feats.cpu().numpy()
-    X = np.concatenate([standardise(host[b, :, :frames[b]].astype(np.float64)) for b in range(B)])
-    idx, C = thumbnail_batch(torch.from_numpy(X).to(feats.device), frames, int(round(thumb_size / short_step)),
+    # clip b's StandardScaler().fit_transform(features.T) (column-major: pairwise column sums), packed C-contiguous
+    Xb, frames = _scale_input(feats.transpose(1, 2), frames)
+    F = Xb.shape[2]
+    X = torch.empty((int(frames.sum()), F), dtype=torch.float64, device=feats.device)
+    _scale_into(Xb, frames, X, np.concatenate([[0], np.cumsum(frames)[:-1]]).astype(np.int64) * F, F, 1)
+    idx, C = thumbnail_batch(X, frames, int(round(thumb_size / short_step)),
                              5.0 / short_step, limit_1, limit_2)
     return short_step * idx, C

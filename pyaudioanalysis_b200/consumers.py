@@ -464,6 +464,118 @@ def thumbnail_batch(X, frames, filter_len, diag_gap, limit_1=0, limit_2=1):
     return idx, out
 
 
+def _scale_into(X, rows, out, out_off, out_row_stride, out_col_stride):
+    """b200aa_standard_scale of X [B, n_max, D] (CUDA float32 / float64, strides >= 1) into `out` at the element offsets
+    out_off [B]: (mean, scale) CUDA float64 [B, D].  A matrix holding +-inf is handed to scikit-learn, which raises."""
+    B, n_max, D = X.shape
+    with torch.cuda.device(X.device):
+        mean = torch.empty((B, D), dtype=torch.float64, device=X.device)
+        scale = torch.empty((B, D), dtype=torch.float64, device=X.device)
+        bad = torch.empty(B, dtype=torch.int32, device=X.device)
+        check(lib().b200aa_standard_scale(
+            ctypes.c_void_p(X.data_ptr()), DTYPE_F32 if X.dtype == torch.float32 else DTYPE_F64, B, D,
+            ctypes.c_void_p(rows.ctypes.data), X.stride(0), X.stride(1), X.stride(2), ctypes.c_void_p(out.data_ptr()),
+            ctypes.c_void_p(out_off.ctypes.data), out_row_stride, out_col_stride, ctypes.c_void_p(mean.data_ptr()),
+            ctypes.c_void_p(scale.data_ptr()), ctypes.c_void_p(bad.data_ptr()), _stream()))
+    for b in np.flatnonzero(bad.cpu().numpy()):
+        from sklearn.preprocessing import StandardScaler
+        StandardScaler().fit_transform(X[b, :rows[b]].cpu().numpy().astype(np.float64))
+        raise ValueError("Input X contains infinity or a value too large for dtype('float64').")
+    return mean, scale
+
+
+def _scale_input(X, rows):
+    """X as a CUDA [B, n_max, D] float tensor with strides >= 1 and its row counts as int64 [B]."""
+    _require_cuda(X, "X")
+    if X.dim() not in (2, 3) or X.dtype not in (torch.float32, torch.float64):
+        raise ValueError("X must be float32 / float64 [n, D] or [B, n, D]")
+    X3 = X.unsqueeze(0) if X.dim() == 2 else X
+    B, n_max, D = X3.shape
+    if B < 1 or n_max < 1 or D < 1:
+        raise ValueError("X must hold at least one matrix of one row and one column")
+    if min(X3.stride()) < 1:
+        X3 = X3.contiguous()
+    rows = np.full(B, n_max, dtype=np.int64) if rows is None else np.ascontiguousarray(np.asarray(rows).ravel())
+    if rows.dtype.kind not in "iu" or rows.shape != (B,) or rows.min() < 1 or rows.max() > n_max:
+        raise ValueError("rows must be one count in [1, %d] per matrix" % n_max)
+    return X3, rows.astype(np.int64)
+
+
+def standard_scale_batch(X, rows=None):
+    """StandardScaler().fit_transform of every matrix of a batch, in one call on the current stream
+    (``b200aa_standard_scale``, DESIGN.md kernel 11), bit for bit scikit-learn 1.9.
+
+    X: CUDA float32 (widened) or float64, one matrix [n, D] or a batch [B, n_max, D] at any strides, matrix b its first
+    rows[b] rows (default: all).  As NumPy's axis-0 sums, a matrix whose row stride is below its column stride (a
+    column-major matrix, such as the transpose of a C-contiguous [D, n] array) has each column summed pairwise, any other
+    row by row.  NaN is left out of the statistics and passes through; a matrix holding +-inf raises scikit-learn's
+    ValueError.  Returns (Y, mean, scale): Y CUDA float64 of X's shape in the layout scikit-learn returns (column-major
+    matrices for a column-major X, else C-contiguous), zero past each matrix's rows; mean and scale CUDA float64 [B, D]
+    (or [D]), scikit-learn's mean_ and scale_."""
+    X3, rows = _scale_input(X, rows)
+    B, n_max, D = X3.shape
+    column_major = D == 1 or X3.stride(1) < X3.stride(2)
+    with torch.cuda.device(X3.device):
+        if column_major:
+            Y = torch.zeros((B, D, n_max), dtype=torch.float64, device=X3.device).transpose(1, 2)
+        else:
+            Y = torch.zeros((B, n_max, D), dtype=torch.float64, device=X3.device)
+    mean, scale = _scale_into(X3, rows, Y, np.arange(B, dtype=np.int64) * n_max * D, Y.stride(1), Y.stride(2))
+    if X.dim() == 2:
+        return Y[0], mean[0], scale[0]
+    return Y, mean, scale
+
+
+def outlier_columns(X):
+    """The feature-outlier rule of speaker_diarization (audioSegmentation.py:861-865) for a normalised CUDA float64 [M, D]
+    matrix, in one call on the current stream (``b200aa_outlier_columns``, DESIGN.md kernel 11): dist_all =
+    np.sum(squareform(pdist(X.T)), axis=0) and the columns with dist_all < 1.1 * np.mean(dist_all), bit for bit.  A
+    matrix whose columns are not contiguous is copied.  Returns (i_non_outliers int64 NumPy, dist_all CUDA float64 [D])."""
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64 or X.shape[0] < 1 or X.shape[1] < 1:
+        raise ValueError("X must be float64 [M, D] with M, D >= 1")
+    M, D = X.shape
+    if M > 1 and X.stride(0) != 1 or D > 1 and X.stride(1) < M:
+        X = X.t().contiguous().t()
+    with torch.cuda.device(X.device):
+        dist_all = torch.empty(D, dtype=torch.float64, device=X.device)
+        mean = torch.empty(1, dtype=torch.float64, device=X.device)
+        keep = torch.empty(D, dtype=torch.uint8, device=X.device)
+        check(lib().b200aa_outlier_columns(ctypes.c_void_p(X.data_ptr()), M, D, X.stride(1) if D > 1 else M,
+                                           ctypes.c_void_p(dist_all.data_ptr()), ctypes.c_void_p(mean.data_ptr()),
+                                           ctypes.c_void_p(keep.data_ptr()), _stream()))
+    return np.flatnonzero(keep.cpu().numpy()).astype(np.int64), dist_all
+
+
+def pool_frames_batch(st, ratio, frames=None):
+    """The LDA branch's pooling of speaker_diarization (audioSegmentation.py:884-906, ``audioSegmentation.pool_frames``)
+    for a ragged batch, in one call on the current stream (``b200aa_pool_frames``, DESIGN.md kernel 11).  st: CUDA
+    float32 (widened) or float64 [F, T] or [B, F, T], clip b its first frames[b] frames (default: all).  Returns CUDA
+    float64 [2F, T] / [B, 2F, T]: row f at frame i the np.mean and row F + f the np.std of frames [i, min(i + ratio, T_b))
+    of row f, bit for bit; zero past each clip's frames.  ratio < 1 raises ValueError."""
+    _require_cuda(st, "st")
+    if st.dim() not in (2, 3) or st.dtype not in (torch.float32, torch.float64):
+        raise ValueError("st must be float32 / float64 [F, T] or [B, F, T]")
+    s3 = st.unsqueeze(0) if st.dim() == 2 else st
+    B, F, T = s3.shape
+    if B < 1 or F < 1 or T < 1:
+        raise ValueError("st must hold at least one clip of one row and one frame")
+    if (T > 1 and s3.stride(2) != 1) or min(s3.stride()) < 0:
+        s3 = s3.contiguous()
+    frames = np.full(B, T, dtype=np.int64) if frames is None else np.ascontiguousarray(np.asarray(frames).ravel())
+    if frames.dtype.kind not in "iu" or frames.shape != (B,) or frames.min() < 1 or frames.max() > T:
+        raise ValueError("frames must be one count in [1, %d] per clip" % T)
+    frames = frames.astype(np.int64)
+    if int(ratio) != ratio or ratio < 1:
+        raise ValueError("ratio must be an integer >= 1")
+    with torch.cuda.device(s3.device):
+        out = torch.zeros((B, 2 * F, T), dtype=torch.float64, device=s3.device)
+        check(lib().b200aa_pool_frames(ctypes.c_void_p(s3.data_ptr()), DTYPE_F32 if s3.dtype == torch.float32 else DTYPE_F64,
+                                       B, F, s3.stride(0), s3.stride(1), ctypes.c_void_p(frames.ctypes.data), int(ratio),
+                                       ctypes.c_void_p(out.data_ptr()), T, _stream()))
+    return out[0] if st.dim() == 2 else out
+
+
 TREE_FOREST, TREE_BOOST = 0, 1
 _TREE_TYPES = ("randomforest", "extratrees", "gradientboosting")
 

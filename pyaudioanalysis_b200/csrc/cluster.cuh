@@ -212,3 +212,9 @@ __host__ __device__ inline int64_t dist_index(const Segment &s, int64_t u, int64
 
 }  // namespace cluster
 }  // namespace b200aa
+
+// The distance tile kernel (cluster.cu): segments [s0, s1) of a pass, G's rows `D` doubles apart.  Kernel 11's outlier rule
+// (front.cu) launches it too, on one kBlock segment of every pair of columns.
+__global__ void __launch_bounds__(b200aa::cluster::kThreads, 2)
+cluster_dist_kernel(const b200aa::cluster::Segment *__restrict__ segs, int64_t s0, int64_t s1, const double *__restrict__ G,
+                    int D, double *__restrict__ dist);

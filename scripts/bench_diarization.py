@@ -1,5 +1,6 @@
-"""Time speaker diarization's silhouette stage (kernel 9 against scipy + NumPy on the host) and ``diarize`` end to end on
-a synthetic 1 h mid-term matrix with a per-stage breakdown.  Prints one JSON line per measurement.
+"""Time speaker diarization's silhouette stage (kernel 9 against scipy + NumPy on the host), its scaler, outlier rule and
+LDA pooling (kernel 11 against scikit-learn, scipy and NumPy on the host), and ``diarize`` end to end on a synthetic 1 h
+mid-term matrix with a per-stage breakdown.  Prints one JSON line per measurement.
 
     python scripts/bench_diarization.py [--host-max 3600] [--skip-diarize]
 
@@ -29,6 +30,64 @@ def host_means(X, labels, K):
                 if c2 != c:
                     B[c, c2] = np.mean(distance.cdist(xc, X[labels == c2]))
     return A, B
+
+
+def front_stage(rng, dev):
+    """Kernel 11 against the host steps it replaces: the scaler and the outlier rule of a 1 h matrix (M = 36 000 windows
+    of D = 146), and the LDA branch's pooling plus its scaler at T = 72 000 short-term frames (1 h at 50 ms, ratio 40).
+    Device times include the upload of the host matrix and the copies back that diarize makes."""
+    import torch
+    from scipy.spatial import distance
+    from sklearn.preprocessing import StandardScaler
+    from pyaudioanalysis_b200 import audioSegmentation as S
+    from pyaudioanalysis_b200.consumers import outlier_columns, pool_frames_batch, standard_scale_batch
+
+    def best(fn, reps):
+        out, ts = None, []
+        for _ in range(reps):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = fn()
+            torch.cuda.synchronize()
+            ts.append(time.perf_counter() - t0)
+        return out, min(ts) * 1e3
+
+    def same(a, b):
+        return bool(np.array_equal(np.asarray(a).view(np.uint64), np.asarray(b).view(np.uint64)))
+
+    feats = rng.normal(size=(146, 36000)) * np.exp(rng.normal(size=(146, 1)))
+
+    def host_a():
+        x = StandardScaler().fit_transform(feats.T)
+        d = np.sum(distance.squareform(distance.pdist(x.T)), axis=0)
+        return x, np.nonzero(d < 1.1 * np.mean(d))[0]
+
+    def dev_a():
+        y = standard_scale_batch(torch.from_numpy(feats).cuda().t())[0]
+        return y.t().cpu().numpy().T, outlier_columns(y)[0]
+    (hx, hk), host_ms = best(host_a, 3)
+    best(dev_a, 2)
+    (dx, dk), dev_ms = best(dev_a, 5)
+    print(json.dumps({"stage": "scaler_outliers", "M": 36000, "D": 146, "host_ms": round(host_ms, 2),
+                      "gpu_ms": round(dev_ms, 3), "bit_equal": same(hx, dx) and bool(np.array_equal(hk, dk)),
+                      "device": dev}), flush=True)
+    st = (rng.normal(size=(68, 72000)) * 3).astype(np.float32)
+    post = rng.random((72000, 12))
+
+    def host_b():
+        pooled = S.pool_frames(st, 40)
+        return pooled, StandardScaler().fit_transform(S._with_posteriors(pooled, [post]).T).T
+
+    def dev_b():
+        pooled_dev = pool_frames_batch(torch.from_numpy(st).cuda(), 40)
+        pooled = pooled_dev.cpu().numpy()
+        red = torch.cat([pooled_dev, torch.from_numpy(post.T + 1e-4).cuda()])
+        return pooled, standard_scale_batch(red.t())[0].t().cpu().numpy()
+    (hp, hr), host_ms = best(host_b, 1)
+    best(dev_b, 2)
+    (dp, dr), dev_ms = best(dev_b, 5)
+    print(json.dumps({"stage": "lda_pool_scaler", "T": 72000, "ratio": 40, "host_ms": round(host_ms, 1),
+                      "gpu_ms": round(dev_ms, 3), "bit_equal": same(hp, dp) and same(hr, dr), "device": dev}), flush=True)
 
 
 def main():
@@ -64,6 +123,7 @@ def main():
             else:
                 row["host_ms"] = "not measured"
             print(json.dumps(row), flush=True)
+    front_stage(rng, dev)
     if args.skip_diarize:
         return
     # diarize on a synthetic 1 h matrix at the default 0.1 s step: 36 000 windows, 136 features, two seeded SVCs

@@ -12,6 +12,7 @@ measurement, the first naming the card and its power limit.
   signals already on the GPU and from WAV files decoded by ``audioio.load_batch`` (files written to a temporary
   directory first, not timed)."""
 import argparse
+import hashlib
 import ctypes
 import json
 import os
@@ -127,7 +128,8 @@ def main():
     torch.cuda.synchronize()
     wall = time.perf_counter() - t0
     print(json.dumps({"batch": "signals on the GPU", "tracks": n_chunks * args.chunk, "seconds_per_track": seconds,
-                      "wall_s": wall}), flush=True)
+                      "wall_s": wall, "times_sha1": hashlib.sha1(np.ascontiguousarray(times).tobytes()).hexdigest()}),
+          flush=True)
     with tempfile.TemporaryDirectory() as d:
         paths = []
         for b in range(args.chunk):
