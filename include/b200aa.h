@@ -42,7 +42,7 @@ typedef enum b200aa_status {
 /* sample formats of the clip buffer */
 #define B200AA_DTYPE_I16 0        /* int16 PCM as scipy.io.wavfile.read returns it (audioBasicIO.py:99) */
 #define B200AA_DTYPE_F32 1        /* float32 samples (any scale; the path is scale invariant)           */
-#define B200AA_DTYPE_F64 2        /* float64 (b200aa_knn_classify's query vectors only)                  */
+#define B200AA_DTYPE_F64 2        /* float64 (the float64 feature path, b200aa_knn_classify's query vectors) */
 
 #define B200AA_N_BASE 34          /* ShortTermFeatures.py:580-585 */
 #define B200AA_N_MEL 40           /* ShortTermFeatures.py:191-192 */
@@ -58,6 +58,13 @@ typedef struct b200aa_clip_norm {
     float hi;       /* smallest representable sample value >= mean, minus m   */
     float rsv[3];   /* scratch used while the statistics are accumulated       */
 } b200aa_clip_norm;
+
+/* Per-clip normalisation of the float64 path: y = (x / 32768.0 - mean) / scale, bit for bit the reference's
+ * `signal / 2**15` + dc_normalize() in NumPy float64.  16 bytes. */
+typedef struct b200aa_clip_norm_f64 {
+    double mean;    /* np.mean(x / 32768.0)                          */
+    double scale;   /* np.abs(x / 32768.0 - mean).max() + 1e-10      */
+} b200aa_clip_norm_f64;
 
 typedef struct b200aa_plan b200aa_plan;   /* opaque: constant tables of one (fs, window, step) on one device */
 
@@ -204,6 +211,42 @@ int b200aa_long_term_mean_ragged(const float *d_mid, int64_t n_clips, int n_rows
 int b200aa_normalize_windows(const float *d_mid, int64_t n_clips, int n_rows, int64_t n_windows,
                              const float *d_mean, const float *d_std, float *d_out, void *stream);
 
+/* ------------------------------------------------------------------ float64 path (kernel family 12)
+ * The float64 counterparts of the entry points above: the same arguments, float64 outputs, and d_sig may also be
+ * float64 (B200AA_DTYPE_F64, read unrounded).  Every value is computed in float64 as the float64 oracle computes it
+ * (csrc/f64.cuh): the normalisation and rows 0-1 (zcr, energy) bit for bit NumPy, the transform an fp64 mixed-radix
+ * FFT, the other rows in the order of the oracle's loop.  Argument checks and refusals are the float32 entry points'. */
+
+/* Normalisation records of the float64 path: d_norm [n_clips] (d_len as in b200aa_clip_stats). */
+int b200aa_clip_stats_f64(const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples, int64_t clip_stride,
+                          const int64_t *d_len, b200aa_clip_norm_f64 *d_norm, void *stream);
+/* d_out float64 [n_clips, F, t_stride] as b200aa_st_features; d_norm from b200aa_clip_stats_f64 with the same d_len. */
+int b200aa_st_features_f64(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                           int64_t clip_stride, const int64_t *d_len, const b200aa_clip_norm_f64 *d_norm, int deltas,
+                           double *d_out, int64_t t_stride, void *stream);
+int b200aa_spectrogram_f64(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                           int64_t clip_stride, const b200aa_clip_norm_f64 *d_norm, double *d_out, void *stream);
+int b200aa_spectrogram_ragged_f64(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                                  int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                                  const b200aa_clip_norm_f64 *d_norm, double *d_out, void *stream);
+int b200aa_chromagram_f64(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips, int64_t n_samples,
+                          int64_t clip_stride, const b200aa_clip_norm_f64 *d_norm, double *d_out, void *stream);
+int b200aa_chromagram_ragged_f64(const b200aa_plan *plan, const void *d_sig, int dtype, int64_t n_clips,
+                                 int64_t n_samples, int64_t clip_stride, const int64_t *d_len,
+                                 const b200aa_clip_norm_f64 *d_norm, double *d_out, void *stream);
+/* Mid-term pooling of float64 rows, bit for bit np.mean / np.std of each window and np.nan_to_num
+ * (MidTermFeatures.py:110-126); windows, ratio and step_ratio as in b200aa_mid_pool / b200aa_mid_pool_ragged. */
+int b200aa_mid_pool_f64(const double *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
+                        int ratio, int step_ratio, double *d_mid, void *stream);
+int b200aa_mid_pool_ragged_f64(const double *d_st, int64_t n_clips, int n_feats, int64_t t_stride,
+                               const int64_t *d_frames, int ratio, int step_ratio, double *d_mid, void *stream);
+/* Long-term mean of float64 mid-term rows, bit for bit `mid.T.mean(axis=0)` (MidTermFeatures.py:200-201); windows as in
+ * b200aa_long_term_mean / b200aa_long_term_mean_ragged. */
+int b200aa_long_term_mean_f64(const double *d_mid, int64_t n_clips, int n_rows, int64_t n_windows, double *d_out,
+                              void *stream);
+int b200aa_long_term_mean_ragged_f64(const double *d_mid, int64_t n_clips, int n_rows, int64_t m_stride,
+                                     const int64_t *d_windows, double *d_out, void *stream);
+
 /* PCM WAV decode (SURVEY 8f rank 2): data-chunk formats of a byte arena, as scipy.io.wavfile.read returns them */
 #define B200AA_PCM_U8 0           /* PCM 8-bit, unsigned                                        */
 #define B200AA_PCM_S16 1          /* PCM 16-bit                                                 */
@@ -244,6 +287,10 @@ int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const b200aa_pcm
  * Replaces: MidTermFeatures.beat_extraction (:18-84) and utilities.peakdet (:33-103). */
 int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
                            const int64_t *d_frames, double window_size, double *d_out, void *stream);
+/* Kernel 4 on float64 rows (the float64 path's short-term features): the same arguments and result, bit for bit the host
+ * beat_extraction(st[b, :, :T_b], window_size). */
+int b200aa_beat_extraction_f64(const double *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
+                               const int64_t *d_frames, double window_size, double *d_out, void *stream);
 
 /* Kernel 5: the library's kNN classifier on a matrix of query vectors (SURVEY 8f rank 4).  Training set on the device:
  * d_feats float64 [n_train, n_feats]; d_slots int32 [n_train], the class a training row votes for (its label when that is

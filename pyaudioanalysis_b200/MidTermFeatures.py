@@ -10,10 +10,10 @@ import os
 
 import numpy as np
 
-from . import _lib
+from . import _lib, precision
 from ._lib import lib, check, get_plan
 from . import ShortTermFeatures
-from .ShortTermFeatures import _as_clip, _fs_int, _ptr
+from .ShortTermFeatures import _as_clip, _as_clip64, _device64, _fs_int, _ptr
 from .batch import mid_ratios
 
 
@@ -35,12 +35,18 @@ def mid_feature_extraction(signal, sampling_rate, mid_window, mid_step, short_wi
     ratio, stepr = mid_ratios(mid_window, mid_step, short_window, short_step)
     if stepr < 1:
         raise ValueError("mid-term step shorter than half a short-term step")
+    st_names = ShortTermFeatures.feature_names(True)
+    names = [n + "_mean" for n in st_names] + [n + "_std" for n in st_names]
+    if precision.wide():
+        import torch
+        from .batch import mid_feature_extraction_batch
+        mid, st = mid_feature_extraction_batch(_device64(signal), plan.fs, mid_window, mid_step, short_window, short_step,
+                                               dtype=torch.float64)
+        return mid[0].cpu().numpy(), st[0].cpu().numpy(), names
     M = lib().b200aa_mid_windows(T, stepr)
     mid = np.empty((136, M), dtype=np.float32)
     st = np.empty((68, T), dtype=np.float32)
     check(lib().b200aa_mid_features_host(plan.handle, _ptr(x), code, x.shape[0], ratio, stepr, _ptr(mid), _ptr(st)))
-    st_names = ShortTermFeatures.feature_names(True)
-    names = [n + "_mean" for n in st_names] + [n + "_std" for n in st_names]
     return mid.astype(np.float64), st.astype(np.float64), names
 
 
@@ -116,19 +122,34 @@ class _Clip:
         self.path, self.fs, self.n, self.data, self.code, self.layout = path, int(fs), int(n), data, code, layout
 
 
+def _staged_exactly(fmt, ch):
+    """Whether the device decode's int16 / float32 staging of a WAV data chunk is the host decode's signal exactly
+    (DESIGN §7's table): not for stereo 24 / 32-bit PCM, mono 32-bit PCM and float64, which the float64 path reads on
+    the host as float64."""
+    from . import audioio
+    if fmt == audioio.PCM_F64:
+        return False
+    if fmt == audioio.PCM_S32:
+        return False
+    return not (fmt == audioio.PCM_S24 and ch == 2)
+
+
 def _open_clip(path):
     """audioBasicIO.read_audio_file + stereo_to_mono for one file, lazily for every WAV flavour audioio.wav_pcm_layout
-    accepts: mono 8 / 16-bit PCM stages as int16, everything else as float32, the code _as_clip gives."""
+    accepts: mono 8 / 16-bit PCM stages as int16, everything else as float32, the code _as_clip gives.  Under
+    set_precision("float64") a file whose staged form would not be exact is decoded on the host and staged as float64
+    (_as_clip64)."""
     from . import audioio
     from ._lib import DTYPE_I16, DTYPE_F32
+    wide = precision.wide()
     if os.path.splitext(path)[1].lower() == ".wav":
         lay = audioio.wav_pcm_layout(path)
-        if lay is not None:
+        if lay is not None and (not wide or _staged_exactly(lay[4], lay[1])):
             fs, ch, n, off, fmt = lay
             code = DTYPE_I16 if ch == 1 and fmt in (audioio.PCM_U8, audioio.PCM_S16) else DTYPE_F32
             return _Clip(path, fs, n, None, code, layout=(off, fmt, ch))
     fs, x = audioio.read_audio_file(path)
-    clip, code = _as_clip(audioio.stereo_to_mono(x))
+    clip, code = (_as_clip64 if wide else _as_clip)(audioio.stereo_to_mono(x))
     return _Clip(path, fs, clip.shape[0], clip, code)
 
 
@@ -139,7 +160,7 @@ def _plan_chunks(clips, max_bytes=None, max_padding=None):
     chunk is closed when the next clip would bring its padded bytes above ``max_bytes`` or its padding above
     ``max_padding`` times its clips' samples; a clip larger than ``max_bytes`` on its own is a chunk of its own.  The
     bounds default to _MAX_CHUNK_BYTES and _MAX_PADDING."""
-    from ._lib import DTYPE_I16
+    from ._lib import DTYPE_I16, DTYPE_F64
     max_bytes = _MAX_CHUNK_BYTES if max_bytes is None else max_bytes
     max_padding = _MAX_PADDING if max_padding is None else max_padding
     groups = {}
@@ -147,7 +168,7 @@ def _plan_chunks(clips, max_bytes=None, max_padding=None):
         groups.setdefault((c.fs, c.code), []).append(idx)
     chunks = []
     for (_, code), idxs in groups.items():
-        item = 2 if code == DTYPE_I16 else 4
+        item = 2 if code == DTYPE_I16 else (8 if code == DTYPE_F64 else 4)
         cur, n_max, payload = [], 0, 0
         for i in sorted(idxs, key=lambda i: (-clips[i].n, i)):
             n, k = clips[i].n, len(cur) + 1
@@ -169,9 +190,12 @@ def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_sh
     st float64 [68 x T] | None, (bpm, ratio) of beat_extraction(st, short_step) | None).  Clips of one (rate, format)
     share launches as ragged batches (_plan_chunks); every clip's results are bit for bit those of the clip alone.  The
     long-term mean and the beat are computed on the GPU from the resident features."""
+    import torch
     from .batch import mid_feature_extraction_batch, long_term_mean_batch, beat_extraction_batch, frame_counts
     from . import audioio
+    from ._lib import DTYPE_F64
     L = lib()
+    dtype = precision.torch_dtype()
     results = [None] * len(clips)
     for part in _plan_chunks(clips):
         chunk = [clips[i] for i in part]
@@ -180,14 +204,20 @@ def _mid_per_clip(clips, mid_window, mid_step, short_window, short_step, want_sh
         mw, ms = round(mid_window * fs), round(mid_step * fs)
         if L.b200aa_num_frames(chunk[-1].n, w, s) <= 0:
             check(_lib.ERR_TOO_SHORT)       # alone, the shortest clip has no frames: a ragged batch would give it none
-        dev, lengths = audioio.stage(chunk)            # one arena, one H2D copy, one decode launch
-        mid, st = mid_feature_extraction_batch(dev, fs, mw, ms, w, s, lengths=lengths)
+        if chunk[0].code == DTYPE_F64:                 # decoded on the host in float64: one H2D copy of the padded batch
+            host = np.zeros((len(chunk), chunk[0].n), dtype=np.float64)
+            for k, c in enumerate(chunk):
+                host[k, :c.n] = c.data
+            dev, lengths = torch.from_numpy(host).cuda(), torch.tensor([c.n for c in chunk], dtype=torch.int64).cuda()
+        else:
+            dev, lengths = audioio.stage(chunk)        # one arena, one H2D copy, one decode launch
+        mid, st = mid_feature_extraction_batch(dev, fs, mw, ms, w, s, lengths=lengths, dtype=dtype)
         stepr = mid_ratios(mw, ms, w, s)[1]
         if want_long_term or want_beat:
             n_frames, n_windows = frame_counts(lengths, w, s, stepr)
         first = (long_term_mean_batch(mid, n_windows=n_windows) if want_long_term else mid).cpu().numpy().astype(np.float64)
         st_h = st.cpu().numpy().astype(np.float64) if want_short else None
-        beat = beat_extraction_batch(st, short_step, n_frames=n_frames).cpu().numpy() if want_beat else None
+        beat = beat_extraction_batch(st, short_step, n_frames=n_frames, dtype=dtype).cpu().numpy() if want_beat else None
         for k, (i, c) in enumerate(zip(part, chunk)):
             T = L.b200aa_num_frames(c.n, w, s)
             results[i] = (first[k] if want_long_term else first[k][:, :L.b200aa_mid_windows(T, stepr)],

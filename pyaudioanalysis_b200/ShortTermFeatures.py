@@ -2,14 +2,15 @@
 
 Signatures, return types, feature names, frame-count rules and error behaviour follow the
 reference (ShortTermFeatures.py:324, :389, :543); the arithmetic runs in libb200aa.so on the GPU
-through the C ABI's host-buffer entry points (NumPy in, NumPy float64 out).
+through the C ABI's host-buffer entry points (NumPy in, NumPy float64 out), or, under
+``set_precision("float64")``, through the float64 path (kernel 12).
 """
 import ctypes
 
 import numpy as np
 
-from . import _lib
-from ._lib import lib, check, get_plan, DTYPE_I16, DTYPE_F32
+from . import _lib, precision
+from ._lib import lib, check, get_plan, DTYPE_I16, DTYPE_F32, DTYPE_F64
 
 PRINT_SPECTROGRAM_SHAPE = True   # the reference prints specgram.shape (ShortTermFeatures.py:451)
 
@@ -49,6 +50,21 @@ def _as_clip(signal):
     return np.ascontiguousarray(x.astype(np.float32)), DTYPE_F32
 
 
+def _as_clip64(signal):
+    """1-D host array for the float64 path: int16 (and 8-bit PCM) as _as_clip stages it, every other format as float64,
+    which holds every int32 and float32 value exactly and a float64 signal unrounded."""
+    x, code = _as_clip(signal)
+    if code == DTYPE_I16:
+        return x, code
+    return np.ascontiguousarray(np.asarray(signal, dtype=np.float64).reshape(x.shape)), DTYPE_F64
+
+
+def _device64(signal):
+    """The clip on the current CUDA device, for the float64 path."""
+    import torch
+    return torch.from_numpy(_as_clip64(signal)[0]).cuda()
+
+
 def _fs_int(sampling_rate):
     fs = int(sampling_rate)
     if fs != sampling_rate:
@@ -80,6 +96,11 @@ def feature_extraction(signal, sampling_rate, window, step, deltas=True):
     T = lib().b200aa_num_frames(x.shape[0], window, step)
     if T <= 0:
         _raise_no_frames(plan.fs, window)
+    if precision.wide():
+        import torch
+        from .batch import feature_extraction_batch
+        out = feature_extraction_batch(_device64(signal), plan.fs, window, step, deltas=deltas, plan=plan, dtype=torch.float64)
+        return out[0].cpu().numpy(), feature_names(deltas)
     F = 68 if deltas else 34
     out = np.empty((F, T), dtype=np.float32)
     check(lib().b200aa_st_features_host(plan.handle, _ptr(x), code, 1, x.shape[0], 1 if deltas else 0, _ptr(out)))
@@ -96,9 +117,14 @@ def spectrogram(signal, sampling_rate, window, step, plot=False, show_progress=F
     R = lib().b200aa_spectrogram_rows(x.shape[0], window, step)
     if R <= 0:
         check(_lib.ERR_TOO_SHORT)
-    out = np.empty((R, K), dtype=np.float32)
-    check(lib().b200aa_spectrogram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
-    specgram = out.astype(np.float64)
+    if precision.wide():
+        import torch
+        from .batch import spectrogram_batch
+        specgram = spectrogram_batch(_device64(signal), plan.fs, window, step, plan=plan, dtype=torch.float64)[0].cpu().numpy()
+    else:
+        out = np.empty((R, K), dtype=np.float32)
+        check(lib().b200aa_spectrogram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
+        specgram = out.astype(np.float64)
     freq_axis = [float((f + 1) * fs) / (2 * K) for f in range(K)]
     time_axis = [float(t * step) / fs for t in range(R)]
     if plot:
@@ -117,9 +143,14 @@ def chromagram(signal, sampling_rate, window, step, plot=False, show_progress=Fa
     R = lib().b200aa_chromagram_rows(x.shape[0], window, step)
     if R <= 0 or x.shape[0] - step - window < 0:
         check(_lib.ERR_TOO_SHORT)
-    out = np.empty((R, 12), dtype=np.float32)
-    check(lib().b200aa_chromagram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
-    chromogram = out.astype(np.float64)
+    if precision.wide():
+        import torch
+        from .batch import chromagram_batch
+        chromogram = chromagram_batch(_device64(signal), plan.fs, window, step, plan=plan, dtype=torch.float64)[0].cpu().numpy()
+    else:
+        out = np.empty((R, 12), dtype=np.float32)
+        check(lib().b200aa_chromagram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
+        chromogram = out.astype(np.float64)
     time_axis = [(t * step) / fs for t in range(R)]
     if plot:
         _plot(chromogram.transpose()[::-1, :])

@@ -14,8 +14,9 @@ from .batch import (feature_extraction_batch, mid_feature_extraction_batch, clip
                     long_term_mean_batch, row_counts)
 from .audioio import load_batch  # noqa: F401
 from .install import install, install_segmentation, install_training, uninstall  # noqa: F401
+from .precision import set_precision, get_precision  # noqa: F401
 
 __all__ = ["ShortTermFeatures", "MidTermFeatures", "consumers", "feature_extraction_batch", "mid_feature_extraction_batch",
            "spectrogram_batch", "chromagram_batch", "beat_extraction_batch", "frame_counts", "mid_pool_batch",
            "long_term_mean_batch", "row_counts", "clip_stats", "load_batch", "install", "install_segmentation",
-           "install_training", "uninstall"]
+           "install_training", "uninstall", "set_precision", "get_precision"]

@@ -57,6 +57,7 @@ SIGNATURES = {
     # (d_arena, arena_bytes, h_clips, n_clips, out_dtype, d_out, n_out, out_stride, stream)
     "b200aa_decode_pcm": (c_int, [c_vp, c_i64, c_vp, c_i64, c_int, c_vp, c_i64, c_i64, c_vp]),
     "b200aa_beat_extraction": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
+    "b200aa_beat_extraction_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_vp, ctypes.c_double, c_vp, c_vp]),
     # (d_feats, d_slots, n_train, n_feats, n_classes, k, d_query, dtype, n_query, q_stride, d_ids, d_P, stream)
     "b200aa_knn_classify": (c_int, [c_vp, c_vp, c_i64, c_int, c_int, c_i64, c_vp, c_int, c_i64, c_i64, c_vp, c_vp, c_vp]),
     # (d_X, d_y, n, n_feats, n_classes, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx, h_k, h_classes, d_pred,
@@ -90,6 +91,17 @@ SIGNATURES = {
     # (model, d_query, dtype, n_query, n_feats, q_stride, d_ids, d_scores, d_bad, stream)
     "b200aa_trees_classify": (c_int, [c_vp, c_vp, c_int, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "b200aa_trees_destroy": (c_int, [c_vp]),
+    # float64 path: (d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, stream)
+    "b200aa_clip_stats_f64": (c_int, [c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    "b200aa_st_features_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]),
+    "b200aa_spectrogram_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    "b200aa_spectrogram_ragged_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "b200aa_chromagram_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
+    "b200aa_chromagram_ragged_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
+    "b200aa_mid_pool_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_i64, c_int, c_int, c_vp, c_vp]),
+    "b200aa_mid_pool_ragged_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_int, c_int, c_vp, c_vp]),
+    "b200aa_long_term_mean_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp]),
+    "b200aa_long_term_mean_ragged_f64": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_st_features_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_int, c_vp]),
     "b200aa_spectrogram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),
     "b200aa_chromagram_host": (c_int, [c_vp, c_vp, c_int, c_i64, c_vp]),

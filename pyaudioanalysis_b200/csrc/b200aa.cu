@@ -164,6 +164,9 @@ struct b200aa_plan {
     static constexpr int kPipe = 3;     // streams of the chunked host pipeline, each with its own clips / records / features buffers
     cudaStream_t pipe_stream[kPipe] = {nullptr, nullptr, nullptr};
     GrowBuffer pipe_ws[kPipe][3];
+    // tables of the float64 path, built by its first call (f64.cu)
+    std::mutex f64_mu;
+    std::shared_ptr<const F64Tables> f64;
     ~b200aa_plan()
     {
         for (cudaStream_t s : pipe_stream) if (s) cudaStreamDestroy(s);
@@ -283,6 +286,25 @@ static int plan_device_check(const b200aa_plan *pl)
     int dev = -1;
     CK(cudaGetDevice(&dev));
     return dev == pl->device ? B200AA_OK : B200AA_ERR_INVALID;
+}
+
+int plan_f64(const b200aa_plan *plan, PlanF64 &out)
+{
+    out = PlanF64{plan->fs, plan->window, plan->step, plan->K, plan->sm_count, plan->tables_status, nullptr};
+    return B200AA_OK;
+}
+
+int plan_f64_device(const b200aa_plan *plan) { return plan_device_check(plan); }
+
+int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out)
+{
+    int rc = plan_device_check(plan);
+    if (rc != B200AA_OK) return rc;
+    b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
+    std::lock_guard<std::mutex> g(pl->f64_mu);
+    if (!pl->f64 && (rc = f64_tables_build(pl->fs, pl->window, pl->tables_status, pl->f64)) != B200AA_OK) return rc;
+    out.tables = pl->f64.get();
+    return B200AA_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -13,16 +13,18 @@ using namespace b200aa;
 // ------------------------------------------------------------------------------------------------
 // One CTA of P = blockDim.x threads (a power of two, 32 .. 256) per (clip, beat row): threshold, chunked peak scan, and the
 // distances between successive peaks counted into the row's integer histogram counts[row][d - 1], d = 1 .. min(mbt, T - 1).
-__global__ void __launch_bounds__(256) beat_rows_kernel(const float *st, int F, int64_t n_frames, int64_t t_stride,
-                                                        const int64_t *frames, int64_t b0, int64_t mbt, int nb, int chunk,
-                                                        int nch_max, beat::Chunk *recs, unsigned *counts)
+// The rows are float32 (b200aa_beat_extraction) or float64 (b200aa_beat_extraction_f64); both are read as double.
+template <class Real>
+__device__ __forceinline__ void beat_rows(const Real *st, int F, int64_t n_frames, int64_t t_stride, const int64_t *frames,
+                                          int64_t b0, int64_t mbt, int nb, int chunk, int nch_max, beat::Chunk *recs,
+                                          unsigned *counts)
 {
     __shared__ double part[256];
     const int64_t bl = blockIdx.x / beat::kRows;
     const int r = int(blockIdx.x - bl * beat::kRows);
     const int64_t b = b0 + bl;
     const int64_t T = frames ? min(max(frames[b], int64_t(0)), n_frames) : n_frames;
-    const float *row = st + (size_t(b) * F + beat::row_index(r)) * t_stride;
+    const Real *row = st + (size_t(b) * F + beat::row_index(r)) * t_stride;
     const int P = blockDim.x, k = threadIdx.x;
     auto v = [row](int64_t i) { return double(row[i]); };
     auto absdiff = [row](int64_t i) { return fabs(beat::dsub(double(row[i]), double(row[i + 1]))); };
@@ -65,6 +67,18 @@ __global__ void __launch_bounds__(256) beat_rows_kernel(const float *st, int F, 
                              last = p;
                          });
     }
+}
+__global__ void __launch_bounds__(256) beat_rows_kernel(const float *st, int F, int64_t n_frames, int64_t t_stride,
+                                                        const int64_t *frames, int64_t b0, int64_t mbt, int nb, int chunk,
+                                                        int nch_max, beat::Chunk *recs, unsigned *counts)
+{
+    beat_rows(st, F, n_frames, t_stride, frames, b0, mbt, nb, chunk, nch_max, recs, counts);
+}
+__global__ void __launch_bounds__(256) beat_rows_f64_kernel(const double *st, int F, int64_t n_frames, int64_t t_stride,
+                                                            const int64_t *frames, int64_t b0, int64_t mbt, int nb, int chunk,
+                                                            int nch_max, beat::Chunk *recs, unsigned *counts)
+{
+    beat_rows(st, F, n_frames, t_stride, frames, b0, mbt, nb, chunk, nch_max, recs, counts);
 }
 
 // One warp per clip: hist[k] = sum over the rows, in _BEAT_ROWS order, of counts[row][k] / T; its first maximum k, and its
@@ -117,10 +131,11 @@ __global__ void __launch_bounds__(256) beat_finish_kernel(const int64_t *frames,
     }
 }
 
-extern "C" int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
-                                      const int64_t *d_frames, double window_size, double *d_out, void *stream)
+// b200aa_beat_extraction and b200aa_beat_extraction_f64: `rows` is the row kernel of the rows' element type
+template <class Real, class RowsKernel>
+static int beat_launch(RowsKernel rows, const Real *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
+                       const int64_t *d_frames, double window_size, double *d_out, void *stream)
 {
-    NvtxRange nvtx_("b200aa_beat_extraction");
     if (!d_st || !d_out || n_clips < 0 || n_feats < 19 || n_frames < 0 || n_frames > INT32_MAX - beat::kChunk ||
         t_stride < n_frames)
         return B200AA_ERR_INVALID;
@@ -149,12 +164,27 @@ extern "C" int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_
         const int64_t ns = std::min<int64_t>(slice, n_clips - b0);
         const cudaError_t e = nb ? cudaMemsetAsync(counts, 0, size_t(ns) * beat::kRows * nb * sizeof(unsigned), st) : cudaSuccess;
         if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync");
-        beat_rows_kernel<<<(unsigned)(ns * beat::kRows), P, 0, st>>>(d_st, n_feats, n_frames, t_stride, d_frames, b0, mbt, nb, chunk,
-                                                                     nch_max, recs, counts);
+        rows<<<(unsigned)(ns * beat::kRows), P, 0, st>>>(d_st, n_feats, n_frames, t_stride, d_frames, b0, mbt, nb, chunk,
+                                                         nch_max, recs, counts);
         CK_LAUNCH("beat_rows_kernel");
         beat_finish_kernel<<<(unsigned)((ns * 32 + 255) / 256), 256, 0, st>>>(d_frames, n_frames, b0, ns, window_size, mbt, nb,
                                                                                counts, d_out);
         CK_LAUNCH("beat_finish_kernel");
     }
     return scratch.done(B200AA_OK);
+}
+
+extern "C" int b200aa_beat_extraction(const float *d_st, int64_t n_clips, int n_feats, int64_t n_frames, int64_t t_stride,
+                                      const int64_t *d_frames, double window_size, double *d_out, void *stream)
+{
+    NvtxRange nvtx_("b200aa_beat_extraction");
+    return beat_launch(beat_rows_kernel, d_st, n_clips, n_feats, n_frames, t_stride, d_frames, window_size, d_out, stream);
+}
+
+extern "C" int b200aa_beat_extraction_f64(const double *d_st, int64_t n_clips, int n_feats, int64_t n_frames,
+                                          int64_t t_stride, const int64_t *d_frames, double window_size, double *d_out,
+                                          void *stream)
+{
+    NvtxRange nvtx_("b200aa_beat_extraction_f64");
+    return beat_launch(beat_rows_f64_kernel, d_st, n_clips, n_feats, n_frames, t_stride, d_frames, window_size, d_out, stream);
 }

@@ -9,6 +9,7 @@
 #include <atomic>
 #include <cstddef>
 #include <cstdint>
+#include <memory>
 #include <string>
 
 #include "../../include/b200aa.h"
@@ -94,3 +95,20 @@ auto with_real_type(int dtype, F f)
 {
     return dtype == B200AA_DTYPE_F32 ? f(float{}) : f(double{});
 }
+
+// ------------------------------------------------------------------------------------------------
+// a plan as the float64 path (f64.cu) sees it
+// ------------------------------------------------------------------------------------------------
+struct F64Tables;                               // the plan's float64 device tables (f64.cu)
+struct PlanF64 {
+    int fs, window, step, K, sm_count, tables_status;
+    const F64Tables *tables;                    // set by plan_f64_tables
+};
+// the plan's shape (b200aa.cu)
+int plan_f64(const b200aa_plan *plan, PlanF64 &out);
+// B200AA_OK when the current device is the plan's (b200aa.cu)
+int plan_f64_device(const b200aa_plan *plan);
+// the same after the device check, with the float64 tables, built on the plan's first float64 call (b200aa.cu)
+int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out);
+// builds them (f64.cu); tables_status: the plan's, the feature tables are only built when it is B200AA_OK
+int f64_tables_build(int fs, int window, int tables_status, std::shared_ptr<const F64Tables> &out);

@@ -7,9 +7,13 @@ Every caller in the reference looks the four functions up on the module object a
 _saved = {}
 
 
-def install(pyaudioanalysis_pkg=None):
-    """Patch an importable ``pyAudioAnalysis``; returns the list of attributes rebound."""
+def install(pyaudioanalysis_pkg=None, precision=None):
+    """Patch an importable ``pyAudioAnalysis``; returns the list of attributes rebound.  ``precision`` ("float32" /
+    "float64", None: leave it as it is) sets the drop-ins' result contract (``precision.set_precision``)."""
     from . import ShortTermFeatures as ours_st, MidTermFeatures as ours_mt
+    if precision is not None:
+        from .precision import set_precision
+        set_precision(precision)
     if pyaudioanalysis_pkg is None:
         import importlib
         ref_st = importlib.import_module("pyAudioAnalysis.ShortTermFeatures")
