@@ -36,7 +36,10 @@ typedef enum b200aa_status {
                                      (ShortTermFeatures.py:230-231)                                       */
     B200AA_ERR_CUDA = -5,         /* a CUDA call failed; see b200aa_last_cuda_error()                     */
     B200AA_ERR_UNSUPPORTED = -6,  /* window too large for the on-chip transform buffers                  */
-    B200AA_ERR_NO_DEVICE = -7     /* no CUDA device / not an sm_90 device                                 */
+    B200AA_ERR_NO_DEVICE = -7,    /* no CUDA device / not an sm_90 device                                 */
+    B200AA_ERR_CAPTURE = -8       /* the stream is capturing a CUDA graph and this call cannot be captured: make it once
+                                     outside capture first, or call it eagerly; b200aa_last_cuda_error() names the entry
+                                     point and the reason                                                 */
 } b200aa_status;
 
 /* sample formats of the clip buffer */
@@ -71,8 +74,19 @@ typedef struct b200aa_plan b200aa_plan;   /* opaque: constant tables of one (fs,
 /* ------------------------------------------------------------------ library ---------- */
 int         b200aa_abi_version(void);
 const char *b200aa_status_string(int status);
-const char *b200aa_last_cuda_error(void);        /* thread-local text of the last CUDA failure */
+const char *b200aa_last_cuda_error(void);        /* thread-local text of the last CUDA failure or capture refusal */
 int         b200aa_device_ok(void);              /* B200AA_OK iff the current device is sm_90 */
+
+/* CUDA graph capture.  These device entry points may be called on a stream that is capturing a graph (any capture mode),
+ * and the graph's replays give their eager results bit for bit: b200aa_clip_stats, b200aa_st_features, b200aa_spectrogram,
+ * b200aa_chromagram (and _ragged), b200aa_frame_counts, b200aa_row_counts, b200aa_mid_pool (and _ragged),
+ * b200aa_long_term_mean (and _ragged), b200aa_beat_extraction, and their _f64 forms.  A captured launch of a persistent
+ * kernel takes its work slot from stream-ordered scratch (an allocation and a free node of the graph) instead of the plan's
+ * ring, so no graph shares a slot with another launch or replay.  Every other device entry point, the host-buffer entry
+ * points, b200aa_plan_create and b200aa_trees_create return B200AA_ERR_CAPTURE on a capturing stream before any other CUDA
+ * call, and so does a float64 call whose plan has not built its float64 tables in an eager call yet.  The entry points
+ * without a stream argument can only see the legacy default stream: they refuse when it is capturing, or when a blocking
+ * stream captures and any use of it would break that capture.  A plan a graph uses must outlive the graph. */
 
 /* ------------------------------------------------------------------ host tables -------
  * Pure host code, usable without a GPU (the CPU test-suite checks them against the oracle).

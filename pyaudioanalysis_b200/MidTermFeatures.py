@@ -46,6 +46,7 @@ def mid_feature_extraction(signal, sampling_rate, mid_window, mid_step, short_wi
     M = lib().b200aa_mid_windows(T, stepr)
     mid = np.empty((136, M), dtype=np.float32)
     st = np.empty((68, T), dtype=np.float32)
+    _lib.refuse_capture("b200aa_mid_features_host", _lib.HOST_BUFFER_WHY)
     check(lib().b200aa_mid_features_host(plan.handle, _ptr(x), code, x.shape[0], ratio, stepr, _ptr(mid), _ptr(st)))
     return mid.astype(np.float64), st.astype(np.float64), names
 

@@ -103,6 +103,7 @@ def feature_extraction(signal, sampling_rate, window, step, deltas=True):
         return out[0].cpu().numpy(), feature_names(deltas)
     F = 68 if deltas else 34
     out = np.empty((F, T), dtype=np.float32)
+    _lib.refuse_capture("b200aa_st_features_host", _lib.HOST_BUFFER_WHY)
     check(lib().b200aa_st_features_host(plan.handle, _ptr(x), code, 1, x.shape[0], 1 if deltas else 0, _ptr(out)))
     return out.astype(np.float64), feature_names(deltas)
 
@@ -123,6 +124,7 @@ def spectrogram(signal, sampling_rate, window, step, plot=False, show_progress=F
         specgram = spectrogram_batch(_device64(signal), plan.fs, window, step, plan=plan, dtype=torch.float64)[0].cpu().numpy()
     else:
         out = np.empty((R, K), dtype=np.float32)
+        _lib.refuse_capture("b200aa_spectrogram_host", _lib.HOST_BUFFER_WHY)
         check(lib().b200aa_spectrogram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
         specgram = out.astype(np.float64)
     freq_axis = [float((f + 1) * fs) / (2 * K) for f in range(K)]
@@ -149,6 +151,7 @@ def chromagram(signal, sampling_rate, window, step, plot=False, show_progress=Fa
         chromogram = chromagram_batch(_device64(signal), plan.fs, window, step, plan=plan, dtype=torch.float64)[0].cpu().numpy()
     else:
         out = np.empty((R, 12), dtype=np.float32)
+        _lib.refuse_capture("b200aa_chromagram_host", _lib.HOST_BUFFER_WHY)
         check(lib().b200aa_chromagram_host(plan.handle, _ptr(x), code, x.shape[0], _ptr(out)))
         chromogram = out.astype(np.float64)
     time_axis = [(t * step) / fs for t in range(R)]

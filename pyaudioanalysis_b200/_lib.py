@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("B200AA_LIB") or os.path.join(_HERE, "libb200aa.so")  
 
 OK = 0
 ERR_INVALID, ERR_TOO_SHORT, ERR_CHROMA, ERR_MEL_RANGE, ERR_CUDA, ERR_UNSUPPORTED, ERR_NO_DEVICE = -1, -2, -3, -4, -5, -6, -7
+ERR_CAPTURE = -8
 DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2
 
 _lib = None
@@ -147,9 +148,25 @@ def check(status):
         raise ValueError(text)          # ShortTermFeatures.py:684 / :290-294 raise ValueError
     if status == ERR_MEL_RANGE:
         raise IndexError(text)          # ShortTermFeatures.py:230-231 raises IndexError
-    if status == ERR_CUDA:
+    if status in (ERR_CUDA, ERR_CAPTURE):       # the text names the failed call, or the entry point that refused and why
         raise RuntimeError(text + ": " + L.b200aa_last_cuda_error().decode())
     raise RuntimeError(text)
+
+
+def capturing():
+    """True while the current CUDA stream captures a graph."""
+    import torch
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+HOST_BUFFER_WHY = "host-buffer entry points allocate, copy and synchronise; call them eagerly"
+
+
+def refuse_capture(entry, why):
+    """Raise the capture error of ``check(ERR_CAPTURE)`` for ``entry`` while the current stream captures: for calls the
+    library cannot see the stream of (plan creation, the host-buffer entry points)."""
+    if capturing():
+        raise RuntimeError("%s: %s: %s" % (lib().b200aa_status_string(ERR_CAPTURE).decode(), entry, why))
 
 
 class Plan:
@@ -158,6 +175,7 @@ class Plan:
     def __init__(self, fs, window, step):
         self.fs, self.window, self.step = int(fs), int(window), int(step)
         self.K = self.window // 2
+        refuse_capture("b200aa_plan_create", "allocates and uploads device tables; create the plan outside capture first")
         h = c_vp()
         check(lib().b200aa_plan_create(ctypes.byref(h), self.fs, self.window, self.step))
         self.handle = h
@@ -192,10 +210,22 @@ import collections
 _plans = collections.OrderedDict()
 _plans_lock = threading.Lock()
 MAX_CACHED_PLANS = 32       # least recently used plans beyond this are dropped (their device tables and workspaces are freed)
+_pinned = []                # plans a captured call used: a graph reads their tables at every replay, so they live for good
+
+
+def pin_if_capturing(plan):
+    """Keep ``plan`` alive for the life of the process when the current stream captures a graph that will use it."""
+    if capturing():
+        with _plans_lock:
+            if not any(p is plan for p in _pinned):
+                _pinned.append(plan)
+    return plan
 
 
 def get_plan(fs, window, step, device=None):
-    """Plans are cached per (device, fs, window, step), least recently used first out."""
+    """Plans are cached per (device, fs, window, step), least recently used first out.  While the current stream
+    captures a graph, only a cached plan is returned, and it is pinned (never freed); an uncached one raises the capture
+    error, since creating it cannot be captured."""
     if device is None:
         try:
             import torch
@@ -212,7 +242,7 @@ def get_plan(fs, window, step, device=None):
                 _plans.popitem(last=False)          # Plan.__del__ destroys it once no caller holds it any more
         else:
             _plans.move_to_end(key)
-        return pl
+    return pin_if_capturing(pl)
 
 
 def host_table(fs, window, which):

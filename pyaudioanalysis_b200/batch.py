@@ -8,7 +8,7 @@ import ctypes
 import torch
 
 from . import _lib
-from ._lib import lib, check, get_plan, DTYPE_I16, DTYPE_F32, DTYPE_F64
+from ._lib import lib, check, get_plan, pin_if_capturing, DTYPE_I16, DTYPE_F32, DTYPE_F64
 
 NORM_BYTES = 32
 NORM_F64_BYTES = 16
@@ -125,7 +125,7 @@ def feature_extraction_batch(signals, sampling_rate, window, step, deltas=True, 
     signals, B, N, stride, lengths, len_ptr = _prep(signals, lengths)
     F = 68 if deltas else 34
     with torch.cuda.device(signals.device):
-        plan = plan or get_plan(sampling_rate, window, step, signals.device.index)
+        plan = pin_if_capturing(plan) if plan else get_plan(sampling_rate, window, step, signals.device.index)
         T = lib().b200aa_num_frames(N, window, step)
         if T <= 0:
             check(_lib.ERR_TOO_SHORT)
@@ -340,7 +340,7 @@ def spectrogram_batch(signals, sampling_rate, window, step, plan=None, norm=None
     sfx = "_f64" if wide else ""
     signals, B, N, stride, lengths, len_ptr = _prep(signals, lengths)
     with torch.cuda.device(signals.device):
-        plan = plan or get_plan(sampling_rate, window, step, signals.device.index)
+        plan = pin_if_capturing(plan) if plan else get_plan(sampling_rate, window, step, signals.device.index)
         R = lib().b200aa_spectrogram_rows(N, window, step)
         if R <= 0:
             check(_lib.ERR_TOO_SHORT)
@@ -371,7 +371,7 @@ def chromagram_batch(signals, sampling_rate, window, step, plan=None, norm=None,
     sfx = "_f64" if wide else ""
     signals, B, N, stride, lengths, len_ptr = _prep(signals, lengths)
     with torch.cuda.device(signals.device):
-        plan = plan or get_plan(sampling_rate, window, step, signals.device.index)
+        plan = pin_if_capturing(plan) if plan else get_plan(sampling_rate, window, step, signals.device.index)
         R = lib().b200aa_chromagram_rows(N, window, step)
         if R <= 0 or (lengths is None and N - step - window < 0):
             check(_lib.ERR_TOO_SHORT)

@@ -20,6 +20,7 @@ import ctypes
 import numpy as np
 import torch
 
+from . import _lib
 from ._lib import DTYPE_F32, DTYPE_F64, ERR_UNSUPPORTED, check, lib
 from .batch import _require_cuda, _stream, beat_extraction_batch, long_term_mean_batch, mid_feature_extraction_batch
 
@@ -661,6 +662,7 @@ class TreeEnsembleModel:
         self.mode, self.n_classes, self.n_feats = flat["mode"], flat["n_classes"], flat["n_feats"]
         self.device = _cuda_device(device, "a TreeEnsembleModel")
         nodes, roots, values, init = flat["nodes"], flat["roots"], flat["values"], flat["init"]
+        _lib.refuse_capture("b200aa_trees_create", "allocates and uploads the model; create it outside capture")
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
             status = lib().b200aa_trees_create(

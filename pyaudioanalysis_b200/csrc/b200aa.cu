@@ -41,6 +41,7 @@ extern "C" const char *b200aa_status_string(int s)
     case B200AA_ERR_CUDA: return "CUDA error";
     case B200AA_ERR_UNSUPPORTED: return "window too large for the on-chip transform";
     case B200AA_ERR_NO_DEVICE: return "no sm_90 CUDA device";
+    case B200AA_ERR_CAPTURE: return "this call cannot be captured; make it once outside capture first, or call it eagerly";
     default: return "unknown status";
     }
 }
@@ -176,6 +177,7 @@ struct b200aa_plan {
 extern "C" int b200aa_plan_create(b200aa_plan **out, int fs, int window, int step)
 {
     if (!out || fs <= 0 || window < 2 || step < 1) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(nullptr, "b200aa_plan_create", kWhyAllocates);
     int rc = b200aa_device_ok();
     if (rc != B200AA_OK) return rc;
     std::unique_ptr<b200aa_plan> pl(new b200aa_plan);
@@ -220,14 +222,26 @@ extern "C" void b200aa_plan_destroy(b200aa_plan *plan) { delete plan; }
 // One launch of a persistent kernel: the constructor takes a work-counter slot of the plan's ring (status in rc, counter
 // in ctr), finish() gets the launcher's status, counts the launch, maps the status and frees the slot.
 // B200AA_ERR_UNSUPPORTED = the launcher declined the shape and launched nothing; the caller tries the next kernel.
+// On a capturing stream the slot is the launch's own stream-ordered scratch instead (an allocation and a free node of the
+// graph): the ring's events cannot be waited on or recorded across a capture, and a graph keeps its slot for every replay,
+// so a ring slot would be handed to eager launches that run at the same time as a replay.  The launcher zeroes either
+// slot on the stream before its kernel.
 struct SlotLaunch {
     b200aa_plan *pl;
     cudaStream_t st;
     unsigned slot = 0;
     unsigned int *ctr = nullptr;
     int rc;
-    SlotLaunch(b200aa_plan *plan, cudaStream_t stream) : pl(plan), st(stream)
+    bool captured = false;
+    StreamScratch own;
+    SlotLaunch(b200aa_plan *plan, cudaStream_t stream) : pl(plan), st(stream), own(stream)
     {
+        if (stream_capturing(st)) {
+            captured = true;
+            rc = own.alloc(b200aa_plan::kSlotBytes);
+            ctr = static_cast<unsigned int *>(own.get());
+            return;
+        }
         rc = pl->slots.acquire(st, slot);
         if (rc == B200AA_OK)
             ctr = reinterpret_cast<unsigned int *>(static_cast<unsigned char *>(pl->counters.get()) + size_t(slot) * b200aa_plan::kSlotBytes);
@@ -236,6 +250,7 @@ struct SlotLaunch {
     {
         const int r = launch_rc == B200AA_OK ? launched(name)
                                              : (launch_rc == B200AA_ERR_CUDA ? cuda_fail(cudaGetLastError(), name) : launch_rc);
+        if (captured) return own.done(r);
         const int done = pl->slots.done(st, slot);    // after launched(): a failed record keeps its own message
         return r != B200AA_OK ? r : done;
     }
@@ -296,13 +311,18 @@ int plan_f64(const b200aa_plan *plan, PlanF64 &out)
 
 int plan_f64_device(const b200aa_plan *plan) { return plan_device_check(plan); }
 
-int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out)
+int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out, cudaStream_t st, const char *entry)
 {
     int rc = plan_device_check(plan);
     if (rc != B200AA_OK) return rc;
     b200aa_plan *pl = const_cast<b200aa_plan *>(plan);
     std::lock_guard<std::mutex> g(pl->f64_mu);
-    if (!pl->f64 && (rc = f64_tables_build(pl->fs, pl->window, pl->tables_status, pl->f64)) != B200AA_OK) return rc;
+    if (!pl->f64) {         // the build allocates and copies synchronously
+        if ((rc = refuse_capture(st, entry, "the plan's float64 tables are built by its first float64 call; make one "
+                                            "outside capture first")) != B200AA_OK)
+            return rc;
+        if ((rc = f64_tables_build(pl->fs, pl->window, pl->tables_status, pl->f64)) != B200AA_OK) return rc;
+    }
     out.tables = pl->f64.get();
     return B200AA_OK;
 }
@@ -832,6 +852,7 @@ extern "C" int b200aa_st_features_host(const b200aa_plan *plan, const void *h_si
 {
     NvtxRange nvtx_("b200aa_st_features_host");
     if (!plan || !h_sig || !h_out || n_clips < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(nullptr, "b200aa_st_features_host", kWhyHostBuffer);
     if (plan->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
     const int64_t T = rows::frames(n_samples, plan->window, plan->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;
@@ -856,6 +877,7 @@ extern "C" int b200aa_st_features_host(const b200aa_plan *plan, const void *h_si
 extern "C" int b200aa_spectrogram_host(const b200aa_plan *plan, const void *h_sig, int dtype, int64_t n_samples, float *h_out)
 {
     if (!plan || !h_sig || !h_out || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(nullptr, "b200aa_spectrogram_host", kWhyHostBuffer);
     const int64_t R = b200aa_spectrogram_rows(n_samples, plan->window, plan->step);
     if (R <= 0) return B200AA_ERR_TOO_SHORT;
     const size_t out_b = size_t(R) * plan->K * 4;
@@ -873,6 +895,7 @@ extern "C" int b200aa_spectrogram_host(const b200aa_plan *plan, const void *h_si
 extern "C" int b200aa_chromagram_host(const b200aa_plan *plan, const void *h_sig, int dtype, int64_t n_samples, float *h_out)
 {
     if (!plan || !h_sig || !h_out || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(nullptr, "b200aa_chromagram_host", kWhyHostBuffer);
     const int64_t R = b200aa_chromagram_rows(n_samples, plan->window, plan->step);
     if (R <= 0 || n_samples - plan->step - plan->window < 0) return B200AA_ERR_TOO_SHORT;
     if (plan->tables_status == B200AA_ERR_CHROMA) return B200AA_ERR_CHROMA;
@@ -893,6 +916,7 @@ extern "C" int b200aa_mid_features_host(const b200aa_plan *plan, const void *h_s
 {
     NvtxRange nvtx_("b200aa_mid_features_host");
     if (!plan || !h_sig || !h_mid || step_ratio < 1 || (dtype != 0 && dtype != 1)) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(nullptr, "b200aa_mid_features_host", kWhyHostBuffer);
     if (plan->tables_status == B200AA_ERR_MEL_RANGE) return B200AA_ERR_MEL_RANGE;
     const int64_t T = rows::frames(n_samples, plan->window, plan->step);
     if (T == 0) return B200AA_ERR_TOO_SHORT;
@@ -958,6 +982,7 @@ extern "C" int b200aa_peer_buffer_open(const unsigned char *handle, void **d_out
 extern "C" int b200aa_peer_copy(void *d_dst, const void *d_src, size_t bytes, void *stream)
 {
     if (!d_dst || !d_src) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(stream, "b200aa_peer_copy", "peer copies are not captured; call it eagerly");
     if (bytes == 0) return B200AA_OK;
     // unified addressing: the copy engines move the block over NVLink, no SM on either side is involved
     CK(cudaMemcpyAsync(d_dst, d_src, bytes, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));

@@ -160,6 +160,7 @@ extern "C" int b200aa_cluster_distance_means(const double *d_X, int64_t n, int n
                                              double *d_A, double *d_B, void *stream)
 {
     NvtxRange nvtx_("b200aa_cluster_distance_means");
+    REFUSE_CAPTURE(stream, "b200aa_cluster_distance_means", kWhyHostArrays);
     const int K = n_clusters, D = n_feats;
     if (!d_X || !h_labels || !d_A || !d_B || n < 1 || D < 1 || D > cluster::kMaxFeats || x_stride < D || K < 1 ||
         K > B200AA_CLUSTER_MAX)

@@ -1,5 +1,5 @@
-// Host-side plumbing of every C ABI entry point of libb200aa.so: CUDA error reporting and the launch count, stream-ordered
-// scratch, NVTX ranges, scratch alignment and slicing, and the float32 / float64 dispatch of a launch.
+// Host-side plumbing of every C ABI entry point of libb200aa.so: CUDA error reporting and the launch count, the capture
+// guard, stream-ordered scratch, NVTX ranges, scratch alignment and slicing, and the float32 / float64 dispatch of a launch.
 // g_cuda_err and g_launches are defined once, in b200aa.cu, so that b200aa_last_cuda_error() and b200aa_launch_count()
 // see every file's entry points.
 #pragma once
@@ -42,6 +42,39 @@ inline int launched(const char *name)
         const int rc_ = launched(name);                              \
         if (rc_ != B200AA_OK) return rc_;                            \
     } while (0)
+
+// ------------------------------------------------------------------------------------------------
+// CUDA graph capture (include/b200aa.h)
+// ------------------------------------------------------------------------------------------------
+// True when `st` is capturing a graph, or is the legacy default stream while a blocking stream captures (any use of it
+// would invalidate that capture).  The query is legal in every capture mode.  A query that fails otherwise (no device, a
+// bad stream) answers false and clears its error, so the call goes on to meet that error where it met it before.
+inline bool stream_capturing(cudaStream_t st)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+    if (e != cudaSuccess) cudaGetLastError();
+    return e == cudaErrorStreamCaptureImplicit || (e == cudaSuccess && cs != cudaStreamCaptureStatusNone);
+}
+
+// The guard of an entry point that cannot be captured: B200AA_ERR_CAPTURE, with "entry: why" as the thread's error text,
+// when `st` is capturing, before any other CUDA call
+inline int refuse_capture(cudaStream_t st, const char *entry, const char *why)
+{
+    if (!stream_capturing(st)) return B200AA_OK;
+    g_cuda_err = std::string(entry) + ": " + why;
+    return B200AA_ERR_CAPTURE;
+}
+#define REFUSE_CAPTURE(stream, entry, why)                                                   \
+    do {                                                                                     \
+        const int rc_ = refuse_capture(static_cast<cudaStream_t>(stream), entry, why);      \
+        if (rc_ != B200AA_OK) return rc_;                                                    \
+    } while (0)
+// reasons of the refusals
+constexpr const char *kWhyHostArrays = "copies host arrays to the device, which a graph would read after they are freed; "
+                                       "call it eagerly";
+constexpr const char *kWhyHostBuffer = "host-buffer entry points allocate, copy and synchronise; call them eagerly";
+constexpr const char *kWhyAllocates = "allocates and uploads device tables; make this call outside capture first";
 
 // Stream-ordered device scratch of one entry point, bound to its scope: alloc() takes it with cudaMallocAsync, done(rc)
 // frees it after everything queued on the stream and returns rc, else the free's error.  A scope left early (its error
@@ -108,7 +141,8 @@ struct PlanF64 {
 int plan_f64(const b200aa_plan *plan, PlanF64 &out);
 // B200AA_OK when the current device is the plan's (b200aa.cu)
 int plan_f64_device(const b200aa_plan *plan);
-// the same after the device check, with the float64 tables, built on the plan's first float64 call (b200aa.cu)
-int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out);
+// the same after the device check, with the float64 tables, built on the plan's first float64 call (b200aa.cu); that
+// build cannot be captured: B200AA_ERR_CAPTURE (as `entry`) when st is capturing and the tables are not built yet
+int plan_f64_tables(const b200aa_plan *plan, PlanF64 &out, cudaStream_t st, const char *entry);
 // builds them (f64.cu); tables_status: the plan's, the feature tables are only built when it is B200AA_OK
 int f64_tables_build(int fs, int window, int tables_status, std::shared_ptr<const F64Tables> &out);

@@ -535,12 +535,12 @@ extern "C" int b200aa_st_features_f64(const b200aa_plan *plan, const void *d_sig
     if ((rc = plan_f64_device(plan)) != B200AA_OK) return rc;       // where b200aa_st_features checks it
     if (t_stride < T) return B200AA_ERR_INVALID;
     if (n_clips == 0) return B200AA_OK;
-    if ((rc = plan_f64_tables(plan, pl)) != B200AA_OK) return rc;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if ((rc = plan_f64_tables(plan, pl, st, "b200aa_st_features_f64")) != B200AA_OK) return rc;
     F64Params q;
     fill_f64(q, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     q.t_stride = t_stride;
     q.n_out = deltas ? 2 * B200AA_N_BASE : B200AA_N_BASE;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     if ((rc = launch_frames<kModeFeatures>(pl, q, T, st)) != B200AA_OK || !deltas) return rc;
     const int64_t n = n_clips * B200AA_N_BASE * T;
     f64_deltas_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_out, n_clips, T, t_stride, d_len, n_samples,
@@ -562,7 +562,8 @@ static int spectrogram_f64(const b200aa_plan *plan, const void *d_sig, int dtype
     const rows::Rows r = rows::spectrogram(n_samples, pl.window, pl.step);
     if (r.refused) return B200AA_ERR_TOO_SHORT;
     if (n_clips == 0) return B200AA_OK;
-    if ((rc = plan_f64_tables(plan, pl)) != B200AA_OK) return rc;
+    const char *entry = d_len ? "b200aa_spectrogram_ragged_f64" : "b200aa_spectrogram_f64";
+    if ((rc = plan_f64_tables(plan, pl, static_cast<cudaStream_t>(stream), entry)) != B200AA_OK) return rc;
     F64Params q;
     fill_f64(q, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     q.rows_launch = r.R;
@@ -603,7 +604,8 @@ static int chromagram_f64(const b200aa_plan *plan, const void *d_sig, int dtype,
     if (pl.tables_status == B200AA_ERR_CHROMA) return B200AA_ERR_CHROMA;
     if (n_clips == 0) return B200AA_OK;
     if (!d_len && r.refused) return B200AA_ERR_INVALID;
-    if ((rc = plan_f64_tables(plan, pl)) != B200AA_OK) return rc;
+    const char *entry = d_len ? "b200aa_chromagram_ragged_f64" : "b200aa_chromagram_f64";
+    if ((rc = plan_f64_tables(plan, pl, static_cast<cudaStream_t>(stream), entry)) != B200AA_OK) return rc;
     F64Params q;
     fill_f64(q, pl, d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, d_out);
     q.rows_launch = r.R;

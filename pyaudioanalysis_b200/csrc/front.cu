@@ -64,6 +64,7 @@ extern "C" int b200aa_standard_scale(const void *d_X, int dtype, int64_t n_mats,
                                      double *d_mean, double *d_scale, int32_t *d_bad, void *stream)
 {
     NvtxRange nvtx_("b200aa_standard_scale");
+    REFUSE_CAPTURE(stream, "b200aa_standard_scale", "kernel 11 is not captured; call it eagerly");
     const int D = n_feats;
     if (!d_X || !h_rows || !d_out || !h_out_off || !d_mean || !d_scale || !d_bad || n_mats < 1 || D < 1 ||
         mat_stride < 0 || row_stride < 1 || col_stride < 1 || out_row_stride < 1 || out_col_stride < 1 ||
@@ -129,6 +130,7 @@ extern "C" int b200aa_outlier_columns(const double *d_X, int64_t n_rows, int n_f
                                       double *d_dist_all, double *d_mean, unsigned char *d_keep, void *stream)
 {
     NvtxRange nvtx_("b200aa_outlier_columns");
+    REFUSE_CAPTURE(stream, "b200aa_outlier_columns", "kernel 11 is not captured; call it eagerly");
     const int D = n_feats;
     if (!d_X || !d_dist_all || !d_mean || !d_keep || n_rows < 1 || D < 1 || D > front::kMaxFeats || col_stride < n_rows ||
         col_stride > INT_MAX)
@@ -183,6 +185,7 @@ extern "C" int b200aa_pool_frames(const void *d_st, int dtype, int64_t n_clips, 
                                   int64_t out_stride, void *stream)
 {
     NvtxRange nvtx_("b200aa_pool_frames");
+    REFUSE_CAPTURE(stream, "b200aa_pool_frames", "kernel 11 is not captured; call it eagerly");
     const int F = n_feats;
     if (!d_st || !h_frames || !d_out || n_clips < 1 || F < 1 || ratio < 1 || clip_stride < 0 || row_stride < 0 ||
         (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))

@@ -118,6 +118,7 @@ extern "C" int b200aa_hmm_statistics(const void *d_mid, int dtype, int64_t n_cli
                                      const int64_t *h_idx, double *d_out, void *stream)
 {
     NvtxRange nvtx_("b200aa_hmm_statistics");
+    REFUSE_CAPTURE(stream, "b200aa_hmm_statistics", kWhyHostArrays);
     if (!d_mid || !h_n_windows || !h_class_off || !h_idx || !d_out || n_clips < 1 || n_feats < 1 || m_stride < 1 ||
         n_classes < 1 || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64) || h_class_off[0] != 0 ||
         !hmm_counts_ok(h_n_windows, n_clips, m_stride, 0))
@@ -221,6 +222,7 @@ extern "C" int b200aa_hmm_decode(const float *d_mid, int64_t n_clips, int n_feat
                                  const double *d_vars, const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
 {
     NvtxRange nvtx_("b200aa_hmm_decode");
+    REFUSE_CAPTURE(stream, "b200aa_hmm_decode", kWhyHostArrays);
     if (!hmm_decode_ok(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars,
                        d_const, d_ids, d_bad))
         return B200AA_ERR_INVALID;
@@ -234,6 +236,7 @@ extern "C" int b200aa_hmm_decode_f64(const double *d_mid, int64_t n_clips, int n
                                      const double *d_const, int32_t *d_ids, int32_t *d_bad, void *stream)
 {
     NvtxRange nvtx_("b200aa_hmm_decode_f64");
+    REFUSE_CAPTURE(stream, "b200aa_hmm_decode_f64", kWhyHostArrays);
     if ((window_major != 0 && window_major != 1) ||
         !hmm_decode_ok(d_mid, n_clips, n_feats, m_stride, h_n_windows, n_states, d_log_start, d_log_trans, d_means, d_vars,
                        d_const, d_ids, d_bad))

@@ -203,6 +203,7 @@ extern "C" int b200aa_knn_classify(const double *d_feats, const int32_t *d_slots
                                    double *d_P, void *stream)
 {
     NvtxRange nvtx_("b200aa_knn_classify");
+    REFUSE_CAPTURE(stream, "b200aa_knn_classify", kWhyHostArrays);
     if (!d_feats || !d_slots || !d_query || !d_ids || !d_P || n_train < 1 || n_train > INT32_MAX || n_feats < 1 ||
         n_classes < 1 || k < 1 || n_query < 0 || q_stride < n_feats || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
         return B200AA_ERR_INVALID;
@@ -274,6 +275,7 @@ extern "C" int b200aa_knn_cross_validate(const double *d_X, const int32_t *d_y, 
                                          const int32_t *h_classes, int32_t *d_pred, int64_t *d_counts, void *stream)
 {
     NvtxRange nvtx_("b200aa_knn_cross_validate");
+    REFUSE_CAPTURE(stream, "b200aa_knn_cross_validate", kWhyHostArrays);
     if (!d_X || !d_y || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !h_k || !h_classes || !d_pred ||
         !d_counts || n < 1 || n > INT32_MAX || n_feats < 1 || n_classes < 1 || n_problems < 0 || h_train_off[0] != 0 ||
         h_test_off[0] != 0)

@@ -205,6 +205,7 @@ extern "C" int b200aa_normalize_windows(const float *d_mid, int64_t n_clips, int
                                         const float *d_std, float *d_out, void *stream)
 {
     if (!d_mid || !d_out || !d_mean || !d_std || n_clips < 0 || n_rows < 1 || n_windows < 0) return B200AA_ERR_INVALID;
+    REFUSE_CAPTURE(stream, "b200aa_normalize_windows", "not captured; call it eagerly");
     if (n_clips == 0 || n_windows == 0) return B200AA_OK;
     if (n_clips > 65535 || (n_rows + 31) / 32 > 65535) return B200AA_ERR_UNSUPPORTED;
     const dim3 grid((unsigned)((n_windows + 31) / 32), (unsigned)((n_rows + 31) / 32), (unsigned)n_clips), block(32, 8);

@@ -14,6 +14,7 @@ extern "C" int b200aa_decode_pcm(const void *d_arena, int64_t arena_bytes, const
                                  int out_dtype, void *d_out, int64_t n_out, int64_t out_stride, void *stream)
 {
     NvtxRange nvtx_("b200aa_decode_pcm");
+    REFUSE_CAPTURE(stream, "b200aa_decode_pcm", kWhyHostArrays);
     if (!d_arena || !h_clips || !d_out || arena_bytes < 0 || n_clips < 0 || n_out < 0 || out_stride < n_out ||
         (out_dtype != B200AA_DTYPE_I16 && out_dtype != B200AA_DTYPE_F32))
         return B200AA_ERR_INVALID;

@@ -258,6 +258,7 @@ extern "C" int b200aa_music_thumbnail(const double *d_X, int n_feats, int64_t x_
                                       double *d_sim, double *d_out, int64_t *d_idx, void *stream)
 {
     NvtxRange nvtx_("b200aa_music_thumbnail");
+    REFUSE_CAPTURE(stream, "b200aa_music_thumbnail", kWhyHostArrays);
     using thumb::Track;
     const int F = n_feats, m = filter_len;
     const bool sim_only = d_sim != nullptr;

@@ -93,6 +93,7 @@ extern "C" int b200aa_trees_create(b200aa_trees **out, const b200aa_tree_node *h
 {
     if (!out) return B200AA_ERR_INVALID;
     *out = nullptr;
+    REFUSE_CAPTURE(nullptr, "b200aa_trees_create", kWhyAllocates);
     if (!h_nodes || !h_roots || !h_values || n_nodes < 1 || n_nodes > INT32_MAX || n_trees < 1 || n_leaves < 1 ||
         n_leaves > INT32_MAX || n_classes < 1 || n_feats < 1 || (mode != trees::kForestMean && mode != trees::kBoostSum) ||
         (mode == trees::kBoostSum && !h_init))
@@ -176,6 +177,7 @@ extern "C" int b200aa_trees_classify(const b200aa_trees *model, const void *d_qu
                                      void *stream)
 {
     NvtxRange nvtx_("b200aa_trees_classify");
+    REFUSE_CAPTURE(stream, "b200aa_trees_classify", "kernel 8 is not captured; call it eagerly");
     if (!model || !d_query || !d_ids || !d_scores || !d_bad || n_query < 0 || n_feats != model->n_feats ||
         q_stride < n_feats || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
         return B200AA_ERR_INVALID;

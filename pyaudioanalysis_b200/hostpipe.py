@@ -10,6 +10,7 @@ import ctypes
 
 import numpy as np
 
+from . import _lib
 from ._lib import lib, check, get_plan, DTYPE_I16, DTYPE_F32
 from . import numa
 
@@ -79,6 +80,7 @@ class HostPipeline:
             raise ValueError("out must be C-contiguous float32 [>=B, %d, %d]" % (self.F, self.T))
         import torch
         with torch.cuda.device(self.device):
+            _lib.refuse_capture("b200aa_st_features_host", _lib.HOST_BUFFER_WHY)
             check(lib().b200aa_st_features_host(self.plan.handle, x.ctypes.data_as(ctypes.c_void_p), _NP_CODES[self.dtype], B,
                                                 self.n, 1 if self.deltas else 0, dst.ctypes.data_as(ctypes.c_void_p)))
         return dst[:B]
