@@ -487,6 +487,57 @@ int b200aa_trees_classify(const b200aa_trees *model, const void *d_query, int dt
                           int64_t q_stride, int64_t *d_ids, double *d_scores, int32_t *d_bad, void *stream);
 int b200aa_trees_destroy(b200aa_trees *model);
 
+/* Kernel 13 (csrc/forest.cuh): training of the forests of extract_features_and_train / evaluate_classifier
+ * (audioTrainTest.py:52-93), bit for bit scikit-learn 1.9's RandomForestClassifier(n_estimators=T).fit (kind 0, best
+ * splitter) and ExtraTreesClassifier(n_estimators=T).fit (kind 1, random splitter) with every other argument at its
+ * default: gini, max_features = max(1, int(sqrt(n_feats))), min_samples_split 2, min_samples_leaf 1, no depth limit.
+ *
+ * b200aa_forest_fit: d_X [n, row_stride] float32 or float64 on the current device (n_feats columns read, cast to float32
+ * with round to nearest as fit casts; no NaN and nothing that is or becomes +-inf: the caller refuses those), h_y int32
+ * [n] class indices in [0, n_classes), h_weights int32 [n_trees, n] every tree's sample weights (np.bincount of its
+ * bootstrap indices) or NULL for weight 1 everywhere, h_seeds uint32 [n_trees] every tree's splitter rand_r_state.
+ * Writes the trees one after another to h_nodes / h_values (node_capacity nodes; 2 n - 1 per tree always suffice):
+ * tree t has h_node_count[t] nodes in Tree.__getstate__'s order and fields (left / right -1 and feature -2, threshold
+ * -2.0 at a leaf) and values [node, n_classes] (class fractions), and h_max_depth[t].  NULL pointers, n < 1 or n > 2^29,
+ * n_feats < 1, row_stride < n_feats, n_classes < 1, n_trees < 1, an unknown kind or dtype, max_features outside [1,
+ * n_feats], a class index out of range, a negative weight or one above 2^29, and a forest larger than node_capacity are
+ * B200AA_ERR_INVALID (all but the last before any CUDA call); more than 512 features or 32 classes is
+ * B200AA_ERR_UNSUPPORTED.  Not restated: for kind 1, when a node's minimum of the drawn feature is a zero present with
+ * both signs and our_rand_r returns exactly RAND_R_MAX, the stored threshold's zero sign may differ from scikit-learn's
+ * (the partition is the same).  One CTA builds one tree; trees run in slices whose stream-ordered scratch stays under 256 MB.
+ * The call returns once the nodes are on the host; it refuses a capturing stream (B200AA_ERR_CAPTURE).
+ *
+ * Replaces: RandomForestClassifier / ExtraTreesClassifier .fit in train_random_forest / train_extra_trees. */
+typedef struct b200aa_forest_node {
+    int32_t left, right, feature, n_node_samples;
+    double threshold, impurity, weighted_n_node_samples;
+    int32_t missing_go_to_left, pad;
+} b200aa_forest_node;
+int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride, const int32_t *h_y,
+                      int n_classes, int kind, int n_trees, int max_features, const int32_t *h_weights,
+                      const uint32_t *h_seeds, b200aa_forest_node *h_nodes, double *h_values, int64_t node_capacity,
+                      int64_t *h_node_count, int32_t *h_max_depth, void *stream);
+
+/* b200aa_forest_cross_validate: the model selection of evaluate_classifier (audioTrainTest.py:576-771) for
+ * "randomforest" (kind 0) and "extratrees" (kind 1), every (parameter, experiment) problem in one call.  d_X float64
+ * [n, n_feats] C-contiguous on the current device, h_y int32 [n] class indices in [0, n_classes).  Problem p trains on
+ * rows h_train_idx [h_train_off[p], h_train_off[p + 1]) and tests on h_test_idx [h_test_off[p], h_test_off[p + 1]), in
+ * split order (h_train_off[0] = h_test_off[0] = 0).  Per problem, on the device: StandardScaler().fit on the training
+ * rows and transform of both (kernel 6's knn::scaler_fit), the forest of h_n_trees[p] trees built by kernel 13 on the
+ * training rows cast to float32 with labels the indices into the training rows' sorted classes, and every test row
+ * classified as the forest's predict (tree sums in tree order over T, first maximum).  Problem p's trees take
+ * h_seeds [sum of the earlier h_n_trees, + h_n_trees[p]) and, for kind 0, h_weights int32 [h_n_trees[p], n_train(p)]
+ * (problems one after another; NULL for kind 1, required for kind 0).  Writes d_pred int32 [h_test_off[P]] (each test
+ * row's class index) and d_counts int64 [P, n_classes, n_classes] = counts[p, y_test, y_pred], the format of
+ * b200aa_knn_cross_validate.  The forests never leave the device.  Argument checks as b200aa_forest_fit's, plus an empty
+ * training set, an index outside [0, n) and h_n_trees < 1 are B200AA_ERR_INVALID before any CUDA call.  The call is
+ * stream-ordered and returns without waiting for the stream; it refuses a capturing stream. */
+int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_feats, const int32_t *h_y, int n_classes, int kind,
+                                 int64_t n_problems, const int64_t *h_train_off, const int32_t *h_train_idx,
+                                 const int64_t *h_test_off, const int32_t *h_test_idx, const int32_t *h_n_trees,
+                                 const int32_t *h_weights, const uint32_t *h_seeds, int32_t *d_pred, int64_t *d_counts,
+                                 void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

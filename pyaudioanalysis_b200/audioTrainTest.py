@@ -1,4 +1,5 @@
-"""The kNN model selection of the reference's audioTrainTest.evaluate_classifier (audioTrainTest.py:576-771) on the GPU.
+"""The kNN and forest model selection of the reference's audioTrainTest.evaluate_classifier (audioTrainTest.py:576-771)
+on the GPU.
 
 For every neighbour count in `params` and each of `n_exp` experiments the reference draws a train / test split, fits a
 StandardScaler on the training rows, classifies every test row with its Knn and scores the experiment with scikit-learn.
@@ -8,13 +9,20 @@ The reference's scores follow from those counts: its confusion_matrix is the cou
 y_test or y_pred, and its macro f1_score is the mean over those classes of 2 tp / (n_true + n_pred).  The printed table
 and the returned parameter are the reference's, text for text.
 
-Only classifier_name "knn" without SMOTE on finite float64 features runs here (``unsupported`` says why not otherwise);
-``install.install_training`` sends everything else to the reference's own function.
+The forests ("randomforest", "extratrees") go the same way: each problem's split and then its forest's tree seeds are
+drawn in the reference's order, and ``consumers.forest_cross_validate`` (kernel 13) scales, trains and classifies every
+problem on the device, bit for bit scikit-learn 1.9's fit and predict.
+
+Only "knn", "randomforest" and "extratrees" without SMOTE on finite float64 features run here (``unsupported`` says why
+not otherwise); ``install.install_training`` sends everything else to the reference's own function.
 """
 import math
 
 import numpy as np
 from sklearn.model_selection import GroupShuffleSplit
+
+
+_FORESTS = ("randomforest", "extratrees")
 
 
 def features_to_matrix(features):
@@ -26,8 +34,12 @@ def features_to_matrix(features):
 
 def unsupported(features, classifier_name, params, train_percentage=0.90, smote=False):
     """None when evaluate_classifier runs on the GPU for these arguments, else the reason it does not."""
-    if classifier_name != "knn":
-        return "classifier %r: only 'knn' runs on the GPU" % (classifier_name,)
+    if classifier_name not in ("knn",) + _FORESTS:
+        return "classifier %r: only 'knn', 'randomforest' and 'extratrees' run on the GPU" % (classifier_name,)
+    if classifier_name in _FORESTS:
+        import sklearn
+        if not sklearn.__version__.startswith("1.9."):
+            return "scikit-learn %s: the forest trainer restates 1.9.x" % sklearn.__version__
     if smote:
         return "SMOTE resamples the training rows"
     if len(features) < 2:
@@ -44,9 +56,15 @@ def unsupported(features, classifier_name, params, train_percentage=0.90, smote=
     # single contiguous column pairwise)
     if len(shapes) != 1 or shapes.pop() < 2:
         return "the classes need the same number (>= 2) of features"
+    if classifier_name in _FORESTS:
+        if features[0].shape[1] > 512 or len(features) > 32:
+            return "more than 512 features or 32 classes: the forest trainer's shared-memory layout"
+        with np.errstate(over="ignore"):
+            if not all(np.isfinite(np.asarray(f).astype(np.float32)).all() for f in features):
+                return "features that become inf as float32"
     for k in params:
-        if not (isinstance(k, (int, np.integer)) and k >= 1):
-            return "every kNN parameter must be an integer >= 1, got %r" % (k,)
+        if not (isinstance(k, (int, np.integer)) and not isinstance(k, bool) and k >= 1):
+            return "every parameter (kNN neighbours, forest trees) must be an integer >= 1, got %r" % (k,)
     if not 0 < 1 - train_percentage < 1:
         return "train_percentage must leave a test fraction in (0, 1)"
     return None
@@ -76,6 +94,20 @@ def draw_splits(X, y, n_params, n_exp, train_percentage, list_of_ids=None):
         perm = np.random.permutation(n)
         splits.append((perm[n_test:n_test + n_train], perm[:n_test]))
     return splits
+
+
+def draw_forest_problems(X, params, n_exp, train_percentage, kind, list_of_ids=None):
+    """(splits, seeds) of every (param, experiment) of the forest branch, params outer, drawn from NumPy's global RNG in
+    the reference's order: GroupShuffleSplit's splits once up front (list_of_ids), then per problem its
+    train_test_split permutation (without list_of_ids) followed by the seeds its forest's fit draws, one per tree."""
+    fixed = draw_splits(X, None, 1, n_exp, train_percentage, list_of_ids) if list_of_ids else None
+    from .forests import tree_seeds
+    splits, seeds = [], []
+    for C in params:
+        for e in range(n_exp):
+            splits.append(fixed[e] if fixed else draw_splits(X, None, 1, 1, train_percentage)[0])
+            seeds.append(tree_seeds(int(C), kind))
+    return splits, seeds
 
 
 def experiment_scores(counts, all_classes):
@@ -159,16 +191,21 @@ def report(y, class_names, params, parameter_mode, n_exp, counts):
 
 def evaluate_classifier(features, class_names, classifier_name, params, parameter_mode, list_of_ids=None, n_exp=-1,
                         train_percentage=0.90, smote=False):
-    """audioTrainTest.evaluate_classifier (:576-771) for classifier_name "knn": the same prints and return value, every
-    (param, experiment) problem classified on the GPU in one call.  Raises ValueError for arguments it does not cover
+    """audioTrainTest.evaluate_classifier (:576-771) for classifier_name "knn", "randomforest" and "extratrees": the same
+    prints and return value, every (param, experiment) problem trained (forests) and classified on the GPU in one call.  Raises ValueError for arguments it does not cover
     (``unsupported``); there is no CPU path."""
-    from .consumers import knn_cross_validate
+    from .consumers import forest_cross_validate, knn_cross_validate
     why = unsupported(features, classifier_name, params, train_percentage, smote)
     if why is not None:
         raise ValueError("evaluate_classifier on the GPU: " + why)
     X, y = features_to_matrix(features)
     if n_exp == -1:
         n_exp = int(50000 / X.shape[0]) + 1
+    if classifier_name in _FORESTS:
+        splits, seeds = draw_forest_problems(X, params, n_exp, train_percentage, classifier_name, list_of_ids)
+        trees = [int(C) for C in params for _ in range(n_exp)]
+        _, counts = forest_cross_validate(X, y, splits, seeds, trees, classifier_name, n_classes=len(features))
+        return report(y, class_names, params, parameter_mode, n_exp, counts.cpu().numpy())
     splits = draw_splits(X, y, len(params), n_exp, train_percentage, list_of_ids)
     ks = [int(C) for C in params for _ in range(n_exp)]
     _, counts = knn_cross_validate(X, y, splits, ks, n_classes=len(features))
@@ -184,3 +221,26 @@ def dispatcher(original):
                    train_percentage=train_percentage, smote=smote)
     evaluate_classifier_dispatch.original = original
     return evaluate_classifier_dispatch
+
+
+def _train_forest(kind, features, labels, n_estimators):
+    from . import forests
+    from .consumers import forest_fit
+    X = np.asarray(features) if not isinstance(features, np.ndarray) else features
+    if forests.unsupported(X, labels, n_estimators, kind) is None:
+        return forest_fit(X, labels, n_estimators, kind)
+    from sklearn.ensemble import ExtraTreesClassifier, RandomForestClassifier
+    cls = RandomForestClassifier if kind == "randomforest" else ExtraTreesClassifier
+    return cls(n_estimators=n_estimators).fit(features, labels)
+
+
+def train_random_forest(features, labels, n_estimators):
+    """audioTrainTest.train_random_forest (:158-178): RandomForestClassifier(n_estimators).fit(features, labels), trained
+    on the GPU (``consumers.forest_fit``) tree for tree as scikit-learn trains it; arguments the trainer does not
+    reproduce (``forests.unsupported``) go to scikit-learn."""
+    return _train_forest("randomforest", features, labels, n_estimators)
+
+
+def train_extra_trees(features, labels, n_estimators):
+    """audioTrainTest.train_extra_trees (:202-219), as ``train_random_forest`` with ExtraTreesClassifier."""
+    return _train_forest("extratrees", features, labels, n_estimators)

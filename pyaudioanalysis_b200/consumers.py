@@ -681,6 +681,104 @@ class TreeEnsembleModel:
             lib().b200aa_trees_destroy(h)
 
 
+def forest_fit(X, y, n_estimators, kind):
+    """``RandomForestClassifier(n_estimators).fit(X, y)`` (kind "randomforest") or ``ExtraTreesClassifier`` (kind
+    "extratrees") trained on the GPU (``b200aa_forest_fit``, DESIGN.md kernel 13), tree for tree scikit-learn 1.9's under
+    the same NumPy global state, which it leaves as ``fit`` leaves it.  Returns the fitted scikit-learn estimator.
+
+    X: float64 / float32 [n, F] host array (or a CUDA tensor, which is read from the device); y: n labels.  Raises
+    ValueError with ``forests.unsupported``'s reason for what it does not reproduce; ``train_random_forest`` /
+    ``train_extra_trees`` hand those calls to scikit-learn."""
+    from . import forests as FO
+    Xh = X.detach().cpu().numpy() if isinstance(X, torch.Tensor) else X
+    why = FO.unsupported(Xh, y, n_estimators, kind)
+    if why is not None:
+        raise ValueError("forest_fit on the GPU: " + why)
+    n, F = Xh.shape
+    classes, y_idx = np.unique(np.asarray(y), return_inverse=True)
+    C = len(classes)
+    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64) and X.stride(1) == 1:
+        d_X = X                                     # cast to float32 on the device, round to nearest, as fit casts
+    else:
+        # fit's own cast, straight to float32 (any integer or float dtype rounds once)
+        d_X = torch.from_numpy(np.ascontiguousarray(Xh, dtype=np.float32)).cuda()
+    est, trees, weights, seeds = FO.draw(int(n_estimators), kind, n)
+    cap = int(n_estimators) * (2 * n - 1)
+    nodes = np.empty(cap, dtype=FO.NODE_DTYPE)
+    values = np.empty((cap, C), dtype=np.float64)
+    counts = np.empty(int(n_estimators), dtype=np.int64)
+    depth = np.empty(int(n_estimators), dtype=np.int32)
+    y32 = np.ascontiguousarray(y_idx, dtype=np.int32)
+
+    def ptr(a):
+        return ctypes.c_void_p(a.ctypes.data) if a is not None else None
+    with torch.cuda.device(d_X.device):
+        check(lib().b200aa_forest_fit(
+            ctypes.c_void_p(d_X.data_ptr()), DTYPE_F32 if d_X.dtype == torch.float32 else DTYPE_F64, n, F, d_X.stride(0),
+            ptr(y32), C, FO.KINDS[kind], int(n_estimators), max(1, int(np.sqrt(F))), ptr(weights), ptr(seeds), ptr(nodes),
+            ptr(values), cap, ptr(counts), ptr(depth), _stream()))
+    states, off = [], 0
+    for t in range(int(n_estimators)):
+        nc = int(counts[t])
+        states.append(FO.tree_state(nodes[off:off + nc], values[off:off + nc], depth[t], C))
+        off += nc
+    return FO.assemble(est, trees, F, n, classes, states)
+
+
+def forest_cross_validate(X, y, splits, seeds, n_estimators, kind, n_classes=None):
+    """The forest branch of evaluate_classifier's model selection (audioTrainTest.py:631-699) as one batch on the GPU
+    (``b200aa_forest_cross_validate``, DESIGN.md kernel 13): per (train, test) split, StandardScaler fit on the training
+    rows, ``RandomForestClassifier`` / ``ExtraTreesClassifier(n_estimators[p]).fit`` (kind "randomforest" /
+    "extratrees") on them, and predict of every test row, bit for bit scikit-learn's.  The forests stay on the device.
+
+    X: float64 [n, F] (host, or a CUDA tensor); y: the n class indices in [0, n_classes); splits: (train, test) row
+    indices per problem; seeds: per problem the tree seeds fit would draw (``forests.tree_seeds``); n_estimators: the tree
+    count per problem.  Returns CUDA (pred int32 [sum of the test counts], counts int64 [P, n_classes, n_classes])."""
+    from . import forests as FO
+    if kind not in FO.KINDS:
+        raise ValueError("kind must be 'randomforest' or 'extratrees', got %r" % (kind,))
+    if not isinstance(X, torch.Tensor):
+        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, F]")
+    X = X.contiguous()
+    n = X.shape[0]
+    y = np.asarray(y.cpu() if isinstance(y, torch.Tensor) else y)
+    if y.shape != (n,) or not np.array_equal(y, np.floor(y)) or (n and y.min() < 0):
+        raise ValueError("y must hold one class index >= 0 per row of X")
+    y = y.astype(np.int32)
+    n_classes = int(y.max()) + 1 if n_classes is None else int(n_classes)
+    if not len(splits) == len(seeds) == len(n_estimators):
+        raise ValueError("one seed list and one tree count per split")
+    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
+    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
+    train_off, train_idx = _concat_indices(train, np.int32)
+    test_off, test_idx = _concat_indices(test, np.int32)
+    n_trees = np.ascontiguousarray(n_estimators, dtype=np.int32)
+    if any(len(s) != t for s, t in zip(seeds, n_trees)):
+        raise ValueError("every problem needs one seed per tree")
+    ws, rs = [], []
+    for s, tr in zip(seeds, train):
+        w, r = FO.derive(s, kind, tr.size)
+        if w is not None:
+            ws.append(w.ravel())
+        rs.append(r)
+    weights = np.ascontiguousarray(np.concatenate(ws), dtype=np.int32) if ws else None
+    rand_r = np.ascontiguousarray(np.concatenate(rs), dtype=np.uint32)
+    with torch.cuda.device(X.device):
+        pred = torch.empty(int(test_off[-1]), dtype=torch.int32, device=X.device)
+        counts = torch.empty((len(splits), n_classes, n_classes), dtype=torch.int64, device=X.device)
+
+        def ptr(a):
+            return ctypes.c_void_p(a.ctypes.data) if a is not None else None
+        check(lib().b200aa_forest_cross_validate(
+            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], ptr(y), n_classes, FO.KINDS[kind], len(splits), ptr(train_off),
+            ptr(train_idx), ptr(test_off), ptr(test_idx), ptr(n_trees), ptr(weights), ptr(rand_r),
+            ctypes.c_void_p(pred.data_ptr()), ctypes.c_void_p(counts.data_ptr()), _stream()))
+    return pred, counts
+
+
 def tree_classify_batch(model, vectors):
     """predict / predict_proba of a tree ensemble for every row of a CUDA float32 / float64 [n, F] tensor, in one kernel on
     the current stream (DESIGN.md, kernel 8): CUDA (ids int64 [n], indices into the model's classes_; P float64 [n, C]),

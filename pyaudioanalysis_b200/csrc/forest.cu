@@ -1,0 +1,331 @@
+// libb200aa.so -- Forest training (kernel 13).
+#include <algorithm>
+#include <vector>
+
+#include "../../include/b200aa.h"
+#include "entry.h"
+#include "forest.cuh"
+#include "knn_cv.cuh"
+
+using namespace b200aa;
+
+// ------------------------------------------------------------------------------------------------
+// kernel 13: random forest / extra trees training, bit for bit scikit-learn 1.9's fit (csrc/forest.cuh)
+// ------------------------------------------------------------------------------------------------
+static_assert(sizeof(b200aa_forest_node) == sizeof(forest::NodeOut), "node layout of the C ABI");
+
+namespace {
+
+// the global scratch of one tree: [samples | tmp | keys | stack | nodes | values | meta]
+struct TreeLayout {
+    size_t samples, tmp, keys, stack, nodes, values, meta, bytes;
+};
+TreeLayout tree_layout(int64_t n, int C)
+{
+    const int64_t cap = 2 * n - 1;
+    TreeLayout L;
+    L.samples = 0;
+    L.tmp = L.samples + align256(size_t(n) * 4);
+    L.keys = L.tmp + align256(size_t(n) * 4);
+    L.stack = L.keys + align256(size_t(forest::pow2_at_least(n)) * 8);
+    L.nodes = L.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
+    L.values = L.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
+    L.meta = L.values + align256(size_t(cap) * C * 8);
+    L.bytes = align256(L.meta + 16);
+    return L;
+}
+
+// team-shared arrays of build_tree in dynamic shared memory
+inline size_t smem_bytes(int F, int C)
+{
+    return sizeof(forest::Shared) + size_t(F) * (3 * 4 + 2 * 4 + 8) + size_t(forest::kThreads) * (size_t(C) * 8 + 16) + 64;
+}
+
+}  // namespace
+
+__global__ void forest_cast_kernel(const double *__restrict__ X, int64_t n, int F, int64_t stride, float *__restrict__ out)
+{
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n * F; i += int64_t(gridDim.x) * blockDim.x)
+        out[i] = __double2float_rn(X[(i / F) * stride + i % F]);
+}
+__global__ void forest_cast_kernel(const float *__restrict__ X, int64_t n, int F, int64_t stride, float *__restrict__ out)
+{
+    for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n * F; i += int64_t(gridDim.x) * blockDim.x)
+        out[i] = X[(i / F) * stride + i % F];
+}
+
+// One CTA per tree of the slice: build_tree with the block as its team.
+__global__ void __launch_bounds__(forest::kThreads) forest_build_kernel(const float *__restrict__ X,
+                                                                       const int32_t *__restrict__ y, int64_t n, int F,
+                                                                       int C, int max_features, int kind,
+                                                                       const int32_t *__restrict__ w,
+                                                                       const uint32_t *__restrict__ seeds,
+                                                                       char *__restrict__ scratch, TreeLayout L)
+{
+    extern __shared__ __align__(16) unsigned char forest_smem[];
+    const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
+    char *base = scratch + size_t(blockIdx.x) * L.bytes;
+    unsigned char *s = forest_smem;
+    forest::Shared *st = reinterpret_cast<forest::Shared *>(s);
+    s += (sizeof(forest::Shared) + 15) & ~size_t(15);
+    double *thr = reinterpret_cast<double *>(s);
+    s += size_t(F) * 8;
+    int64_t *cnt = reinterpret_cast<int64_t *>(s);
+    s += size_t(blockDim.x) * C * 8;
+    double *red_proxy = reinterpret_cast<double *>(s);
+    s += size_t(blockDim.x) * 8;
+    int64_t *red_pos = reinterpret_cast<int64_t *>(s);
+    s += size_t(blockDim.x) * 8;
+    float *mn = reinterpret_cast<float *>(s);
+    float *mx = mn + F;
+    int32_t *features = reinterpret_cast<int32_t *>(mx + F);
+    int32_t *constf = features + F, *drawn = constf + F;
+    const forest::Tree T{X, y, w ? w + int64_t(blockIdx.x) * n : nullptr, n, F, C, max_features, kind,
+                         reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.tmp),
+                         reinterpret_cast<uint64_t *>(base + L.keys), reinterpret_cast<forest::StackRec *>(base + L.stack),
+                         reinterpret_cast<forest::NodeOut *>(base + L.nodes), reinterpret_cast<double *>(base + L.values),
+                         features, constf, drawn, mn, mx, thr, cnt, red_proxy, red_pos, st};
+    forest::build_tree(T, tm, seeds[blockIdx.x]);
+    if (threadIdx.x == 0) {
+        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
+        meta[0] = st->node_count;
+        meta[1] = st->max_depth;
+    }
+}
+
+extern "C" int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride,
+                                 const int32_t *h_y, int n_classes, int kind, int n_trees, int max_features,
+                                 const int32_t *h_weights, const uint32_t *h_seeds, b200aa_forest_node *h_nodes,
+                                 double *h_values, int64_t node_capacity, int64_t *h_node_count, int32_t *h_max_depth,
+                                 void *stream)
+{
+    NvtxRange nvtx_("b200aa_forest_fit");
+    REFUSE_CAPTURE(stream, "b200aa_forest_fit", kWhyHostArrays);
+    if (!d_X || !h_y || !h_seeds || !h_nodes || !h_values || !h_node_count || !h_max_depth || n < 1 ||
+        n > (int64_t(1) << 29) || n_feats < 1 || row_stride < n_feats || n_classes < 1 || n_trees < 1 ||
+        (kind != forest::kBest && kind != forest::kRandom) || max_features < 1 || max_features > n_feats ||
+        node_capacity < 0 || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
+        return B200AA_ERR_INVALID;
+    for (int64_t i = 0; i < n; ++i)
+        if (h_y[i] < 0 || h_y[i] >= n_classes) return B200AA_ERR_INVALID;
+    if (h_weights)
+        for (int64_t i = 0; i < int64_t(n_trees) * n; ++i)
+            if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t smem = smem_bytes(n_feats, n_classes);
+    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const TreeLayout L = tree_layout(n, n_classes);
+    const size_t per_tree = L.bytes + (h_weights ? align256(size_t(n) * 4) : 0);
+    const size_t fixed = align256(size_t(n) * n_feats * 4) + align256(size_t(n) * 4) + align256(size_t(n_trees) * 4);
+    const int64_t slice = std::max<int64_t>(
+        1, std::min<int64_t>(n_trees, fixed + per_tree < kScratchSliceBytes ? int64_t((kScratchSliceBytes - fixed) / per_tree) : 1));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
+    if (rc != B200AA_OK) return rc;
+    char *base = static_cast<char *>(scratch.get());
+    float *Xf = reinterpret_cast<float *>(base);
+    int32_t *y = reinterpret_cast<int32_t *>(base + align256(size_t(n) * n_feats * 4));
+    uint32_t *seeds = reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(y) + align256(size_t(n) * 4));
+    char *trees = base + fixed;
+    int32_t *w = h_weights ? reinterpret_cast<int32_t *>(trees + size_t(slice) * L.bytes) : nullptr;
+    const unsigned cast_blocks = unsigned(std::min<int64_t>((n * n_feats + 255) / 256, 4096));
+    with_real_type(dtype, [&](auto t) {
+        forest_cast_kernel<<<cast_blocks, 256, 0, st>>>(static_cast<const decltype(t) *>(d_X), n, n_feats, row_stride, Xf);
+    });
+    CK_LAUNCH("forest_cast_kernel");
+    CK(cudaMemcpyAsync(y, h_y, size_t(n) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
+    int64_t written = 0;
+    std::vector<int64_t> meta(size_t(slice) * 2);
+    for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
+        const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
+        if (w) CK(cudaMemcpyAsync(w, h_weights + t0 * n, size_t(nt * n) * 4, cudaMemcpyHostToDevice, st));
+        forest_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(Xf, y, n, n_feats, n_classes, max_features, kind,
+                                                                         w, seeds + t0, trees, L);
+        CK_LAUNCH("forest_build_kernel");
+        for (int64_t i = 0; i < nt; ++i)
+            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], trees + size_t(i) * L.bytes + L.meta, 16,
+                               cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (int64_t i = 0; i < nt; ++i) {
+            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
+            h_node_count[t] = nc;
+            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
+            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
+            const char *tb = trees + size_t(i) * L.bytes;
+            CK(cudaMemcpyAsync(h_nodes + written, tb + L.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(h_values + written * n_classes, tb + L.values, size_t(nc) * n_classes * 8,
+                               cudaMemcpyDeviceToHost, st));
+            written += nc;
+        }
+        CK(cudaStreamSynchronize(st));    // the next slice reuses the scratch the copies read
+    }
+    return scratch.done(B200AA_OK);
+}
+
+// ------------------------------------------------------------------------------------------------
+// kernel 13 in model selection: every (parameter, experiment) problem of evaluate_classifier for the two forests
+// ------------------------------------------------------------------------------------------------
+// One thread per column: StandardScaler().fit over the problem's training rows in split order (kernel 6's
+// knn::scaler_fit), then the training and test rows standardised and cast to float32 as fit / predict cast them.
+__global__ void forest_cv_scale_kernel(const double *__restrict__ X, int F, const int32_t *__restrict__ train, int64_t n_train,
+                                       const int32_t *__restrict__ test, int64_t n_test, float *__restrict__ Xtr,
+                                       float *__restrict__ Xte)
+{
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    const knn::Scale sc = knn::scaler_fit([&](int64_t i) { return X[int64_t(train[i]) * F + f]; }, n_train);
+    for (int64_t i = 0; i < n_train; ++i) Xtr[i * F + f] = __double2float_rn(knn::standardise(X[int64_t(train[i]) * F + f], sc));
+    for (int64_t i = 0; i < n_test; ++i) Xte[i * F + f] = __double2float_rn(knn::standardise(X[int64_t(test[i]) * F + f], sc));
+}
+
+// One thread per test row: walk every tree of the slice (left iff x <= threshold, tree/_tree.pyx _apply_dense) and add
+// its leaf's values to the row's class sums in tree order (forest predict_proba); after the last slice P = sum / T, the
+// first maximum is the prediction (classes_.take(argmax)), mapped to its class over all problems and counted.
+__global__ void forest_cv_classify_kernel(const float *__restrict__ Xte, int64_t n_test, int F, int C, const char *__restrict__ trees,
+                                          TreeLayout L, int nt, bool first, bool last, int n_trees,
+                                          double *__restrict__ acc, const int32_t *__restrict__ to_global,
+                                          const int32_t *__restrict__ y_test, int n_classes, int32_t *__restrict__ pred,
+                                          unsigned long long *__restrict__ counts)
+{
+    const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (r >= n_test) return;
+    const float *x = Xte + r * F;
+    double *a = acc + r * C;
+    if (first)
+        for (int c = 0; c < C; ++c) a[c] = 0.0;
+    for (int t = 0; t < nt; ++t) {
+        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * L.bytes + L.nodes);
+        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * L.bytes + L.values);
+        int32_t i = 0;
+        while (nodes[i].left != forest::kTreeLeaf) i = double(x[nodes[i].feature]) <= nodes[i].threshold ? nodes[i].left : nodes[i].right;
+        for (int c = 0; c < C; ++c) a[c] = forest::dadd(a[c], values[int64_t(i) * C + c]);
+    }
+    if (!last) return;
+    double best = 0.0;
+    int bi = -1;
+    for (int c = 0; c < C; ++c) {
+        const double pc = forest::ddiv(a[c], double(n_trees));
+        if (bi < 0 || pc > best) {
+            best = pc;
+            bi = c;
+        }
+    }
+    const int32_t g = to_global[bi];
+    pred[r] = g;
+    atomicAdd(&counts[int64_t(y_test[r]) * n_classes + g], 1ull);
+}
+
+extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_feats, const int32_t *h_y, int n_classes,
+                                            int kind, int64_t n_problems, const int64_t *h_train_off,
+                                            const int32_t *h_train_idx, const int64_t *h_test_off,
+                                            const int32_t *h_test_idx, const int32_t *h_n_trees,
+                                            const int32_t *h_weights, const uint32_t *h_seeds, int32_t *d_pred,
+                                            int64_t *d_counts, void *stream)
+{
+    NvtxRange nvtx_("b200aa_forest_cross_validate");
+    REFUSE_CAPTURE(stream, "b200aa_forest_cross_validate", kWhyHostArrays);
+    if (!d_X || !h_y || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !h_n_trees || !h_seeds || !d_pred ||
+        !d_counts || n < 1 || n > (int64_t(1) << 29) || n_feats < 1 || n_classes < 1 || n_problems < 1 ||
+        (kind != forest::kBest && kind != forest::kRandom) || (kind == forest::kBest) != (h_weights != nullptr))
+        return B200AA_ERR_INVALID;
+    for (int64_t i = 0; i < n; ++i)
+        if (h_y[i] < 0 || h_y[i] >= n_classes) return B200AA_ERR_INVALID;
+    if (h_train_off[0] != 0 || h_test_off[0] != 0) return B200AA_ERR_INVALID;
+    int64_t ntr_max = 0, nte_max = 0, trees_total = 0, weights_total = 0, t_max = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
+        if (ntr < 1 || ntr > n || nte < 0 || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
+        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
+            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
+        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
+            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
+        ntr_max = std::max(ntr_max, ntr);
+        nte_max = std::max(nte_max, nte);
+        t_max = std::max<int64_t>(t_max, h_n_trees[p]);
+        trees_total += h_n_trees[p];
+        weights_total += int64_t(h_n_trees[p]) * ntr;
+    }
+    if (h_weights)
+        for (int64_t i = 0; i < weights_total; ++i)
+            if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int C = n_classes, F = n_feats, max_features = forest::sqrt_features(F);
+    const size_t smem = smem_bytes(F, C);
+    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    // scratch: [y_local | train | test | map | Xtr | Xte | acc | seeds | weights of a slice | trees of a slice]
+    const TreeLayout Lmax = tree_layout(ntr_max, C);
+    const size_t b_y = align256(size_t(ntr_max) * 4), b_tr = b_y, b_te = align256(size_t(std::max<int64_t>(nte_max, 1)) * 4),
+                 b_map = 256, b_xtr = align256(size_t(ntr_max) * F * 4), b_xte = align256(size_t(std::max<int64_t>(nte_max, 1)) * F * 4),
+                 b_acc = align256(size_t(std::max<int64_t>(nte_max, 1)) * C * 8), b_seeds = align256(size_t(t_max) * 4),
+                 b_yt = b_te;
+    const size_t fixed = b_y + b_tr + b_te + b_map + b_xtr + b_xte + b_acc + b_seeds + b_yt;
+    const size_t per_tree = Lmax.bytes + (h_weights ? align256(size_t(ntr_max) * 4) : 0);
+    const int64_t slice = std::max<int64_t>(
+        1, std::min<int64_t>(t_max, fixed + per_tree < kScratchSliceBytes ? int64_t((kScratchSliceBytes - fixed) / per_tree) : 1));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
+    if (rc != B200AA_OK) return rc;
+    char *q = static_cast<char *>(scratch.get());
+    int32_t *d_ylocal = reinterpret_cast<int32_t *>(q); q += b_y;
+    int32_t *d_train = reinterpret_cast<int32_t *>(q); q += b_tr;
+    int32_t *d_test = reinterpret_cast<int32_t *>(q); q += b_te;
+    int32_t *d_map = reinterpret_cast<int32_t *>(q); q += b_map;
+    float *d_xtr = reinterpret_cast<float *>(q); q += b_xtr;
+    float *d_xte = reinterpret_cast<float *>(q); q += b_xte;
+    double *d_acc = reinterpret_cast<double *>(q); q += b_acc;
+    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
+    int32_t *d_ytest = reinterpret_cast<int32_t *>(q); q += b_yt;
+    char *d_trees = q;
+    int32_t *d_w = h_weights ? reinterpret_cast<int32_t *>(d_trees + size_t(slice) * Lmax.bytes) : nullptr;
+    CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * C * C * sizeof(int64_t), st));
+    std::vector<int32_t> ylocal(ntr_max), ytest(std::max<int64_t>(nte_max, 1)), map(forest::kMaxClasses);
+    int64_t tree0 = 0, w0 = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
+        const int32_t *tr = h_train_idx + h_train_off[p], *te = h_test_idx + h_test_off[p];
+        const int T = h_n_trees[p];
+        // the classifier's classes_: the sorted class indices present in the training rows
+        int32_t local_of[forest::kMaxClasses];
+        for (int c = 0; c < C; ++c) local_of[c] = -1;
+        for (int64_t i = 0; i < ntr; ++i) local_of[h_y[tr[i]]] = 0;
+        int Cl = 0;
+        for (int c = 0; c < C; ++c)
+            if (local_of[c] == 0) {
+                local_of[c] = Cl;
+                map[Cl++] = c;
+            }
+        for (int64_t i = 0; i < ntr; ++i) ylocal[i] = local_of[h_y[tr[i]]];
+        for (int64_t i = 0; i < nte; ++i) ytest[i] = h_y[te[i]];
+        CK(cudaMemcpyAsync(d_train, tr, size_t(ntr) * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_ylocal, ylocal.data(), size_t(ntr) * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_map, map.data(), size_t(Cl) * 4, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_seeds, h_seeds + tree0, size_t(T) * 4, cudaMemcpyHostToDevice, st));
+        if (nte) {
+            CK(cudaMemcpyAsync(d_test, te, size_t(nte) * 4, cudaMemcpyHostToDevice, st));
+            CK(cudaMemcpyAsync(d_ytest, ytest.data(), size_t(nte) * 4, cudaMemcpyHostToDevice, st));
+        }
+        forest_cv_scale_kernel<<<unsigned((F + 63) / 64), 64, 0, st>>>(d_X, F, d_train, ntr, d_test, nte, d_xtr, d_xte);
+        CK_LAUNCH("forest_cv_scale_kernel");
+        const TreeLayout L = tree_layout(ntr, Cl);
+        const size_t smem_p = smem_bytes(F, Cl);
+        for (int64_t t0 = 0; t0 < T; t0 += slice) {
+            const int64_t nt = std::min<int64_t>(slice, T - t0);
+            if (d_w) CK(cudaMemcpyAsync(d_w, h_weights + w0 + t0 * ntr, size_t(nt * ntr) * 4, cudaMemcpyHostToDevice, st));
+            forest_build_kernel<<<unsigned(nt), forest::kThreads, smem_p, st>>>(d_xtr, d_ylocal, ntr, F, Cl, max_features, kind,
+                                                                               d_w, d_seeds + t0, d_trees, L);
+            CK_LAUNCH("forest_build_kernel");
+            if (nte) {
+                forest_cv_classify_kernel<<<unsigned((nte + 127) / 128), 128, 0, st>>>(
+                    d_xte, nte, F, Cl, d_trees, L, int(nt), t0 == 0, t0 + nt == T, T, d_acc, d_map, d_ytest, C,
+                    d_pred + h_test_off[p], reinterpret_cast<unsigned long long *>(d_counts + p * C * C));
+                CK_LAUNCH("forest_cv_classify_kernel");
+            }
+        }
+        tree0 += T;
+        w0 += int64_t(T) * ntr;
+    }
+    return scratch.done(B200AA_OK);
+}

@@ -36,14 +36,25 @@ def install_training(audio_train_test=None):
     """Rebind an importable ``pyAudioAnalysis.audioTrainTest`` (or the module given) so that its evaluate_classifier runs
     the kNN model selection on the GPU (``audioTrainTest.evaluate_classifier`` here) and every other classifier, SMOTE
     and non-finite input through the saved original.  extract_features_and_train looks the function up on the module at
-    call time (audioTrainTest.py:309), so it trains kNN models through the GPU unchanged.  Returns the attribute rebound."""
+    call time (audioTrainTest.py:309), so it trains kNN models through the GPU unchanged.  train_random_forest and
+    train_extra_trees, where the module has them, are rebound to the GPU trainers here (kernel 13): the final forest
+    extract_features_and_train fits and pickles is built on the GPU, tree for tree scikit-learn's.  Returns the
+    attributes rebound."""
     from .audioTrainTest import dispatcher
     if audio_train_test is None:
         import importlib
         audio_train_test = importlib.import_module("pyAudioAnalysis.audioTrainTest")
     original = _saved.setdefault((audio_train_test, "evaluate_classifier"), audio_train_test.evaluate_classifier)
     audio_train_test.evaluate_classifier = dispatcher(original)
-    return ["%s.evaluate_classifier" % audio_train_test.__name__]
+    done = ["%s.evaluate_classifier" % audio_train_test.__name__]
+    from . import audioTrainTest as ours
+    for n in ("train_random_forest", "train_extra_trees"):
+        if not hasattr(audio_train_test, n):
+            continue
+        _saved.setdefault((audio_train_test, n), getattr(audio_train_test, n))
+        setattr(audio_train_test, n, getattr(ours, n))
+        done.append("%s.%s" % (audio_train_test.__name__, n))
+    return done
 
 
 def install_segmentation(audio_segmentation=None):
