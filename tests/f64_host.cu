@@ -6,6 +6,8 @@
 //   time w Y (w)                 -> zcr, energy, energy entropy of one normalised frame
 //   pool F T ratio stepr X (FxT) -> the [2F, M] mid-term matrix
 //   fft n RE (n)                 -> re (n), im (n) of the fp64 mixed-radix transform of a real frame
+//   spec n Y (n)                 -> |X|[0:K] / K of that transform (f64::magnitude), as the frame kernel writes it
+//   specrec n Y (n)              -> the same with twiddles built by recurrence, w^j = w^(j-1) w (a planted defect)
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -71,7 +73,7 @@ int main()
             printf("P");
             for (double v : out) pr(v);
             printf("\n");
-        } else if (!strcmp(cmd, "fft")) {
+        } else if (!strcmp(cmd, "fft") || !strcmp(cmd, "spec") || !strcmp(cmd, "specrec")) {
             const int n = int(rl());
             const std::vector<double> re = rv(size_t(n));
             std::vector<f64::Cplx> a(n), b(n), tw(n);
@@ -79,6 +81,8 @@ int main()
                 a[j] = {re[j], 0.0};
                 const double ang = -2.0 * b200aa_host::kPi * double(j) / double(n);
                 tw[j] = {std::cos(ang), std::sin(ang)};
+                if (!strcmp(cmd, "specrec") && j > 1)
+                    tw[j] = {tw[j - 1].x * tw[1].x - tw[j - 1].y * tw[1].y, tw[j - 1].x * tw[1].y + tw[j - 1].y * tw[1].x};
             }
             std::vector<int> radix = b200aa_host::radix_list(n);
             if (n == 1) radix.clear();
@@ -88,6 +92,12 @@ int main()
                     b[o] = f64::stockham_output([&](int i) { return a[i]; }, o, n, Ns, R, [&](int i) { return tw[i]; });
                 std::swap(a, b);
                 Ns *= R;
+            }
+            if (strcmp(cmd, "fft")) {
+                printf("S");
+                for (int k = 0; k < n / 2; ++k) pr(f64::magnitude(a[k], n / 2));
+                printf("\n");
+                continue;
             }
             printf("F");
             for (int k = 0; k < n; ++k) pr(a[k].x);
