@@ -538,6 +538,39 @@ int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_feats, cons
                                  const int32_t *h_weights, const uint32_t *h_seeds, int32_t *d_pred, int64_t *d_counts,
                                  void *stream);
 
+/* Kernel 13, regression (csrc/forest.cuh build_regression_tree): scikit-learn 1.9's RandomForestRegressor(n_estimators=T)
+ * .fit with the library's arguments (squared_error, max_features=1.0, bootstrap, no depth limit), tree for tree in bits.
+ *
+ * b200aa_forest_regressor_fit: as b200aa_forest_fit, with h_y float64 [n] finite targets, h_weights int32 [n_trees, n]
+ * required (the bootstrap counts), no classes, kind or max_features, and one float64 value per node in h_values
+ * [node_capacity].  A non-finite target is B200AA_ERR_INVALID; more than 512 features, or a problem whose single tree's
+ * scratch (its sort keys alone take 8 n_feats pow2(n) bytes: at 136 features, n above 131 072) does not fit the 256 MB
+ * scratch bound, B200AA_ERR_UNSUPPORTED; all before any CUDA call.  Returns after the stream drained; it refuses a
+ * capturing stream.
+ * Replaces: RandomForestRegressor.fit in train_random_forest_regression. */
+int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride, const double *h_y,
+                                int n_trees, const int32_t *h_weights, const uint32_t *h_seeds, b200aa_forest_node *h_nodes,
+                                double *h_values, int64_t node_capacity, int64_t *h_node_count, int32_t *h_max_depth,
+                                void *stream);
+
+/* b200aa_forest_regression_cross_validate: the "randomforest" model selection of evaluate_regression, every (parameter,
+ * experiment) problem in one call.  d_X float64 [n, n_feats] C-contiguous on the current device, h_y float64 [n] finite.
+ * The whole matrix is standardised once (kernel 11's scaler: StandardScaler().fit_transform) and cast to float32.
+ * Problem p trains on rows h_train_idx [h_train_off[p], h_train_off[p + 1]) and predicts them and its test rows
+ * h_test_idx [h_test_off[p], h_test_off[p + 1]) with its forest of h_n_trees[p] trees (seeds h_seeds and weights
+ * h_weights int32 [h_n_trees[p], n_train(p)], problems one after another).  The trees of many problems are built in one
+ * launch.  Writes float64 predictions (ForestRegressor.predict: tree values added in tree order, then / T) to d_pred_test
+ * [h_test_off[P]] and d_pred_train [h_train_off[P]], in split order.  Argument checks as b200aa_forest_regressor_fit's,
+ * plus an empty training set, an index outside [0, n) and h_n_trees < 1 are B200AA_ERR_INVALID before any CUDA call
+ * (the scratch bound applies to the largest training set together with the call's fixed arrays).  It refuses a
+ * capturing stream and waits for its stream between launches.
+ * Replaces: the "randomforest" loop of evaluate_regression (train_random_forest_regression and regression_wrapper per
+ * problem). */
+int b200aa_forest_regression_cross_validate(const double *d_X, int64_t n, int n_feats, const double *h_y, int64_t n_problems,
+                                            const int64_t *h_train_off, const int32_t *h_train_idx, const int64_t *h_test_off,
+                                            const int32_t *h_test_idx, const int32_t *h_n_trees, const int32_t *h_weights,
+                                            const uint32_t *h_seeds, double *d_pred_test, double *d_pred_train, void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

@@ -100,6 +100,14 @@ SIGNATURES = {
     #  h_weights, h_seeds, d_pred, d_counts, stream)
     "b200aa_forest_cross_validate": (c_int, [c_vp, c_i64, c_int, c_vp, c_int, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
                                              c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (d_X, dtype, n, n_feats, row_stride, h_y, n_trees, h_weights, h_seeds, h_nodes, h_values, node_capacity,
+    #  h_node_count, h_max_depth, stream)
+    "b200aa_forest_regressor_fit": (c_int, [c_vp, c_int, c_i64, c_int, c_i64, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                            c_vp, c_vp, c_vp]),
+    # (d_X, n, n_feats, h_y, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx, h_n_trees, h_weights, h_seeds,
+    #  d_pred_test, d_pred_train, stream)
+    "b200aa_forest_regression_cross_validate": (c_int, [c_vp, c_i64, c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                        c_vp, c_vp, c_vp, c_vp, c_vp]),
     # float64 path: (d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, stream)
     "b200aa_clip_stats_f64": (c_int, [c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_st_features_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]),

@@ -244,3 +244,145 @@ def train_random_forest(features, labels, n_estimators):
 def train_extra_trees(features, labels, n_estimators):
     """audioTrainTest.train_extra_trees (:202-219), as ``train_random_forest`` with ExtraTreesClassifier."""
     return _train_forest("extratrees", features, labels, n_estimators)
+
+
+# ---- regression: evaluate_regression's "randomforest" branch and train_random_forest_regression ----
+
+def train_random_forest_regression(features, labels, n_estimators):
+    """audioTrainTest.train_random_forest_regression: ``(rf, train_err)`` with rf =
+    RandomForestRegressor(n_estimators).fit(features, labels) trained on the GPU (``consumers.forest_regressor_fit``) tree
+    for tree as scikit-learn trains it, and train_err = np.mean(np.abs(rf.predict(features) - labels)); arguments the
+    trainer does not reproduce (``forests.unsupported_regressor``) or whose trees would exceed its scratch bound
+    (``forests.Unsupported``) go to scikit-learn."""
+    from . import forests
+    from .consumers import forest_regressor_fit
+    X = np.asarray(features) if not isinstance(features, np.ndarray) else features
+    rf = None
+    if forests.unsupported_regressor(X, labels, n_estimators) is None:
+        try:
+            rf = forest_regressor_fit(X, labels, n_estimators)
+        except forests.Unsupported:
+            pass                        # one tree over the scratch bound; NumPy's state is untouched
+    if rf is None:
+        from sklearn.ensemble import RandomForestRegressor
+        rf = RandomForestRegressor(n_estimators=n_estimators).fit(features, labels)
+    train_err = np.mean(np.abs(rf.predict(features) - labels))
+    return rf, train_err
+
+
+def unsupported_regression(features, labels, n_exp, method_name, params):
+    """None when evaluate_regression here reproduces the reference's for these arguments, else the reason it does not."""
+    import sklearn
+    if method_name != "randomforest":
+        return "method %r: only 'randomforest' runs on the GPU" % (method_name,)
+    if not sklearn.__version__.startswith("1.9."):
+        return "scikit-learn %s: the forest trainer restates 1.9.x" % sklearn.__version__
+    if not (isinstance(features, np.ndarray) and features.dtype == np.float64 and features.ndim == 2 and
+            features.flags.c_contiguous and features.shape[0] >= 1 and features.shape[1] >= 1):
+        return "features must be a non-empty C-contiguous float64 matrix (the scaler's column sums follow the layout)"
+    if features.shape[1] > 512:
+        return "more than 512 features: the forest trainer's shared-memory layout"
+    if not np.isfinite(features).all():
+        return "NaN or inf in the features"
+    if not isinstance(labels, np.ndarray) or labels.ndim != 1 or labels.shape[0] != features.shape[0]:
+        return "labels must be a 1-d array with one target per row"
+    if labels.dtype.kind not in "fiub" or not np.isfinite(labels.astype(np.float64)).all():
+        return "labels must be finite numbers"
+    n = labels.shape[0]
+    if int(round(0.9 * n)) == n:
+        return "no test rows (n_train == n): the reference's errors are NaN"
+    if not (isinstance(n_exp, (int, np.integer)) and n_exp >= 1):
+        return "n_exp must be an integer >= 1"
+    for C in params:
+        if not (isinstance(C, (int, np.integer)) and not isinstance(C, bool) and C >= 1):
+            return "every parameter (forest trees) must be an integer >= 1, got %r" % (C,)
+    return None
+
+
+def draw_regression_problems(n, params, n_exp):
+    """(splits, seeds) of every (param, experiment) of evaluate_regression's forest branch, params outer, drawn from
+    NumPy's global RNG in the reference's order: per problem np.random.permutation(range(n)), then the seeds its forest's
+    fit draws.  The first int(round(0.9 n)) rows of the permutation train, the rest test."""
+    from .forests import REGRESSOR, tree_seeds
+    n_train = int(round(0.9 * n))
+    splits, seeds = [], []
+    for C in params:
+        for _ in range(n_exp):
+            randperm = np.random.permutation(range(n))
+            splits.append((randperm[:n_train], randperm[n_train:]))
+            seeds.append(tree_seeds(int(C), REGRESSOR))
+    return splits, seeds
+
+
+def evaluate_regression(features, labels, n_exp, method_name, params):
+    """audioTrainTest.evaluate_regression for method_name "randomforest": the same prints and return value, every
+    (param, experiment) problem's forest trained and its test and training rows predicted on the GPU in one call
+    (``consumers.forest_regression_cross_validate``); the errors and means are the reference's NumPy expressions on the
+    host.  Raises ValueError for arguments it does not cover (``unsupported_regression``), and ``forests.Unsupported``
+    (a ValueError), with NumPy's global state as before the call, when one tree would exceed the trainer's scratch
+    bound."""
+    from .consumers import forest_regression_cross_validate
+    from .forests import Unsupported
+    why = unsupported_regression(features, labels, n_exp, method_name, params)
+    if why is not None:
+        raise ValueError("evaluate_regression on the GPU: " + why)
+    n_samples = labels.shape[0]
+    state = np.random.get_state()
+    splits, seeds = draw_regression_problems(n_samples, params, n_exp)
+    trees = [int(C) for C in params for _ in range(n_exp)]
+    try:
+        pred_test, pred_train = forest_regression_cross_validate(features, labels, splits, seeds, trees)
+    except Unsupported:
+        np.random.set_state(state)
+        raise
+    pred_test, pred_train = pred_test.cpu().numpy(), pred_train.cpu().numpy()
+    errors_all, er_train_all, er_base_all = [], [], []
+    k, o_te, o_tr = 0, 0, 0
+    for C in params:
+        errors, errors_train, errors_baseline = [], [], []
+        for _ in range(n_exp):
+            tr, te = splits[k]
+            k += 1
+            l_train = [labels[i] for i in tr]
+            l_test = [labels[i] for i in te]
+            p_tr, p_te = pred_train[o_tr:o_tr + tr.size], pred_test[o_te:o_te + te.size]
+            o_tr += tr.size
+            o_te += te.size
+            train_err = np.mean(np.abs(p_tr - l_train))
+            error_test, error_test_baseline = [], []
+            for itest in range(te.size):
+                R = p_te[itest]
+                Rbaseline = np.mean(l_train)
+                error_test.append((R - l_test[itest]) * (R - l_test[itest]))
+                error_test_baseline.append((Rbaseline - l_test[itest]) * (Rbaseline - l_test[itest]))
+            errors.append(np.array(error_test).mean())
+            errors_train.append(train_err)
+            errors_baseline.append(np.array(error_test_baseline).mean())
+        errors_all.append(np.array(errors).mean())
+        er_train_all.append(np.array(errors_train).mean())
+        er_base_all.append(np.array(errors_baseline).mean())
+    best_ind = np.argmin(errors_all)
+    print("{0:s}\t\t{1:s}\t\t{2:s}\t\t{3:s}".format("Param", "MSE", "T-MSE", "R-MSE"))
+    for i in range(len(errors_all)):
+        print("{0:.4f}\t\t{1:.2f}\t\t{2:.2f}\t\t{3:.2f}".format(params[i], errors_all[i], er_train_all[i], er_base_all[i]),
+              end="")
+        if i == best_ind:
+            print("\t\t best", end="")
+        print("")
+    return params[best_ind], errors_all[best_ind], er_base_all[best_ind]
+
+
+def regression_dispatcher(original):
+    """An evaluate_regression that runs the arguments the GPU covers here ("randomforest") and hands the rest ("svm",
+    "svm_rbf", anything ``unsupported_regression`` names, and trees over the scratch bound) to `original`."""
+    from .forests import Unsupported
+
+    def evaluate_regression_dispatch(features, labels, n_exp, method_name, params):
+        if unsupported_regression(features, labels, n_exp, method_name, params) is None:
+            try:
+                return evaluate_regression(features, labels, n_exp, method_name, params)
+            except Unsupported:
+                pass                    # NumPy's state is as before the call: the original draws the same problems
+        return original(features, labels, n_exp, method_name, params)
+    evaluate_regression_dispatch.original = original
+    return evaluate_regression_dispatch

@@ -779,6 +779,110 @@ def forest_cross_validate(X, y, splits, seeds, n_estimators, kind, n_classes=Non
     return pred, counts
 
 
+def forest_regressor_fit(X, y, n_estimators):
+    """``RandomForestRegressor(n_estimators).fit(X, y)`` trained on the GPU (``b200aa_forest_regressor_fit``, DESIGN.md
+    kernel 13, regression), tree for tree scikit-learn 1.9's under the same NumPy global state, which it leaves as ``fit``
+    leaves it.  Returns the fitted scikit-learn estimator.
+
+    X: float64 / float32 [n, F] host array (or a CUDA tensor, which is read from the device); y: n finite targets.
+    Raises ValueError with ``forests.unsupported_regressor``'s reason for what it does not reproduce, and
+    ``forests.Unsupported`` (a ValueError), with NumPy's global state as before the call, when one tree's scratch would
+    exceed the trainer's 256 MB bound (at 136 features, more than 131 072 rows); ``train_random_forest_regression`` hands
+    those calls to scikit-learn."""
+    from . import forests as FO
+    Xh = X.detach().cpu().numpy() if isinstance(X, torch.Tensor) else X
+    why = FO.unsupported_regressor(Xh, y, n_estimators)
+    if why is not None:
+        raise ValueError("forest_regressor_fit on the GPU: " + why)
+    n, F = Xh.shape
+    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64) and X.stride(1) == 1:
+        d_X = X                                     # cast to float32 on the device, round to nearest, as fit casts
+    else:
+        d_X = torch.from_numpy(np.ascontiguousarray(Xh, dtype=np.float32)).cuda()
+    T = int(n_estimators)
+    state = np.random.get_state()
+    est, trees, weights, seeds = FO.draw(T, FO.REGRESSOR, n)
+    cap = T * (2 * n - 1)
+    nodes = np.empty(cap, dtype=FO.NODE_DTYPE)
+    values = np.empty(cap, dtype=np.float64)
+    counts = np.empty(T, dtype=np.int64)
+    depth = np.empty(T, dtype=np.int32)
+    y64 = np.ascontiguousarray(y, dtype=np.float64)
+
+    def ptr(a):
+        return ctypes.c_void_p(a.ctypes.data)
+    with torch.cuda.device(d_X.device):
+        status = lib().b200aa_forest_regressor_fit(
+            ctypes.c_void_p(d_X.data_ptr()), DTYPE_F32 if d_X.dtype == torch.float32 else DTYPE_F64, n, F, d_X.stride(0),
+            ptr(y64), T, ptr(weights), ptr(seeds), ptr(nodes), ptr(values), cap, ptr(counts), ptr(depth), _stream())
+    if status == ERR_UNSUPPORTED:
+        np.random.set_state(state)
+        raise FO.Unsupported("forest_regressor_fit on the GPU: one tree of %d rows x %d features needs more scratch than "
+                             "the trainer's 256 MB bound" % (n, F))
+    check(status)
+    states, off = [], 0
+    for t in range(T):
+        nc = int(counts[t])
+        states.append(FO.tree_state(nodes[off:off + nc], values[off:off + nc], depth[t], 1))
+        off += nc
+    return FO.assemble_regressor(est, trees, F, n, states)
+
+
+def forest_regression_cross_validate(X, y, splits, seeds, n_estimators):
+    """The "randomforest" branch of evaluate_regression's model selection as one batch on the GPU
+    (``b200aa_forest_regression_cross_validate``, DESIGN.md kernel 13, regression): StandardScaler().fit_transform of
+    the whole matrix once, then per (train, test) split ``RandomForestRegressor(n_estimators[p]).fit`` on the training
+    rows and predict of the test and training rows, bit for bit scikit-learn's.  The forests stay on the device.
+
+    X: C-contiguous float64 [n, F] (host, or a CUDA tensor); y: n finite targets; splits: (train, test) row indices per
+    problem; seeds: per problem the tree seeds fit would draw (``forests.tree_seeds(T, forests.REGRESSOR)``); n_estimators: the tree
+    count per problem.  Returns CUDA float64 (test predictions [sum of the test counts], training predictions [sum of the
+    training counts]), each problem's rows in its split's order.  Raises ``forests.Unsupported`` when one tree of the
+    largest training set would exceed the trainer's 256 MB scratch bound."""
+    from . import forests as FO
+    if not isinstance(X, torch.Tensor):
+        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, F]")
+    X = X.contiguous()
+    n = X.shape[0]
+    y = np.ascontiguousarray(y.cpu() if isinstance(y, torch.Tensor) else y, dtype=np.float64)
+    if y.shape != (n,) or not np.isfinite(y).all():
+        raise ValueError("y must hold one finite target per row of X")
+    if not len(splits) == len(seeds) == len(n_estimators):
+        raise ValueError("one seed list and one tree count per split")
+    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
+    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
+    train_off, train_idx = _concat_indices(train, np.int32)
+    test_off, test_idx = _concat_indices(test, np.int32)
+    n_trees = np.ascontiguousarray(n_estimators, dtype=np.int32)
+    if any(len(s) != t for s, t in zip(seeds, n_trees)):
+        raise ValueError("every problem needs one seed per tree")
+    ws, rs = [], []
+    for s, tr in zip(seeds, train):
+        w, r = FO.derive(s, FO.REGRESSOR, tr.size)
+        ws.append(w.ravel())
+        rs.append(r)
+    weights = np.ascontiguousarray(np.concatenate(ws), dtype=np.int32)
+    rand_r = np.ascontiguousarray(np.concatenate(rs), dtype=np.uint32)
+    with torch.cuda.device(X.device):
+        pred_test = torch.empty(int(test_off[-1]), dtype=torch.float64, device=X.device)
+        pred_train = torch.empty(int(train_off[-1]), dtype=torch.float64, device=X.device)
+
+        def ptr(a):
+            return ctypes.c_void_p(a.ctypes.data)
+        status = lib().b200aa_forest_regression_cross_validate(
+            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], ptr(y), len(splits), ptr(train_off), ptr(train_idx),
+            ptr(test_off), ptr(test_idx), ptr(n_trees), ptr(weights), ptr(rand_r), ctypes.c_void_p(pred_test.data_ptr()),
+            ctypes.c_void_p(pred_train.data_ptr()), _stream())
+    if status == ERR_UNSUPPORTED:
+        raise FO.Unsupported("forest_regression_cross_validate on the GPU: one tree of %d training rows x %d features "
+                             "needs more scratch than the trainer's 256 MB bound" % (max(t.size for t in train), X.shape[1]))
+    check(status)
+    return pred_test, pred_train
+
+
 def tree_classify_batch(model, vectors):
     """predict / predict_proba of a tree ensemble for every row of a CUDA float32 / float64 [n, F] tensor, in one kernel on
     the current stream (DESIGN.md, kernel 8): CUDA (ids int64 [n], indices into the model's classes_; P float64 [n, C]),

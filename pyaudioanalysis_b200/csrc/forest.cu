@@ -5,6 +5,7 @@
 #include "../../include/b200aa.h"
 #include "entry.h"
 #include "forest.cuh"
+#include "front.cuh"
 #include "knn_cv.cuh"
 
 using namespace b200aa;
@@ -326,6 +327,328 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
         }
         tree0 += T;
         w0 += int64_t(T) * ntr;
+    }
+    return scratch.done(B200AA_OK);
+}
+
+// ------------------------------------------------------------------------------------------------
+// kernel 13, regression: RandomForestRegressor fit, bit for bit scikit-learn 1.9's (csrc/forest.cuh,
+// build_regression_tree), and the forest branch of evaluate_regression's model selection
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// the global scratch of one regression tree of at most n samples: [samples | idx | fv | keys | stack | nodes | values |
+// meta | weights]
+struct RegLayout {
+    size_t samples, idx, fv, keys, stack, nodes, values, meta, weights, bytes;
+};
+RegLayout reg_layout(int64_t n, int F)
+{
+    const int64_t cap = 2 * n - 1;
+    RegLayout L;
+    L.samples = 0;
+    L.idx = L.samples + align256(size_t(n) * 4);
+    L.fv = L.idx + align256(size_t(n) * 4);
+    L.keys = L.fv + align256(size_t(n) * 4);
+    L.stack = L.keys + align256(size_t(F) * size_t(forest::pow2_at_least(n)) * 8);
+    L.nodes = L.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
+    L.values = L.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
+    L.meta = L.values + align256(size_t(cap) * 8);
+    L.weights = L.meta + 256;
+    L.bytes = L.weights + align256(size_t(n) * 4);
+    return L;
+}
+
+// team-shared arrays of build_regression_tree in dynamic shared memory
+inline size_t reg_smem_bytes(int F) { return sizeof(forest::RegShared) + size_t(F) * (5 * 4 + 2 * 4 + 16) + 64; }
+
+// one tree of a launch: its training rows (NULL: rows 0 .. n - 1 of X) and their number
+struct RegJob {
+    const int32_t *rows;
+    int64_t n;
+};
+
+}  // namespace
+
+// One CTA per tree of the launch: build_regression_tree with the block as its team.  Tree i's scratch (its weights
+// included) starts at scratch + i * L.bytes.
+__global__ void __launch_bounds__(forest::kThreads) forest_reg_build_kernel(const float *__restrict__ X,
+                                                                           const double *__restrict__ y, int F,
+                                                                           const RegJob *__restrict__ jobs,
+                                                                           const uint32_t *__restrict__ seeds,
+                                                                           char *__restrict__ scratch, RegLayout L)
+{
+    extern __shared__ __align__(16) unsigned char forest_reg_smem[];
+    const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
+    char *base = scratch + size_t(blockIdx.x) * L.bytes;
+    unsigned char *s = forest_reg_smem;
+    forest::RegShared *st = reinterpret_cast<forest::RegShared *>(s);
+    s += (sizeof(forest::RegShared) + 15) & ~size_t(15);
+    double *vproxy = reinterpret_cast<double *>(s);
+    s += size_t(F) * 8;
+    int64_t *vpos = reinterpret_cast<int64_t *>(s);
+    s += size_t(F) * 8;
+    float *mn = reinterpret_cast<float *>(s);
+    float *mx = mn + F;
+    int32_t *features = reinterpret_cast<int32_t *>(mx + F);
+    int32_t *constf = features + F, *drawn = constf + F, *vis = drawn + F, *tied = vis + F;
+    const RegJob job = jobs[blockIdx.x];
+    const forest::RegTree T{X, y, job.rows, reinterpret_cast<const int32_t *>(base + L.weights), job.n, F,
+                            reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.idx),
+                            reinterpret_cast<float *>(base + L.fv), reinterpret_cast<uint64_t *>(base + L.keys),
+                            reinterpret_cast<forest::StackRec *>(base + L.stack), reinterpret_cast<forest::NodeOut *>(base + L.nodes),
+                            reinterpret_cast<double *>(base + L.values), features, constf, drawn, vis, tied, mn, mx, vproxy,
+                            vpos, st};
+    forest::build_regression_tree(T, tm, seeds[blockIdx.x]);
+    if (threadIdx.x == 0) {
+        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
+        meta[0] = st->node_count;
+        meta[1] = st->max_depth;
+    }
+}
+
+namespace {
+
+bool y_finite(double v) { return v - v == 0.0; }
+
+// trees per launch: as many as keep fixed + trees under the scratch slice bound, or 0 when not even one tree fits (the
+// entry points then refuse with B200AA_ERR_UNSUPPORTED before any CUDA call).  A tree's sort keys take 8 F pow2(n)
+// bytes, so at F = 136 one tree fits for n up to 131 072.
+int64_t reg_slice(size_t fixed, size_t per_tree, int64_t n_trees)
+{
+    if (fixed + per_tree > kScratchSliceBytes) return 0;
+    return std::min<int64_t>(n_trees, int64_t((kScratchSliceBytes - fixed) / per_tree));
+}
+
+}  // namespace
+
+extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride,
+                                           const double *h_y, int n_trees, const int32_t *h_weights,
+                                           const uint32_t *h_seeds, b200aa_forest_node *h_nodes, double *h_values,
+                                           int64_t node_capacity, int64_t *h_node_count, int32_t *h_max_depth,
+                                           void *stream)
+{
+    NvtxRange nvtx_("b200aa_forest_regressor_fit");
+    REFUSE_CAPTURE(stream, "b200aa_forest_regressor_fit", kWhyHostArrays);
+    if (!d_X || !h_y || !h_weights || !h_seeds || !h_nodes || !h_values || !h_node_count || !h_max_depth || n < 1 ||
+        n > (int64_t(1) << 29) || n_feats < 1 || row_stride < n_feats || n_trees < 1 || node_capacity < 0 ||
+        (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
+        return B200AA_ERR_INVALID;
+    for (int64_t i = 0; i < n; ++i)
+        if (!y_finite(h_y[i])) return B200AA_ERR_INVALID;
+    for (int64_t i = 0; i < int64_t(n_trees) * n; ++i)
+        if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
+    const RegLayout L = reg_layout(n, n_feats);
+    const size_t b_x = align256(size_t(n) * n_feats * 4), b_y = align256(size_t(n) * 8), b_seeds = align256(size_t(n_trees) * 4),
+                 b_jobs = align256(size_t(n_trees) * sizeof(RegJob));
+    const size_t fixed = b_x + b_y + b_seeds + b_jobs;
+    const int64_t slice = reg_slice(fixed, L.bytes, n_trees);
+    if (slice < 1) return B200AA_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t smem = reg_smem_bytes(n_feats);
+    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
+    if (rc != B200AA_OK) return rc;
+    char *base = static_cast<char *>(scratch.get());
+    float *Xf = reinterpret_cast<float *>(base);
+    double *y = reinterpret_cast<double *>(base + b_x);
+    uint32_t *seeds = reinterpret_cast<uint32_t *>(base + b_x + b_y);
+    RegJob *jobs = reinterpret_cast<RegJob *>(base + b_x + b_y + b_seeds);
+    char *trees = base + fixed;
+    const unsigned cast_blocks = unsigned(std::min<int64_t>((n * n_feats + 255) / 256, 4096));
+    with_real_type(dtype, [&](auto t) {
+        forest_cast_kernel<<<cast_blocks, 256, 0, st>>>(static_cast<const decltype(t) *>(d_X), n, n_feats, row_stride, Xf);
+    });
+    CK_LAUNCH("forest_cast_kernel");
+    std::vector<RegJob> hjobs(size_t(slice), RegJob{nullptr, n});
+    CK(cudaMemcpyAsync(y, h_y, size_t(n) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(jobs, hjobs.data(), size_t(slice) * sizeof(RegJob), cudaMemcpyHostToDevice, st));
+    int64_t written = 0;
+    std::vector<int64_t> meta(size_t(slice) * 2);
+    for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
+        const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
+        for (int64_t i = 0; i < nt; ++i)
+            CK(cudaMemcpyAsync(trees + size_t(i) * L.bytes + L.weights, h_weights + (t0 + i) * n, size_t(n) * 4,
+                               cudaMemcpyHostToDevice, st));
+        forest_reg_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(Xf, y, n_feats, jobs, seeds + t0, trees, L);
+        CK_LAUNCH("forest_reg_build_kernel");
+        for (int64_t i = 0; i < nt; ++i)
+            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], trees + size_t(i) * L.bytes + L.meta, 16, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (int64_t i = 0; i < nt; ++i) {
+            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
+            h_node_count[t] = nc;
+            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
+            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
+            const char *tb = trees + size_t(i) * L.bytes;
+            CK(cudaMemcpyAsync(h_nodes + written, tb + L.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(h_values + written, tb + L.values, size_t(nc) * 8, cudaMemcpyDeviceToHost, st));
+            written += nc;
+        }
+        CK(cudaStreamSynchronize(st));    // the next slice reuses the scratch the copies read
+    }
+    return scratch.done(B200AA_OK);
+}
+
+// StandardScaler().fit_transform of the whole C-contiguous float64 matrix (kernel 11's front::scaler_fit, rows added in
+// sequence), cast to float32 as fit and predict cast it: one thread per column.
+__global__ void forest_reg_scale_kernel(const double *__restrict__ X, int64_t n, int F, float *__restrict__ Xs)
+{
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    bool inf = false;
+    const knn::Scale sc = front::scaler_fit([&](int64_t i) { return X[i * F + f]; }, n, false, inf);
+    for (int64_t i = 0; i < n; ++i) Xs[i * F + f] = __double2float_rn(knn::standardise(X[i * F + f], sc));
+}
+
+namespace {
+// the prediction of one problem's rows by the trees of one launch: problem p's trees are the launch's trees t0 .. t0+nt-1
+struct RegPredJob {
+    const int32_t *rows;        // the problem's test rows, then its training rows (device)
+    int64_t n_rows, acc_off;    // acc_off: the rows' offset in acc and out
+    int32_t t0, nt, first, last, n_trees;
+};
+}  // namespace
+
+// One thread per (problem, row), blockIdx.y the problem: walk its trees of this launch in tree order (left iff x <=
+// threshold) and add their leaf values to the row's sum (ForestRegressor.predict: out += tree.predict(X)); after the
+// problem's last tree, the sum / n_trees in its place (y_hat /= len(estimators_)).
+__global__ void forest_reg_predict_kernel(const float *__restrict__ Xs, int F, const RegPredJob *__restrict__ pjobs,
+                                          const char *__restrict__ trees, RegLayout L, double *__restrict__ acc)
+{
+    const RegPredJob J = pjobs[blockIdx.y];
+    const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (r >= J.n_rows) return;
+    const float *x = Xs + int64_t(J.rows[r]) * F;
+    double a = J.first ? 0.0 : acc[J.acc_off + r];
+    for (int t = J.t0; t < J.t0 + J.nt; ++t) {
+        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * L.bytes + L.nodes);
+        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * L.bytes + L.values);
+        int32_t i = 0;
+        while (nodes[i].left != forest::kTreeLeaf) i = double(x[nodes[i].feature]) <= nodes[i].threshold ? nodes[i].left : nodes[i].right;
+        a = forest::dadd(a, values[i]);
+    }
+    acc[J.acc_off + r] = J.last ? forest::ddiv(a, double(J.n_trees)) : a;
+}
+
+extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_t n, int n_feats, const double *h_y,
+                                                       int64_t n_problems, const int64_t *h_train_off,
+                                                       const int32_t *h_train_idx, const int64_t *h_test_off,
+                                                       const int32_t *h_test_idx, const int32_t *h_n_trees,
+                                                       const int32_t *h_weights, const uint32_t *h_seeds,
+                                                       double *d_pred_test, double *d_pred_train, void *stream)
+{
+    NvtxRange nvtx_("b200aa_forest_regression_cross_validate");
+    REFUSE_CAPTURE(stream, "b200aa_forest_regression_cross_validate", kWhyHostArrays);
+    if (!d_X || !h_y || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !h_n_trees || !h_weights ||
+        !h_seeds || !d_pred_test || !d_pred_train || n < 1 || n > (int64_t(1) << 29) || n_feats < 1 || n_problems < 1)
+        return B200AA_ERR_INVALID;
+    for (int64_t i = 0; i < n; ++i)
+        if (!y_finite(h_y[i])) return B200AA_ERR_INVALID;
+    if (h_train_off[0] != 0 || h_test_off[0] != 0) return B200AA_ERR_INVALID;
+    int64_t ntr_max = 0, trees_total = 0, weights_total = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
+        if (ntr < 1 || ntr > n || nte < 0 || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
+        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
+            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
+        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
+            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
+        ntr_max = std::max(ntr_max, ntr);
+        trees_total += h_n_trees[p];
+        weights_total += int64_t(h_n_trees[p]) * ntr;
+    }
+    for (int64_t i = 0; i < weights_total; ++i)
+        if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
+    const int F = n_feats;
+    const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems], n_rows = n_tr + n_te;
+    // scratch: [Xs | y | train | rows (test then train, per problem) | acc | seeds | jobs | pjobs | trees of a launch]
+    const RegLayout L = reg_layout(ntr_max, F);
+    const size_t b_xs = align256(size_t(n) * F * 4), b_y = align256(size_t(n) * 8), b_tr = align256(size_t(n_tr) * 4),
+                 b_rows = align256(size_t(n_rows) * 4), b_acc = align256(size_t(std::max<int64_t>(n_rows, 1)) * 8),
+                 b_seeds = align256(size_t(trees_total) * 4), b_jobs = align256(size_t(trees_total) * sizeof(RegJob)),
+                 b_pjobs = align256(size_t(n_problems) * sizeof(RegPredJob));
+    const size_t fixed = b_xs + b_y + b_tr + b_rows + b_acc + b_seeds + b_jobs + b_pjobs;
+    const int64_t slice = std::min<int64_t>(reg_slice(fixed, L.bytes, trees_total), 65535);    // problems per launch: grid y
+    if (slice < 1) return B200AA_ERR_UNSUPPORTED;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t smem = reg_smem_bytes(F);
+    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
+    if (rc != B200AA_OK) return rc;
+    char *q = static_cast<char *>(scratch.get());
+    float *d_xs = reinterpret_cast<float *>(q); q += b_xs;
+    double *d_y = reinterpret_cast<double *>(q); q += b_y;
+    int32_t *d_train = reinterpret_cast<int32_t *>(q); q += b_tr;
+    int32_t *d_rows = reinterpret_cast<int32_t *>(q); q += b_rows;
+    double *d_acc = reinterpret_cast<double *>(q); q += b_acc;
+    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
+    RegJob *d_jobs = reinterpret_cast<RegJob *>(q); q += b_jobs;
+    RegPredJob *d_pjobs = reinterpret_cast<RegPredJob *>(q); q += b_pjobs;
+    char *d_trees = q;
+    // every tree's job, and every problem's rows: its test rows, then its training rows
+    std::vector<RegJob> jobs(static_cast<size_t>(trees_total));
+    std::vector<int32_t> rows(size_t(std::max<int64_t>(n_rows, 1)));
+    std::vector<int64_t> tree0(size_t(n_problems) + 1, 0), w0(size_t(n_problems) + 1, 0), row0(size_t(n_problems) + 1, 0);
+    std::vector<int32_t> prob_of(static_cast<size_t>(trees_total));
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
+        for (int32_t t = 0; t < h_n_trees[p]; ++t) {
+            jobs[size_t(tree0[p] + t)] = RegJob{d_train + h_train_off[p], ntr};
+            prob_of[size_t(tree0[p] + t)] = int32_t(p);
+        }
+        std::copy(h_test_idx + h_test_off[p], h_test_idx + h_test_off[p + 1], rows.begin() + row0[p]);
+        std::copy(h_train_idx + h_train_off[p], h_train_idx + h_train_off[p + 1], rows.begin() + row0[p] + nte);
+        tree0[p + 1] = tree0[p] + h_n_trees[p];
+        w0[p + 1] = w0[p] + int64_t(h_n_trees[p]) * ntr;
+        row0[p + 1] = row0[p] + nte + ntr;
+    }
+    CK(cudaMemcpyAsync(d_y, h_y, size_t(n) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_train, h_train_idx, size_t(n_tr) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_rows, rows.data(), size_t(n_rows) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_seeds, h_seeds, size_t(trees_total) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_jobs, jobs.data(), size_t(trees_total) * sizeof(RegJob), cudaMemcpyHostToDevice, st));
+    forest_reg_scale_kernel<<<unsigned((F + 63) / 64), 64, 0, st>>>(d_X, n, F, d_xs);
+    CK_LAUNCH("forest_reg_scale_kernel");
+    // launches of up to `slice` consecutive trees over the problems' trees in order; after each, every problem with trees
+    // in it adds their predictions, in tree order
+    std::vector<RegPredJob> pj(static_cast<size_t>(n_problems));
+    for (int64_t g0 = 0; g0 < trees_total; g0 += slice) {
+        const int64_t nt = std::min<int64_t>(slice, trees_total - g0);
+        for (int64_t i = 0; i < nt; ++i) {
+            const int64_t g = g0 + i, p = prob_of[size_t(g)];
+            const int64_t ntr = h_train_off[p + 1] - h_train_off[p];
+            CK(cudaMemcpyAsync(d_trees + size_t(i) * L.bytes + L.weights, h_weights + w0[p] + (g - tree0[p]) * ntr,
+                               size_t(ntr) * 4, cudaMemcpyHostToDevice, st));
+        }
+        forest_reg_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(d_xs, d_y, F, d_jobs + g0, d_seeds + g0,
+                                                                            d_trees, L);
+        CK_LAUNCH("forest_reg_build_kernel");
+        int np = 0;
+        int64_t max_rows = 0;
+        for (int64_t p = prob_of[size_t(g0)]; p < n_problems && tree0[p] < g0 + nt; ++p) {
+            const int64_t a = std::max(tree0[p], g0), b = std::min(tree0[p + 1], g0 + nt);
+            const int64_t nr = row0[p + 1] - row0[p];
+            pj[size_t(np++)] = RegPredJob{d_rows + row0[p], nr, row0[p], int32_t(a - g0), int32_t(b - a), a == tree0[p],
+                                          b == tree0[p + 1], h_n_trees[p]};
+            max_rows = std::max(max_rows, nr);
+        }
+        CK(cudaMemcpyAsync(d_pjobs, pj.data(), size_t(np) * sizeof(RegPredJob), cudaMemcpyHostToDevice, st));
+        forest_reg_predict_kernel<<<dim3(unsigned((max_rows + 127) / 128), unsigned(np)), 128, 0, st>>>(
+            d_xs, F, d_pjobs, d_trees, L, d_acc);
+        CK_LAUNCH("forest_reg_predict_kernel");
+        CK(cudaStreamSynchronize(st));    // the next launch reuses the scratch and the host job arrays
+    }
+    // every problem's rows: test rows to d_pred_test, training rows to d_pred_train, from the final sums' quotients
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t nte = h_test_off[p + 1] - h_test_off[p], ntr = h_train_off[p + 1] - h_train_off[p];
+        if (nte) CK(cudaMemcpyAsync(d_pred_test + h_test_off[p], d_acc + row0[p], size_t(nte) * 8, cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync(d_pred_train + h_train_off[p], d_acc + row0[p] + nte, size_t(ntr) * 8, cudaMemcpyDeviceToDevice, st));
     }
     return scratch.done(B200AA_OK);
 }

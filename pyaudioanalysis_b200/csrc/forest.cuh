@@ -188,12 +188,16 @@ struct Team {
 
 // Thread 0: the Fisher-Yates draw loop of node_split_best / node_split_random.  Writes the drawn non-constant features in
 // visit order to drawn[] (and, for the random splitter, each one's threshold to thr[]), keeps features / constf as
-// scikit-learn's splitter keeps them across nodes, and returns the node's n_total_constants.
+// scikit-learn's splitter keeps them across nodes, and returns the node's n_total_constants.  With `visited`, it also
+// writes every feature the best splitter sorts, in visit order: the drawn non-constant ones and the ones found constant
+// (not those drawn from the known-constant range), and their number to n_visited_out (the regressor needs the sort order
+// each of them leaves).
 __host__ __device__ inline int64_t draw_features(int32_t *features, int32_t *constf, int F, int max_features, int kind,
                                                  int64_t n_known, const float *mn, const float *mx, uint32_t &rng,
-                                                 int32_t *drawn, double *thr, int64_t &n_drawn)
+                                                 int32_t *drawn, double *thr, int64_t &n_drawn,
+                                                 int32_t *visited = nullptr, int64_t *n_visited_out = nullptr)
 {
-    int64_t f_i = F, n_found = 0, n_drawn_c = 0, n_total = n_known, n_visited = 0;
+    int64_t f_i = F, n_found = 0, n_drawn_c = 0, n_total = n_known, n_visited = 0, n_sorted = 0;
     n_drawn = 0;
     while (f_i > n_total && (n_visited < max_features || n_visited <= n_found + n_drawn_c)) {
         ++n_visited;
@@ -207,6 +211,7 @@ __host__ __device__ inline int64_t draw_features(int32_t *features, int32_t *con
         }
         f_j += n_found;
         const int32_t cur = features[f_j];
+        if (visited) visited[n_sorted++] = cur;
         if (is_constant(mn[cur], mx[cur])) {
             features[f_j] = features[n_total];
             features[n_total] = cur;
@@ -227,6 +232,7 @@ __host__ __device__ inline int64_t draw_features(int32_t *features, int32_t *con
     }
     for (int64_t i = 0; i < n_known; ++i) features[i] = constf[i];
     for (int64_t i = 0; i < n_found; ++i) constf[n_known + i] = features[n_known + i];
+    if (n_visited_out) *n_visited_out = n_sorted;
     return n_total;
 }
 
@@ -508,6 +514,467 @@ __host__ __device__ inline void build_tree(const Tree &T, const Team &tm, uint32
                 else T.nodes[rec.parent].right = int32_t(id);
             }
             for (int c = 0; c < T.C; ++c) T.values[id * T.C + c] = ddiv(double(S.total[c]), S.wn);
+            if (rec.depth > S.max_depth) S.max_depth = rec.depth;
+        }
+        tm.sync();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Regression: RandomForestRegressor(n_estimators=T).fit with the library's arguments (criterion="squared_error",
+// max_features=1.0, bootstrap, min_samples_split=2, min_samples_leaf=1, no depth limit), node for node, bit for bit.
+//
+// A regressor's node sums are float64 sums of w * y, so they depend on the order of samples[start:end] at every step,
+// and that order is the one scikit-learn's splitter leaves:
+//   - node_split_best sorts every visited feature's values in place together with samples[start:end] by introsort_3way
+//     (utils/_sorting.pyx simultaneous_sort, use_three_way_partition=True), each sort starting from the order the
+//     previous one left ("visited" includes a feature then found constant, not one drawn from the known-constant range);
+//   - partition_samples_final, a swap partition, starts from the order the last visited feature left.
+// Where a feature's values in the node are pairwise different (-0 == +0 counts as equal), the sorted order is unique and
+// any sort gives it; otherwise introsort_3way is replayed from the order it starts from.
+//
+// The criterion (tree/_criterion.pyx RegressionCriterion / MSE), every sum sequential in the samples' order:
+//   init:    sum_total += w*y, sq_sum_total += (w*y)*y, weighted_n += w over samples[start:end]
+//   update(new_pos), called only at candidate positions: forward (sum_left += w*y from pos) when new_pos - pos <=
+//            end - new_pos, else reverse_reset (sum_left = sum_total) and sum_left -= w*y from end - 1 down to new_pos
+//   proxy:   sl*sl / wl + sr*sr / wr, sr = sum_total - sl
+//   after the best split: the partition, reset, update(best.pos) over the partitioned order, children_impurity
+//            (sq_sum_left += (w*y)*y over samples[start:pos]) and impurity_improvement.
+// Node values are sum_total / weighted_n.  The leaf tests use tree/_tree.pyx's EPSILON = np.finfo('double').eps.
+//
+// build_regression_tree() runs it for a team of threads.  Per node: the node's sums (thread 0, in order); every feature's
+// min / max; the Fisher-Yates draw (draw_features, recording the visits); every visit's (value, sample) keys sorted at
+// once by one batched bitonic sort (team-parallel); ties detected (team-parallel); thread 0 replays introsort_3way, in
+// visit order, for the visits with ties only; one candidate chain per visit, each on its own thread; thread 0 takes the
+// first strict maximum in (visit order, position), partitions, and computes the children's impurities.
+constexpr double kLeafEpsilon = DBL_EPSILON;                // EPSILON of tree/_tree.pyx
+
+// ---- introsort_3way (utils/_sorting.pyx), on float32 values with int32 sample indices ----
+__host__ __device__ inline void sort_swap(float *v, int32_t *ix, int64_t i, int64_t j)
+{
+    const float tv = v[i];
+    v[i] = v[j];
+    v[j] = tv;
+    const int32_t ti = ix[i];
+    ix[i] = ix[j];
+    ix[j] = ti;
+}
+__host__ __device__ inline float median3(const float *v, int64_t n)
+{
+    const float a = v[0], b = v[n / 2], c = v[n - 1];
+    if (a < b) {
+        if (b < c) return b;
+        if (a < c) return c;
+        return a;
+    }
+    if (b < c) {
+        if (a < c) return a;
+        return c;
+    }
+    return b;
+}
+__host__ __device__ inline void insertion_sort(float *v, int32_t *ix, int64_t n)
+{
+    for (int64_t i = 1; i < n; ++i) {
+        const float tv = v[i];
+        const int32_t ti = ix[i];
+        int64_t j = i;
+        while (j > 0 && v[j - 1] > tv) {
+            v[j] = v[j - 1];
+            ix[j] = ix[j - 1];
+            --j;
+        }
+        v[j] = tv;
+        ix[j] = ti;
+    }
+}
+__host__ __device__ inline void sift_down(float *v, int32_t *ix, int64_t start, int64_t end)
+{
+    int64_t root = start;
+    while (true) {
+        const int64_t child = root * 2 + 1;
+        int64_t maxind = root;
+        if (child < end && v[maxind] < v[child]) maxind = child;
+        if (child + 1 < end && v[maxind] < v[child + 1]) maxind = child + 1;
+        if (maxind == root) break;
+        sort_swap(v, ix, root, maxind);
+        root = maxind;
+    }
+}
+__host__ __device__ inline void heapsort(float *v, int32_t *ix, int64_t n)
+{
+    int64_t start = (n - 2) / 2, end = n;        // n > 15 here: C's and Python's integer division agree
+    while (true) {
+        sift_down(v, ix, start, end);
+        if (start == 0) break;
+        --start;
+    }
+    end = n - 1;
+    while (end > 0) {
+        sort_swap(v, ix, 0, end);
+        sift_down(v, ix, 0, end);
+        --end;
+    }
+}
+// floor(log2(n)) for n >= 1.  simultaneous_sort takes maxd = 2 * (intp)log2(n) with libm's log2; for n < 2^29 they agree:
+// log2(n) is exact at a power of two, and otherwise lies in (k, k + 1) at least log2(2^(k+1)) - log2(2^(k+1) - 1) >
+// 2^-(k+1) / ln 2 >= 2^-29 / ln 2 ~ 2.7e-9 below k + 1, a gap a million times an ulp of a number below 32 (3.6e-15), so
+// a log2 correct to within an ulp cannot reach k + 1 and truncates to k.
+__host__ __device__ inline int64_t floor_log2(int64_t n)
+{
+    int64_t k = 0;
+    while ((n >> (k + 1)) != 0) ++k;
+    return k;
+}
+// simultaneous_sort(values, indices, n, use_three_way_partition=True).  introsort_3way recurses on the left part and
+// loops on the right one; the parts are disjoint and each one's sort depends only on its own contents and depth budget,
+// so an explicit stack of pending (offset, length, maxd) parts gives the same result.  Pending parts <= the initial maxd.
+__host__ __device__ inline void introsort_3way(float *v, int32_t *ix, int64_t n)
+{
+    if (n == 0) return;
+    struct Part {
+        int64_t off, n, maxd;
+    };
+    Part stack[64];
+    int top = 0;
+    stack[top++] = Part{0, n, 2 * floor_log2(n)};
+    while (top > 0) {
+        Part p = stack[--top];
+        float *pv = v + p.off;
+        int32_t *pi = ix + p.off;
+        bool done = false;
+        while (p.n > 15) {
+            if (p.maxd <= 0) {
+                heapsort(pv, pi, p.n);
+                done = true;
+                break;
+            }
+            --p.maxd;
+            const float pivot = median3(pv, p.n);
+            int64_t i = 0, l = 0, r = p.n;
+            while (i < r) {
+                if (pv[i] < pivot) {
+                    sort_swap(pv, pi, i, l);
+                    ++i;
+                    ++l;
+                } else if (pv[i] > pivot) {
+                    --r;
+                    sort_swap(pv, pi, i, r);
+                } else {
+                    ++i;
+                }
+            }
+            stack[top++] = Part{p.off, l, p.maxd};
+            p.off += r;
+            pv += r;
+            pi += r;
+            p.n -= r;
+        }
+        if (!done) insertion_sort(pv, pi, p.n);
+    }
+}
+
+// partition_samples_final (tree/_partitioner.pyx): the swap partition of samples[0, m) by x <= threshold
+template <class Xf>
+__host__ __device__ inline void swap_partition(int32_t *samples, int64_t m, const Xf &x, double threshold)
+{
+    int64_t ps = 0, pe = m;
+    while (ps < pe) {
+        if (double(x(samples[ps])) <= threshold) {
+            ++ps;
+        } else {
+            --pe;
+            const int32_t t = samples[ps];
+            samples[ps] = samples[pe];
+            samples[pe] = t;
+        }
+    }
+}
+
+struct RegShared {
+    int64_t node_count, max_depth, n_vis, n_drawn, n_const_out, best_pos;
+    double best_proxy, best_thr, imp, wn, w_total, sum_total, sq_total, imp_left, imp_right;
+    int32_t best_v, best_f, best_missing_left, leaf, stack_top;
+    uint32_t rng;
+};
+
+// Everything one regression tree reads and writes.  Global: X [rows, F] and y [rows] (shared by every tree; rows[s] is
+// local sample s's row, or s when rows is NULL), w [n] (bootstrap counts), samples / idx [n] and fv [n] (the replay's
+// indices and values), keys [F * pow2_at_least(n)], stack [n + 1], nodes [2 n - 1], values [2 n - 1].  Team-shared:
+// features / constf / drawn / vis / tied [F], mn / mx [F], vproxy / vpos [F] and st.
+struct RegTree {
+    const float *X;
+    const double *y;
+    const int32_t *rows, *w;
+    int64_t n;
+    int F;
+    int32_t *samples, *idx;
+    float *fv;
+    uint64_t *keys;
+    StackRec *stack;
+    NodeOut *nodes;
+    double *values;
+    int32_t *features, *constf, *drawn, *vis, *tied;
+    float *mn, *mx;
+    double *vproxy;
+    int64_t *vpos;
+    RegShared *st;
+    __host__ __device__ int64_t row(int32_t s) const { return rows ? int64_t(rows[s]) : int64_t(s); }
+    __host__ __device__ float x(int32_t s, int f) const { return X[row(s) * F + f]; }
+    __host__ __device__ double yv(int32_t s) const { return y[row(s)]; }
+    __host__ __device__ double wv(int32_t s) const { return double(w[s]); }
+};
+
+__host__ __device__ inline uint64_t reg_key(float v, int32_t s) { return (uint64_t(order_bits(v)) << 32) | uint32_t(s); }
+__host__ __device__ inline float key_value(uint64_t k) { return from_order_bits(uint32_t(k >> 32)); }
+__host__ __device__ inline int32_t key_sample(uint64_t k) { return int32_t(uint32_t(k)); }
+
+// The regressor's criterion at a split position of one sample order: sum_left and weighted_n_left after reset and
+// update(pos) from the current (pos0, sl, wl), forward or from the end as RegressionCriterion.update chooses.
+template <class Sample>
+__host__ __device__ inline void reg_update(const RegTree &T, const Sample &sample, int64_t m, double sum_total, double wn,
+                                           int64_t &pos, double &sl, double &wl, int64_t new_pos)
+{
+    if (new_pos - pos <= m - new_pos) {
+        for (int64_t p = pos; p < new_pos; ++p) {
+            const int32_t s = sample(p);
+            const double w = T.wv(s);
+            sl = dadd(sl, dmul(w, T.yv(s)));
+            wl = dadd(wl, w);
+        }
+    } else {
+        sl = sum_total;                 // reverse_reset
+        wl = wn;
+        for (int64_t p = m - 1; p >= new_pos; --p) {
+            const int32_t s = sample(p);
+            const double w = T.wv(s);
+            sl = dsub(sl, dmul(w, T.yv(s)));
+            wl = dsub(wl, w);
+        }
+    }
+    pos = new_pos;
+}
+// MSE.proxy_impurity_improvement
+__host__ __device__ inline double reg_proxy(double sl, double wl, double sr, double wr)
+{
+    return dadd(ddiv(dadd(0.0, dmul(sl, sl)), wl), ddiv(dadd(0.0, dmul(sr, sr)), wr));
+}
+__host__ __device__ inline double square(double a) { return dmul(a, a); }     // Cython's a ** 2.0 folds to a * a
+
+// One visit's candidate chain over its sorted keys K[0, m): the first strict maximum of the proxy, or bq = -1 when the
+// feature has no candidate.
+__host__ __device__ inline void reg_chain(const RegTree &T, const uint64_t *K, int64_t m, double sum_total, double wn,
+                                          double &bp, int64_t &bq)
+{
+    const auto sample = [K](int64_t p) { return key_sample(K[p]); };
+    int64_t pos = 0;
+    double sl = 0.0, wl = 0.0;                 // reset
+    bp = -INFINITY;
+    bq = -1;
+    float prev = key_value(K[0]);
+    for (int64_t q = 1; q < m; ++q) {
+        const float cur = key_value(K[q]);
+        if (is_candidate(prev, cur)) {
+            reg_update(T, sample, m, sum_total, wn, pos, sl, wl, q);
+            const double proxy_q = reg_proxy(sl, wl, dsub(sum_total, sl), dsub(wn, wl));
+            if (proxy_q > bp) {
+                bp = proxy_q;
+                bq = q;
+            }
+        }
+        prev = cur;
+    }
+}
+
+// The whole tree: DepthFirstTreeBuilder.build with the regressor's parameters.  rand_r_seed: the splitter's
+// rand_r_state.  Writes nodes / values (one per node) and st->node_count, st->max_depth.
+__host__ __device__ inline void build_regression_tree(const RegTree &T, const Team &tm, uint32_t rand_r_seed)
+{
+    RegShared &S = *T.st;
+    if (tm.tid == 0) {
+        int64_t j = 0, wt = 0;
+        for (int64_t i = 0; i < T.n; ++i) {
+            if (T.w[i] != 0) T.samples[j++] = int32_t(i);
+            wt += T.w[i];
+        }
+        S.w_total = double(wt);
+        S.rng = rand_r_seed;
+        S.node_count = 0;
+        S.max_depth = -1;
+        S.stack_top = 1;
+        T.stack[0] = StackRec{0, int32_t(j), 0, kTreeUndefined, 0, 0, INFINITY};
+    }
+    for (int f = tm.tid; f < T.F; f += tm.n) T.features[f] = f;
+    tm.sync();
+    bool first = true;
+    while (S.stack_top > 0) {
+        const StackRec rec = T.stack[S.stack_top - 1];
+        tm.sync();
+        const int64_t lo = rec.start, hi = rec.end, m = hi - lo;
+        int32_t *smp = T.samples + lo;
+        if (tm.tid == 0) {
+            S.stack_top -= 1;
+            // node_reset -> criterion.init, in the node's current order
+            double st_ = 0.0, sq = 0.0, wn = 0.0;
+            for (int64_t p = 0; p < m; ++p) {
+                const int32_t s = smp[p];
+                const double w = T.wv(s), wy = dmul(w, T.yv(s));
+                st_ = dadd(st_, wy);
+                sq = dadd(sq, dmul(wy, T.yv(s)));
+                wn = dadd(wn, w);
+            }
+            S.sum_total = st_;
+            S.sq_total = sq;
+            S.wn = wn;
+            S.imp = first ? dsub(ddiv(sq, wn), square(ddiv(st_, wn))) : rec.impurity;
+            S.best_proxy = -INFINITY;
+            S.best_v = -1;
+            S.n_vis = 0;
+            S.leaf = m < 2 || S.imp <= kLeafEpsilon;
+        }
+        first = false;
+        tm.sync();
+        if (!S.leaf) {
+            for (int f = tm.tid; f < T.F; f += tm.n) {
+                float a = T.x(smp[0], f), b = a;
+                for (int64_t p = 1; p < m; ++p) {
+                    const float v = T.x(smp[p], f);
+                    if (v < a) a = v;
+                    else if (v > b) b = v;
+                }
+                T.mn[f] = a;
+                T.mx[f] = b;
+            }
+            tm.sync();
+            if (tm.tid == 0) {
+                int64_t nd = 0, nv = 0;
+                S.n_const_out = draw_features(T.features, T.constf, T.F, T.F, kBest, rec.n_const, T.mn, T.mx, S.rng, T.drawn,
+                                              nullptr, nd, T.vis, &nv);
+                S.n_drawn = nd;
+                S.n_vis = nv;
+            }
+            tm.sync();
+            const int64_t nv = S.n_vis, m2 = pow2_at_least(m);
+            // every visit's keys, sorted at once: segment v is keys[v m2, (v + 1) m2), padded with keys above any value
+            for (int64_t i = tm.tid; i < nv * m2; i += tm.n) {
+                const int64_t v = i / m2, q = i - v * m2;
+                T.keys[i] = q < m ? reg_key(T.x(smp[q], T.vis[v]), smp[q]) : ~uint64_t(0);
+            }
+            for (int64_t v = tm.tid; v < nv; v += tm.n) T.tied[v] = 0;
+            tm.sync();
+            for (int64_t kk = 2; kk <= m2; kk <<= 1) {
+                for (int64_t j = kk >> 1; j > 0; j >>= 1) {
+                    for (int64_t i = tm.tid; i < nv * m2; i += tm.n) {
+                        const int64_t q = i & (m2 - 1), l = q ^ j;
+                        if (l > q) {
+                            uint64_t *seg = T.keys + (i - q);
+                            const uint64_t a = seg[q], b = seg[l];
+                            if ((a > b) == ((q & kk) == 0)) {
+                                seg[q] = b;
+                                seg[l] = a;
+                            }
+                        }
+                    }
+                    tm.sync();
+                }
+            }
+            for (int64_t i = tm.tid; i < nv * m; i += tm.n) {
+                const int64_t v = i / m, q = i - v * m;
+                if (q >= 1 && key_value(T.keys[v * m2 + q - 1]) == key_value(T.keys[v * m2 + q])) T.tied[v] = 1;
+            }
+            tm.sync();
+            // introsort_3way replayed for the visits with ties, in visit order, each from the order the one before left
+            if (tm.tid == 0) {
+                for (int64_t v = 0; v < nv; ++v) {
+                    if (!T.tied[v]) continue;
+                    const int f = T.vis[v];
+                    for (int64_t q = 0; q < m; ++q) {
+                        const int32_t s = v == 0 ? smp[q] : key_sample(T.keys[(v - 1) * m2 + q]);
+                        T.idx[q] = s;
+                        T.fv[q] = T.x(s, f);
+                    }
+                    introsort_3way(T.fv, T.idx, m);
+                    for (int64_t q = 0; q < m; ++q) T.keys[v * m2 + q] = reg_key(T.fv[q], T.idx[q]);
+                }
+            }
+            tm.sync();
+            // one candidate chain per visit; a visit found constant has no candidate
+            for (int64_t v = tm.tid; v < nv; v += tm.n) {
+                const int f = T.vis[v];
+                double bp = -INFINITY;
+                int64_t bq = -1;
+                if (!is_constant(T.mn[f], T.mx[f])) reg_chain(T, T.keys + v * m2, m, S.sum_total, S.wn, bp, bq);
+                T.vproxy[v] = bp;
+                T.vpos[v] = bq;
+            }
+            tm.sync();
+            if (tm.tid == 0) {
+                for (int64_t v = 0; v < nv; ++v)
+                    if (T.vpos[v] >= 0 && T.vproxy[v] > S.best_proxy) {
+                        const uint64_t *K = T.keys + v * m2;
+                        const int64_t q = T.vpos[v];
+                        S.best_proxy = T.vproxy[v];
+                        S.best_v = int32_t(v);
+                        S.best_f = T.vis[v];
+                        S.best_pos = q;
+                        S.best_thr = mid_threshold(key_value(K[q - 1]), key_value(K[q]));
+                        S.best_missing_left = q > m - q;
+                    }
+                if (S.best_v < 0) {
+                    S.leaf = 1;
+                } else {
+                    // partition_samples_final from the order the last visit left, then reset, update(best.pos) and
+                    // children_impurity over the partitioned order
+                    for (int64_t q = 0; q < m; ++q) smp[q] = key_sample(T.keys[(nv - 1) * m2 + q]);
+                    const int bf = S.best_f;
+                    swap_partition(smp, m, [&T, bf](int32_t s) { return T.x(s, bf); }, S.best_thr);
+                    const int64_t pos = S.best_pos;
+                    int64_t p0 = 0;
+                    double sl = 0.0, wl = 0.0;
+                    reg_update(T, [smp](int64_t p) { return smp[p]; }, m, S.sum_total, S.wn, p0, sl, wl, pos);
+                    double sq_left = 0.0;
+                    for (int64_t p = 0; p < pos; ++p) {
+                        const int32_t s = smp[p];
+                        sq_left = dadd(sq_left, dmul(dmul(T.wv(s), T.yv(s)), T.yv(s)));
+                    }
+                    const double wr = dsub(S.wn, wl), sr = dsub(S.sum_total, sl);
+                    const double gl = dsub(ddiv(sq_left, wl), square(ddiv(sl, wl)));
+                    const double gr = dsub(ddiv(dsub(S.sq_total, sq_left), wr), square(ddiv(sr, wr)));
+                    const double impr = improvement(S.w_total, S.wn, S.imp, wl, gl, wr, gr);
+                    S.leaf = dadd(impr, kLeafEpsilon) < 0.0;
+                    if (!S.leaf) {
+                        const int32_t ps = int32_t(lo + pos), d = rec.depth + 1, id = int32_t(S.node_count);
+                        const int32_t nc = int32_t(S.n_const_out);
+                        T.stack[S.stack_top++] = StackRec{ps, int32_t(hi), d, id, 0, nc, gr};
+                        T.stack[S.stack_top++] = StackRec{int32_t(lo), ps, d, id, 1, nc, gl};
+                    }
+                }
+            }
+            tm.sync();
+        }
+        if (tm.tid == 0) {
+            const int64_t id = S.node_count++;
+            NodeOut &o = T.nodes[id];
+            o.n_samples = int32_t(m);
+            o.impurity = S.imp;
+            o.weighted = S.wn;
+            o.pad = 0;
+            if (S.leaf) {
+                o.left = o.right = kTreeLeaf;
+                o.feature = kTreeUndefined;
+                o.threshold = double(kTreeUndefined);
+                o.missing_left = 0;
+            } else {
+                o.left = o.right = 0;
+                o.feature = S.best_f;
+                o.threshold = S.best_thr;
+                o.missing_left = S.best_missing_left;
+            }
+            if (rec.parent != kTreeUndefined) {
+                if (rec.is_left) T.nodes[rec.parent].left = int32_t(id);
+                else T.nodes[rec.parent].right = int32_t(id);
+            }
+            T.values[id] = ddiv(S.sum_total, S.wn);
             if (rec.depth > S.max_depth) S.max_depth = rec.depth;
         }
         tm.sync();

@@ -38,8 +38,10 @@ def install_training(audio_train_test=None):
     and non-finite input through the saved original.  extract_features_and_train looks the function up on the module at
     call time (audioTrainTest.py:309), so it trains kNN models through the GPU unchanged.  train_random_forest and
     train_extra_trees, where the module has them, are rebound to the GPU trainers here (kernel 13): the final forest
-    extract_features_and_train fits and pickles is built on the GPU, tree for tree scikit-learn's.  Returns the
-    attributes rebound."""
+    extract_features_and_train fits and pickles is built on the GPU, tree for tree scikit-learn's.  Likewise, where the
+    module has them, evaluate_regression (its "randomforest" model selection on the GPU, every other method through the
+    saved original) and train_random_forest_regression, so feature_extraction_train_regression selects and fits its
+    forest on the GPU.  Returns the attributes rebound."""
     from .audioTrainTest import dispatcher
     if audio_train_test is None:
         import importlib
@@ -53,6 +55,15 @@ def install_training(audio_train_test=None):
             continue
         _saved.setdefault((audio_train_test, n), getattr(audio_train_test, n))
         setattr(audio_train_test, n, getattr(ours, n))
+        done.append("%s.%s" % (audio_train_test.__name__, n))
+    if hasattr(audio_train_test, "evaluate_regression"):
+        original = _saved.setdefault((audio_train_test, "evaluate_regression"), audio_train_test.evaluate_regression)
+        audio_train_test.evaluate_regression = ours.regression_dispatcher(original)
+        done.append("%s.evaluate_regression" % audio_train_test.__name__)
+    if hasattr(audio_train_test, "train_random_forest_regression"):
+        n = "train_random_forest_regression"
+        _saved.setdefault((audio_train_test, n), getattr(audio_train_test, n))
+        setattr(audio_train_test, n, ours.train_random_forest_regression)
         done.append("%s.%s" % (audio_train_test.__name__, n))
     return done
 
