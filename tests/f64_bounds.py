@@ -45,6 +45,38 @@ within the ball (full frames) or per-bin eps (clipped frames), c_j' - c_j = sum_
 (``f64_chroma``: each class adds X^2 / share of its taps in sequence, gamma64(taps + 2); E is NumPy's pairwise sum,
 gamma64(pairwise_depth(K)); one IEEE division, u) and the same stage of the reference (X^2, the matrix product over the
 same taps with 1 / share rounded, np.sum, the division): twice the stage.
+
+**Feature rows** (``feature_bounds64``).  X' (kernel) lies in the ball |X' - X|_2 <= e of ``spectrum_bound``; the bound of
+each entry is the largest change of the reference's exact formula over the ball, plus kernel 12's float64 stage and the
+reference's (both sides' roundings counted, so no "2 x" hides in a constant).  pK = pairwise_depth(K).
+* Rows 0-1: bit for bit (bound 0).  Row 2: the samples are exact, so only the stage: s_j = B_j / (E + eps) off by
+  gamma64(pairwise_depth(w / 10)) + gamma64(pairwise_depth(w)) + 2 u per side, then ``_entropy64``: the mean value
+  theorem on h(s) = -s log2(s + eps), the logs (1 ulp CUDA, 4 ulp NumPy's SIMD loops), the products and 10-term sums.
+* Row 3: with ind = fl((k + 1) fs / 2K) (the same double on both sides), cen = N / Dn, N = sum ind X, Dn = S + eps top,
+  top = max X.  top moves by at most e, S by sqrt(K) e, so |cen' - cen| <= (|ind - cen|_2 e + cen eps e) / (Dn - sqrt(K) e
+  - eps e), plus gamma64(2 pK + 6) cen per side.  Row 4: V = sum (ind - c)^2 X / Dn at the computed centroid c (within
+  dc of row 3's): V moves by (|w|_2 e + V eps e) / Dn_lo, w_k = |(ind_k - c)^2 - V| + 2 |ind_k - c| dc + dc^2 + dVc,
+  dVc = dc (dc S + 2 cen eps top) / Dn the change of V with c; the stage adds u |ind - c| per rounded difference and
+  gamma64(2 pK + 8) V; then sqrt over [V - dV, V + dV] and the roundings of sqrt and / (fs / 2).
+* Row 5: X'^2 - X^2 = 2 X d + d^2, so s_j moves by (2 |(1_Bj - s_j) X|_2 e + max |1_Bj - s_j| e^2) / (E + eps - 2 |X|_2 e
+  - e^2), then ``_entropy64``.  Row 6: sqrt(flux) = |X / Sn - Xp / Snp|_2, Sn = S + K eps; each side moves by (e + |X /
+  Sn|_2 sqrt(K) e) / (Sn - sqrt(K) e) =: D, so flux moves by (Dt + Dp)(2 sqrt(flux) + Dt + Dp); the stage's rounded
+  difference errs by gamma64(pK + 2)(|a_k| + |b_k|) + u |a_k - b_k| per bin, carried through the squares and the sum.
+* Row 7: g_k = cumsum_k(X^2) + eps - 0.9 E has weights 1[j <= k] - 0.9 on X^2: it moves by 2 (0.01 C_k + 0.81 (E -
+  C_k))^(1/2) e + 0.9 e^2, plus per side gamma64(k + 3) C_k (the sequential cumsum), (gamma64(pK) + u) 0.9 E and u (C_k +
+  eps).  The kernel's index lies between the first k with g + b > 0 and the first with g - b > 0; the value is k / K
+  correctly rounded (``check_feature_bounds64``: within 4 u of a whole number of quanta).
+* Rows 8-20: m = M X moves by |M_j|_2 e plus gamma64(taps_j + 1) m_j (the kernel's sequential taps) and gamma64(K + 1)
+  m_j (the reference's BLAS product, order unknown).  Both sides' m are sums of non-negative terms, so log10(m + eps)
+  stays in [log10(max(m - dm, 0) + eps), log10(m + dm + eps)]: finite for every frame, constant frames included (written
+  with log1p, which does not cancel).  Plus the + eps roundings (u / ln 10 per side), the logs (5 ulp together) and both
+  sides' 40-term DCT sums, gamma64(41) sum |D| |log10 m| each.
+* Rows 21-32: ``chroma_bound64``.  Row 33: np.std is 1-Lipschitz in the RMS norm of the class errors, plus per side the
+  stage of a 12-value mean, the differences, squares, sum, division and sqrt.
+* Deltas: b[t] + b[t - 1] plus the rounding of both sides' differences; row 41 through the quanta of row 7.
+"Unbounded" has one meaning: a denominator's interval reaches 0 (Dn - sqrt(K) e - eps e, Sn - sqrt(K) e, E + eps - dE
+<= 0); each such entry is counted with its reason.  An exactly zero spectrum (e = 0, top = 0) is bounded by the stage
+alone.
 """
 import math
 
@@ -265,3 +297,335 @@ def feature_chroma_bounds(x, fs, w, s):
     X, e = spectrum_reference(fr)
     cj = _classes(X, C)
     return _finish(cj, chroma_bound64(X, C, cj, e=e), np.full(T, ROW_FULL), False)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The 68 feature rows (derivation: "Feature rows" in the module docstring)
+LOG_HOST_ULP = 4        # NumPy's float64 log2 / log10: its SIMD loops are documented to 4 ulp, libm's to 1
+LOG_CUDA_ULP = 1        # CUDA's double-precision log2 / log10 (CUDA C++ Programming Guide, mathematical functions)
+LOG_ULPS = LOG_HOST_ULP + LOG_CUDA_ULP
+EPS = O_EPS
+
+
+def rowsum(A):
+    """np.sum of every row of A, each a contiguous 1-D reduction: NumPy's pairwise sum, kernel 12's order."""
+    A = np.ascontiguousarray(A, dtype=np.float64)
+    return np.array([np.sum(r) for r in A]) if A.shape[0] else np.zeros(0)
+
+
+def _g(n):
+    return float(gamma64(n))
+
+
+def _entropy64(s, ds):
+    """Bound on |H' - H|, H = sum_j h(s_j), h(s) = -s log2(s + eps), each s_j' within ds_j of s_j, both sides' stage
+    included.  By the mean value theorem |h(s') - h(s)| <= ds max |h'| over [lo, hi] (lo = max(s - ds, 0), hi = s + ds),
+    |h'(s)| = |log2(s + eps) + s / ((s + eps) ln 2)| <= max(|log2(lo + eps)|, |log2(hi + eps)|) + 1 / ln 2.  (parity's
+    concave-h interval gives the same bound, but its endpoint differences h(s) - h(lo) cancel in float64 at these
+    widths.)  Then the logs of both sides, LOG_ULPS ulp <= 2 LOG_ULPS u |log2|, times s; the products and the 10-term
+    pairwise sums of both sides, 2 gamma64(pairwise_depth(10))."""
+    lo = np.maximum(s - ds, 0.0)
+    hi = s + ds
+    lg = np.maximum(np.abs(np.log2(lo + EPS)), np.abs(np.log2(hi + EPS)))
+    dev = ds * (lg + 1 / math.log(2.0)) + hi * 2 * LOG_ULPS * U64 * lg
+    stage = 2 * _g(pairwise_depth(10)) * (np.abs(s * np.log2(s + EPS)) + dev)
+    return MARGIN * (dev + stage).sum(axis=-1)
+
+
+def _blocks(V, n_blocks=10):
+    """[T, 10] block sums of squares of the rows of V: blocks of len // 10 values, NumPy's pairwise sum each."""
+    blk = V.shape[1] // n_blocks
+    return np.stack([rowsum(V[:, j * blk:(j + 1) * blk] ** 2) for j in range(n_blocks)], axis=1), blk
+
+
+def feature_bounds64(x, fs, w, s, deltas=False):
+    """The float64 reference of all 68 (34 without deltas) short-term feature rows of clip x at (fs, w, s), every frame,
+    and a per-entry bound on what kernel 12 may return, as a parity.FeatureBounds (rolloff: admissible quanta)."""
+    from oracle import st_oracle as O
+    from tests.parity import FeatureBounds
+    K = w // 2
+    y = O.normalize_clip(np.asarray(x, dtype=np.float64))
+    T = O.frame_count(y.size, w, s)
+    fr = np.stack([y[s * t:s * t + w] for t in range(T)])
+    X, e = spectrum_reference(fr)
+    ref = O.base_features_from_frames(fr, X, fs)
+    ref[0] = [O._zcr(f) for f in fr]
+    ref[1] = [O._energy(f) for f in fr]
+    M, D, C = _tables(fs, K)
+    u = U64
+    bound = np.zeros_like(ref)
+    unb = {}
+
+    def unbounded(rows, mask, reason):
+        if mask.any():
+            bound[np.ix_(rows, np.nonzero(mask)[0])] = np.inf
+            unb[reason] = unb.get(reason, 0) + int(mask.sum()) * len(rows)
+
+    pK = pairwise_depth(K)
+    # row 2: the samples are exact; both sides round the block sums, the total, + eps and the division
+    Bt, blk = _blocks(fr)
+    Et = rowsum(fr ** 2)
+    sj = Bt / (Et + EPS)[:, None]
+    bound[2] = _entropy64(sj, 2 * sj * (_g(pairwise_depth(blk)) + _g(pairwise_depth(w)) + 2 * u))
+
+    # rows 3, 4: in Hz, ind = fl((k + 1) fs / (2 K)) the same value on both sides; cen = N / Dn with N = sum ind X and
+    # Dn = S + eps top (X / top and sum + eps, top = max X); top moves by at most e
+    ind = np.arange(1, K + 1) * (fs / (2.0 * K))
+    half = fs / 2.0
+    S = X.sum(axis=1)
+    top = X.max(axis=1)
+    Dn = S + EPS * top
+    silent = (top == 0) & (e == 0)                       # an exactly zero spectrum: both sides compute 0 exactly
+    Dlo = _ratio_den(Dn, math.sqrt(K) * e + EPS * e)
+    Dlo = np.where(silent, 1.0, Dlo)
+    c = ref[3] * half
+    dc_t = (np.linalg.norm(ind[None, :] - c[:, None], axis=1) * e + c * EPS * e) / Dlo
+    dc = MARGIN * (dc_t + 2 * _g(2 * pK + 6) * c)
+    bound[3] = dc / half
+    V = (ref[4] * half) ** 2
+    Dsafe = np.where(silent, 1.0, Dn)
+    dVc = dc * (dc * S + 2 * c * EPS * top) / Dsafe       # V at a centroid dc away
+    dk = np.abs(ind[None, :] - c[:, None])
+    wv = np.abs(dk ** 2 - V[:, None]) + 2 * dk * dc[:, None] + dc[:, None] ** 2 + dVc[:, None]
+    dV_t = (np.linalg.norm(wv, axis=1) * e + (V + dVc) * EPS * e) / Dlo + dVc
+    zeta = u * (dk + dc[:, None])                        # the rounded ind - cen
+    dV_a = 2 * (((2 * dk * zeta + zeta ** 2) * X).sum(axis=1) / Dlo + _g(2 * pK + 8) * (V + dVc))
+    dV = MARGIN * (dV_t + dV_a)
+    sv = np.sqrt(V)
+    up = np.where(dV > 0, dV / np.maximum(np.sqrt(V + dV) + sv, 1e-300), 0.0)
+    down = np.where(V > dV, dV / np.maximum(sv + np.sqrt(np.maximum(V - dV, 0.0)), 1e-300), sv)
+    bound[4] = (np.maximum(up, down) + 4 * u * np.sqrt(V + dV)) / half
+    unbounded([3, 4], np.isnan(Dlo), "sum X interval contains 0 (centroid, spread)")
+
+    # row 5: s_j = B_j / (E + eps) over blocks of K // 10 bins; X'^2 - X^2 = 2 X d + d^2
+    P = X ** 2
+    E = P.sum(axis=1)
+    dE = 2 * np.linalg.norm(X, axis=1) * e + e ** 2
+    Bs, blk = _blocks(X)
+    sjs = Bs / (E + EPS)[:, None]
+    Bm = np.zeros((10, K))
+    for j in range(10):
+        Bm[j, j * blk:(j + 1) * blk] = 1.0
+    a = Bm[None] - sjs[:, :, None]                                             # [T, 10, K]
+    Elo = _ratio_den(E + EPS, dE)
+    ds = (2 * np.linalg.norm(a * X[:, None, :], axis=2) * e[:, None] + np.abs(a).max(axis=2) * (e ** 2)[:, None]) / Elo[:, None]
+    bound[5] = _entropy64(sjs, ds + 2 * sjs * (_g(pairwise_depth(blk)) + _g(pK) + 2 * u))
+
+    # row 6: sqrt(flux) = |X / Sn - Xp / Snp|_2, Sn = sum(X + eps); each side moves by (e + |X / Sn|_2 dSn) / (Sn - dSn)
+    Sn = S + K * EPS
+    dSn = math.sqrt(K) * e
+    Snlo = _ratio_den(Sn, dSn)
+    nrm = np.linalg.norm(X, axis=1) / Sn
+    Dt = (e + nrm * dSn) / Snlo
+    Dp = np.concatenate([Dt[:1], Dt[:-1]])
+    Xn = X / Sn[:, None]
+    Pn = np.concatenate([Xn[:1], Xn[:-1]])
+    dd = np.abs(Xn - Pn)
+    eta = _g(pK + 2) * (Xn + Pn) + u * dd                                      # one side's rounded difference
+    sq = (2 * dd * eta + eta ** 2).sum(axis=1)
+    rf = np.sqrt(ref[6])
+    bound[6] = MARGIN * ((Dt + Dp) * (2 * rf + Dt + Dp) + 2 * (sq + _g(pK) * (ref[6] + sq)))
+    unbounded([6], np.isnan(Snlo) | np.isnan(np.concatenate([Snlo[:1], Snlo[:-1]])), "sum (X + eps) interval contains 0")
+
+    # row 7: first k with g_k = cumsum_k(X^2) + eps - 0.9 E > 0; weights 1[j <= k] - 0.9 on X^2; both sides' stage
+    Pc = np.cumsum(P, axis=1)
+    g = Pc + EPS - 0.9 * E[:, None]
+    aX2 = 0.01 * Pc + 0.81 * np.maximum(E[:, None] - Pc, 0.0)
+    kk = np.arange(K)[None, :]
+    b = MARGIN * (2 * np.sqrt(aX2) * e[:, None] + 0.9 * (e ** 2)[:, None]
+                  + 2 * (_g(1) * (kk + 3) * Pc + (_g(pK) + u) * 0.9 * E[:, None] + u * (Pc + EPS)))
+    first = lambda cnd: np.where(cnd.any(axis=1), np.argmax(cnd, axis=1), -1)
+    lo, hi = first(g + b > 0), first(g - b > 0)
+    lo = np.where((lo < 0) | (hi < 0), 0, lo)
+    hi = np.where(hi < 0, K - 1, hi)
+    roll = np.stack([lo, hi])
+
+    # rows 8 .. 20: mel bands m = M X (non-negative sums on both sides), log10(m + eps), the DCT
+    m = X @ M.T
+    taps = np.array([np.ptp(np.nonzero(r)[0]) + 1 if r.any() else 0 for r in M])
+    dm = np.linalg.norm(M, axis=1)[None, :] * e[:, None] + (gamma64(taps + 1)[None, :] + _g(K + 1)) * m
+    lm = np.log10(m + EPS)
+    lo_m = np.maximum(m - dm, 0.0)
+    dL = np.maximum(np.log1p((m - lo_m) / (lo_m + EPS)), np.log1p(dm / (m + EPS))) / math.log(10.0)
+    dL = dL + 2 * u / math.log(10.0) + 2 * LOG_ULPS * u * np.abs(lm)
+    aD = np.abs(D)
+    bound[8:21] = MARGIN * (dL @ aD.T + 2 * _g(41) * (np.abs(lm) @ aD.T)).T
+
+    # rows 21 .. 33: the chroma bound; chroma_std 1-Lipschitz in the RMS norm of the class errors, plus np.std's stage
+    cj = ref[21:33].T
+    dcj = chroma_bound64(X, C, cj, e=e)
+    bound[21:33] = dcj.T
+    mu_e = _g(pairwise_depth(12) + 1) * np.abs(cj).mean(axis=1)
+    bound[33] = np.sqrt((dcj ** 2).mean(axis=1)) + 2 * MARGIN * (mu_e + (_g(pairwise_depth(12) + 4) + u) * (ref[33] + mu_e))
+    unbounded([5] + list(range(21, 34)), np.isnan(Elo) | np.isnan(dcj).any(axis=1), "sum X^2 interval contains 0")
+    bound = np.where(np.isnan(bound), np.inf, bound)
+    bound[7] = 0.0
+    if deltas:
+        d = np.zeros_like(ref)
+        d[:, 1:] = ref[:, 1:] - ref[:, :-1]
+        db = np.zeros_like(bound)
+        db[:, 1:] = bound[:, 1:] + bound[:, :-1]
+        db[:, 1:] += 2 * u * (np.abs(d[:, 1:]) + db[:, 1:])
+        for reason in list(unb):
+            unb["delta: " + reason] = unb[reason]
+        ref, bound = np.concatenate([ref, d]), np.concatenate([bound, db])
+    return FeatureBounds(ref, bound, roll, unb, K)
+
+
+def check_feature_bounds64(got, fb, what=""):
+    """parity.check_feature_bounds at float64: the rolloff k / K within 4 u64 of a whole number of quanta."""
+    from tests.parity import check_feature_bounds
+    return check_feature_bounds(got, fb, what, roll_slack=4 * U64)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The stage model: kernel 12's feature stage (csrc/f64.cu f64_spectrum's time rows, f64_spectral) restated in NumPy in
+# its documented order, logs correctly rounded
+def _cr(fn, v):
+    """fn (mpmath.log, base 2 or 10) of every value of v, correctly rounded to float64."""
+    import mpmath
+    v = np.asarray(v, dtype=np.float64)
+    uq, inv = np.unique(v, return_inverse=True)
+    with mpmath.workprec(160):
+        out = np.array([float(fn(mpmath.mpf(float(a)))) if a > 0 else (-np.inf if a == 0 else np.nan) for a in uq])
+    return out[inv].reshape(v.shape)
+
+
+def cr_log2(v):
+    import mpmath
+    return _cr(lambda a: mpmath.log(a, 2), v)
+
+
+def cr_log10(v):
+    import mpmath
+    return _cr(mpmath.log10, v)
+
+
+def _entropy_stage(Bsum, tot):
+    """-np.sum of s_j log2(s_j + eps), s_j = B_j / (tot + eps), with correctly rounded logs; and the margin of a kernel
+    whose log2 is within LOG_CUDA_ULP ulp: its logs differ by at most 1.5 ulp <= 3 u |L|, so each term by 3 u |t| plus
+    both products' roundings, and each 10-term sum lies within gamma64(pairwise_depth(10)) sum |t| of the exact sum."""
+    s = Bsum / (tot + EPS)[:, None]
+    t = s * cr_log2(s + EPS)
+    H = -rowsum(t)
+    at = np.abs(t).sum(axis=1)
+    return H, MARGIN * (5 * U64 + 2 * _g(pairwise_depth(10))) * at
+
+
+def stage_tables(exe, fs, K):
+    """(mel [40, K], dct [13, 40]) as the host builds them for the plan (tests/f64_host.cu ``tables``)."""
+    from tests.host_exe import floats, run
+    v = floats(run(exe, "tables %d %d\n" % (fs, K))[0][1:])
+    return v[:40 * K].reshape(40, K), v[40 * K:].reshape(13, 40)
+
+
+class Stage:
+    """stage_model's result: ``rows`` [34, T] (rows 0 .. 1 nan: the model starts from the spectra), ``margin`` [34, T]
+    (0: bit for bit; rows 2, 5, 8 .. 20: the log margin) and the mask ``have`` [34] of the rows it states."""
+
+    def __init__(self, rows, margin, have):
+        self.rows, self.margin, self.have = rows, margin, have
+
+
+def stage_model(X, Xp, fs, mel, dct, frames=None):
+    """Kernel 12's rows 3 .. 33 (and row 2 from the frames' samples, when given) of frames whose spectra are X [T, K]
+    and whose previous frames' spectra are Xp [T, K], in the order DESIGN section 4 (kernel 12) states: NumPy's pairwise
+    sums (np.sum of a contiguous row), IEEE division and sqrt, a sequential cumsum, sequential mel taps and a sequential
+    40-term DCT, the chroma fold in ascending slot order, np.std of the 12 classes."""
+    from oracle import st_oracle as O
+    X = np.ascontiguousarray(X, dtype=np.float64)
+    Xp = np.ascontiguousarray(Xp, dtype=np.float64)
+    T, K = X.shape
+    rows = np.full((34, T), np.nan)
+    margin = np.zeros((34, T))
+    have = np.zeros(34, dtype=bool)
+    if frames is not None:
+        Bt, _ = _blocks(np.asarray(frames, dtype=np.float64))
+        rows[2], margin[2] = _entropy_stage(Bt, rowsum(np.asarray(frames, dtype=np.float64) ** 2))
+        have[2] = True
+    top = X.max(axis=1)
+    dv = np.where(top == 0.0, EPS, top)
+    Xt = X / dv[:, None]
+    ind = np.arange(1, K + 1).astype(np.float64) * (fs / (2.0 * K))
+    den = rowsum(Xt) + EPS
+    cen = rowsum(ind[None, :] * Xt) / den
+    spr = np.sqrt(rowsum(((ind[None, :] - cen[:, None]) ** 2) * Xt) / den)
+    rows[3], rows[4] = cen / (fs / 2.0), spr / (fs / 2.0)
+    tot = rowsum(X * X)
+    Bs, _ = _blocks(X)
+    rows[5], margin[5] = _entropy_stage(Bs, tot)
+    d = X / rowsum(X + EPS)[:, None] - Xp / rowsum(Xp + EPS)[:, None]
+    rows[6] = rowsum(d * d)
+    over = np.cumsum(X * X, axis=1) + EPS > (0.90 * tot)[:, None]
+    rows[7] = np.where(over.any(axis=1), np.argmax(over, axis=1) / float(K), 0.0)
+    acc = np.zeros((T, 40))
+    for i in range(40):
+        nz = np.nonzero(mel[i])[0]
+        if nz.size:
+            for k in range(nz[0], nz[-1] + 1):
+                acc[:, i] = acc[:, i] + mel[i, k] * X[:, k]
+    lm = cr_log10(acc + EPS)
+    mf = np.zeros((T, 13))
+    for n in range(40):
+        mf = mf + dct[None, :, n] * lm[:, n:n + 1]
+    rows[8:21] = mf.T
+    margin[8:21] = (MARGIN * (5 * U64 + 2 * _g(41)) * (np.abs(lm) @ np.abs(dct).T)).T
+    semis, share = O.chroma_tables(fs, K)
+    wrap = lambda j: j + K if j < 0 else j
+    winner = {}
+    for k in range(K):
+        winner[wrap(int(semis[k]))] = k
+    ch = np.zeros((T, 12))
+    for cl in range(12):
+        for j in range(cl, K, 12):
+            if j in winner:
+                b = winner[j]
+                ch[:, cl] = ch[:, cl] + (X[:, b] * X[:, b]) / share[wrap(int(semis[j]))]
+    ch = ch / np.where(tot == 0.0, EPS, tot)[:, None]
+    rows[21:33] = ch.T
+    rows[33] = [np.std(r) for r in ch]
+    have[3:34] = True
+    return Stage(rows, margin, have)
+
+
+EXACT_ROWS = (3, 4, 6, 7) + tuple(range(21, 34))
+LOG_ROWS = (2, 5) + tuple(range(8, 21))
+
+
+def check_stage(got, st, what="", rows=None):
+    """Kernel rows ``got`` [34, T] against a Stage: rows 3, 4, 6, 7, 21 .. 33 equal (+0 == -0), rows 2, 5, 8 .. 20 within
+    the log margin.  ``rows``: the subset to check (default: every row the model states).  Returns the worst
+    |got - model| / margin of the log rows."""
+    got = np.asarray(got, dtype=np.float64)
+    rows = [r for r in (rows if rows is not None else range(34)) if st.have[r]]
+    assert np.isfinite(got[rows]).all(), what + ": non-finite rows"
+    worst = 0.0
+    for r in rows:
+        if r in EXACT_ROWS:
+            bad = got[r] != st.rows[r]
+            if bad.any():
+                t = int(np.nonzero(bad)[0][0])
+                raise AssertionError("%s: row %d differs from the stage model in %d frames, first %d: %r vs %r"
+                                     % (what, r, int(bad.sum()), t, got[r, t], st.rows[r, t]))
+        else:
+            err = np.abs(got[r] - st.rows[r])
+            bad = err > st.margin[r]
+            if bad.any():
+                t = int(np.nonzero(bad)[0][0])
+                raise AssertionError("%s: row %d outside the stage model's log margin in %d frames, first %d: %r vs %r, "
+                                     "margin %.3g" % (what, r, int(bad.sum()), t, got[r, t], st.rows[r, t], st.margin[r, t]))
+            if err.size:
+                worst = max(worst, float(np.max(np.where(err > 0, err / np.where(st.margin[r] > 0, st.margin[r], 1), 0))))
+    return worst
+
+
+def check_deltas(F, T, what=""):
+    """Rows 34 .. 67 of a [68, >= T] feature block: column 0 zero, column t the kernel's own row difference, in bits."""
+    F = np.asarray(F, dtype=np.float64)[:, :T]
+    d = np.zeros((34, T))
+    d[:, 1:] = F[:34, 1:] - F[:34, :-1]
+    same = (F[34:] == d) | (np.isnan(F[34:]) & np.isnan(d))
+    same &= np.signbit(F[34:]) == np.signbit(d)
+    if not same.all():
+        r, t = (int(v[0]) for v in np.nonzero(~same))
+        raise AssertionError("%s: delta row %d frame %d is %r, the row difference %r" % (what, 34 + r, t, F[34 + r, t], d[r, t]))

@@ -8,6 +8,8 @@
 //   fft n RE (n)                 -> re (n), im (n) of the fp64 mixed-radix transform of a real frame
 //   spec n Y (n)                 -> |X|[0:K] / K of that transform (f64::magnitude), as the frame kernel writes it
 //   specrec n Y (n)              -> the same with twiddles built by recurrence, w^j = w^(j-1) w (a planted defect)
+//   tables fs K                  -> the plan's dense [40 x K] mel bank, then the [13 x 40] DCT (b200aa_host::build_mel,
+//                                   build_dct: the tables kernel 12's MFCC stage reads)
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
@@ -72,6 +74,15 @@ int main()
                                     out[size_t(f * M + j)], out[size_t((F + f) * M + j)]);
             printf("P");
             for (double v : out) pr(v);
+            printf("\n");
+        } else if (!strcmp(cmd, "tables")) {
+            const int fs = int(rl()), K = int(rl());
+            std::vector<double> mel, dct;
+            b200aa_host::build_mel(fs, K, mel);
+            b200aa_host::build_dct(dct);
+            printf("M");
+            for (double v : mel) pr(v);
+            for (double v : dct) pr(v);
             printf("\n");
         } else if (!strcmp(cmd, "fft") || !strcmp(cmd, "spec") || !strcmp(cmd, "specrec")) {
             const int n = int(rl());

@@ -513,9 +513,9 @@ def feature_bounds(x, fs, w, s, deltas=False):
     return FeatureBounds(ref, bound, roll, unb, K)
 
 
-def check_feature_bounds(got, fb, what=""):
+def check_feature_bounds(got, fb, what="", roll_slack=4 * U32):
     """Rows ``got`` [F, T] against a FeatureBounds: every bounded entry within its bound, rolloff (and its delta) a whole
-    number of quanta inside the admissible range, no exception lists and no flip allowance.  Returns ({row group:
+    number of quanta inside the admissible range (within roll_slack of it), no exception lists and no flip allowance.  Returns ({row group:
     worst err / bound}, {reason: unbounded entries})."""
     got = np.asarray(got, dtype=np.float64)
     assert got.shape == fb.ref.shape, (what, got.shape, fb.ref.shape)
@@ -537,7 +537,7 @@ def check_feature_bounds(got, fb, what=""):
             qlo = np.concatenate([[0], lo[1:] - hi[:-1]])
             qhi = np.concatenate([[0], hi[1:] - lo[:-1]])
             scale = np.abs(fb.ref[ROLLOFF_ROW] * K) + np.abs(np.concatenate([[0], fb.ref[ROLLOFF_ROW, :-1] * K]))
-        off = (q < qlo) | (q > qhi) | (np.abs(got[r] * K - q) > 4 * U32 * (scale + 1))
+        off = (q < qlo) | (q > qhi) | (np.abs(got[r] * K - q) > roll_slack * (scale + 1))
         if off.any():
             t = int(np.nonzero(off)[0][0])
             raise AssertionError("%s: row %d (rolloff) outside its admissible quanta in %d frames, first %d: %r quanta, "

@@ -4,7 +4,11 @@ Held to the tolerances the oracle itself is held to against the reference (tests
 atol 1e-11), with the exceptions documented there (digitally silent frames, whose non-DC bins are float64 round-off).
 Bit for bit: the normalisation records and rows 0-1 against NumPy, the mid-term pooling and the long-term mean against
 NumPy on the kernel's own rows, every clip of a ragged batch against the clip alone, concurrent calls against the same
-calls alone, and the float32 path's bits before and after float64 calls."""
+calls alone, and the float32 path's bits before and after float64 calls.
+
+These tolerances are the path's published contract.  Beside them, tests/test_gpu_f64_feature_bounds.py holds rows 2-67
+of every frame, constant frames and the deltas after them included, to a per-entry float64 error bound, and the feature
+stage bit for bit to its NumPy statement on the kernel's own spectra."""
 import threading
 
 import numpy as np
