@@ -571,6 +571,63 @@ int b200aa_forest_regression_cross_validate(const double *d_X, int64_t n, int n_
                                             const int32_t *h_test_idx, const int32_t *h_n_trees, const int32_t *h_weights,
                                             const uint32_t *h_seeds, double *d_pred_test, double *d_pred_train, void *stream);
 
+/* Kernel 13, gradient boosting (csrc/forest.cuh boost_leaves): the device side of scikit-learn 1.9's
+ * GradientBoostingClassifier(n_estimators=T).fit with the library's arguments (log_loss, learning_rate 0.1, max_depth 3,
+ * subsample 1.0), one stage per call.  The caller computes each stage's negative gradient with scikit-learn's own loss
+ * (the only step that needs exp / log) and draws every tree's splitter seed; the device builds the stage's trees in bits
+ * and does the ordered float64 rest.
+ *
+ * b200aa_boosting_stage: one stage of many problems.  d_X float32 [n_rows, n_feats] C-contiguous on the current device.
+ * Problem p trains on rows h_train_rows [h_train_off[p], h_train_off[p + 1]) (h_train_off[0] = 0) and, when h_test_off /
+ * h_test_rows are given (both or neither), also updates its test rows h_test_rows [h_test_off[p], h_test_off[p + 1]).
+ * h_n_trees[p] = K, the trees per stage (1: binomial loss, else the multinomial loss over K classes, 3 <= K <= 32), and
+ * h_active[p] (0 / 1) whether p fits a tree in this stage.  Device blocks, problems one after another: d_y int32
+ * [h_train_off[P]] each training row's class index (0 / 1 for K = 1, else in [0, K)), d_neg_grad float64 and d_raw_train
+ * float64 (updated) [n_train(p), K] per problem, d_raw_test float64 (updated) [n_test(p), K] per problem.  h_seeds uint32:
+ * the splitter rand_r_state of every tree of the stage, active problems in order, k inner.  Per tree k of an active problem,
+ * on its training rows: a DecisionTreeRegressor (squared_error, max_depth 3, every feature, unit weights) on column k of
+ * the negative gradient, node for node as build_regression_tree builds it; every leaf's value replaced by
+ * _update_terminal_regions' Newton step over the leaf's rows in ascending row order (NumPy pairwise sums, the (K - 1) / K
+ * factor for the multinomial loss, 0.0 below |denominator| 1e-150); raw[:, k] += learning_rate * value[leaf] for the
+ * training rows and, walking the tree, the test rows.  With h_nodes (and h_values, h_node_count, h_max_depth; all or
+ * none) the stage's trees are written as b200aa_forest_fit writes them (one float64 value per node) and the call returns
+ * after the stream drained; without, the trees stay on the device and the call is stream-ordered.  NULL pointers,
+ * n_rows < 1 or > 2^29, n_feats < 1, n_problems < 1, a non-finite learning_rate, an empty training set, a row outside [0,
+ * n_rows), a K outside {1} and [3, 32], an active flag other than 0 / 1, test rows without d_raw_test, and a negative
+ * node_capacity are B200AA_ERR_INVALID before any CUDA call, trees beyond node_capacity after; more than 512 features, or
+ * a tree whose scratch does not fit the 256 MB scratch bound (its sort keys take 8 n_feats pow2(n_train) bytes),
+ * B200AA_ERR_UNSUPPORTED before any CUDA call.  It refuses a capturing stream.
+ * Replaces: _fit_stage of GradientBoostingClassifier.fit in train_gradient_boosting, and predict_stages on the test rows
+ * of evaluate_classifier's "gradientboosting" branch. */
+int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_feats, int64_t n_problems, const int64_t *h_train_off,
+                          const int32_t *h_train_rows, const int64_t *h_test_off, const int32_t *h_test_rows,
+                          const int32_t *h_n_trees, const int32_t *h_active, const int32_t *d_y, const double *d_neg_grad,
+                          double *d_raw_train, double *d_raw_test, const uint32_t *h_seeds, double learning_rate,
+                          b200aa_forest_node *h_nodes, double *h_values, int64_t node_capacity, int64_t *h_node_count,
+                          int32_t *h_max_depth, void *stream);
+
+/* b200aa_boosting_scale: evaluate_classifier's per-split scaling for the boosting model selection.  d_X float64 [n,
+ * n_feats] C-contiguous on the current device; per problem p, StandardScaler().fit on rows h_train_idx [h_train_off[p],
+ * h_train_off[p + 1]) in split order (kernel 6's knn::scaler_fit) and transform of them and of its test rows h_test_idx
+ * [h_test_off[p], h_test_off[p + 1]), cast to float32 as fit and predict cast them.  Writes d_Xs float32 [h_train_off[P] +
+ * h_test_off[P], n_feats]: problem p's training rows at row h_train_off[p], its test rows at row h_train_off[P] +
+ * h_test_off[p].  NULL pointers, n < 1 or n > 2^29, n_feats < 1, n_problems < 1, an empty training set and an index
+ * outside [0, n) are B200AA_ERR_INVALID before any CUDA call.  Stream-ordered; it refuses a capturing stream. */
+int b200aa_boosting_scale(const double *d_X, int64_t n, int n_feats, int64_t n_problems, const int64_t *h_train_off,
+                          const int32_t *h_train_idx, const int64_t *h_test_off, const int32_t *h_test_idx, float *d_Xs,
+                          void *stream);
+
+/* b200aa_boosting_count: the confusion counts of the boosting model selection from the test rows' final raw scores
+ * d_raw_test (float64 [n_test(p), K] per problem, problems one after another, K = h_n_trees[p]).  Each row's predicted
+ * class is predict's: raw >= 0 for K = 1, else the first maximum, mapped through h_classes int32 [P, 32] (problem p's
+ * present classes in sorted order, as label indices in [0, n_classes)).  Writes d_pred int32 [h_test_off[P]] and d_counts
+ * int64 [P, n_classes, n_classes] = counts[p, y_test, y_pred] with h_y_test int32 [h_test_off[P]], the format of
+ * b200aa_knn_cross_validate.  NULL pointers, n_problems < 1, n_classes outside [2, 32], a bad K, offset or label are
+ * B200AA_ERR_INVALID before any CUDA call.  Stream-ordered; it refuses a capturing stream. */
+int b200aa_boosting_count(const double *d_raw_test, int64_t n_problems, const int64_t *h_test_off, const int32_t *h_n_trees,
+                          const int32_t *h_classes, const int32_t *h_y_test, int n_classes, int32_t *d_pred,
+                          int64_t *d_counts, void *stream);
+
 /* ------------------------------------------------------------------ host entry points --
  * Same operations on HOST buffers: pinned or pageable input is copied to the device, the
  * kernels run, the result is copied back and the call returns after the stream drained.

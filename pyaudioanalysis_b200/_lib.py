@@ -108,6 +108,15 @@ SIGNATURES = {
     #  d_pred_test, d_pred_train, stream)
     "b200aa_forest_regression_cross_validate": (c_int, [c_vp, c_i64, c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
                                                         c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (d_X, n_rows, n_feats, n_problems, h_train_off, h_train_rows, h_test_off, h_test_rows, h_n_trees, h_active, d_y,
+    #  d_neg_grad, d_raw_train, d_raw_test, h_seeds, learning_rate, h_nodes, h_values, node_capacity, h_node_count,
+    #  h_max_depth, stream)
+    "b200aa_boosting_stage": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                      c_vp, ctypes.c_double, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    # (d_X, n, n_feats, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx, d_Xs, stream)
+    "b200aa_boosting_scale": (c_int, [c_vp, c_i64, c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    # (d_raw_test, n_problems, h_test_off, h_n_trees, h_classes, h_y_test, n_classes, d_pred, d_counts, stream)
+    "b200aa_boosting_count": (c_int, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     # float64 path: (d_sig, dtype, n_clips, n_samples, clip_stride, d_len, d_norm, stream)
     "b200aa_clip_stats_f64": (c_int, [c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b200aa_st_features_f64": (c_int, [c_vp, c_vp, c_int, c_i64, c_i64, c_i64, c_vp, c_vp, c_int, c_vp, c_i64, c_vp]),

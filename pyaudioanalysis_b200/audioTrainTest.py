@@ -11,10 +11,13 @@ and the returned parameter are the reference's, text for text.
 
 The forests ("randomforest", "extratrees") go the same way: each problem's split and then its forest's tree seeds are
 drawn in the reference's order, and ``consumers.forest_cross_validate`` (kernel 13) scales, trains and classifies every
-problem on the device, bit for bit scikit-learn 1.9's fit and predict.
+problem on the device, bit for bit scikit-learn 1.9's fit and predict.  So does "gradientboosting": each problem's split,
+then the n_estimators * K splitter seeds its fit draws, and ``consumers.boosting_cross_validate`` runs every problem's
+stages together, the gradients on the host with scikit-learn's loss and the trees on the device.
 
-Only "knn", "randomforest" and "extratrees" without SMOTE on finite float64 features run here (``unsupported`` says why
-not otherwise); ``install.install_training`` sends everything else to the reference's own function.
+Only "knn", "randomforest", "extratrees" and "gradientboosting" without SMOTE on finite float64 features run here
+(``unsupported`` says why not otherwise); ``install.install_training`` sends everything else to the reference's own
+function.
 """
 import math
 
@@ -23,6 +26,7 @@ from sklearn.model_selection import GroupShuffleSplit
 
 
 _FORESTS = ("randomforest", "extratrees")
+_TREES = _FORESTS + ("gradientboosting",)
 
 
 def features_to_matrix(features):
@@ -34,9 +38,10 @@ def features_to_matrix(features):
 
 def unsupported(features, classifier_name, params, train_percentage=0.90, smote=False):
     """None when evaluate_classifier runs on the GPU for these arguments, else the reason it does not."""
-    if classifier_name not in ("knn",) + _FORESTS:
-        return "classifier %r: only 'knn', 'randomforest' and 'extratrees' run on the GPU" % (classifier_name,)
-    if classifier_name in _FORESTS:
+    if classifier_name not in ("knn",) + _TREES:
+        return "classifier %r: only 'knn', 'randomforest', 'extratrees' and 'gradientboosting' run on the GPU" % (
+            classifier_name,)
+    if classifier_name in _TREES:
         import sklearn
         if not sklearn.__version__.startswith("1.9."):
             return "scikit-learn %s: the forest trainer restates 1.9.x" % sklearn.__version__
@@ -56,7 +61,7 @@ def unsupported(features, classifier_name, params, train_percentage=0.90, smote=
     # single contiguous column pairwise)
     if len(shapes) != 1 or shapes.pop() < 2:
         return "the classes need the same number (>= 2) of features"
-    if classifier_name in _FORESTS:
+    if classifier_name in _TREES:
         if features[0].shape[1] > 512 or len(features) > 32:
             return "more than 512 features or 32 classes: the forest trainer's shared-memory layout"
         with np.errstate(over="ignore"):
@@ -107,6 +112,25 @@ def draw_forest_problems(X, params, n_exp, train_percentage, kind, list_of_ids=N
         for e in range(n_exp):
             splits.append(fixed[e] if fixed else draw_splits(X, None, 1, 1, train_percentage)[0])
             seeds.append(tree_seeds(int(C), kind))
+    return splits, seeds
+
+
+def draw_boosting_problems(X, y, params, n_exp, train_percentage, list_of_ids=None):
+    """(splits, seeds) of every (param, experiment) of the "gradientboosting" branch, params outer, drawn from NumPy's
+    global RNG in the reference's order: GroupShuffleSplit's splits once up front (list_of_ids), then per problem its
+    train_test_split permutation (without list_of_ids) followed by the n_estimators * K seeds its fit draws, K from the
+    classes in its training rows.  None when a training set holds a single class (the reference's fit raises there)."""
+    from .boosting import draw_seeds, trees_per_stage
+    fixed = draw_splits(X, None, 1, n_exp, train_percentage, list_of_ids) if list_of_ids else None
+    splits, seeds = [], []
+    for C in params:
+        for e in range(n_exp):
+            split = fixed[e] if fixed else draw_splits(X, None, 1, 1, train_percentage)[0]
+            present = np.unique(y[split[0]]).size
+            if present < 2:
+                return None
+            splits.append(split)
+            seeds.append(draw_seeds(int(C) * trees_per_stage(present)))
     return splits, seeds
 
 
@@ -191,16 +215,32 @@ def report(y, class_names, params, parameter_mode, n_exp, counts):
 
 def evaluate_classifier(features, class_names, classifier_name, params, parameter_mode, list_of_ids=None, n_exp=-1,
                         train_percentage=0.90, smote=False):
-    """audioTrainTest.evaluate_classifier (:576-771) for classifier_name "knn", "randomforest" and "extratrees": the same
-    prints and return value, every (param, experiment) problem trained (forests) and classified on the GPU in one call.  Raises ValueError for arguments it does not cover
-    (``unsupported``); there is no CPU path."""
-    from .consumers import forest_cross_validate, knn_cross_validate
+    """audioTrainTest.evaluate_classifier (:576-771) for classifier_name "knn", "randomforest", "extratrees" and
+    "gradientboosting": the same prints and return value, every (param, experiment) problem trained (trees) and
+    classified on the GPU in one call.  Raises ValueError for arguments it does not cover (``unsupported``), and
+    ``boosting.SingleClass`` (a ValueError), with NumPy's global state as before the call, when a boosting training set
+    holds one class; there is no CPU path."""
+    from .consumers import boosting_cross_validate, forest_cross_validate, knn_cross_validate
     why = unsupported(features, classifier_name, params, train_percentage, smote)
     if why is not None:
         raise ValueError("evaluate_classifier on the GPU: " + why)
     X, y = features_to_matrix(features)
     if n_exp == -1:
         n_exp = int(50000 / X.shape[0]) + 1
+    if classifier_name == "gradientboosting":
+        from .boosting import SingleClass
+        state = np.random.get_state()
+        drawn = draw_boosting_problems(X, y, params, n_exp, train_percentage, list_of_ids)
+        if drawn is None:
+            np.random.set_state(state)
+            raise SingleClass("evaluate_classifier on the GPU: a training split holds a single class")
+        stages = [int(C) for C in params for _ in range(n_exp)]
+        try:
+            _, counts = boosting_cross_validate(X, y, drawn[0], drawn[1], stages, n_classes=len(features))
+        except ValueError:
+            np.random.set_state(state)
+            raise
+        return report(y, class_names, params, parameter_mode, n_exp, counts.cpu().numpy())
     if classifier_name in _FORESTS:
         splits, seeds = draw_forest_problems(X, params, n_exp, train_percentage, classifier_name, list_of_ids)
         trees = [int(C) for C in params for _ in range(n_exp)]
@@ -214,11 +254,18 @@ def evaluate_classifier(features, class_names, classifier_name, params, paramete
 
 def dispatcher(original):
     """An evaluate_classifier that runs the arguments the GPU covers here and hands the rest to `original`."""
+    from .boosting import SingleClass
+    from .forests import Unsupported
+
     def evaluate_classifier_dispatch(features, class_names, classifier_name, params, parameter_mode, list_of_ids=None,
                                      n_exp=-1, train_percentage=0.90, smote=False):
-        run = evaluate_classifier if unsupported(features, classifier_name, params, train_percentage, smote) is None else original
-        return run(features, class_names, classifier_name, params, parameter_mode, list_of_ids=list_of_ids, n_exp=n_exp,
-                   train_percentage=train_percentage, smote=smote)
+        kw = dict(list_of_ids=list_of_ids, n_exp=n_exp, train_percentage=train_percentage, smote=smote)
+        if unsupported(features, classifier_name, params, train_percentage, smote) is None:
+            try:
+                return evaluate_classifier(features, class_names, classifier_name, params, parameter_mode, **kw)
+            except (SingleClass, Unsupported):
+                pass                    # NumPy's state is as before the call: the original draws the same problems
+        return original(features, class_names, classifier_name, params, parameter_mode, **kw)
     evaluate_classifier_dispatch.original = original
     return evaluate_classifier_dispatch
 
@@ -244,6 +291,23 @@ def train_random_forest(features, labels, n_estimators):
 def train_extra_trees(features, labels, n_estimators):
     """audioTrainTest.train_extra_trees (:202-219), as ``train_random_forest`` with ExtraTreesClassifier."""
     return _train_forest("extratrees", features, labels, n_estimators)
+
+
+def train_gradient_boosting(features, labels, n_estimators):
+    """audioTrainTest.train_gradient_boosting (:181-199): GradientBoostingClassifier(n_estimators).fit(features,
+    labels), trained on the GPU (``consumers.boosting_fit``) stage for stage as scikit-learn trains it; arguments the
+    trainer does not reproduce (``boosting.unsupported``) or whose trees would exceed its scratch bound
+    (``forests.Unsupported``) go to scikit-learn."""
+    from . import boosting, forests
+    from .consumers import boosting_fit
+    X = np.asarray(features) if not isinstance(features, np.ndarray) else features
+    if boosting.unsupported(X, labels, n_estimators) is None:
+        try:
+            return boosting_fit(X, labels, n_estimators)
+        except forests.Unsupported:
+            pass                        # one tree over the scratch bound; NumPy's state is untouched
+    from sklearn.ensemble import GradientBoostingClassifier
+    return GradientBoostingClassifier(n_estimators=n_estimators).fit(features, labels)
 
 
 # ---- regression: evaluate_regression's "randomforest" branch and train_random_forest_regression ----

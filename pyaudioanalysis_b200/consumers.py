@@ -883,6 +883,184 @@ def forest_regression_cross_validate(X, y, splits, seeds, n_estimators):
     return pred_test, pred_train
 
 
+def _boost_scratch_refusal(status, what, n, F):
+    from . import forests as FO
+    if status == ERR_UNSUPPORTED:
+        raise FO.Unsupported("%s on the GPU: one tree of %d training rows x %d features needs more scratch than the "
+                             "trainer's 256 MB bound" % (what, n, F))
+    check(status)
+
+
+def boosting_fit(X, y, n_estimators):
+    """``GradientBoostingClassifier(n_estimators).fit(X, y)`` trained on the GPU (``b200aa_boosting_stage``, DESIGN.md
+    kernel 13, gradient boosting), stage for stage scikit-learn 1.9's under the same NumPy global state, which it leaves
+    as ``fit`` leaves it.  Each stage's negative gradient and train_score_ are computed on the host by scikit-learn's own
+    loss; the trees, their Newton leaf values and the raw-prediction update run on the device.  Returns the fitted
+    scikit-learn estimator.
+
+    X: float64 / float32 [n, F] host array (or a CUDA tensor, which is read from the device); y: n labels.  Raises
+    ValueError with ``boosting.unsupported``'s reason for what it does not reproduce, and ``forests.Unsupported`` (a
+    ValueError), with NumPy's global state as before the call, when one tree's scratch would exceed the trainer's 256 MB
+    bound; ``train_gradient_boosting`` hands those calls to scikit-learn."""
+    from . import boosting as BO
+    from . import forests as FO
+    Xh = X.detach().cpu().numpy() if isinstance(X, torch.Tensor) else X
+    why = BO.unsupported(Xh, y, n_estimators)
+    if why is not None:
+        raise ValueError("boosting_fit on the GPU: " + why)
+    n, F = Xh.shape
+    T = int(n_estimators)
+    est, X32, y_enc, raw0 = BO.begin(Xh, y, T)
+    K = est.n_trees_per_iteration_
+    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64):
+        d_X = X.to(torch.float32).contiguous()     # fit's cast to float32, round to nearest
+    else:
+        d_X = torch.from_numpy(np.ascontiguousarray(X32)).to(X.device if isinstance(X, torch.Tensor) and X.is_cuda else "cuda")
+    state = np.random.get_state()
+    seeds = BO.draw_seeds(T * K)
+    raw = np.ascontiguousarray(np.broadcast_to(raw0, (n, K)), dtype=np.float64)
+    sw = np.ones(n)
+    factor = BO.loss_factor(est._loss)
+    train_off, test_off = np.array([0, n], np.int64), None
+    rows = np.arange(n, dtype=np.int32)
+    K_arr, active = np.array([K], np.int32), np.ones(1, np.int32)
+    cap = K * (2 * n - 1)
+    nodes = np.empty(cap, dtype=FO.NODE_DTYPE)
+    values = np.empty(cap, dtype=np.float64)
+    counts = np.empty(K, dtype=np.int64)
+    depth = np.empty(K, dtype=np.int32)
+
+    def ptr(a):
+        return ctypes.c_void_p(a.ctypes.data)
+    with torch.cuda.device(d_X.device):
+        d_y = torch.from_numpy(y_enc.astype(np.int32)).to(d_X.device)
+        d_raw = torch.from_numpy(raw).to(d_X.device)
+        d_neg = torch.empty((n, K), dtype=torch.float64, device=d_X.device)
+        for i in range(T):
+            d_neg.copy_(torch.from_numpy(BO.neg_gradient(est._loss, y_enc, raw)))
+            status = lib().b200aa_boosting_stage(
+                ctypes.c_void_p(d_X.data_ptr()), n, F, 1, ptr(train_off), ptr(rows), None, None, ptr(K_arr), ptr(active),
+                ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()), ctypes.c_void_p(d_raw.data_ptr()),
+                None, ptr(seeds[i * K:(i + 1) * K]), float(est.learning_rate), ptr(nodes), ptr(values), cap, ptr(counts),
+                ptr(depth), _stream())
+            if status == ERR_UNSUPPORTED:
+                np.random.set_state(state)
+            _boost_scratch_refusal(status, "boosting_fit", n, F)
+            raw = d_raw.cpu().numpy()
+            est.train_score_[i] = factor * est._loss(y_true=y_enc, raw_prediction=raw, sample_weight=sw)
+            off = 0
+            for k in range(K):
+                nc = int(counts[k])
+                est.estimators_[i, k] = BO.make_tree(est, F, FO.tree_state(nodes[off:off + nc], values[off:off + nc],
+                                                                           depth[k], 1))
+                off += nc
+    est.n_estimators_ = T
+    return est
+
+
+def boosting_cross_validate(X, y, splits, seeds, n_estimators, n_classes=None):
+    """The "gradientboosting" branch of evaluate_classifier's model selection (audioTrainTest.py:631-699) on the GPU:
+    per (train, test) split, StandardScaler fit on the training rows (``b200aa_boosting_scale``),
+    ``GradientBoostingClassifier(n_estimators[p]).fit`` on them stage for stage scikit-learn's, every problem's stage in
+    one call (``b200aa_boosting_stage``; problems drop out once their stages are done), the test rows' raw scores updated
+    with each stage's trees, and predict's class of every test row counted (``b200aa_boosting_count``).  The trees stay
+    on the device; each stage's negative gradients are computed on the host with scikit-learn's loss.
+
+    X: float64 [n, F] (host, or a CUDA tensor); y: the n class indices in [0, n_classes); splits: (train, test) row
+    indices per problem, every training set holding at least two classes; seeds: per problem the n_estimators[p] * K_p
+    splitter seeds its fit draws (``boosting.draw_seeds``; K_p from the classes in its training rows).  Returns CUDA (pred
+    int32 [sum of the test counts], counts int64 [P, n_classes, n_classes]).  Raises ``forests.Unsupported`` when one tree
+    of the largest training set would exceed the trainer's 256 MB scratch bound."""
+    from . import boosting as BO
+    if not isinstance(X, torch.Tensor):
+        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, F]")
+    X = X.contiguous()
+    n, F = X.shape
+    y = np.asarray(y.cpu() if isinstance(y, torch.Tensor) else y)
+    if y.shape != (n,) or not np.array_equal(y, np.floor(y)) or (n and y.min() < 0):
+        raise ValueError("y must hold one class index >= 0 per row of X")
+    n_classes = int(y.max()) + 1 if n_classes is None else int(n_classes)
+    P = len(splits)
+    if not P == len(seeds) == len(n_estimators):
+        raise ValueError("one seed list and one stage count per split")
+    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
+    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
+    train_off, train_idx = _concat_indices(train, np.int32)
+    test_off, test_idx = _concat_indices(test, np.int32)
+    n_tr, n_te = int(train_off[-1]), int(test_off[-1])
+    stages = np.asarray(n_estimators, dtype=np.int64)
+    # each problem's fit preamble on the host: present classes, K, loss, encoded labels, initial raw prediction
+    init = [BO.problem_init(y[tr].astype(np.float64)) for tr in train]
+    K = np.array([k for _, k, _, _, _ in init], dtype=np.int32)
+    if any(c.size < 2 for c, _, _, _, _ in init):
+        raise ValueError("every training set needs two classes (fit raises otherwise)")
+    if any(len(s) != t * k for s, t, k in zip(seeds, stages, K)):
+        raise ValueError("every problem needs n_estimators * K seeds")
+    seeds = [np.asarray(s, dtype=np.uint32) for s in seeds]
+    g_off = np.concatenate([[0], np.cumsum([tr.size * k for tr, k in zip(train, K)])]).astype(np.int64)
+    t_off = np.concatenate([[0], np.cumsum([te.size * k for te, k in zip(test, K)])]).astype(np.int64)
+    raw_tr = np.concatenate([np.broadcast_to(r0, (tr.size, k)).ravel() for (_, k, _, _, r0), tr in zip(init, train)])
+    raw_te = np.concatenate([np.broadcast_to(r0, (te.size, k)).ravel() for (_, k, _, _, r0), te in zip(init, test)] +
+                            [np.zeros(0)])
+    y_loc = np.ascontiguousarray(np.concatenate([ye for _, _, _, ye, _ in init]), dtype=np.int32)
+    classes = np.zeros((P, 32), dtype=np.int32)
+    for p, (c, _, _, _, _) in enumerate(init):
+        classes[p, :c.size] = c.astype(np.int32)
+    # the losses of the problems grouped by K: the gradient is row by row, so one call per group computes every problem's
+    groups = {}
+    for p, (_, k, loss, _, _) in enumerate(init):
+        groups.setdefault(int(k), (loss, []))[1].append(p)
+    rows_tr = np.arange(n_tr, dtype=np.int32)
+    rows_te = np.arange(n_tr, n_tr + n_te, dtype=np.int32)
+    lr = 0.1                                        # GradientBoostingClassifier's learning_rate
+
+    def ptr(a):
+        return ctypes.c_void_p(a.ctypes.data) if a is not None else None
+    with torch.cuda.device(X.device):
+        d_Xs = torch.empty((n_tr + n_te, F), dtype=torch.float32, device=X.device)
+        check(lib().b200aa_boosting_scale(ctypes.c_void_p(X.data_ptr()), n, F, P, ptr(train_off), ptr(train_idx),
+                                          ptr(test_off), ptr(test_idx), ctypes.c_void_p(d_Xs.data_ptr()), _stream()))
+        d_y = torch.from_numpy(y_loc).to(X.device)
+        d_raw_tr = torch.from_numpy(np.ascontiguousarray(raw_tr, dtype=np.float64)).to(X.device)
+        d_raw_te = torch.from_numpy(np.ascontiguousarray(raw_te, dtype=np.float64)).to(X.device)
+        d_neg = torch.empty(max(int(g_off[-1]), 1), dtype=torch.float64, device=X.device)
+        neg = np.zeros(max(int(g_off[-1]), 1))
+        for s in range(int(stages.max())):
+            active = (stages > s).astype(np.int32)
+            raw = d_raw_tr.cpu().numpy()
+            for k, (loss, probs) in groups.items():
+                ps = [p for p in probs if active[p]]
+                if not ps:
+                    continue
+                yk = np.concatenate([init[p][3] for p in ps])
+                rk = np.concatenate([raw[g_off[p]:g_off[p + 1]].reshape(-1, k) for p in ps])
+                gk = BO.neg_gradient(loss, yk, rk).ravel()
+                o = 0
+                for p in ps:
+                    m = int(g_off[p + 1] - g_off[p])
+                    neg[g_off[p]:g_off[p + 1]] = gk[o:o + m]
+                    o += m
+            d_neg.copy_(torch.from_numpy(neg))
+            st_seeds = np.ascontiguousarray(np.concatenate([seeds[p][s * K[p]:(s + 1) * K[p]] for p in range(P) if active[p]]),
+                                            dtype=np.uint32)
+            status = lib().b200aa_boosting_stage(
+                ctypes.c_void_p(d_Xs.data_ptr()), n_tr + n_te, F, P, ptr(train_off), ptr(rows_tr), ptr(test_off),
+                ptr(rows_te), ptr(K), ptr(active), ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()),
+                ctypes.c_void_p(d_raw_tr.data_ptr()), ctypes.c_void_p(d_raw_te.data_ptr()), ptr(st_seeds), lr,
+                None, None, 0, None, None, _stream())
+            _boost_scratch_refusal(status, "boosting_cross_validate", max(t.size for t in train), F)
+        pred = torch.empty(max(n_te, 1), dtype=torch.int32, device=X.device)
+        counts = torch.empty((P, n_classes, n_classes), dtype=torch.int64, device=X.device)
+        y_test = np.ascontiguousarray(y[test_idx] if n_te else np.zeros(1), dtype=np.int32)
+        check(lib().b200aa_boosting_count(ctypes.c_void_p(d_raw_te.data_ptr()), P, ptr(test_off), ptr(K), ptr(classes),
+                                          ptr(y_test), n_classes, ctypes.c_void_p(pred.data_ptr()),
+                                          ctypes.c_void_p(counts.data_ptr()), _stream()))
+    return pred[:n_te], counts
+
+
 def tree_classify_batch(model, vectors):
     """predict / predict_proba of a tree ensemble for every row of a CUDA float32 / float64 [n, F] tensor, in one kernel on
     the current stream (DESIGN.md, kernel 8): CUDA (ids int64 [n], indices into the model's classes_; P float64 [n, C]),

@@ -652,3 +652,322 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
     }
     return scratch.done(B200AA_OK);
 }
+
+// ------------------------------------------------------------------------------------------------
+// kernel 13, gradient boosting: one stage of GradientBoostingClassifier fit for many problems (csrc/forest.cuh,
+// build_regression_tree with max_depth 3 and boost_leaves), the test rows' raw scores, and the final class counts
+// ------------------------------------------------------------------------------------------------
+namespace {
+
+// one tree of a stage: problem p's training rows, its [n, K] gradient / raw blocks (tree k reads and updates column k),
+// its class indices, and its test rows with their [n_test, K] raw block
+struct BoostJob {
+    const int32_t *rows;
+    int64_t n;
+    const double *neg_g;
+    const int32_t *y;
+    double *raw;
+    int32_t k, K;
+    const int32_t *test_rows;
+    int64_t n_test;
+    double *raw_test;
+};
+
+// a boosting tree's scratch: the regression tree's, then leaf_of [n] and leaf_rows [n]
+struct BoostLayout {
+    RegLayout reg;
+    size_t leaf_of, leaf_rows, bytes;
+};
+BoostLayout boost_layout(int64_t n, int F)
+{
+    BoostLayout B;
+    B.reg = reg_layout(n, F);
+    B.leaf_of = B.reg.bytes;
+    B.leaf_rows = B.leaf_of + align256(size_t(n) * 4);
+    B.bytes = B.leaf_rows + align256(size_t(n) * 4);
+    return B;
+}
+
+inline size_t boost_smem_bytes(int F) { return reg_smem_bytes(F) + size_t(forest::kThreads) * 8; }
+
+}  // namespace
+
+// One CTA per tree of the launch: unit weights, build_regression_tree (max_depth 3) on column k of the problem's negative
+// gradient, then boost_leaves: the Newton leaf values and the training rows' raw column k.
+__global__ void __launch_bounds__(forest::kThreads) boost_build_kernel(const float *__restrict__ X, int F,
+                                                                      const BoostJob *__restrict__ jobs,
+                                                                      const uint32_t *__restrict__ seeds, double lr,
+                                                                      char *__restrict__ scratch, BoostLayout B)
+{
+    extern __shared__ __align__(16) unsigned char boost_smem[];
+    const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
+    const RegLayout &L = B.reg;
+    char *base = scratch + size_t(blockIdx.x) * B.bytes;
+    unsigned char *s = boost_smem;
+    forest::RegShared *st = reinterpret_cast<forest::RegShared *>(s);
+    s += (sizeof(forest::RegShared) + 15) & ~size_t(15);
+    double *vproxy = reinterpret_cast<double *>(s);
+    s += size_t(F) * 8;
+    int64_t *vpos = reinterpret_cast<int64_t *>(s);
+    s += size_t(F) * 8;
+    int64_t *part = reinterpret_cast<int64_t *>(s);
+    s += size_t(forest::kThreads) * 8;
+    float *mn = reinterpret_cast<float *>(s);
+    float *mx = mn + F;
+    int32_t *features = reinterpret_cast<int32_t *>(mx + F);
+    int32_t *constf = features + F, *drawn = constf + F, *vis = drawn + F, *tied = vis + F;
+    const BoostJob J = jobs[blockIdx.x];
+    int32_t *w = reinterpret_cast<int32_t *>(base + L.weights);
+    for (int64_t i = threadIdx.x; i < J.n; i += blockDim.x) w[i] = 1;
+    __syncthreads();
+    const forest::RegTree T{X, J.neg_g + J.k, J.rows, w, J.n, F,
+                            reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.idx),
+                            reinterpret_cast<float *>(base + L.fv), reinterpret_cast<uint64_t *>(base + L.keys),
+                            reinterpret_cast<forest::StackRec *>(base + L.stack), reinterpret_cast<forest::NodeOut *>(base + L.nodes),
+                            reinterpret_cast<double *>(base + L.values), features, constf, drawn, vis, tied, mn, mx, vproxy,
+                            vpos, st, J.K, forest::kBoostDepth};
+    forest::build_regression_tree(T, tm, seeds[blockIdx.x]);
+    forest::boost_leaves(T, forest::BoostTree{J.y, J.k, J.K, J.raw, lr, reinterpret_cast<int32_t *>(base + B.leaf_of),
+                                              reinterpret_cast<int32_t *>(base + B.leaf_rows), part}, tm);
+    if (threadIdx.x == 0) {
+        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
+        meta[0] = st->node_count;
+        meta[1] = st->max_depth;
+    }
+}
+
+// One thread per (tree, test row), blockIdx.y the tree of the launch: the row's leaf, and raw_test[:, k] += lr * value
+// (predict_stages' update; a stage's trees touch different columns, so their order does not matter)
+__global__ void boost_test_kernel(const float *__restrict__ X, int F, const BoostJob *__restrict__ jobs, double lr,
+                                  const char *__restrict__ scratch, BoostLayout B)
+{
+    const BoostJob J = jobs[blockIdx.y];
+    const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (r >= J.n_test) return;
+    const char *base = scratch + size_t(blockIdx.y) * B.bytes;
+    const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(base + B.reg.nodes);
+    const double *values = reinterpret_cast<const double *>(base + B.reg.values);
+    const float *x = X + int64_t(J.test_rows[r]) * F;
+    const int32_t leaf = forest::tree_apply(nodes, [x](int f) { return x[f]; });
+    double &o = J.raw_test[r * J.K + J.k];
+    o = forest::dadd(o, forest::dmul(lr, values[leaf]));
+}
+
+namespace {
+bool valid_trees_per_stage(int32_t K) { return K == 1 || (K >= 3 && K <= forest::kMaxClasses); }
+}  // namespace
+
+extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_feats, int64_t n_problems,
+                                     const int64_t *h_train_off, const int32_t *h_train_rows, const int64_t *h_test_off,
+                                     const int32_t *h_test_rows, const int32_t *h_n_trees, const int32_t *h_active,
+                                     const int32_t *d_y, const double *d_neg_grad, double *d_raw_train, double *d_raw_test,
+                                     const uint32_t *h_seeds, double learning_rate, b200aa_forest_node *h_nodes,
+                                     double *h_values, int64_t node_capacity, int64_t *h_node_count, int32_t *h_max_depth,
+                                     void *stream)
+{
+    NvtxRange nvtx_("b200aa_boosting_stage");
+    REFUSE_CAPTURE(stream, "b200aa_boosting_stage", kWhyHostArrays);
+    const bool out = h_nodes != nullptr;
+    if (!d_X || !h_train_off || !h_train_rows || !h_n_trees || !h_active || !d_y || !d_neg_grad || !d_raw_train ||
+        !h_seeds || n_rows < 1 || n_rows > (int64_t(1) << 29) || n_feats < 1 || n_problems < 1 ||
+        !(learning_rate - learning_rate == 0.0) || (h_test_off == nullptr) != (h_test_rows == nullptr) ||
+        out != (h_values != nullptr) || out != (h_node_count != nullptr) || out != (h_max_depth != nullptr) ||
+        node_capacity < 0 || h_train_off[0] != 0 || (h_test_off && h_test_off[0] != 0))
+        return B200AA_ERR_INVALID;
+    int64_t ntr_max = 0, nte_max = 0, n_trees = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off ? h_test_off[p + 1] - h_test_off[p] : 0;
+        if (ntr < 1 || nte < 0 || !valid_trees_per_stage(h_n_trees[p]) || (h_active[p] != 0 && h_active[p] != 1))
+            return B200AA_ERR_INVALID;
+        if (nte > 0 && !d_raw_test) return B200AA_ERR_INVALID;
+        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
+            if (h_train_rows[i] < 0 || h_train_rows[i] >= n_rows) return B200AA_ERR_INVALID;
+        for (int64_t i = h_test_off ? h_test_off[p] : 0; i < (h_test_off ? h_test_off[p + 1] : 0); ++i)
+            if (h_test_rows[i] < 0 || h_test_rows[i] >= n_rows) return B200AA_ERR_INVALID;
+        if (!h_active[p]) continue;
+        ntr_max = std::max(ntr_max, ntr);
+        nte_max = std::max(nte_max, nte);
+        n_trees += h_n_trees[p];
+    }
+    if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
+    const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off ? h_test_off[n_problems] : 0;
+    const BoostLayout B = boost_layout(std::max<int64_t>(ntr_max, 1), n_feats);
+    // scratch: [train rows | test rows | seeds | jobs | trees of a launch]
+    const size_t b_tr = align256(size_t(n_tr) * 4), b_te = align256(size_t(std::max<int64_t>(n_te, 1)) * 4),
+                 b_seeds = align256(size_t(std::max<int64_t>(n_trees, 1)) * 4),
+                 b_jobs = align256(size_t(std::max<int64_t>(n_trees, 1)) * sizeof(BoostJob));
+    const size_t fixed = b_tr + b_te + b_seeds + b_jobs;
+    const int64_t slice = std::min<int64_t>(reg_slice(fixed, B.bytes, std::max<int64_t>(n_trees, 1)), 65535);    // grid y
+    if (slice < 1) return B200AA_ERR_UNSUPPORTED;
+    if (n_trees == 0) return B200AA_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t smem = boost_smem_bytes(n_feats);
+    CK(cudaFuncSetAttribute(boost_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(fixed + size_t(slice) * B.bytes);
+    if (rc != B200AA_OK) return rc;
+    char *q = static_cast<char *>(scratch.get());
+    int32_t *d_tr = reinterpret_cast<int32_t *>(q); q += b_tr;
+    int32_t *d_te = reinterpret_cast<int32_t *>(q); q += b_te;
+    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
+    BoostJob *d_jobs = reinterpret_cast<BoostJob *>(q); q += b_jobs;
+    char *d_trees = q;
+    // every active problem's trees, k inner
+    std::vector<BoostJob> jobs;
+    jobs.reserve(size_t(n_trees));
+    int64_t g_off = 0, t_off = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off ? h_test_off[p + 1] - h_test_off[p] : 0;
+        const int32_t K = h_n_trees[p];
+        if (h_active[p])
+            for (int32_t k = 0; k < K; ++k)
+                jobs.push_back(BoostJob{d_tr + h_train_off[p], ntr, d_neg_grad + g_off, d_y + h_train_off[p], d_raw_train + g_off,
+                                        k, K, nte ? d_te + h_test_off[p] : nullptr, nte, nte ? d_raw_test + t_off : nullptr});
+        g_off += ntr * K;
+        t_off += nte * K;
+    }
+    CK(cudaMemcpyAsync(d_tr, h_train_rows, size_t(n_tr) * 4, cudaMemcpyHostToDevice, st));
+    if (n_te) CK(cudaMemcpyAsync(d_te, h_test_rows, size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_jobs, jobs.data(), size_t(n_trees) * sizeof(BoostJob), cudaMemcpyHostToDevice, st));
+    int64_t written = 0;
+    std::vector<int64_t> meta(size_t(slice) * 2);
+    for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
+        const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
+        boost_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(d_X, n_feats, d_jobs + t0, d_seeds + t0,
+                                                                         learning_rate, d_trees, B);
+        CK_LAUNCH("boost_build_kernel");
+        int64_t te_max = 0;
+        for (int64_t i = t0; i < t0 + nt; ++i) te_max = std::max(te_max, jobs[size_t(i)].n_test);
+        if (te_max) {
+            boost_test_kernel<<<dim3(unsigned((te_max + 127) / 128), unsigned(nt)), 128, 0, st>>>(d_X, n_feats, d_jobs + t0,
+                                                                                                learning_rate, d_trees, B);
+            CK_LAUNCH("boost_test_kernel");
+        }
+        if (!out) continue;             // the next launch reuses the scratch in stream order
+        for (int64_t i = 0; i < nt; ++i)
+            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], d_trees + size_t(i) * B.bytes + B.reg.meta, 16, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (int64_t i = 0; i < nt; ++i) {
+            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
+            h_node_count[t] = nc;
+            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
+            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
+            const char *tb = d_trees + size_t(i) * B.bytes;
+            CK(cudaMemcpyAsync(h_nodes + written, tb + B.reg.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(h_values + written, tb + B.reg.values, size_t(nc) * 8, cudaMemcpyDeviceToHost, st));
+            written += nc;
+        }
+        CK(cudaStreamSynchronize(st));
+    }
+    return scratch.done(B200AA_OK);
+}
+
+extern "C" int b200aa_boosting_scale(const double *d_X, int64_t n, int n_feats, int64_t n_problems,
+                                     const int64_t *h_train_off, const int32_t *h_train_idx, const int64_t *h_test_off,
+                                     const int32_t *h_test_idx, float *d_Xs, void *stream)
+{
+    NvtxRange nvtx_("b200aa_boosting_scale");
+    REFUSE_CAPTURE(stream, "b200aa_boosting_scale", kWhyHostArrays);
+    if (!d_X || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !d_Xs || n < 1 || n > (int64_t(1) << 29) ||
+        n_feats < 1 || n_problems < 1 || h_train_off[0] != 0 || h_test_off[0] != 0)
+        return B200AA_ERR_INVALID;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        if (h_train_off[p + 1] - h_train_off[p] < 1 || h_test_off[p + 1] < h_test_off[p]) return B200AA_ERR_INVALID;
+        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
+            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
+        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
+            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
+    }
+    const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems];
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    StreamScratch scratch(st);
+    const size_t b_tr = align256(size_t(n_tr) * 4);
+    const int rc = scratch.alloc(b_tr + align256(size_t(std::max<int64_t>(n_te, 1)) * 4));
+    if (rc != B200AA_OK) return rc;
+    int32_t *d_tr = static_cast<int32_t *>(scratch.get());
+    int32_t *d_te = reinterpret_cast<int32_t *>(static_cast<char *>(scratch.get()) + b_tr);
+    CK(cudaMemcpyAsync(d_tr, h_train_idx, size_t(n_tr) * 4, cudaMemcpyHostToDevice, st));
+    if (n_te) CK(cudaMemcpyAsync(d_te, h_test_idx, size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
+        forest_cv_scale_kernel<<<unsigned((n_feats + 63) / 64), 64, 0, st>>>(
+            d_X, n_feats, d_tr + h_train_off[p], ntr, d_te + h_test_off[p], nte, d_Xs + h_train_off[p] * n_feats,
+            d_Xs + (n_tr + h_test_off[p]) * n_feats);
+        CK_LAUNCH("forest_cv_scale_kernel");
+    }
+    return scratch.done(B200AA_OK);
+}
+
+// One thread per test row: predict's class from the row's K raw scores (boost_class), mapped through the problem's present
+// classes, and counted as counts[p, y_test, y_pred].
+__global__ void boost_count_kernel(const double *__restrict__ raw_test, int64_t n_test, const int32_t *__restrict__ prob,
+                                   const int64_t *__restrict__ raw_off, const int64_t *__restrict__ test_off,
+                                   const int32_t *__restrict__ trees, const int32_t *__restrict__ classes,
+                                   const int32_t *__restrict__ y_test, int n_classes, int32_t *__restrict__ pred,
+                                   unsigned long long *__restrict__ counts)
+{
+    const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (r >= n_test) return;
+    const int32_t p = prob[r], K = trees[p];
+    const int c = forest::boost_class(raw_test + raw_off[p] + (r - test_off[p]) * K, K);
+    const int32_t g = classes[int64_t(p) * forest::kMaxClasses + c];
+    pred[r] = g;
+    atomicAdd(&counts[(int64_t(p) * n_classes + y_test[r]) * n_classes + g], 1ull);
+}
+
+extern "C" int b200aa_boosting_count(const double *d_raw_test, int64_t n_problems, const int64_t *h_test_off,
+                                     const int32_t *h_n_trees, const int32_t *h_classes, const int32_t *h_y_test,
+                                     int n_classes, int32_t *d_pred, int64_t *d_counts, void *stream)
+{
+    NvtxRange nvtx_("b200aa_boosting_count");
+    REFUSE_CAPTURE(stream, "b200aa_boosting_count", kWhyHostArrays);
+    if (!d_raw_test || !h_test_off || !h_n_trees || !h_classes || !h_y_test || !d_pred || !d_counts || n_problems < 1 ||
+        n_classes < 2 || n_classes > forest::kMaxClasses || h_test_off[0] != 0)
+        return B200AA_ERR_INVALID;
+    std::vector<int64_t> raw_off(static_cast<size_t>(n_problems));
+    int64_t o = 0;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        const int32_t K = h_n_trees[p];
+        if (!valid_trees_per_stage(K) || h_test_off[p + 1] < h_test_off[p]) return B200AA_ERR_INVALID;
+        for (int c = 0; c < (K == 1 ? 2 : K); ++c)
+            if (h_classes[p * forest::kMaxClasses + c] < 0 || h_classes[p * forest::kMaxClasses + c] >= n_classes)
+                return B200AA_ERR_INVALID;
+        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
+            if (h_y_test[i] < 0 || h_y_test[i] >= n_classes) return B200AA_ERR_INVALID;
+        raw_off[size_t(p)] = o;
+        o += (h_test_off[p + 1] - h_test_off[p]) * K;
+    }
+    const int64_t n_te = h_test_off[n_problems];
+    std::vector<int32_t> prob(size_t(std::max<int64_t>(n_te, 1)));
+    for (int64_t p = 0; p < n_problems; ++p)
+        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i) prob[size_t(i)] = int32_t(p);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * n_classes * n_classes * sizeof(int64_t), st));
+    if (n_te == 0) return B200AA_OK;
+    // scratch: [prob | raw_off | test_off | trees | classes | y_test]
+    const size_t b_prob = align256(size_t(n_te) * 4), b_off = align256(size_t(n_problems) * 8),
+                 b_toff = align256(size_t(n_problems + 1) * 8), b_trees = align256(size_t(n_problems) * 4),
+                 b_cls = align256(size_t(n_problems) * forest::kMaxClasses * 4), b_y = align256(size_t(n_te) * 4);
+    StreamScratch scratch(st);
+    const int rc = scratch.alloc(b_prob + b_off + b_toff + b_trees + b_cls + b_y);
+    if (rc != B200AA_OK) return rc;
+    char *q = static_cast<char *>(scratch.get());
+    int32_t *d_prob = reinterpret_cast<int32_t *>(q); q += b_prob;
+    int64_t *d_off = reinterpret_cast<int64_t *>(q); q += b_off;
+    int64_t *d_toff = reinterpret_cast<int64_t *>(q); q += b_toff;
+    int32_t *d_trees = reinterpret_cast<int32_t *>(q); q += b_trees;
+    int32_t *d_cls = reinterpret_cast<int32_t *>(q); q += b_cls;
+    int32_t *d_y = reinterpret_cast<int32_t *>(q);
+    CK(cudaMemcpyAsync(d_prob, prob.data(), size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_off, raw_off.data(), size_t(n_problems) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_toff, h_test_off, size_t(n_problems + 1) * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_trees, h_n_trees, size_t(n_problems) * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cls, h_classes, size_t(n_problems) * forest::kMaxClasses * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_y, h_y_test, size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
+    boost_count_kernel<<<unsigned((n_te + 127) / 128), 128, 0, st>>>(d_raw_test, n_te, d_prob, d_off, d_toff, d_trees, d_cls,
+                                                                     d_y, n_classes, d_pred,
+                                                                     reinterpret_cast<unsigned long long *>(d_counts));
+    CK_LAUNCH("boost_count_kernel");
+    return scratch.done(B200AA_OK);
+}

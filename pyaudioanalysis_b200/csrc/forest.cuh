@@ -24,6 +24,7 @@
 #include <cstdint>
 #include <cstring>
 
+#include "front.cuh"
 #include "npsum.cuh"
 
 namespace b200aa {
@@ -719,9 +720,14 @@ struct RegTree {
     double *vproxy;
     int64_t *vpos;
     RegShared *st;
+    // y_stride 0: the target of local sample s is y[row(s)] (the forest's targets of every row); else y[s * y_stride]
+    // (gradient boosting: column k of the problem's [n, K] negative gradients)
+    int32_t y_stride = 0;
+    // DepthFirstTreeBuilder's max_depth: the forest has none (np.iinfo(np.int32).max), gradient boosting 3
+    int32_t max_depth = INT32_MAX;
     __host__ __device__ int64_t row(int32_t s) const { return rows ? int64_t(rows[s]) : int64_t(s); }
     __host__ __device__ float x(int32_t s, int f) const { return X[row(s) * F + f]; }
-    __host__ __device__ double yv(int32_t s) const { return y[row(s)]; }
+    __host__ __device__ double yv(int32_t s) const { return y_stride ? y[int64_t(s) * y_stride] : y[row(s)]; }
     __host__ __device__ double wv(int32_t s) const { return double(w[s]); }
 };
 
@@ -830,7 +836,7 @@ __host__ __device__ inline void build_regression_tree(const RegTree &T, const Te
             S.best_proxy = -INFINITY;
             S.best_v = -1;
             S.n_vis = 0;
-            S.leaf = m < 2 || S.imp <= kLeafEpsilon;
+            S.leaf = rec.depth >= T.max_depth || m < 2 || S.imp <= kLeafEpsilon;
         }
         first = false;
         tm.sync();
@@ -979,6 +985,116 @@ __host__ __device__ inline void build_regression_tree(const RegTree &T, const Te
         }
         tm.sync();
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Gradient boosting: GradientBoostingClassifier(n_estimators).fit with the library's arguments (loss="log_loss",
+// learning_rate=0.1, max_depth=3, subsample=1.0), one stage's trees.  _fit_stage (ensemble/_gb.py) fits k = 0 .. K - 1
+// DecisionTreeRegressor(squared_error, best splitter, max_depth=3, max_features=None) on column k of the stage's negative
+// gradient with unit weights: build_regression_tree with max_depth 3, all-ones weights and y_stride K.  The gradient
+// itself (exp / log) is computed on the host by scikit-learn's own loss object; everything here is ordered float64
+// arithmetic.  _update_terminal_regions then replaces every leaf's value by one Newton step over the rows tree.apply puts
+// in it, in ascending row order:
+//   numerator   = np.average(neg_g, weights=1) = pairwise_sum(neg_g) / count, times (K - 1) / K for the multinomial loss
+//   denominator = np.average(prob * (1 - prob), weights=1), prob = y_k - neg_g (y_k: y for the binomial loss, the
+//                 one-hot column y == k for the multinomial one)
+//   value       = 0.0 when |denominator| < 1e-150 (_safe_divide), else numerator / denominator
+// and adds learning_rate * value[leaf] to raw[:, k].  Internal nodes keep the builder's mean.
+constexpr int kBoostDepth = 3;                              // GradientBoostingClassifier's max_depth
+
+// One boosting tree's extras: its problem's class indices y [n] (0 / 1 for the binomial loss), the tree's raw column k of
+// K, the training raw predictions raw [n, K], the learning rate, leaf_of / leaf_rows [n] (global) and part [team size].
+struct BoostTree {
+    const int32_t *y;
+    int k, K;
+    double *raw;
+    double lr;
+    int32_t *leaf_of, *leaf_rows;
+    int64_t *part;
+};
+
+// tree.apply for one row: left iff x <= threshold (tree/_tree.pyx _apply_dense, float32 compared in float64)
+template <class Xf>
+__host__ __device__ inline int32_t tree_apply(const NodeOut *nodes, const Xf &x)
+{
+    int32_t i = 0;
+    while (nodes[i].left != kTreeLeaf) i = double(x(nodes[i].feature)) <= nodes[i].threshold ? nodes[i].left : nodes[i].right;
+    return i;
+}
+
+// np.add.reduce of a leaf's cnt terms: +0.0 plus NumPy's pairwise sum, without the recursion of npy::pairwise_sum (its
+// frames are not in the kernel's static stack size)
+template <class G>
+__host__ __device__ inline double leaf_sum(const G &get, int64_t cnt)
+{
+    return front::np_sum(get, cnt, true);
+}
+
+// _safe_divide(numerator, denominator) of one leaf from its sums over cnt rows
+__host__ __device__ inline double newton_value(double num_sum, double den_sum, int64_t cnt, int K)
+{
+    double num = ddiv(num_sum, double(cnt));
+    if (K > 1) num = dmul(num, ddiv(double(K - 1), double(K)));
+    const double den = ddiv(den_sum, double(cnt));
+    return fabs(den) < 1e-150 ? 0.0 : ddiv(num, den);
+}
+
+// After build_regression_tree(T): every leaf's Newton value into T.values, then raw[:, k] += lr * value[leaf] for every
+// training row.  Team-parallel but for the leaf sums (thread 0, one leaf after another).
+__host__ __device__ inline void boost_leaves(const RegTree &T, const BoostTree &B, const Team &tm)
+{
+    const int64_t n = T.n;
+    for (int64_t s = tm.tid; s < n; s += tm.n)
+        B.leaf_of[s] = tree_apply(T.nodes, [&T, s](int f) { return T.x(int32_t(s), f); });
+    tm.sync();
+    const int64_t node_count = T.st->node_count, chunk = (n + tm.n - 1) / tm.n;
+    const int64_t q0 = tm.tid * chunk, q1 = q0 + chunk < n ? q0 + chunk : n;
+    for (int64_t id = 0; id < node_count; ++id) {
+        if (T.nodes[id].left != kTreeLeaf) continue;
+        // np.nonzero(masked_terminal_regions == leaf): the leaf's rows in ascending order, each thread's chunk after the
+        // earlier chunks'
+        int64_t c = 0;
+        for (int64_t q = q0; q < q1; ++q) c += B.leaf_of[q] == id;
+        B.part[tm.tid] = c;
+        tm.sync();
+        int64_t o = 0;
+        for (int t = 0; t < tm.tid; ++t) o += B.part[t];
+        for (int64_t q = q0; q < q1; ++q) {
+            const int32_t s = int32_t(q);
+            if (B.leaf_of[s] == id) B.leaf_rows[o++] = s;
+        }
+        tm.sync();
+        if (tm.tid == 0) {
+            int64_t cnt = 0;
+            for (int t = 0; t < tm.n; ++t) cnt += B.part[t];
+            const int32_t *rw = B.leaf_rows;
+            const double num = leaf_sum([&T, rw](int64_t i) { return T.yv(rw[i]); }, cnt);
+            const double den = leaf_sum([&T, &B, rw](int64_t i) {
+                const int32_t s = rw[i];
+                const double yk = B.K == 1 ? double(B.y[s]) : (B.y[s] == B.k ? 1.0 : 0.0);
+                const double prob = dsub(yk, T.yv(s));
+                return dmul(prob, dsub(1.0, prob));
+            }, cnt);
+            T.values[id] = newton_value(num, den, cnt, B.K);
+        }
+        tm.sync();
+    }
+    for (int64_t s = tm.tid; s < n; s += tm.n) {
+        double &r = B.raw[s * B.K + B.k];
+        r = dadd(r, dmul(B.lr, T.values[B.leaf_of[s]]));
+    }
+    tm.sync();
+}
+
+// predict's class of one row from its K raw scores (local class index): raw >= 0 for the binomial loss, else the first
+// maximum (np.argmax)
+__host__ __device__ inline int boost_class(const double *raw, int K)
+{
+    if (K == 1) return raw[0] >= 0.0 ? 1 : 0;
+    int b = 0;
+    for (int c = 1; c < K; ++c)
+        if (raw[c] > raw[b]) b = c;
+    return b;
 }
 
 }  // namespace forest

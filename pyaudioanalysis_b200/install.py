@@ -37,8 +37,9 @@ def install_training(audio_train_test=None):
     the kNN model selection on the GPU (``audioTrainTest.evaluate_classifier`` here) and every other classifier, SMOTE
     and non-finite input through the saved original.  extract_features_and_train looks the function up on the module at
     call time (audioTrainTest.py:309), so it trains kNN models through the GPU unchanged.  train_random_forest and
-    train_extra_trees, where the module has them, are rebound to the GPU trainers here (kernel 13): the final forest
-    extract_features_and_train fits and pickles is built on the GPU, tree for tree scikit-learn's.  Likewise, where the
+    train_extra_trees and train_gradient_boosting, where the module has them, are rebound to the GPU trainers here
+    (kernel 13): the final forest or boosting model extract_features_and_train fits and pickles is built on the GPU, tree
+    for tree scikit-learn's.  Likewise, where the
     module has them, evaluate_regression (its "randomforest" model selection on the GPU, every other method through the
     saved original) and train_random_forest_regression, so feature_extraction_train_regression selects and fits its
     forest on the GPU.  Returns the attributes rebound."""
@@ -50,7 +51,7 @@ def install_training(audio_train_test=None):
     audio_train_test.evaluate_classifier = dispatcher(original)
     done = ["%s.evaluate_classifier" % audio_train_test.__name__]
     from . import audioTrainTest as ours
-    for n in ("train_random_forest", "train_extra_trees"):
+    for n in ("train_random_forest", "train_extra_trees", "train_gradient_boosting"):
         if not hasattr(audio_train_test, n):
             continue
         _saved.setdefault((audio_train_test, n), getattr(audio_train_test, n))
