@@ -36,12 +36,6 @@ TreeLayout tree_layout(int64_t n, int C)
     return L;
 }
 
-// team-shared arrays of build_tree in dynamic shared memory
-inline size_t smem_bytes(int F, int C)
-{
-    return sizeof(forest::Shared) + size_t(F) * (3 * 4 + 2 * 4 + 8) + size_t(forest::kThreads) * (size_t(C) * 8 + 16) + 64;
-}
-
 }  // namespace
 
 __global__ void forest_cast_kernel(const double *__restrict__ X, int64_t n, int F, int64_t stride, float *__restrict__ out)
@@ -114,8 +108,8 @@ extern "C" int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_fe
             if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t smem = smem_bytes(n_feats, n_classes);
-    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const size_t smem = forest::smem_bytes(n_feats, n_classes);
+    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kSmemCap)));
     const TreeLayout L = tree_layout(n, n_classes);
     const size_t per_tree = L.bytes + (h_weights ? align256(size_t(n) * 4) : 0);
     const size_t fixed = align256(size_t(n) * n_feats * 4) + align256(size_t(n) * 4) + align256(size_t(n_trees) * 4);
@@ -254,8 +248,7 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
     if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int C = n_classes, F = n_feats, max_features = forest::sqrt_features(F);
-    const size_t smem = smem_bytes(F, C);
-    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kSmemCap)));
     // scratch: [y_local | train | test | map | Xtr | Xte | acc | seeds | weights of a slice | trees of a slice]
     const TreeLayout Lmax = tree_layout(ntr_max, C);
     const size_t b_y = align256(size_t(ntr_max) * 4), b_tr = b_y, b_te = align256(size_t(std::max<int64_t>(nte_max, 1)) * 4),
@@ -311,7 +304,7 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
         forest_cv_scale_kernel<<<unsigned((F + 63) / 64), 64, 0, st>>>(d_X, F, d_train, ntr, d_test, nte, d_xtr, d_xte);
         CK_LAUNCH("forest_cv_scale_kernel");
         const TreeLayout L = tree_layout(ntr, Cl);
-        const size_t smem_p = smem_bytes(F, Cl);
+        const size_t smem_p = forest::smem_bytes(F, Cl);
         for (int64_t t0 = 0; t0 < T; t0 += slice) {
             const int64_t nt = std::min<int64_t>(slice, T - t0);
             if (d_w) CK(cudaMemcpyAsync(d_w, h_weights + w0 + t0 * ntr, size_t(nt * ntr) * 4, cudaMemcpyHostToDevice, st));
@@ -358,9 +351,6 @@ RegLayout reg_layout(int64_t n, int F)
     L.bytes = L.weights + align256(size_t(n) * 4);
     return L;
 }
-
-// team-shared arrays of build_regression_tree in dynamic shared memory
-inline size_t reg_smem_bytes(int F) { return sizeof(forest::RegShared) + size_t(F) * (5 * 4 + 2 * 4 + 16) + 64; }
 
 // one tree of a launch: its training rows (NULL: rows 0 .. n - 1 of X) and their number
 struct RegJob {
@@ -446,8 +436,8 @@ extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n
     const int64_t slice = reg_slice(fixed, L.bytes, n_trees);
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t smem = reg_smem_bytes(n_feats);
-    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const size_t smem = forest::reg_smem_bytes(n_feats);
+    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
     const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
     if (rc != B200AA_OK) return rc;
@@ -576,8 +566,8 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
     const int64_t slice = std::min<int64_t>(reg_slice(fixed, L.bytes, trees_total), 65535);    // problems per launch: grid y
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t smem = reg_smem_bytes(F);
-    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const size_t smem = forest::reg_smem_bytes(F);
+    CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
     const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
     if (rc != B200AA_OK) return rc;
@@ -687,8 +677,6 @@ BoostLayout boost_layout(int64_t n, int F)
     B.bytes = B.leaf_rows + align256(size_t(n) * 4);
     return B;
 }
-
-inline size_t boost_smem_bytes(int F) { return reg_smem_bytes(F) + size_t(forest::kThreads) * 8; }
 
 }  // namespace
 
@@ -801,8 +789,8 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     if (n_trees == 0) return B200AA_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t smem = boost_smem_bytes(n_feats);
-    CK(cudaFuncSetAttribute(boost_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+    const size_t smem = forest::boost_smem_bytes(n_feats);
+    CK(cudaFuncSetAttribute(boost_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kBoostSmemCap)));
     StreamScratch scratch(st);
     const int rc = scratch.alloc(fixed + size_t(slice) * B.bytes);
     if (rc != B200AA_OK) return rc;

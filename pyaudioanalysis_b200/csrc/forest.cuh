@@ -9,7 +9,7 @@
 // operations of npsum.cuh: no contraction) and the splitter's our_rand_r stream, restated below.
 //
 // build_tree() is the whole DepthFirstTreeBuilder loop for one tree, written for a team of threads: on the device one
-// CTA (Team = the block, sync = __syncthreads), in tests/forest_host.cu a team of one thread on the CPU.  Per node:
+// CTA (Team = the block, sync = __syncthreads), in tests/forest_host.cu a team of std::threads on the CPU.  Per node:
 //   1. class totals and, for every feature, min / max over the node's samples (team-parallel);
 //   2. thread 0 runs node_split_best / node_split_random's Fisher-Yates draw loop with the known / found / drawn
 //      constant bookkeeping and the two memcpys (draw_features); the random splitter's thresholds are drawn there too;
@@ -177,12 +177,28 @@ struct Tree {
     Shared *st;
 };
 
+// Dynamic shared memory of forest_build_kernel (csrc/forest.cu): st, thr [F], cnt [kThreads C], red_proxy / red_pos
+// [kThreads], mn / mx / features / constf / drawn [F].  Every launcher sets the kernel's attribute to kSmemCap, the size at
+// the largest shape it accepts, never to its own call's size: a thread setting a smaller size between another thread's
+// set and launch would make that launch fail.
+constexpr size_t smem_bytes(int F, int C)
+{
+    return sizeof(Shared) + size_t(F) * (3 * 4 + 2 * 4 + 8) + size_t(kThreads) * (size_t(C) * 8 + 16) + 64;
+}
+constexpr size_t kSmemCap = smem_bytes(kMaxFeats, kMaxClasses);
+
+// The team building one tree: on the device the CTA (sync = __syncthreads); on the host, tid / n of threads that meet at
+// wait(wait_ctx), a barrier (tests/ run the builders on std::threads), or a team of one with no wait.
 struct Team {
     int tid, n;
+    void (*wait)(void *) = nullptr;
+    void *wait_ctx = nullptr;
     __host__ __device__ void sync() const
     {
 #ifdef __CUDA_ARCH__
         __syncthreads();
+#else
+        if (wait) wait(wait_ctx);
 #endif
     }
 };
@@ -699,6 +715,11 @@ struct RegShared {
     uint32_t rng;
 };
 
+// Dynamic shared memory of forest_reg_build_kernel: st, vproxy / vpos [F], mn / mx / features / constf / drawn / vis /
+// tied [F]; the attribute is set to kRegSmemCap (as kSmemCap)
+constexpr size_t reg_smem_bytes(int F) { return sizeof(RegShared) + size_t(F) * (5 * 4 + 2 * 4 + 16) + 64; }
+constexpr size_t kRegSmemCap = reg_smem_bytes(kMaxFeats);
+
 // Everything one regression tree reads and writes.  Global: X [rows, F] and y [rows] (shared by every tree; rows[s] is
 // local sample s's row, or s when rows is NULL), w [n] (bootstrap counts), samples / idx [n] and fv [n] (the replay's
 // indices and values), keys [F * pow2_at_least(n)], stack [n + 1], nodes [2 n - 1], values [2 n - 1].  Team-shared:
@@ -730,6 +751,17 @@ struct RegTree {
     __host__ __device__ double yv(int32_t s) const { return y_stride ? y[int64_t(s) * y_stride] : y[row(s)]; }
     __host__ __device__ double wv(int32_t s) const { return double(w[s]); }
 };
+
+// Sets a flag that several of the team's threads may set between two syncs: a plain store on the device, a relaxed
+// atomic one on the host, where concurrent plain stores (even of one value) are a data race to C++ and ThreadSanitizer.
+__host__ __device__ inline void set_flag(int32_t &f)
+{
+#ifdef __CUDA_ARCH__
+    f = 1;
+#else
+    __atomic_store_n(&f, 1, __ATOMIC_RELAXED);
+#endif
+}
 
 __host__ __device__ inline uint64_t reg_key(float v, int32_t s) { return (uint64_t(order_bits(v)) << 32) | uint32_t(s); }
 __host__ __device__ inline float key_value(uint64_t k) { return from_order_bits(uint32_t(k >> 32)); }
@@ -886,7 +918,7 @@ __host__ __device__ inline void build_regression_tree(const RegTree &T, const Te
             }
             for (int64_t i = tm.tid; i < nv * m; i += tm.n) {
                 const int64_t v = i / m, q = i - v * m;
-                if (q >= 1 && key_value(T.keys[v * m2 + q - 1]) == key_value(T.keys[v * m2 + q])) T.tied[v] = 1;
+                if (q >= 1 && key_value(T.keys[v * m2 + q - 1]) == key_value(T.keys[v * m2 + q])) set_flag(T.tied[v]);
             }
             tm.sync();
             // introsort_3way replayed for the visits with ties, in visit order, each from the order the one before left
@@ -1001,6 +1033,11 @@ __host__ __device__ inline void build_regression_tree(const RegTree &T, const Te
 //   value       = 0.0 when |denominator| < 1e-150 (_safe_divide), else numerator / denominator
 // and adds learning_rate * value[leaf] to raw[:, k].  Internal nodes keep the builder's mean.
 constexpr int kBoostDepth = 3;                              // GradientBoostingClassifier's max_depth
+
+// Dynamic shared memory of boost_build_kernel: the regression tree's and part [kThreads]; the attribute is set to
+// kBoostSmemCap (as kSmemCap)
+constexpr size_t boost_smem_bytes(int F) { return reg_smem_bytes(F) + size_t(kThreads) * 8; }
+constexpr size_t kBoostSmemCap = boost_smem_bytes(kMaxFeats);
 
 // One boosting tree's extras: its problem's class indices y [n] (0 / 1 for the binomial loss), the tree's raw column k of
 // K, the training raw predictions raw [n, K], the learning rate, leaf_of / leaf_rows [n] (global) and part [team size].

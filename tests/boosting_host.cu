@@ -1,7 +1,9 @@
 // Host program for tests/test_boosting_cpu.py: runs one gradient boosting stage of kernel 13 (pyaudioanalysis_b200/csrc/
-// forest.cuh: build_regression_tree with max_depth 3, then boost_leaves) on the CPU, with a team of one thread.
+// forest.cuh: build_regression_tree with max_depth 3, then boost_leaves) on the CPU, with a team of TEAM threads
+// (tests/team_host.h; default 1).
 //
-//   boosting_host stage IN OUT     IN: int64 n, n_feats, K; float32 X [n, n_feats]; float64 neg_g [n, K]; int32 y [n];
+//   boosting_host stage IN OUT [TEAM]
+//                                  IN: int64 n, n_feats, K; float32 X [n, n_feats]; float64 neg_g [n, K]; int32 y [n];
 //                                      float64 raw [n, K]; uint32 rand_r seeds [K]; float64 learning_rate
 //                                  OUT: per tree k: int64 node_count, max_depth; nodes [node_count] (48-byte
 //                                       forest::NodeOut); float64 values [node_count]; then float64 raw [n, K]
@@ -12,6 +14,7 @@
 #include <vector>
 
 #include "forest.cuh"
+#include "team_host.h"
 
 using namespace b200aa;
 
@@ -25,7 +28,9 @@ static std::vector<T> rd(FILE *f, size_t n)
 
 int main(int argc, char **argv)
 {
-    if (argc != 4) return 2;
+    if (argc != 4 && argc != 5) return 2;
+    const int team = argc == 5 ? atoi(argv[4]) : 1;
+    if (team < 1 || team > forest::kThreads) return 2;
     FILE *in = fopen(argv[2], "rb");
     FILE *out = fopen(argv[3], "wb");
     if (!in || !out) return 2;
@@ -56,16 +61,18 @@ int main(int argc, char **argv)
     std::vector<forest::StackRec> stack(n + 1);
     std::vector<forest::NodeOut> nodes(2 * n - 1);
     std::vector<double> values(2 * n - 1), vproxy(F);
-    std::vector<int64_t> vpos(F), part(1);
+    std::vector<int64_t> vpos(F), part(team);
     forest::RegShared st{};
     for (int k = 0; k < K; ++k) {
         const forest::RegTree T{X.data(), neg_g.data() + k, nullptr, w.data(), n, F, samples.data(), idx.data(), fv.data(),
                                 keys.data(), stack.data(), nodes.data(), values.data(), features.data(), constf.data(),
                                 drawn.data(), vis.data(), tied.data(), mn.data(), mx.data(), vproxy.data(), vpos.data(), &st,
                                 K, forest::kBoostDepth};
-        const forest::Team tm{0, 1};
-        forest::build_regression_tree(T, tm, seeds[k]);
-        forest::boost_leaves(T, forest::BoostTree{y.data(), k, K, raw.data(), lr, leaf_of.data(), rows.data(), part.data()}, tm);
+        const forest::BoostTree B{y.data(), k, K, raw.data(), lr, leaf_of.data(), rows.data(), part.data()};
+        team_host::run_team(team, [&](const forest::Team &tm) {
+            forest::build_regression_tree(T, tm, seeds[k]);
+            forest::boost_leaves(T, B, tm);
+        });
         const int64_t head[2] = {st.node_count, st.max_depth};
         fwrite(head, sizeof(int64_t), 2, out);
         fwrite(nodes.data(), sizeof(forest::NodeOut), size_t(st.node_count), out);

@@ -47,12 +47,35 @@ def problems():
     return out
 
 
-def palindrome(seed):
-    """Labels symmetric along the sorted values, so splits at p and n - p tie in exact arithmetic: the proxy's rounding
-    decides between them (a fused multiply-add breaks the tie the other way for this seed)."""
+def palindrome(seed, n=40):
+    """n (even) labels symmetric along the sorted values, so splits at p and n - p tie in exact arithmetic: the proxy's
+    rounding decides between them (a fused multiply-add breaks the tie the other way for seed 39 at n = 40).  At n of a
+    few hundred the tied positions fall in different threads' chunks of a 128-thread team."""
     r = np.random.RandomState(seed)
-    h = r.randint(0, 3, 20)
-    return np.stack([np.arange(40.0), r.permutation(40).astype(float)], 1), np.concatenate([h, h[::-1]])
+    h = r.randint(0, 3, n // 2)
+    return np.stack([np.arange(float(n)), r.permutation(n).astype(float)], 1), np.concatenate([h, h[::-1]])
+
+
+# root sizes at the builders' team and padding edges: the 128-thread team, and the bitonic sort's power-of-two padding
+ROOT_SIZES = (127, 128, 129, 255, 256, 257, 1025)
+
+
+def limits(seed=41, n=400):
+    """(X, y) at the launchers' limits: 512 features (kMaxFeats) and 32 classes (kMaxClasses), each class present."""
+    r = np.random.RandomState(seed)
+    X = r.randn(n, 512)
+    y = r.permutation(np.arange(n) % 32)
+    X[:, :8] += 0.5 * (y[:, None] % 8 == np.arange(8))          # some signal, so the trees grow deep and wide
+    return X, y
+
+
+def duplicated_columns(seed, n=300, F=6, decimals=None):
+    """(X, y) whose columns F .. 2F - 1 repeat columns 0 .. F - 1: every split found on one copy ties with the other, and
+    the copy visited first must win; `decimals` rounds X so that the values tie within a column too."""
+    r = np.random.RandomState(seed)
+    X = r.randn(n, F) if decimals is None else np.round(r.randn(n, F), decimals)
+    y = (X[:, 0] + X[:, 1] > 0).astype(int) + (X[:, 2] > 0.5)
+    return np.hstack([X, X]), y
 
 
 def compare(got, ref):

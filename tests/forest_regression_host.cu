@@ -1,9 +1,10 @@
 // Host program for tests/test_forest_regression_cpu.py: runs kernel 13's regression pieces (pyaudioanalysis_b200/csrc/
-// forest.cuh) on the CPU, with a team of one thread for the tree builder.
+// forest.cuh) on the CPU, with a team of TEAM threads for the tree builder (tests/team_host.h; default 1).
 //
 //   forest_regression_host sort IN OUT   IN: int64 n; float32 values [n]; int32 indices [n]
 //                                        OUT: the values and indices after introsort_3way
-//   forest_regression_host fit IN OUT    IN: int64 n, n_feats, n_trees; float32 X [n, n_feats]; float64 y [n];
+//   forest_regression_host fit IN OUT [TEAM]
+//                                        IN: int64 n, n_feats, n_trees; float32 X [n, n_feats]; float64 y [n];
 //                                            int32 weights [n_trees, n]; uint32 rand_r seeds [n_trees]
 //                                        OUT: per tree: int64 node_count, max_depth; nodes [node_count] (48-byte
 //                                             forest::NodeOut); float64 values [node_count]
@@ -13,6 +14,7 @@
 #include <vector>
 
 #include "forest.cuh"
+#include "team_host.h"
 
 using namespace b200aa;
 
@@ -26,7 +28,9 @@ static std::vector<T> rd(FILE *f, size_t n)
 
 int main(int argc, char **argv)
 {
-    if (argc != 4) return 2;
+    if (argc != 4 && argc != 5) return 2;
+    const int team = argc == 5 ? atoi(argv[4]) : 1;
+    if (team < 1 || team > forest::kThreads) return 2;
     FILE *in = fopen(argv[2], "rb");
     FILE *out = fopen(argv[3], "wb");
     if (!in || !out) return 2;
@@ -60,7 +64,7 @@ int main(int argc, char **argv)
         const forest::RegTree T{X.data(), y.data(), nullptr, w.data() + t * n, n, F, samples.data(), idx.data(), fv.data(),
                                 keys.data(), stack.data(), nodes.data(), values.data(), features.data(), constf.data(),
                                 drawn.data(), vis.data(), tied.data(), mn.data(), mx.data(), vproxy.data(), vpos.data(), &st};
-        forest::build_regression_tree(T, forest::Team{0, 1}, seeds[t]);
+        team_host::run_team(team, [&](const forest::Team &tm) { forest::build_regression_tree(T, tm, seeds[t]); });
         const int64_t head[2] = {st.node_count, st.max_depth};
         fwrite(head, sizeof(int64_t), 2, out);
         fwrite(nodes.data(), sizeof(forest::NodeOut), size_t(st.node_count), out);

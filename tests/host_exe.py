@@ -34,6 +34,45 @@ def build(tmp_path_factory, source, *flags):
     return exe
 
 
+TEAMS = (1, 3, 8)
+
+
+def team_params(cases, big_rows=2000):
+    """pytest params (case, team) running every case of kernel 13's builders at each team size of TEAMS: the team of one
+    with the ids the cases had before teams, the others as "<case>-team<t>"; cases of big_rows rows or more at teams 1
+    and 3 only (a team of 8 host threads meets its barrier thousands of times per node).  A case is (name, X, ...)."""
+    out = []
+    for c in cases:
+        for t in TEAMS:
+            if t == 1 or t == 3 or c[1].shape[0] < big_rows:
+                out.append(pytest.param(c, t, id=c[0] if t == 1 else "%s-team%d" % (c[0], t)))
+    return out
+
+
+def tsan_flags():
+    """nvcc flags of a ThreadSanitizer build of a host harness, or skip the test when the toolchain has no libtsan."""
+    res = subprocess.run(["gcc", "-print-file-name=libtsan.so"], capture_output=True, text=True) if shutil.which("gcc") else None
+    if res is None or res.returncode != 0 or not os.path.isabs(res.stdout.strip()):
+        pytest.skip("libtsan not available")
+    return ("-g", "-Xcompiler", "-fsanitize=thread", "-Xlinker", "-ltsan")
+
+
+def tsan_reports(cmd, log_prefix, timeout=120):
+    """Run a ThreadSanitizer build of a harness (``cmd``) with its reports logged to ``log_prefix``.<pid>, and return them.
+
+    Meant for builds with a barrier deleted: such a build reads what another thread has not written yet, and what it
+    does next (a wrong tree, an index past a buffer, a crash, a loop that does not end) depends on timing.  So its exit
+    status and output are ignored and it is killed after ``timeout`` seconds; only the race reports count, and
+    ThreadSanitizer writes those at the racing access, before anything that access leads to."""
+    env = dict(os.environ, TSAN_OPTIONS="exitcode=0 log_path=%s" % log_prefix)
+    try:
+        subprocess.run(cmd, capture_output=True, timeout=timeout, env=env)
+    except subprocess.TimeoutExpired:
+        pass
+    d, base = os.path.split(str(log_prefix))
+    return "".join(open(os.path.join(d, f), errors="replace").read() for f in sorted(os.listdir(d)) if f.startswith(base + "."))
+
+
 def hexes(values):
     """values (any shape) as float64 hex floats separated by spaces."""
     return " ".join(float(x).hex() for x in np.asarray(values, dtype=np.float64).ravel())

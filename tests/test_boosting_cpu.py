@@ -1,8 +1,9 @@
 """CPU: kernel 13's gradient boosting stage (csrc/forest.cuh build_regression_tree with max_depth 3, boost_leaves) run on
-the host by tests/boosting_host.cu, driven stage by stage with scikit-learn's own loss (pyaudioanalysis_b200.boosting),
+the host by tests/boosting_host.cu with teams of 1, 3 and 8 threads (tests/team_host.h), driven stage by stage with scikit-learn's own loss (pyaudioanalysis_b200.boosting),
 against GradientBoostingClassifier.fit on the case bank (tests/boosting_cases.py): every tree in bits, train_score_,
 init_, classes_, NumPy's global state and the predictions.  Also: one stage on crafted gradients against scikit-learn's own
-_update_terminal_regions, named mutants caught, the refusals, the entry points' argument checks and the scratch refusal."""
+_update_terminal_regions, named mutants caught (those of the team-parallel code at a team of 3), a ThreadSanitizer build
+free of races that finds a deleted barrier, the refusals, the entry points' argument checks and the scratch refusal."""
 import ctypes
 import os
 import subprocess
@@ -18,7 +19,7 @@ pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not availa
 CSRC = os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc")
 
 
-def _build(tmp_path_factory, replaces=()):
+def _build(tmp_path_factory, replaces=(), flags=("-O1",)):
     """The harness over forest.cuh, or over a copy with (old, new) replacements made (a mutant)."""
     inc = CSRC
     if replaces:
@@ -29,7 +30,7 @@ def _build(tmp_path_factory, replaces=()):
         d = tmp_path_factory.mktemp("mutant")
         (d / "forest.cuh").write_text(src)
         inc = str(d)
-    return host_exe.build(tmp_path_factory, "boosting_host.cu", "-O1", "-I" + inc, "-I" + CSRC)
+    return host_exe.build(tmp_path_factory, "boosting_host.cu", *flags, "-I" + inc, "-I" + CSRC)
 
 
 @pytest.fixture(scope="module")
@@ -37,17 +38,25 @@ def exe(tmp_path_factory):
     return _build(tmp_path_factory)
 
 
-def host_stage(exe, tmp_path, X32, neg_g, y, raw, seeds, lr=0.1):
-    """One stage through the harness: ([(node_count, max_depth, nodes, values)] per tree, raw after the stage)."""
+def stage_input(tmp_path, X32, neg_g, y, raw, seeds, lr=0.1):
+    """The harness's input for one stage: (src, dst)."""
+    n, F = X32.shape
+    src, dst = str(tmp_path / "in.bin"), str(tmp_path / "out.bin")
+    with open(src, "wb") as f:
+        for a in (np.array([n, F, raw.shape[1]], np.int64), X32.astype(np.float32), neg_g.astype(np.float64),
+                  np.asarray(y, np.int32), raw.astype(np.float64), np.asarray(seeds, np.uint32), np.float64(lr)):
+            f.write(np.ascontiguousarray(a).tobytes())
+    return src, dst
+
+
+def host_stage(exe, tmp_path, X32, neg_g, y, raw, seeds, lr=0.1, team=1):
+    """One stage through the harness with a team of `team` threads: ([(node_count, max_depth, nodes, values)] per tree,
+    raw after the stage)."""
     from pyaudioanalysis_b200 import forests as FO
     n, F = X32.shape
     K = raw.shape[1]
-    src, dst = str(tmp_path / "in.bin"), str(tmp_path / "out.bin")
-    with open(src, "wb") as f:
-        for a in (np.array([n, F, K], np.int64), X32.astype(np.float32), neg_g.astype(np.float64),
-                  np.asarray(y, np.int32), raw.astype(np.float64), np.asarray(seeds, np.uint32), np.float64(lr)):
-            f.write(np.ascontiguousarray(a).tobytes())
-    res = subprocess.run([exe, "stage", src, dst], capture_output=True, text=True)
+    src, dst = stage_input(tmp_path, X32, neg_g, y, raw, seeds, lr)
+    res = subprocess.run([exe, "stage", src, dst, str(team)], capture_output=True, text=True)
     assert res.returncode == 0, res.stderr
     raw_out, off, trees = open(dst, "rb").read(), 0, []
     for _ in range(K):
@@ -61,7 +70,7 @@ def host_stage(exe, tmp_path, X32, neg_g, y, raw, seeds, lr=0.1):
     return trees, np.frombuffer(raw_out, np.float64, n * K, off).reshape(n, K).copy()
 
 
-def host_fit(exe, tmp_path, X, y, T):
+def host_fit(exe, tmp_path, X, y, T, team=1):
     """GradientBoostingClassifier(T).fit(X, y) with every stage's trees built by the host harness."""
     from pyaudioanalysis_b200 import boosting as BO
     est, X32, y_enc, raw0 = BO.begin(X, y, T)
@@ -71,7 +80,7 @@ def host_fit(exe, tmp_path, X, y, T):
     factor, sw = BO.loss_factor(est._loss), np.ones(X32.shape[0])
     for i in range(T):
         states, raw = host_stage(exe, tmp_path, X32, BO.neg_gradient(est._loss, y_enc, raw), y_enc, raw,
-                                 seeds[i * K:(i + 1) * K])
+                                 seeds[i * K:(i + 1) * K], team=team)
         est.train_score_[i] = factor * est._loss(y_true=y_enc, raw_prediction=raw, sample_weight=sw)
         for k, s in enumerate(states):
             est.estimators_[i, k] = BO.make_tree(est, X32.shape[1], s)
@@ -79,10 +88,10 @@ def host_fit(exe, tmp_path, X, y, T):
     return est
 
 
-def _check(exe, tmp_path, X, y, T, seed=7):
+def _check(exe, tmp_path, X, y, T, seed=7, team=1):
     from sklearn.ensemble import GradientBoostingClassifier
     np.random.seed(seed)
-    got = host_fit(exe, tmp_path, X, y, T)
+    got = host_fit(exe, tmp_path, X, y, T, team)
     s_got = np.random.get_state()
     np.random.seed(seed)
     ref = GradientBoostingClassifier(n_estimators=T).fit(X, y)
@@ -90,10 +99,10 @@ def _check(exe, tmp_path, X, y, T, seed=7):
     BC.compare(got, ref, BC.held_out(X))
 
 
-@pytest.mark.parametrize("case", [c[0] for c in BC.problems()])
-def test_fit_equals_sklearn(exe, tmp_path, case):
-    _, X, y, T = next(c for c in BC.problems() if c[0] == case)
-    _check(exe, tmp_path, X, y, T)
+@pytest.mark.parametrize("case,team", host_exe.team_params(BC.problems()))
+def test_fit_equals_sklearn(exe, tmp_path, case, team):
+    _, X, y, T = case
+    _check(exe, tmp_path, X, y, T, team=team)
 
 
 def _sk_stage(X32, neg_g, y_enc, raw, seeds, lr=0.1):
@@ -169,7 +178,8 @@ def _predict_cases(exe, tmp_path):
     return host_predict(exe, tmp_path, raw1).tolist() == [1, 1, 1, 0]
 
 
-# (name, replacements): each mutant must fail at least one case of the bank, the crafted stage or the predict rule
+# (name, replacements): each mutant must fail at least one case of the bank, the crafted stage or the predict rule (those
+# in TEAM_MUTANTS at a team of 3)
 MUTANTS = [
     ("no_depth_limit", [("S.leaf = rec.depth >= T.max_depth || m < 2", "S.leaf = m < 2")]),
     ("partition_order", [("            const int32_t s = int32_t(q);\n", "            const int32_t s = T.samples[q];\n")]),
@@ -180,16 +190,22 @@ MUTANTS = [
     ("fma_raw_update", [("        r = dadd(r, dmul(B.lr, T.values[B.leaf_of[s]]));",
                          "        r = std::fma(B.lr, T.values[B.leaf_of[s]], r);")]),
     ("strict_binary_predict", [("    if (K == 1) return raw[0] >= 0.0 ? 1 : 0;", "    if (K == 1) return raw[0] > 0.0 ? 1 : 0;")]),
+    # every thread writes its rows of a leaf from offset 0 instead of after the earlier threads' rows
+    ("leaf_rows_from_zero", [("        for (int t = 0; t < tm.tid; ++t) o += B.part[t];\n", "")]),
 ]
+TEAM_MUTANTS = {"leaf_rows_from_zero"}
 
 
 @pytest.mark.parametrize("name", [m[0] for m in MUTANTS])
 def test_mutants_are_caught(tmp_path_factory, tmp_path, name):
     exe = _build(tmp_path_factory, dict(MUTANTS)[name])
+    team = 3 if name in TEAM_MUTANTS else 1
     failed = []
     if not _predict_cases(exe, tmp_path):
         failed.append("predict")
     for K in (1, 3):
+        if team > 1:
+            break
         try:
             test_crafted_gradients_hit_the_guard(exe, tmp_path, K)
         except AssertionError:
@@ -198,10 +214,41 @@ def test_mutants_are_caught(tmp_path_factory, tmp_path, name):
         if failed:
             break
         try:
-            _check(exe, tmp_path, X, y, min(T, 3))
+            _check(exe, tmp_path, X, y, min(T, 3), team=team)
         except AssertionError:
             failed.append(case)
     assert failed, name
+
+
+# A barrier deleted from boost_leaves (thread 0 sums a leaf's rows before the other threads have written theirs): a race
+# whose outcome depends on timing, so it is ThreadSanitizer's to find
+SYNC_MUTANT = ("            if (B.leaf_of[s] == id) B.leaf_rows[o++] = s;\n        }\n        tm.sync();\n",
+               "            if (B.leaf_of[s] == id) B.leaf_rows[o++] = s;\n        }\n")
+
+
+@pytest.mark.parametrize("mutant", [False, True], ids=["builder", "deleted_sync"])
+def test_thread_sanitizer(tmp_path_factory, tmp_path, monkeypatch, mutant):
+    """The stage built with ThreadSanitizer, at a team of 4 on small binary and multiclass problems: no report (and the
+    fit still equals scikit-learn's); with one barrier deleted, a data race is reported on every problem's first stage.
+    The mutant's run is judged by its reports alone (host_exe.tsan_reports): after the racing read it may sum rows that
+    are not the leaf's, crash or not end, as timing has it."""
+    from pyaudioanalysis_b200 import boosting as BO
+    tsan = _build(tmp_path_factory, [SYNC_MUTANT] if mutant else (), ("-O1",) + host_exe.tsan_flags())
+    for name, X, y, T in [c for c in BC.problems() if c[0] in ("binary", "three_class", "tiny_three", "dup_rows")]:
+        if mutant:
+            np.random.seed(3)
+            est, X32, y_enc, raw0 = BO.begin(X, y, 1)
+            K = est.n_trees_per_iteration_
+            raw = np.ascontiguousarray(np.broadcast_to(raw0, (X32.shape[0], K)))
+            src, dst = stage_input(tmp_path, X32, BO.neg_gradient(est._loss, y_enc, raw), y_enc, raw, BO.draw_seeds(K))
+            logs = tmp_path / ("tsan_" + name)
+            assert "WARNING: ThreadSanitizer: data race" in host_exe.tsan_reports([tsan, "stage", src, dst, "4"], logs), name
+        else:
+            monkeypatch.setenv("TSAN_OPTIONS", "exitcode=0 log_path=%s" % (tmp_path / "tsan"))
+            _check(tsan, tmp_path, X, y, 2, team=4)
+    if not mutant:
+        reports = "".join(p.read_text() for p in tmp_path.glob("tsan*"))
+        assert reports == "", reports[:4000]
 
 
 def test_refusals():

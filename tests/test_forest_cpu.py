@@ -1,8 +1,9 @@
-"""CPU: kernel 13's tree builder (csrc/forest.cuh, build_tree) run on the host by tests/forest_host.cu with a team of
-one thread, fed by the host draws of pyaudioanalysis_b200.forests, against scikit-learn 1.9's RandomForestClassifier /
-ExtraTreesClassifier fit on seeded problems: every tree's state in bits, the estimators' fitted attributes and NumPy's
-global state afterwards.  Also: named mutants of the builder are caught, the refusals, and the argument checks of
-b200aa_forest_fit."""
+"""CPU: kernel 13's tree builder (csrc/forest.cuh, build_tree) run on the host by tests/forest_host.cu with teams of 1, 3
+and 8 threads (tests/team_host.h), fed by the host draws of pyaudioanalysis_b200.forests, against scikit-learn 1.9's
+RandomForestClassifier / ExtraTreesClassifier fit on seeded problems: every tree's state in bits, the estimators' fitted
+attributes and NumPy's global state afterwards.  Also: named mutants of the builder are caught (those of its
+team-parallel code at a team of 3), a ThreadSanitizer build finds no race in the builder and finds a deleted barrier, the
+refusals, and the argument checks of b200aa_forest_fit."""
 import ctypes
 import os
 import subprocess
@@ -18,7 +19,7 @@ pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not availa
 CSRC = os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc")
 
 
-def _build(tmp_path_factory, replace=None):
+def _build(tmp_path_factory, replace=None, flags=("-O1",)):
     """The harness over forest.cuh, or over a copy with one (old, new) replacement made (a mutant)."""
     inc = CSRC
     if replace is not None:
@@ -28,7 +29,7 @@ def _build(tmp_path_factory, replace=None):
         d = tmp_path_factory.mktemp("mutant")
         (d / "forest.cuh").write_text(src.replace(old, new))
         inc = str(d)
-    return host_exe.build(tmp_path_factory, "forest_host.cu", "-O1", "-I" + inc, "-I" + CSRC)
+    return host_exe.build(tmp_path_factory, "forest_host.cu", *flags, "-I" + inc, "-I" + CSRC)
 
 
 @pytest.fixture(scope="module")
@@ -36,19 +37,29 @@ def exe(tmp_path_factory):
     return _build(tmp_path_factory)
 
 
-def host_fit(exe, tmp_path, X, y, n_estimators, kind):
-    """The estimator fit builds, every tree built by the host harness."""
+def fit_input(tmp_path, X, y, n_estimators, kind):
+    """The harness's input for the fit of X, y, drawn from NumPy's global state as fit draws: (src, dst, est, trees,
+    classes)."""
     from pyaudioanalysis_b200 import forests as FO
     classes, y_idx = np.unique(y, return_inverse=True)
     n, F = X.shape
-    C = len(classes)
     est, trees, w, seeds = FO.draw(n_estimators, kind, n)
-    head = np.array([n, F, C, FO.KINDS[kind], n_estimators, max(1, int(np.sqrt(F))), w is not None], dtype=np.int64)
+    head = np.array([n, F, len(classes), FO.KINDS[kind], n_estimators, max(1, int(np.sqrt(F))), w is not None],
+                    dtype=np.int64)
     src, dst = str(tmp_path / "in.bin"), str(tmp_path / "out.bin")
     with open(src, "wb") as f:
         for a in (head, X.astype(np.float32), y_idx.astype(np.int32)) + ((w,) if w is not None else ()) + (seeds,):
             f.write(np.ascontiguousarray(a).tobytes())
-    res = subprocess.run([exe, src, dst], capture_output=True, text=True)
+    return src, dst, est, trees, classes
+
+
+def host_fit(exe, tmp_path, X, y, n_estimators, kind, team=1):
+    """The estimator fit builds, every tree built by the host harness with a team of `team` threads."""
+    from pyaudioanalysis_b200 import forests as FO
+    n, F = X.shape
+    src, dst, est, trees, classes = fit_input(tmp_path, X, y, n_estimators, kind)
+    C = len(classes)
+    res = subprocess.run([exe, src, dst, str(team)], capture_output=True, text=True)
     assert res.returncode == 0, res.stderr
     raw, off, states = open(dst, "rb").read(), 0, []
     for _ in range(n_estimators):
@@ -67,27 +78,27 @@ def _sklearn(kind):
     return RandomForestClassifier if kind == "randomforest" else ExtraTreesClassifier
 
 
-def _check(exe, tmp_path, X, y, kind, n_estimators=4, seed=11):
+def _check(exe, tmp_path, X, y, kind, n_estimators=4, seed=11, team=1):
     np.random.seed(seed)
     ref = _sklearn(kind)(n_estimators=n_estimators).fit(X, y)
     ref_state = np.random.get_state()
     np.random.seed(seed)
-    got = host_fit(exe, tmp_path, X, y, n_estimators, kind)
+    got = host_fit(exe, tmp_path, X, y, n_estimators, kind, team)
     assert FC.same_state(np.random.get_state(), ref_state)
     FC.compare(got, ref)
     return got, ref
 
 
 @pytest.mark.parametrize("kind", ["randomforest", "extratrees"])
-@pytest.mark.parametrize("case", FC.problems(), ids=lambda c: c[0])
-def test_trees_equal_sklearn(exe, tmp_path, kind, case):
+@pytest.mark.parametrize("case,team", host_exe.team_params(FC.problems()))
+def test_trees_equal_sklearn(exe, tmp_path, kind, case, team):
     _, X, y = case
-    got, ref = _check(exe, tmp_path, X, y, kind)
+    got, ref = _check(exe, tmp_path, X, y, kind, team=team)
     assert np.array_equal(got.predict_proba(X), ref.predict_proba(X))
     assert np.array_equal(got.feature_importances_, ref.feature_importances_)
 
 
-# Named mutants of the builder: each must change some tree of these problems.
+# Named mutants of the builder: each must change some tree of these problems (those in TEAM_MUTANTS at a team of 3).
 MUTANTS = {
     # every node draws from a fresh 0..F-1 permutation with no known constants, instead of the carried splitter state
     "sequential_feature_state": (
@@ -98,26 +109,66 @@ MUTANTS = {
     "ge_instead_of_gt": ("if (pr > bp) {", "if (pr >= bp) {"),
     # a fused multiply-add in the proxy
     "fma_in_proxy": ("return dsub(dmul(-wr, gr), dmul(wl, gl));", "return std::fma(-wl, gl, dmul(-wr, gr));"),
+    # the cross-thread reduction of eval_best keeps the last thread of a tied proxy instead of the first
+    "reduction_keeps_last_tie": ("if (T.red_pos[t] >= 0 && T.red_proxy[t] > fp) {", "if (T.red_pos[t] >= 0 && T.red_proxy[t] >= fp) {"),
+    # eval_best starts every thread's chunk at zero counts instead of the earlier chunks' sums
+    "chunk_counts_from_zero": ("for (int t = 0; t < tm.tid; ++t) a += T.cnt[int64_t(t) * T.C + c];", ""),
+    # partition places every chunk's right-hand samples as if no earlier chunk had any
+    "partition_drops_right_offsets": ("rb += len - T.red_pos[t2];", "(void)len;"),
 }
+TEAM_MUTANTS = {"reduction_keeps_last_tie", "chunk_counts_from_zero", "partition_drops_right_offsets"}
 
 
 @pytest.mark.parametrize("name", sorted(MUTANTS))
 def test_mutants_are_caught(tmp_path_factory, tmp_path, name):
     mexe = _build(tmp_path_factory, MUTANTS[name])
+    team = 3 if name in TEAM_MUTANTS else 1
     kinds = ["randomforest"] if name != "sequential_feature_state" else ["randomforest", "extratrees"]
     cases = [(5, X, y) for _, X, y in FC.problems() if X.shape[0] >= 3] + [(39, *FC.palindrome(39))]
+    if team > 1:
+        cases = [c for c in cases if c[1].shape[0] <= 1000]
     caught = 0
     for kind in kinds:
         for seed, X, y in cases:
             np.random.seed(seed)
             ref = _sklearn(kind)(n_estimators=3).fit(X, y)
             np.random.seed(seed)
-            got = host_fit(mexe, tmp_path, X, y, 3, kind)
+            got = host_fit(mexe, tmp_path, X, y, 3, kind, team)
             try:
                 FC.compare(got, ref)
             except AssertionError:
                 caught += 1
     assert caught > 0, name
+
+
+# A barrier deleted from the builder (class_counts sums the per-thread counts before every thread has written its own):
+# a race whose outcome depends on timing, so it is ThreadSanitizer's to find, not the comparison's
+SYNC_MUTANT = ("    T.red_pos[tm.tid] = k;\n    tm.sync();\n", "    T.red_pos[tm.tid] = k;\n")
+
+
+@pytest.mark.parametrize("mutant", [False, True], ids=["builder", "deleted_sync"])
+def test_thread_sanitizer(tmp_path_factory, tmp_path, monkeypatch, mutant):
+    """The builder built with ThreadSanitizer, at a team of 4 on small problems of both kinds: no report (and the trees
+    still equal scikit-learn's); with one barrier deleted, a data race is reported on every problem.  The mutant's run
+    is judged by its reports alone (host_exe.tsan_reports): after the racing read it may build a wrong tree, crash or
+    not end, as timing has it."""
+    tsan = _build(tmp_path_factory, SYNC_MUTANT if mutant else None, ("-O1",) + host_exe.tsan_flags())
+    cases = [c for c in FC.problems() if c[0] in ("one_row", "single_class", "strings_f2", "gauss_11x300_c4")]
+    if mutant:
+        cases = cases[2:]                       # one_row and single_class build no split: nothing to count
+    for kind in ("randomforest", "extratrees"):
+        for name, X, y in cases + [("palindrome", *FC.palindrome(39))]:
+            if mutant:
+                np.random.seed(3)
+                src, dst = fit_input(tmp_path, X, y, 2, kind)[:2]
+                logs = tmp_path / ("tsan_%s_%s" % (kind, name))
+                assert "WARNING: ThreadSanitizer: data race" in host_exe.tsan_reports([tsan, src, dst, "4"], logs), (kind, name)
+            else:
+                monkeypatch.setenv("TSAN_OPTIONS", "exitcode=0 log_path=%s" % (tmp_path / "tsan"))
+                _check(tsan, tmp_path, X, y, kind, n_estimators=2, team=4)
+    if not mutant:
+        reports = "".join(p.read_text() for p in tmp_path.glob("tsan*"))
+        assert reports == "", reports[:4000]
 
 
 def test_global_state_after_many_trees(exe, tmp_path):

@@ -1,8 +1,10 @@
 """CPU: kernel 13's regression pieces (csrc/forest.cuh) run on the host by tests/forest_regression_host.cu: the
 introsort_3way replay against scikit-learn's own simultaneous_sort permutation for permutation, and the tree builder, with
-a team of one thread fed by pyaudioanalysis_b200.forests' host draws, against RandomForestRegressor.fit on the case bank
-(tests/forest_regression_cases.py): every tree's state in bits, the fitted attributes and NumPy's global state.  Also:
-named mutants of the builder are caught, the refusals, and the argument checks of both entry points."""
+teams of 1, 3 and 8 threads (tests/team_host.h) fed by pyaudioanalysis_b200.forests' host draws, against
+RandomForestRegressor.fit on the case bank (tests/forest_regression_cases.py): every tree's state in bits, the fitted
+attributes and NumPy's global state.  Also: named mutants of the builder are caught (those of its team-parallel code at
+a team of 3), a ThreadSanitizer build finds no race in the builder and finds a deleted barrier, the refusals, and the
+argument checks of both entry points."""
 import ctypes
 import os
 import subprocess
@@ -18,7 +20,7 @@ pytestmark = pytest.mark.skipif(host_exe.nvcc() is None, reason="nvcc not availa
 CSRC = os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc")
 
 
-def _build(tmp_path_factory, replaces=()):
+def _build(tmp_path_factory, replaces=(), flags=("-O1",)):
     """The harness over forest.cuh, or over a copy with (old, new) replacements made (a mutant)."""
     inc = CSRC
     if replaces:
@@ -29,7 +31,7 @@ def _build(tmp_path_factory, replaces=()):
         d = tmp_path_factory.mktemp("mutant")
         (d / "forest.cuh").write_text(src)
         inc = str(d)
-    return host_exe.build(tmp_path_factory, "forest_regression_host.cu", "-O1", "-I" + inc, "-I" + CSRC)
+    return host_exe.build(tmp_path_factory, "forest_regression_host.cu", *flags, "-I" + inc, "-I" + CSRC)
 
 
 @pytest.fixture(scope="module")
@@ -48,8 +50,8 @@ def host_sort(exe, tmp_path, values, indices):
     return np.frombuffer(raw, np.float32, n), np.frombuffer(raw, np.int32, n, 4 * n)
 
 
-def host_fit(exe, tmp_path, X, y, n_estimators):
-    """The regressor fit builds, every tree built by the host harness."""
+def fit_input(tmp_path, X, y, n_estimators):
+    """The harness's input for the fit of X, y, drawn from NumPy's global state as fit draws: (src, dst, est, trees)."""
     from pyaudioanalysis_b200 import forests as FO
     n, F = X.shape
     est, trees, w, seeds = FO.draw(n_estimators, FO.REGRESSOR, n)
@@ -57,7 +59,15 @@ def host_fit(exe, tmp_path, X, y, n_estimators):
     with open(src, "wb") as f:
         for a in (np.array([n, F, n_estimators], np.int64), X.astype(np.float32), np.asarray(y, np.float64), w, seeds):
             f.write(np.ascontiguousarray(a).tobytes())
-    res = subprocess.run([exe, "fit", src, dst], capture_output=True, text=True)
+    return src, dst, est, trees
+
+
+def host_fit(exe, tmp_path, X, y, n_estimators, team=1):
+    """The regressor fit builds, every tree built by the host harness with a team of `team` threads."""
+    from pyaudioanalysis_b200 import forests as FO
+    n, F = X.shape
+    src, dst, est, trees = fit_input(tmp_path, X, y, n_estimators)
+    res = subprocess.run([exe, "fit", src, dst, str(team)], capture_output=True, text=True)
     assert res.returncode == 0, res.stderr
     raw, off, states = open(dst, "rb").read(), 0, []
     for _ in range(n_estimators):
@@ -71,10 +81,10 @@ def host_fit(exe, tmp_path, X, y, n_estimators):
     return FO.assemble_regressor(est, trees, F, n, states)
 
 
-def _check(exe, tmp_path, X, y, n_estimators=3, seed=5):
+def _check(exe, tmp_path, X, y, n_estimators=3, seed=5, team=1):
     from sklearn.ensemble import RandomForestRegressor
     np.random.seed(seed)
-    got = host_fit(exe, tmp_path, X, y, n_estimators)
+    got = host_fit(exe, tmp_path, X, y, n_estimators, team)
     s_got = np.random.get_state()
     np.random.seed(seed)
     ref = RandomForestRegressor(n_estimators=n_estimators).fit(X, y)
@@ -113,13 +123,13 @@ def test_introsort_replay_equals_sklearn(exe, tmp_path, case):
         assert np.array_equal(gv.view(np.uint32), vals.view(np.uint32)), case
 
 
-@pytest.mark.parametrize("case", [c[0] for c in RC.problems()])
-def test_trees_equal_sklearn(exe, tmp_path, case):
-    name, X, y = next(c for c in RC.problems() if c[0] == case)
-    _check(exe, tmp_path, X, y)
+@pytest.mark.parametrize("case,team", host_exe.team_params(RC.problems(), big_rows=1500))
+def test_trees_equal_sklearn(exe, tmp_path, case, team):
+    name, X, y = case
+    _check(exe, tmp_path, X, y, team=team)
 
 
-# (name, replacements): each mutant must fail at least one problem of the bank
+# (name, replacements): each mutant must fail at least one problem of the bank (those in TEAM_MUTANTS at a team of 3)
 MUTANTS = [
     ("stable_partition", [("    int64_t ps = 0, pe = m;\n",
                            "    int64_t k = 0;\n    for (int64_t p = 0; p < m; ++p)\n        if (double(x(samples[p])) <= threshold) {\n"
@@ -131,19 +141,52 @@ MUTANTS = [
     ("no_tie_replay", [("                    if (!T.tied[v]) continue;", "                    continue;")]),
     ("kEpsilon_leaf_tests", [("constexpr double kLeafEpsilon = DBL_EPSILON; ", "constexpr double kLeafEpsilon = kEpsilon; ")]),
     ("fma_sums", [("            sl = dadd(sl, dmul(w, T.yv(s)));", "            sl = std::fma(w, T.yv(s), sl);")]),
+    # only thread 0's positions can mark a visit tied: visits whose ties lie in other threads' positions skip the replay
+    ("tie_detection_thread0_only", [("                if (q >= 1 && key_value(T.keys[v * m2 + q - 1])",
+                                     "                if (tm.tid == 0 && q >= 1 && key_value(T.keys[v * m2 + q - 1])")]),
 ]
+TEAM_MUTANTS = {"tie_detection_thread0_only"}
 
 
 @pytest.mark.parametrize("name", [m[0] for m in MUTANTS])
 def test_mutants_are_caught(tmp_path_factory, tmp_path, name):
     exe = _build(tmp_path_factory, dict(MUTANTS)[name])
+    team = 3 if name in TEAM_MUTANTS else 1
     failed = []
     for case, X, y in RC.problems():
         try:
-            _check(exe, tmp_path, X, y, n_estimators=2)
+            _check(exe, tmp_path, X, y, n_estimators=2, team=team)
         except AssertionError:
             failed.append(case)
     assert failed, name
+
+
+# A barrier deleted from the builder (thread 0 reads every visit's best candidate before the other threads have written
+# theirs): a race whose outcome depends on timing, so it is ThreadSanitizer's to find
+SYNC_MUTANT = ("                T.vpos[v] = bq;\n            }\n            tm.sync();\n", "                T.vpos[v] = bq;\n            }\n")
+
+
+@pytest.mark.parametrize("mutant", [False, True], ids=["builder", "deleted_sync"])
+def test_thread_sanitizer(tmp_path_factory, tmp_path, monkeypatch, mutant):
+    """The builder built with ThreadSanitizer, at a team of 4 on small problems (ties and replays included): no report
+    (and the trees still equal scikit-learn's); with one barrier deleted, a data race is reported on every problem.  The
+    mutant's run is judged by its reports alone (host_exe.tsan_reports): after the racing read it may index past its
+    buffers, crash or not end, as timing has it."""
+    tsan = _build(tmp_path_factory, [SYNC_MUTANT] if mutant else (), ("-O1",) + host_exe.tsan_flags())
+    for name, X, y in [c for c in RC.problems() if c[0] in ("two_rows_f1", "four_eps", "ratings_ties", "f32_collisions_pm0")]:
+        if mutant and X.shape[1] < 4:
+            continue                            # one feature: thread 0 writes and reads the only visit's candidate itself
+        if mutant:
+            np.random.seed(3)
+            src, dst = fit_input(tmp_path, X, y, 2)[:2]
+            logs = tmp_path / ("tsan_" + name)
+            assert "WARNING: ThreadSanitizer: data race" in host_exe.tsan_reports([tsan, "fit", src, dst, "4"], logs), name
+        else:
+            monkeypatch.setenv("TSAN_OPTIONS", "exitcode=0 log_path=%s" % (tmp_path / "tsan"))
+            _check(tsan, tmp_path, X, y, n_estimators=2, team=4)
+    if not mutant:
+        reports = "".join(p.read_text() for p in tmp_path.glob("tsan*"))
+        assert reports == "", reports[:4000]
 
 
 def test_refusals():

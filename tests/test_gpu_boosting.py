@@ -1,9 +1,9 @@
 """GPU: kernel 13's gradient boosting (b200aa_boosting_stage, consumers.boosting_fit and boosting_cross_validate) against
 scikit-learn 1.9's GradientBoostingClassifier fit under the same NumPy global state: every tree in bits, train_score_,
-init_, classes_, the predictions and the global state afterwards, on the CPU harness's case bank, 100 and 500 stages and
-stages spanning several scratch slices; float32 / float64 device input; pickling; kernel 8 on the GPU-trained model;
-concurrent streams and threads; the batched model selection against scikit-learn problem by problem, in one launch and
-across launches; the scratch bound's refusal going to scikit-learn; evaluate_classifier directly and through
+init_, classes_, the predictions and the global state afterwards, on the CPU harness's case bank, 100 and 500 stages,
+stages spanning several scratch slices, 32 classes at 512 features and root sizes on the team and padding edges; float32 / float64 device input; pickling; kernel 8 on the GPU-trained model;
+concurrent streams and threads; the batched model selection against scikit-learn problem by problem, in one launch,
+across launches and at 32 classes; the scratch bound's refusal going to scikit-learn; evaluate_classifier directly and through
 install_training against the unmodified reference's output (tests/golden/boosting_cv.npz); the final fit of
 extract_features_and_train through the rebound train_gradient_boosting."""
 import contextlib
@@ -38,6 +38,30 @@ def _check(X, y, T, seed=7, X_in=None):
 def test_case_bank_in_bits(case):
     _, X, y, T = next(c for c in BC.problems() if c[0] == case)
     _check(X, y, T)
+
+
+def _limits(seed, n):
+    """n rows of 512 features and 32 classes (kMaxFeats, kMaxClasses: 32 trees per stage), each class present at least
+    twice"""
+    r = np.random.RandomState(seed)
+    y = r.permutation(np.arange(n) % 32)
+    X = r.randn(n, 512)
+    X[:, :32] += 1.5 * (y[:, None] == np.arange(32))
+    return X, y
+
+
+def test_32_classes_512_features():
+    X, y = _limits(71, 160)
+    got, _ = _check(X, y, 3)
+    assert got.n_trees_per_iteration_ == 32
+
+
+@pytest.mark.parametrize("n", (127, 128, 129, 255, 256, 257, 1025))
+def test_root_sizes_at_team_and_padding_edges(n):
+    """Unit-weight roots of exactly n rows: one row per thread and one over, and the bitonic sort's padding."""
+    r = np.random.RandomState(n)
+    X = np.round(r.randn(n, 4), 1)
+    _check(X, (X[:, 0] + 0.5 * r.randn(n) > 0).astype(int) + (X[:, 1] > 0.8), 3)
 
 
 def test_100_and_500_stages():
@@ -147,6 +171,12 @@ def test_cross_validate_one_launch_against_sklearn():
     X = r.randn(90, 6)
     y = np.concatenate([np.zeros(50), np.ones(38), 2 * np.ones(2)])
     _cv_against_sklearn(X, y, [3, 7], 4, tp=0.7)
+
+
+def test_cross_validate_32_classes_512_features():
+    """Every training set holds all 32 classes: 32 trees per stage and the count kernel's full class table."""
+    X, y = _limits(72, 192)
+    _cv_against_sklearn(X, y.astype(np.float64), [2], 2, tp=0.85)
 
 
 def test_cross_validate_across_launches_against_sklearn():

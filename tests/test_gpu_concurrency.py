@@ -336,3 +336,91 @@ def test_concurrent_equals_serial(P, tmp_path, monkeypatch, capfd):
     worst = {"%s %s" % k: {n: round(v, 4) for n, v in acc["worst"].items()} for k, acc in accs.items()}
     with capfd.disabled():
         print(json.dumps(dict(report, chromagram_worst=worst)))
+
+
+def test_kernel13_mixed_shapes_concurrent_equals_alone():
+    """Kernel 13's batched entry points of different shapes on six threads, each on its own stream and with no lock, two
+    calls of different shapes per build kernel: forest model selection (random forest at 11 features and 3 classes;
+    extra trees at 512 features and 32 classes), forest regression model selection at 136 and at 11 features, and
+    gradient boosting model selection at 40 features and 10 classes and at 512 features and 3 classes.  Each kernel's
+    two callers need different amounts of dynamic shared memory; every launcher sets the kernel's limit to the one size
+    of its largest accepted shape, so no thread's setting can undercut another's launch (a launcher that set its own
+    size could fail the larger call, when the interleaving falls that way; tests/test_smem_budget_cpu.py checks the rule
+    itself deterministically).
+    Each thread makes its call three times; every result equals, in bits, the same call made alone beforehand.  Seeds
+    are explicit, so no call touches NumPy's global state."""
+    import torch
+    from pyaudioanalysis_b200.consumers import (boosting_cross_validate, forest_cross_validate,
+                                                forest_regression_cross_validate)
+
+    def splits_of(r, n, P, n_train):
+        out = []
+        for _ in range(P):
+            perm = r.permutation(n)
+            out.append((perm[:n_train], perm[n_train:]))
+        return out
+
+    def forest_job(seed, n, F, C, kind, trees):
+        r = np.random.RandomState(seed)
+        y = (np.arange(n) % C).astype(np.float64)
+        X = torch.from_numpy(r.randn(n, F) + 0.4 * (y[:, None] % 3 == np.arange(F) % 3)).cuda()
+        sp = splits_of(r, n, len(trees), int(0.8 * n))
+        seeds = [[int(s) for s in r.randint(0, 2 ** 31 - 1, T)] for T in trees]
+        return lambda: forest_cross_validate(X, y, sp, seeds, trees, kind, n_classes=C)
+
+    def regression_job(seed, n, F, trees):
+        r = np.random.RandomState(seed)
+        Xh = r.randn(n, F)
+        X, y = torch.from_numpy(Xh).cuda(), Xh[:, 2] + 0.3 * r.randn(n)
+        sp = splits_of(r, n, len(trees), int(0.8 * n))
+        seeds = [[int(s) for s in r.randint(0, 2 ** 31 - 1, T)] for T in trees]
+        return lambda: forest_regression_cross_validate(X, y, sp, seeds, trees)
+
+    def boosting_job(seed, n, F, C, stages):
+        r = np.random.RandomState(seed)
+        y = r.permutation(np.arange(n) % C).astype(np.float64)
+        X = torch.from_numpy(r.randn(n, F) + (y[:, None] == np.arange(F) % C)).cuda()
+        sp = splits_of(r, n, len(stages), int(0.8 * n))
+        K = [np.unique(y[tr]).size for tr, _ in sp]
+        K = [1 if k == 2 else k for k in K]
+        seeds = [r.randint(0, 2 ** 31 - 1, T * k).astype(np.uint32) for T, k in zip(stages, K)]
+        return lambda: boosting_cross_validate(X, y, sp, seeds, stages, n_classes=C)
+
+    jobs = [forest_job(81, 300, 11, 3, "randomforest", [6, 4]),
+            forest_job(82, 320, 512, 32, "extratrees", [3, 2]),
+            regression_job(83, 250, 136, [3, 2]),
+            regression_job(85, 300, 11, [4, 3]),
+            boosting_job(84, 300, 40, 10, [2, 3]),
+            boosting_job(86, 240, 512, 3, [3, 2])]
+    alone = []
+    for job in jobs:
+        out = job()
+        torch.cuda.synchronize()
+        alone.append([bits(o) for o in out])
+    reps, results, errors = 3, [[None] * 3 for _ in jobs], []
+    barrier = threading.Barrier(len(jobs))
+
+    def worker(i):
+        try:
+            s = torch.cuda.Stream()
+            barrier.wait()
+            with torch.cuda.stream(s):
+                for k in range(reps):
+                    results[i][k] = jobs[i]()
+            s.synchronize()
+        except BaseException as e:           # noqa: BLE001 -- re-raised on the main thread
+            errors.append(e)
+            barrier.abort()
+
+    threads = [threading.Thread(target=worker, args=(i,)) for i in range(len(jobs))]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    torch.cuda.synchronize()
+    if errors:
+        raise errors[0]
+    for i, (want, got) in enumerate(zip(alone, results)):
+        for k, out in enumerate(got):
+            for a, b in zip(want, out):
+                assert np.array_equal(a, bits(b)), (i, k)

@@ -1,7 +1,8 @@
 """GPU: kernel 13 (b200aa_forest_fit, consumers.forest_fit) against scikit-learn 1.9's RandomForestClassifier /
 ExtraTreesClassifier fit under the same NumPy global state: every tree's state in bits, the fitted attributes and the
 global state afterwards, on the CPU harness's problems, a 500-tree forest and a forest spanning several scratch slices;
-GPU-built models through kernel 8 and pickle; concurrent streams and threads; the drop-ins and install_training."""
+at 512 features and 32 classes, at root sizes on the team and padding edges, on proxy ties across thread chunks and on
+duplicated columns; GPU-built models through kernel 8 and pickle; concurrent streams and threads; the drop-ins and install_training."""
 import pickle
 import threading
 import types
@@ -52,6 +53,62 @@ def test_several_scratch_slices():
     r = np.random.RandomState(8)
     X, y = r.randn(20000, 11), r.randint(0, 4, 20000)
     _check(X, y, "randomforest", 150, seed=2)
+
+
+@pytest.mark.parametrize("kind", ["randomforest", "extratrees"])
+def test_512_features_32_classes(kind):
+    """The launchers' limits: forest_build_kernel asks for 49 832 B of dynamic shared memory, past the 48 KB default, and
+    every class-count array runs full."""
+    X, y = FC.limits()
+    got, ref = _check(X, y, kind, 4)
+    assert np.array_equal(got.predict_proba(X), ref.predict_proba(X))
+
+
+def _draw_unweighted(n_estimators, kind, n):
+    """FO.draw for RandomForestClassifier(bootstrap=False): the best splitter on every sample with weight 1, as
+    b200aa_forest_fit builds it when given no weights."""
+    from sklearn.ensemble import RandomForestClassifier
+    from pyaudioanalysis_b200 import forests as FO
+    assert kind == "randomforest"
+    est = RandomForestClassifier(n_estimators=n_estimators, bootstrap=False)
+    est._validate_estimator()
+    rs = np.random.mtrand._rand
+    trees = [est._make_estimator(append=False, random_state=rs) for _ in range(n_estimators)]
+    return est, trees, None, FO.derive([t.random_state for t in trees], "extratrees", n)[1]
+
+
+@pytest.mark.parametrize("n", FC.ROOT_SIZES)
+def test_root_sizes_at_team_and_padding_edges(n, monkeypatch):
+    """Roots of exactly n rows (unweighted: extra trees, and the best splitter with h_weights = NULL against
+    RandomForestClassifier(bootstrap=False)): one row per thread and one over, and the bitonic sort's padding."""
+    from sklearn.ensemble import RandomForestClassifier
+    from pyaudioanalysis_b200 import forests as FO
+    from pyaudioanalysis_b200.consumers import forest_fit
+    r = np.random.RandomState(n)
+    X, y = np.round(r.randn(n, 7), 1), r.randint(0, 5, n)
+    _check(X, y, "extratrees", 3)
+    np.random.seed(12)
+    ref = RandomForestClassifier(n_estimators=3, bootstrap=False).fit(X, y)
+    monkeypatch.setattr(FO, "draw", _draw_unweighted)
+    np.random.seed(12)
+    got = forest_fit(X, y, 3, "randomforest")
+    FC.compare(got, ref)
+    assert got.estimators_[0].tree_.n_node_samples[0] == n
+
+
+@pytest.mark.parametrize("kind", ["randomforest", "extratrees"])
+@pytest.mark.parametrize("n", [300, 1000])
+def test_proxy_ties_across_thread_chunks(kind, n):
+    """Palindrome labels: splits at p and n - p tie, and at these n the tied positions lie in different threads' chunks,
+    so the cross-thread reduction must keep the first."""
+    X, y = FC.palindrome(39, n)
+    _check(X, y, kind, 4)
+
+
+@pytest.mark.parametrize("kind", ["randomforest", "extratrees"])
+def test_duplicated_columns_first_visit_wins(kind):
+    X, y = FC.duplicated_columns(3)
+    _check(X, y, kind, 6)
 
 
 def test_device_input_and_float32():
@@ -185,6 +242,44 @@ def test_evaluate_classifier_goldens_directly_and_through_install_training():
                 assert ret == int(g[c + "_ret"]), c
     finally:
         uninstall()
+
+
+@pytest.mark.parametrize("kind", ["randomforest", "extratrees"])
+def test_cross_validate_512_features_32_classes_with_splits_missing_classes(kind):
+    """forest_cross_validate at 512 features and 32 classes: one training set holds every class, the others miss some (the local class
+    map runs short of kMaxClasses and the missing classes' test rows are counted against the present ones); problem by
+    problem against scikit-learn."""
+    from sklearn.preprocessing import StandardScaler
+    from pyaudioanalysis_b200 import forests as FO
+    from pyaudioanalysis_b200.consumers import forest_cross_validate
+    r = np.random.RandomState(33)
+    n = 384
+    y = (np.arange(n) % 32).astype(np.float64)
+    X = r.randn(n, 512) + 0.3 * (y[:, None] % 5 == np.arange(512) % 5)
+    perm = r.permutation(n)
+    splits = [(perm[:320], perm[320:])]
+    for missing in ([0, 5, 31], list(range(16, 32))):
+        keep = ~np.isin(y, missing)
+        rows = r.permutation(np.flatnonzero(keep))
+        splits.append((rows[:200], np.concatenate([rows[200:], np.flatnonzero(~keep)[:30]])))
+    trees = [5, 4, 3]
+    seeds = []
+    for p, T in enumerate(trees):
+        np.random.seed(60 + p)
+        seeds.append(FO.tree_seeds(T, kind))
+    pred, counts = forest_cross_validate(X, y, splits, seeds, trees, kind, n_classes=32)
+    pred, counts = pred.cpu().numpy(), counts.cpu().numpy()
+    off = 0
+    for p, ((tr, te), T) in enumerate(zip(splits, trees)):
+        sc = StandardScaler().fit(X[tr])
+        np.random.seed(60 + p)
+        m = _sklearn(kind)(n_estimators=T).fit(sc.transform(X[tr]), y[tr])
+        want = m.predict(sc.transform(X[te])).astype(int)
+        assert np.array_equal(pred[off:off + te.size], want), p
+        c = np.zeros((32, 32), dtype=np.int64)
+        np.add.at(c, (y[te].astype(int), want), 1)
+        assert np.array_equal(counts[p], c), p
+        off += te.size
 
 
 @pytest.mark.parametrize("kind", ["randomforest", "extratrees"])

@@ -1,10 +1,11 @@
 """GPU: kernel 13's regression builder (b200aa_forest_regressor_fit, consumers.forest_regressor_fit) against
 scikit-learn 1.9's RandomForestRegressor fit under the same NumPy global state: every tree's state in bits, the fitted
-attributes and the global state afterwards, on the CPU harness's case bank, 100- and 500-tree forests and a forest
-spanning several scratch slices; float32 / float64 device input; pickling and predict; concurrent streams and threads;
-b200aa_forest_regression_cross_validate against scikit-learn problem by problem, in one launch and across launches; the
-scratch bound's refusal going to scikit-learn; evaluate_regression directly and
-through install_training against the unmodified reference's output (tests/golden/forest_regression_cv.npz)."""
+attributes and the global state afterwards, on the CPU harness's case bank, 100- and 500-tree forests, a forest
+spanning several scratch slices, 512 features, bootstrapped roots near the team and padding edges and tied duplicated
+columns; float32 / float64 device input; pickling and predict; concurrent streams and threads;
+b200aa_forest_regression_cross_validate against scikit-learn problem by problem, in one launch, across launches and at
+512 features; the scratch bound's refusal going to scikit-learn; evaluate_regression directly and through
+install_training against the unmodified reference's output (tests/golden/forest_regression_cv.npz)."""
 import contextlib
 import io
 import pickle
@@ -37,6 +38,33 @@ def _check(X, y, n_estimators, seed=5, X_in=None):
 def test_case_bank_in_bits(case):
     _, X, y = next(c for c in RC.problems() if c[0] == case)
     _check(X, y, 4)
+
+
+def test_512_features():
+    """kMaxFeats: every per-feature array of forest_reg_build_kernel's shared memory runs full, and the batched sort
+    holds 512 visits."""
+    r = np.random.RandomState(61)
+    X = r.randn(300, 512)
+    _check(X, X[:, 7] - 0.5 * X[:, 300] + 0.1 * r.randn(300), 3)
+
+
+@pytest.mark.parametrize("n", (127, 128, 129, 255, 256, 257, 1025))
+def test_bootstrapped_roots_near_team_and_padding_edges(n):
+    """n rows before the bootstrap's zero weights drop some (the root holds the positively weighted ones, about 0.63 n,
+    so not exactly n: the regressor always bootstraps), on tied values, so that the introsort replay and the bitonic
+    padding meet sizes around the team's edges."""
+    r = np.random.RandomState(n)
+    X = np.round(r.randn(n, 5), 1)
+    _check(X, X[:, 0] + r.randint(0, 3, n), 3)
+
+
+def test_tied_duplicated_columns():
+    """Columns 6 .. 11 repeat 0 .. 5 with ties inside each: every visit's introsort replay starts from the order the
+    previous visit left, and the first of two tied copies wins."""
+    r = np.random.RandomState(62)
+    X = np.round(r.randn(400, 6), 1)
+    X = np.hstack([X, X])
+    _check(X, X[:, 0] + 2 * X[:, 1] + r.randint(0, 2, 400), 4)
 
 
 def test_100_and_500_trees():
@@ -135,6 +163,12 @@ def test_cross_validate_one_launch_against_sklearn():
     """Small problems whose trees all go into one launch."""
     r = np.random.RandomState(47)
     _cv_against_sklearn(r.randn(120, 9), r.randn(120) + 10.0, [3, 11], 3)
+
+
+def test_cross_validate_512_features():
+    r = np.random.RandomState(63)
+    X = r.randn(150, 512)
+    _cv_against_sklearn(X, X[:, 3] + 0.2 * r.randn(150), [2, 3], 2)
 
 
 def test_cross_validate_across_launches_against_sklearn():

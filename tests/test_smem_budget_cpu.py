@@ -1,10 +1,13 @@
-"""CPU: shared-memory budgets of the two feature kernels for the shapes the library instantiates.
+"""CPU: shared-memory budgets of the two feature kernels for the shapes the library instantiates, and of kernel 13's three
+build kernels for every shape their launchers accept.
 
 sm_90: 233 472 B of shared memory per SM, 1 024 B reserved per resident CTA, so n CTAs per SM need
 n * (bytes + 1024) <= 233 472.  The CTA kernel (csrc/fast_kernel.cuh) is sized for 3 CTAs per SM on the headline shape;
 the pair kernel (csrc/pair_kernel.cuh) runs one CTA of up to 20 autonomous warps per SM (9.6 KB of shared memory per warp on
 the headline shape, five warps per scheduler at 96 registers).  The generic kernel (csrc/generic_kernel.cuh) takes 8, 4,
 2 or 1 frames per CTA group by the same budget, or keeps its window-sized arrays in global scratch."""
+import os
+import re
 import subprocess
 
 from tests import host_exe
@@ -49,3 +52,30 @@ def test_shared_memory_budget(tmp_path_factory):
         assert ctas_per_sm(nbytes) >= 1 and nbytes <= 227 * 1024, (w, warps, nbytes)     # pair_launch_t's cap (kPairCtaCap)
         assert warps >= 16 and warps % 4 == 0, (w, warps)     # whole rounds over the four schedulers of an SM
     assert pair[800][0] == 20         # 20 autonomous warps per SM on the headline shape
+
+
+# sm_90's largest opt-in dynamic shared memory per CTA (cudaDevAttrMaxSharedMemoryPerBlockOptin: 227 KB)
+SM90_OPTIN = 227 * 1024
+
+
+def test_kernel13_shared_memory_caps(tmp_path_factory):
+    """Kernel 13's three build kernels: every accepted shape (F <= 512, C <= 32) fits under the kernel's cap, the cap is
+    the size at the largest shape, every cap is below sm_90's opt-in maximum, and every cudaFuncSetAttribute in forest.cu
+    passes a cap constant.  A launcher that set its own call's size instead would let a concurrent call of a smaller shape
+    lower the limit between another thread's set and launch, and that launch would fail."""
+    csrc = os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc")
+    exe = host_exe.build(tmp_path_factory, "forest_smem_host.cu", "-I" + csrc)
+    lines = [ln.split() for ln in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.splitlines()]
+    caps = {ln[0]: (int(ln[1]), int(ln[2]), ln[3]) for ln in lines}
+    assert set(caps) == {"forest_build_kernel", "forest_reg_build_kernel", "boost_build_kernel"}
+    for kern, (cap, largest, shape) in caps.items():
+        assert largest == cap, (kern, cap, largest, shape)
+        assert cap <= SM90_OPTIN, (kern, cap)
+    assert caps["forest_build_kernel"] == (49832, 49832, "512:32")          # past the 48 KB default
+    src = open(os.path.join(csrc, "forest.cu")).read()
+    calls = re.findall(r"cudaFuncSetAttribute\(\s*(\w+)\s*,\s*cudaFuncAttributeMaxDynamicSharedMemorySize\s*,\s*([^;]*?)\)\);", src)
+    assert len(calls) == src.count("cudaFuncSetAttribute(") == 5, calls
+    want = {"forest_build_kernel": "int(forest::kSmemCap)", "forest_reg_build_kernel": "int(forest::kRegSmemCap)",
+            "boost_build_kernel": "int(forest::kBoostSmemCap)"}
+    for kern, arg in calls:
+        assert want[kern] == arg.strip(), (kern, arg)
