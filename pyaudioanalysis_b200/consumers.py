@@ -681,6 +681,78 @@ class TreeEnsembleModel:
             lib().b200aa_trees_destroy(h)
 
 
+def _ptr(a):
+    """A host array's address for the C ABI (None: NULL)."""
+    return ctypes.c_void_p(a.ctypes.data) if a is not None else None
+
+
+def _forest_X(X, Xh):
+    """X as the forest trainers read it: a CUDA float32 / float64 tensor with unit column stride as it is (cast to float32
+    on the device, round to nearest, as fit casts), anything else through fit's own cast straight to float32 (any
+    integer or float dtype rounds once)."""
+    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64) and X.stride(1) == 1:
+        return X
+    return torch.from_numpy(np.ascontiguousarray(Xh, dtype=np.float32)).cuda()
+
+
+def _tree_states(nodes, values, counts, depth, n_outputs):
+    """Tree.__getstate__ of every tree of a fit, its nodes and values following the trees before it."""
+    from . import forests as FO
+    states, off = [], 0
+    for nc, d in zip(counts, depth):
+        nc = int(nc)
+        states.append(FO.tree_state(nodes[off:off + nc], values[off:off + nc], d, n_outputs))
+        off += nc
+    return states
+
+
+def _cv_X(X):
+    """A model selection's X as a C-contiguous CUDA float64 [n, F] tensor."""
+    if not isinstance(X, torch.Tensor):
+        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
+    _require_cuda(X, "X")
+    if X.dim() != 2 or X.dtype != torch.float64:
+        raise ValueError("X must be float64 [n, F]")
+    return X.contiguous()
+
+
+def _cv_splits(splits, seeds, n_estimators, what):
+    """A model selection's (train, test) splits, one seed list and one `what` count per split: the training and test row
+    lists, and both as (offsets int64, indices int32)."""
+    if not len(splits) == len(seeds) == len(n_estimators):
+        raise ValueError("one seed list and one %s count per split" % what)
+    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
+    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
+    return train, test, _concat_indices(train, np.int32), _concat_indices(test, np.int32)
+
+
+def _forest_draws(seeds, n_trees, train, kind):
+    """Every problem's bootstrap weights (int32, None for extra trees) and splitter seeds (uint32) from its tree seeds."""
+    from . import forests as FO
+    if any(len(s) != t for s, t in zip(seeds, n_trees)):
+        raise ValueError("every problem needs one seed per tree")
+    ws, rs = [], []
+    for s, tr in zip(seeds, train):
+        w, r = FO.derive(s, kind, tr.size)
+        if w is not None:
+            ws.append(w.ravel())
+        rs.append(r)
+    weights = np.ascontiguousarray(np.concatenate(ws), dtype=np.int32) if ws else None
+    return weights, np.ascontiguousarray(np.concatenate(rs), dtype=np.uint32)
+
+
+def _scratch_refusal(status, what, rows, F, state=None):
+    """forests.Unsupported for a tree over the trainer's scratch bound (NumPy's global state put back to `state` first,
+    when given), else check(status).  rows: the tree's rows, as the message names them."""
+    from . import forests as FO
+    if status == ERR_UNSUPPORTED:
+        if state is not None:
+            np.random.set_state(state)
+        raise FO.Unsupported("%s on the GPU: one tree of %s x %d features needs more scratch than the trainer's 256 MB "
+                             "bound" % (what, rows, F))
+    check(status)
+
+
 def forest_fit(X, y, n_estimators, kind):
     """``RandomForestClassifier(n_estimators).fit(X, y)`` (kind "randomforest") or ``ExtraTreesClassifier`` (kind
     "extratrees") trained on the GPU (``b200aa_forest_fit``, DESIGN.md kernel 13), tree for tree scikit-learn 1.9's under
@@ -697,11 +769,7 @@ def forest_fit(X, y, n_estimators, kind):
     n, F = Xh.shape
     classes, y_idx = np.unique(np.asarray(y), return_inverse=True)
     C = len(classes)
-    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64) and X.stride(1) == 1:
-        d_X = X                                     # cast to float32 on the device, round to nearest, as fit casts
-    else:
-        # fit's own cast, straight to float32 (any integer or float dtype rounds once)
-        d_X = torch.from_numpy(np.ascontiguousarray(Xh, dtype=np.float32)).cuda()
+    d_X = _forest_X(X, Xh)
     est, trees, weights, seeds = FO.draw(int(n_estimators), kind, n)
     cap = int(n_estimators) * (2 * n - 1)
     nodes = np.empty(cap, dtype=FO.NODE_DTYPE)
@@ -709,20 +777,12 @@ def forest_fit(X, y, n_estimators, kind):
     counts = np.empty(int(n_estimators), dtype=np.int64)
     depth = np.empty(int(n_estimators), dtype=np.int32)
     y32 = np.ascontiguousarray(y_idx, dtype=np.int32)
-
-    def ptr(a):
-        return ctypes.c_void_p(a.ctypes.data) if a is not None else None
     with torch.cuda.device(d_X.device):
         check(lib().b200aa_forest_fit(
             ctypes.c_void_p(d_X.data_ptr()), DTYPE_F32 if d_X.dtype == torch.float32 else DTYPE_F64, n, F, d_X.stride(0),
-            ptr(y32), C, FO.KINDS[kind], int(n_estimators), max(1, int(np.sqrt(F))), ptr(weights), ptr(seeds), ptr(nodes),
-            ptr(values), cap, ptr(counts), ptr(depth), _stream()))
-    states, off = [], 0
-    for t in range(int(n_estimators)):
-        nc = int(counts[t])
-        states.append(FO.tree_state(nodes[off:off + nc], values[off:off + nc], depth[t], C))
-        off += nc
-    return FO.assemble(est, trees, F, n, classes, states)
+            _ptr(y32), C, FO.KINDS[kind], int(n_estimators), max(1, int(np.sqrt(F))), _ptr(weights), _ptr(seeds),
+            _ptr(nodes), _ptr(values), cap, _ptr(counts), _ptr(depth), _stream()))
+    return FO.assemble(est, trees, F, n, classes, _tree_states(nodes, values, counts, depth, C))
 
 
 def forest_cross_validate(X, y, splits, seeds, n_estimators, kind, n_classes=None):
@@ -737,44 +797,22 @@ def forest_cross_validate(X, y, splits, seeds, n_estimators, kind, n_classes=Non
     from . import forests as FO
     if kind not in FO.KINDS:
         raise ValueError("kind must be 'randomforest' or 'extratrees', got %r" % (kind,))
-    if not isinstance(X, torch.Tensor):
-        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
-    _require_cuda(X, "X")
-    if X.dim() != 2 or X.dtype != torch.float64:
-        raise ValueError("X must be float64 [n, F]")
-    X = X.contiguous()
+    X = _cv_X(X)
     n = X.shape[0]
     y = np.asarray(y.cpu() if isinstance(y, torch.Tensor) else y)
     if y.shape != (n,) or not np.array_equal(y, np.floor(y)) or (n and y.min() < 0):
         raise ValueError("y must hold one class index >= 0 per row of X")
     y = y.astype(np.int32)
     n_classes = int(y.max()) + 1 if n_classes is None else int(n_classes)
-    if not len(splits) == len(seeds) == len(n_estimators):
-        raise ValueError("one seed list and one tree count per split")
-    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
-    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
-    train_off, train_idx = _concat_indices(train, np.int32)
-    test_off, test_idx = _concat_indices(test, np.int32)
+    train, _, (train_off, train_idx), (test_off, test_idx) = _cv_splits(splits, seeds, n_estimators, "tree")
     n_trees = np.ascontiguousarray(n_estimators, dtype=np.int32)
-    if any(len(s) != t for s, t in zip(seeds, n_trees)):
-        raise ValueError("every problem needs one seed per tree")
-    ws, rs = [], []
-    for s, tr in zip(seeds, train):
-        w, r = FO.derive(s, kind, tr.size)
-        if w is not None:
-            ws.append(w.ravel())
-        rs.append(r)
-    weights = np.ascontiguousarray(np.concatenate(ws), dtype=np.int32) if ws else None
-    rand_r = np.ascontiguousarray(np.concatenate(rs), dtype=np.uint32)
+    weights, rand_r = _forest_draws(seeds, n_trees, train, kind)
     with torch.cuda.device(X.device):
         pred = torch.empty(int(test_off[-1]), dtype=torch.int32, device=X.device)
         counts = torch.empty((len(splits), n_classes, n_classes), dtype=torch.int64, device=X.device)
-
-        def ptr(a):
-            return ctypes.c_void_p(a.ctypes.data) if a is not None else None
         check(lib().b200aa_forest_cross_validate(
-            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], ptr(y), n_classes, FO.KINDS[kind], len(splits), ptr(train_off),
-            ptr(train_idx), ptr(test_off), ptr(test_idx), ptr(n_trees), ptr(weights), ptr(rand_r),
+            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], _ptr(y), n_classes, FO.KINDS[kind], len(splits),
+            _ptr(train_off), _ptr(train_idx), _ptr(test_off), _ptr(test_idx), _ptr(n_trees), _ptr(weights), _ptr(rand_r),
             ctypes.c_void_p(pred.data_ptr()), ctypes.c_void_p(counts.data_ptr()), _stream()))
     return pred, counts
 
@@ -795,10 +833,7 @@ def forest_regressor_fit(X, y, n_estimators):
     if why is not None:
         raise ValueError("forest_regressor_fit on the GPU: " + why)
     n, F = Xh.shape
-    if isinstance(X, torch.Tensor) and X.is_cuda and X.dtype in (torch.float32, torch.float64) and X.stride(1) == 1:
-        d_X = X                                     # cast to float32 on the device, round to nearest, as fit casts
-    else:
-        d_X = torch.from_numpy(np.ascontiguousarray(Xh, dtype=np.float32)).cuda()
+    d_X = _forest_X(X, Xh)
     T = int(n_estimators)
     state = np.random.get_state()
     est, trees, weights, seeds = FO.draw(T, FO.REGRESSOR, n)
@@ -808,24 +843,12 @@ def forest_regressor_fit(X, y, n_estimators):
     counts = np.empty(T, dtype=np.int64)
     depth = np.empty(T, dtype=np.int32)
     y64 = np.ascontiguousarray(y, dtype=np.float64)
-
-    def ptr(a):
-        return ctypes.c_void_p(a.ctypes.data)
     with torch.cuda.device(d_X.device):
         status = lib().b200aa_forest_regressor_fit(
             ctypes.c_void_p(d_X.data_ptr()), DTYPE_F32 if d_X.dtype == torch.float32 else DTYPE_F64, n, F, d_X.stride(0),
-            ptr(y64), T, ptr(weights), ptr(seeds), ptr(nodes), ptr(values), cap, ptr(counts), ptr(depth), _stream())
-    if status == ERR_UNSUPPORTED:
-        np.random.set_state(state)
-        raise FO.Unsupported("forest_regressor_fit on the GPU: one tree of %d rows x %d features needs more scratch than "
-                             "the trainer's 256 MB bound" % (n, F))
-    check(status)
-    states, off = [], 0
-    for t in range(T):
-        nc = int(counts[t])
-        states.append(FO.tree_state(nodes[off:off + nc], values[off:off + nc], depth[t], 1))
-        off += nc
-    return FO.assemble_regressor(est, trees, F, n, states)
+            _ptr(y64), T, _ptr(weights), _ptr(seeds), _ptr(nodes), _ptr(values), cap, _ptr(counts), _ptr(depth), _stream())
+    _scratch_refusal(status, "forest_regressor_fit", "%d rows" % n, F, state)
+    return FO.assemble_regressor(est, trees, F, n, _tree_states(nodes, values, counts, depth, 1))
 
 
 def forest_regression_cross_validate(X, y, splits, seeds, n_estimators):
@@ -840,55 +863,24 @@ def forest_regression_cross_validate(X, y, splits, seeds, n_estimators):
     training counts]), each problem's rows in its split's order.  Raises ``forests.Unsupported`` when one tree of the
     largest training set would exceed the trainer's 256 MB scratch bound."""
     from . import forests as FO
-    if not isinstance(X, torch.Tensor):
-        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
-    _require_cuda(X, "X")
-    if X.dim() != 2 or X.dtype != torch.float64:
-        raise ValueError("X must be float64 [n, F]")
-    X = X.contiguous()
+    X = _cv_X(X)
     n = X.shape[0]
     y = np.ascontiguousarray(y.cpu() if isinstance(y, torch.Tensor) else y, dtype=np.float64)
     if y.shape != (n,) or not np.isfinite(y).all():
         raise ValueError("y must hold one finite target per row of X")
-    if not len(splits) == len(seeds) == len(n_estimators):
-        raise ValueError("one seed list and one tree count per split")
-    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
-    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
-    train_off, train_idx = _concat_indices(train, np.int32)
-    test_off, test_idx = _concat_indices(test, np.int32)
+    train, _, (train_off, train_idx), (test_off, test_idx) = _cv_splits(splits, seeds, n_estimators, "tree")
     n_trees = np.ascontiguousarray(n_estimators, dtype=np.int32)
-    if any(len(s) != t for s, t in zip(seeds, n_trees)):
-        raise ValueError("every problem needs one seed per tree")
-    ws, rs = [], []
-    for s, tr in zip(seeds, train):
-        w, r = FO.derive(s, FO.REGRESSOR, tr.size)
-        ws.append(w.ravel())
-        rs.append(r)
-    weights = np.ascontiguousarray(np.concatenate(ws), dtype=np.int32)
-    rand_r = np.ascontiguousarray(np.concatenate(rs), dtype=np.uint32)
+    weights, rand_r = _forest_draws(seeds, n_trees, train, FO.REGRESSOR)
     with torch.cuda.device(X.device):
         pred_test = torch.empty(int(test_off[-1]), dtype=torch.float64, device=X.device)
         pred_train = torch.empty(int(train_off[-1]), dtype=torch.float64, device=X.device)
-
-        def ptr(a):
-            return ctypes.c_void_p(a.ctypes.data)
         status = lib().b200aa_forest_regression_cross_validate(
-            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], ptr(y), len(splits), ptr(train_off), ptr(train_idx),
-            ptr(test_off), ptr(test_idx), ptr(n_trees), ptr(weights), ptr(rand_r), ctypes.c_void_p(pred_test.data_ptr()),
-            ctypes.c_void_p(pred_train.data_ptr()), _stream())
-    if status == ERR_UNSUPPORTED:
-        raise FO.Unsupported("forest_regression_cross_validate on the GPU: one tree of %d training rows x %d features "
-                             "needs more scratch than the trainer's 256 MB bound" % (max(t.size for t in train), X.shape[1]))
-    check(status)
+            ctypes.c_void_p(X.data_ptr()), n, X.shape[1], _ptr(y), len(splits), _ptr(train_off), _ptr(train_idx),
+            _ptr(test_off), _ptr(test_idx), _ptr(n_trees), _ptr(weights), _ptr(rand_r),
+            ctypes.c_void_p(pred_test.data_ptr()), ctypes.c_void_p(pred_train.data_ptr()), _stream())
+    _scratch_refusal(status, "forest_regression_cross_validate", "%d training rows" % max(t.size for t in train),
+                     X.shape[1])
     return pred_test, pred_train
-
-
-def _boost_scratch_refusal(status, what, n, F):
-    from . import forests as FO
-    if status == ERR_UNSUPPORTED:
-        raise FO.Unsupported("%s on the GPU: one tree of %d training rows x %d features needs more scratch than the "
-                             "trainer's 256 MB bound" % (what, n, F))
-    check(status)
 
 
 def boosting_fit(X, y, n_estimators):
@@ -929,9 +921,6 @@ def boosting_fit(X, y, n_estimators):
     values = np.empty(cap, dtype=np.float64)
     counts = np.empty(K, dtype=np.int64)
     depth = np.empty(K, dtype=np.int32)
-
-    def ptr(a):
-        return ctypes.c_void_p(a.ctypes.data)
     with torch.cuda.device(d_X.device):
         d_y = torch.from_numpy(y_enc.astype(np.int32)).to(d_X.device)
         d_raw = torch.from_numpy(raw).to(d_X.device)
@@ -939,21 +928,15 @@ def boosting_fit(X, y, n_estimators):
         for i in range(T):
             d_neg.copy_(torch.from_numpy(BO.neg_gradient(est._loss, y_enc, raw)))
             status = lib().b200aa_boosting_stage(
-                ctypes.c_void_p(d_X.data_ptr()), n, F, 1, ptr(train_off), ptr(rows), None, None, ptr(K_arr), ptr(active),
-                ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()), ctypes.c_void_p(d_raw.data_ptr()),
-                None, ptr(seeds[i * K:(i + 1) * K]), float(est.learning_rate), ptr(nodes), ptr(values), cap, ptr(counts),
-                ptr(depth), _stream())
-            if status == ERR_UNSUPPORTED:
-                np.random.set_state(state)
-            _boost_scratch_refusal(status, "boosting_fit", n, F)
+                ctypes.c_void_p(d_X.data_ptr()), n, F, 1, _ptr(train_off), _ptr(rows), None, None, _ptr(K_arr),
+                _ptr(active), ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()),
+                ctypes.c_void_p(d_raw.data_ptr()), None, _ptr(seeds[i * K:(i + 1) * K]), float(est.learning_rate),
+                _ptr(nodes), _ptr(values), cap, _ptr(counts), _ptr(depth), _stream())
+            _scratch_refusal(status, "boosting_fit", "%d training rows" % n, F, state)
             raw = d_raw.cpu().numpy()
             est.train_score_[i] = factor * est._loss(y_true=y_enc, raw_prediction=raw, sample_weight=sw)
-            off = 0
-            for k in range(K):
-                nc = int(counts[k])
-                est.estimators_[i, k] = BO.make_tree(est, F, FO.tree_state(nodes[off:off + nc], values[off:off + nc],
-                                                                           depth[k], 1))
-                off += nc
+            for k, tree in enumerate(_tree_states(nodes, values, counts, depth, 1)):
+                est.estimators_[i, k] = BO.make_tree(est, F, tree)
     est.n_estimators_ = T
     return est
 
@@ -972,24 +955,14 @@ def boosting_cross_validate(X, y, splits, seeds, n_estimators, n_classes=None):
     int32 [sum of the test counts], counts int64 [P, n_classes, n_classes]).  Raises ``forests.Unsupported`` when one tree
     of the largest training set would exceed the trainer's 256 MB scratch bound."""
     from . import boosting as BO
-    if not isinstance(X, torch.Tensor):
-        X = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float64)).cuda()
-    _require_cuda(X, "X")
-    if X.dim() != 2 or X.dtype != torch.float64:
-        raise ValueError("X must be float64 [n, F]")
-    X = X.contiguous()
+    X = _cv_X(X)
     n, F = X.shape
     y = np.asarray(y.cpu() if isinstance(y, torch.Tensor) else y)
     if y.shape != (n,) or not np.array_equal(y, np.floor(y)) or (n and y.min() < 0):
         raise ValueError("y must hold one class index >= 0 per row of X")
     n_classes = int(y.max()) + 1 if n_classes is None else int(n_classes)
     P = len(splits)
-    if not P == len(seeds) == len(n_estimators):
-        raise ValueError("one seed list and one stage count per split")
-    train = [np.asarray(tr, dtype=np.int64).ravel() for tr, _ in splits]
-    test = [np.asarray(te, dtype=np.int64).ravel() for _, te in splits]
-    train_off, train_idx = _concat_indices(train, np.int32)
-    test_off, test_idx = _concat_indices(test, np.int32)
+    train, test, (train_off, train_idx), (test_off, test_idx) = _cv_splits(splits, seeds, n_estimators, "stage")
     n_tr, n_te = int(train_off[-1]), int(test_off[-1])
     stages = np.asarray(n_estimators, dtype=np.int64)
     # each problem's fit preamble on the host: present classes, K, loss, encoded labels, initial raw prediction
@@ -1016,13 +989,10 @@ def boosting_cross_validate(X, y, splits, seeds, n_estimators, n_classes=None):
     rows_tr = np.arange(n_tr, dtype=np.int32)
     rows_te = np.arange(n_tr, n_tr + n_te, dtype=np.int32)
     lr = 0.1                                        # GradientBoostingClassifier's learning_rate
-
-    def ptr(a):
-        return ctypes.c_void_p(a.ctypes.data) if a is not None else None
     with torch.cuda.device(X.device):
         d_Xs = torch.empty((n_tr + n_te, F), dtype=torch.float32, device=X.device)
-        check(lib().b200aa_boosting_scale(ctypes.c_void_p(X.data_ptr()), n, F, P, ptr(train_off), ptr(train_idx),
-                                          ptr(test_off), ptr(test_idx), ctypes.c_void_p(d_Xs.data_ptr()), _stream()))
+        check(lib().b200aa_boosting_scale(ctypes.c_void_p(X.data_ptr()), n, F, P, _ptr(train_off), _ptr(train_idx),
+                                          _ptr(test_off), _ptr(test_idx), ctypes.c_void_p(d_Xs.data_ptr()), _stream()))
         d_y = torch.from_numpy(y_loc).to(X.device)
         d_raw_tr = torch.from_numpy(np.ascontiguousarray(raw_tr, dtype=np.float64)).to(X.device)
         d_raw_te = torch.from_numpy(np.ascontiguousarray(raw_te, dtype=np.float64)).to(X.device)
@@ -1047,16 +1017,16 @@ def boosting_cross_validate(X, y, splits, seeds, n_estimators, n_classes=None):
             st_seeds = np.ascontiguousarray(np.concatenate([seeds[p][s * K[p]:(s + 1) * K[p]] for p in range(P) if active[p]]),
                                             dtype=np.uint32)
             status = lib().b200aa_boosting_stage(
-                ctypes.c_void_p(d_Xs.data_ptr()), n_tr + n_te, F, P, ptr(train_off), ptr(rows_tr), ptr(test_off),
-                ptr(rows_te), ptr(K), ptr(active), ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()),
-                ctypes.c_void_p(d_raw_tr.data_ptr()), ctypes.c_void_p(d_raw_te.data_ptr()), ptr(st_seeds), lr,
+                ctypes.c_void_p(d_Xs.data_ptr()), n_tr + n_te, F, P, _ptr(train_off), _ptr(rows_tr), _ptr(test_off),
+                _ptr(rows_te), _ptr(K), _ptr(active), ctypes.c_void_p(d_y.data_ptr()), ctypes.c_void_p(d_neg.data_ptr()),
+                ctypes.c_void_p(d_raw_tr.data_ptr()), ctypes.c_void_p(d_raw_te.data_ptr()), _ptr(st_seeds), lr,
                 None, None, 0, None, None, _stream())
-            _boost_scratch_refusal(status, "boosting_cross_validate", max(t.size for t in train), F)
+            _scratch_refusal(status, "boosting_cross_validate", "%d training rows" % max(t.size for t in train), F)
         pred = torch.empty(max(n_te, 1), dtype=torch.int32, device=X.device)
         counts = torch.empty((P, n_classes, n_classes), dtype=torch.int64, device=X.device)
         y_test = np.ascontiguousarray(y[test_idx] if n_te else np.zeros(1), dtype=np.int32)
-        check(lib().b200aa_boosting_count(ctypes.c_void_p(d_raw_te.data_ptr()), P, ptr(test_off), ptr(K), ptr(classes),
-                                          ptr(y_test), n_classes, ctypes.c_void_p(pred.data_ptr()),
+        check(lib().b200aa_boosting_count(ctypes.c_void_p(d_raw_te.data_ptr()), P, _ptr(test_off), _ptr(K), _ptr(classes),
+                                          _ptr(y_test), n_classes, ctypes.c_void_p(pred.data_ptr()),
                                           ctypes.c_void_p(counts.data_ptr()), _stream()))
     return pred[:n_te], counts
 

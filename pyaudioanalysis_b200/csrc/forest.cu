@@ -15,29 +15,6 @@ using namespace b200aa;
 // ------------------------------------------------------------------------------------------------
 static_assert(sizeof(b200aa_forest_node) == sizeof(forest::NodeOut), "node layout of the C ABI");
 
-namespace {
-
-// the global scratch of one tree: [samples | tmp | keys | stack | nodes | values | meta]
-struct TreeLayout {
-    size_t samples, tmp, keys, stack, nodes, values, meta, bytes;
-};
-TreeLayout tree_layout(int64_t n, int C)
-{
-    const int64_t cap = 2 * n - 1;
-    TreeLayout L;
-    L.samples = 0;
-    L.tmp = L.samples + align256(size_t(n) * 4);
-    L.keys = L.tmp + align256(size_t(n) * 4);
-    L.stack = L.keys + align256(size_t(forest::pow2_at_least(n)) * 8);
-    L.nodes = L.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
-    L.values = L.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
-    L.meta = L.values + align256(size_t(cap) * C * 8);
-    L.bytes = align256(L.meta + 16);
-    return L;
-}
-
-}  // namespace
-
 __global__ void forest_cast_kernel(const double *__restrict__ X, int64_t n, int F, int64_t stride, float *__restrict__ out)
 {
     for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n * F; i += int64_t(gridDim.x) * blockDim.x)
@@ -49,6 +26,147 @@ __global__ void forest_cast_kernel(const float *__restrict__ X, int64_t n, int F
         out[i] = X[(i / F) * stride + i % F];
 }
 
+namespace {
+
+// Argument checks shared by the entry points; each returns false where the entry point returns B200AA_ERR_INVALID.
+// class labels in [0, n_classes)
+bool valid_labels(const int32_t *y, int64_t n, int n_classes)
+{
+    for (int64_t i = 0; i < n; ++i)
+        if (y[i] < 0 || y[i] >= n_classes) return false;
+    return true;
+}
+// finite regression targets
+bool finite_targets(const double *y, int64_t n)
+{
+    for (int64_t i = 0; i < n; ++i)
+        if (!(y[i] - y[i] == 0.0)) return false;
+    return true;
+}
+// bootstrap counts in [0, 2^29]
+bool valid_weights(const int32_t *w, int64_t count)
+{
+    for (int64_t i = 0; i < count; ++i)
+        if (w[i] < 0 || w[i] > (1 << 29)) return false;
+    return true;
+}
+// Ragged splits of n_problems problems over rows [0, n): offsets from 0, at least one training row and no fewer than zero
+// test rows per problem, every index a row.  No test offsets (test_off NULL): no test rows.
+bool valid_splits(int64_t n, int64_t n_problems, const int64_t *train_off, const int32_t *train_idx, const int64_t *test_off,
+                  const int32_t *test_idx)
+{
+    const auto rows_in = [n](const int32_t *idx, int64_t lo, int64_t hi) {
+        for (int64_t i = lo; i < hi; ++i)
+            if (idx[i] < 0 || idx[i] >= n) return false;
+        return true;
+    };
+    if (train_off[0] != 0 || (test_off && test_off[0] != 0)) return false;
+    for (int64_t p = 0; p < n_problems; ++p) {
+        if (train_off[p + 1] - train_off[p] < 1 || (test_off && test_off[p + 1] < test_off[p])) return false;
+        if (!rows_in(train_idx, train_off[p], train_off[p + 1]) || (test_off && !rows_in(test_idx, test_off[p], test_off[p + 1])))
+            return false;
+    }
+    return true;
+}
+
+// One tree's slot of global scratch: its builder's own arrays (the head), then the tail every builder writes: stack
+// [n + 1], nodes [2 n - 1], values [(2 n - 1) per_node], meta (node_count, max_depth).  Every part starts 256-aligned.
+struct Slot {
+    size_t stack, nodes, values, meta, bytes;
+};
+Slot slot_after(size_t head, int64_t n, int per_node)
+{
+    const int64_t cap = 2 * n - 1;
+    Slot S;
+    S.stack = head;
+    S.nodes = S.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
+    S.values = S.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
+    S.meta = S.values + align256(size_t(cap) * per_node * 8);
+    S.bytes = S.meta + 256;
+    return S;
+}
+
+// a classification tree's slot: [samples | tmp | keys | tail]
+struct TreeLayout {
+    size_t samples, tmp, keys;
+    Slot s;
+};
+TreeLayout tree_layout(int64_t n, int C)
+{
+    TreeLayout L;
+    L.samples = 0;
+    L.tmp = L.samples + align256(size_t(n) * 4);
+    L.keys = L.tmp + align256(size_t(n) * 4);
+    L.s = slot_after(L.keys + align256(size_t(forest::pow2_at_least(n)) * 8), n, C);
+    return L;
+}
+
+// Thread 0 of a build kernel: the tree's node count and depth to its slot's meta, where read_trees finds them
+template <class S>
+__device__ void put_meta(char *meta, const S *st)
+{
+    if (threadIdx.x == 0) {
+        int64_t *m = reinterpret_cast<int64_t *>(meta);
+        m[0] = st->node_count;
+        m[1] = st->max_depth;
+    }
+}
+
+// trees per launch: as many as keep fixed + their slots under the scratch slice bound, at most n_trees; 0 when not even
+// one tree fits.  A regression tree's sort keys take 8 F pow2(n) bytes, so at F = 136 one fits for n up to 131 072.
+int64_t trees_per_launch(size_t fixed, size_t per_tree, int64_t n_trees)
+{
+    if (fixed + per_tree > kScratchSliceBytes) return 0;
+    return std::min<int64_t>(n_trees, int64_t((kScratchSliceBytes - fixed) / per_tree));
+}
+
+// Where a fit returns its trees: per_node values per node, each tree's node count and depth, and the nodes written so far
+struct TreesOut {
+    b200aa_forest_node *nodes;
+    double *values;
+    int per_node;
+    int64_t capacity, *node_count;
+    int32_t *max_depth;
+    int64_t written;
+};
+
+// One launch's nt trees (slot i at trees + i * S.bytes) to the host as trees t0 .. t0 + nt - 1, their nodes and values
+// after those already written; B200AA_ERR_INVALID when they pass the capacity.  Returns with the copies done, so the
+// next launch may reuse the slots.
+int read_trees(cudaStream_t st, const char *trees, const Slot &S, int64_t t0, int64_t nt, TreesOut &o)
+{
+    std::vector<int64_t> meta(size_t(nt) * 2);
+    for (int64_t i = 0; i < nt; ++i)
+        CK(cudaMemcpyAsync(&meta[size_t(i) * 2], trees + size_t(i) * S.bytes + S.meta, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int64_t i = 0; i < nt; ++i) {
+        const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
+        o.node_count[t] = nc;
+        o.max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
+        if (o.written + nc > o.capacity) return B200AA_ERR_INVALID;
+        const char *tb = trees + size_t(i) * S.bytes;
+        CK(cudaMemcpyAsync(o.nodes + o.written, tb + S.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(o.values + o.written * o.per_node, tb + S.values, size_t(nc) * o.per_node * 8,
+                           cudaMemcpyDeviceToHost, st));
+        o.written += nc;
+    }
+    CK(cudaStreamSynchronize(st));    // the next launch reuses the scratch the copies read
+    return B200AA_OK;
+}
+
+// X [n, F] (float32 or float64, rows row_stride apart) to dense float32 Xf, rounded to nearest as fit casts
+int cast_to_f32(const void *d_X, int dtype, int64_t n, int F, int64_t row_stride, float *Xf, cudaStream_t st)
+{
+    const unsigned blocks = unsigned(std::min<int64_t>((n * F + 255) / 256, 4096));
+    with_real_type(dtype, [&](auto t) {
+        forest_cast_kernel<<<blocks, 256, 0, st>>>(static_cast<const decltype(t) *>(d_X), n, F, row_stride, Xf);
+    });
+    CK_LAUNCH("forest_cast_kernel");
+    return B200AA_OK;
+}
+
+}  // namespace
+
 // One CTA per tree of the slice: build_tree with the block as its team.
 __global__ void __launch_bounds__(forest::kThreads) forest_build_kernel(const float *__restrict__ X,
                                                                        const int32_t *__restrict__ y, int64_t n, int F,
@@ -59,33 +177,14 @@ __global__ void __launch_bounds__(forest::kThreads) forest_build_kernel(const fl
 {
     extern __shared__ __align__(16) unsigned char forest_smem[];
     const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
-    char *base = scratch + size_t(blockIdx.x) * L.bytes;
-    unsigned char *s = forest_smem;
-    forest::Shared *st = reinterpret_cast<forest::Shared *>(s);
-    s += (sizeof(forest::Shared) + 15) & ~size_t(15);
-    double *thr = reinterpret_cast<double *>(s);
-    s += size_t(F) * 8;
-    int64_t *cnt = reinterpret_cast<int64_t *>(s);
-    s += size_t(blockDim.x) * C * 8;
-    double *red_proxy = reinterpret_cast<double *>(s);
-    s += size_t(blockDim.x) * 8;
-    int64_t *red_pos = reinterpret_cast<int64_t *>(s);
-    s += size_t(blockDim.x) * 8;
-    float *mn = reinterpret_cast<float *>(s);
-    float *mx = mn + F;
-    int32_t *features = reinterpret_cast<int32_t *>(mx + F);
-    int32_t *constf = features + F, *drawn = constf + F;
-    const forest::Tree T{X, y, w ? w + int64_t(blockIdx.x) * n : nullptr, n, F, C, max_features, kind,
-                         reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.tmp),
-                         reinterpret_cast<uint64_t *>(base + L.keys), reinterpret_cast<forest::StackRec *>(base + L.stack),
-                         reinterpret_cast<forest::NodeOut *>(base + L.nodes), reinterpret_cast<double *>(base + L.values),
-                         features, constf, drawn, mn, mx, thr, cnt, red_proxy, red_pos, st};
+    char *base = scratch + size_t(blockIdx.x) * L.s.bytes;
+    forest::Tree T{X, y, w ? w + int64_t(blockIdx.x) * n : nullptr, n, F, C, max_features, kind,
+                   reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.tmp),
+                   reinterpret_cast<uint64_t *>(base + L.keys), reinterpret_cast<forest::StackRec *>(base + L.s.stack),
+                   reinterpret_cast<forest::NodeOut *>(base + L.s.nodes), reinterpret_cast<double *>(base + L.s.values)};
+    forest::carve_smem(forest_smem, blockDim.x, T);
     forest::build_tree(T, tm, seeds[blockIdx.x]);
-    if (threadIdx.x == 0) {
-        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
-        meta[0] = st->node_count;
-        meta[1] = st->max_depth;
-    }
+    put_meta(base + L.s.meta, T.st);
 }
 
 extern "C" int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride,
@@ -101,60 +200,36 @@ extern "C" int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_fe
         (kind != forest::kBest && kind != forest::kRandom) || max_features < 1 || max_features > n_feats ||
         node_capacity < 0 || (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
         return B200AA_ERR_INVALID;
-    for (int64_t i = 0; i < n; ++i)
-        if (h_y[i] < 0 || h_y[i] >= n_classes) return B200AA_ERR_INVALID;
-    if (h_weights)
-        for (int64_t i = 0; i < int64_t(n_trees) * n; ++i)
-            if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (!valid_labels(h_y, n, n_classes) || (h_weights && !valid_weights(h_weights, int64_t(n_trees) * n)))
+        return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::smem_bytes(n_feats, n_classes);
     CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kSmemCap)));
     const TreeLayout L = tree_layout(n, n_classes);
-    const size_t per_tree = L.bytes + (h_weights ? align256(size_t(n) * 4) : 0);
+    const size_t per_tree = L.s.bytes + (h_weights ? align256(size_t(n) * 4) : 0);
     const size_t fixed = align256(size_t(n) * n_feats * 4) + align256(size_t(n) * 4) + align256(size_t(n_trees) * 4);
-    const int64_t slice = std::max<int64_t>(
-        1, std::min<int64_t>(n_trees, fixed + per_tree < kScratchSliceBytes ? int64_t((kScratchSliceBytes - fixed) / per_tree) : 1));
+    const int64_t slice = std::max<int64_t>(1, trees_per_launch(fixed, per_tree, n_trees));    // never refused for scratch
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
+    int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
     if (rc != B200AA_OK) return rc;
     char *base = static_cast<char *>(scratch.get());
     float *Xf = reinterpret_cast<float *>(base);
     int32_t *y = reinterpret_cast<int32_t *>(base + align256(size_t(n) * n_feats * 4));
     uint32_t *seeds = reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(y) + align256(size_t(n) * 4));
     char *trees = base + fixed;
-    int32_t *w = h_weights ? reinterpret_cast<int32_t *>(trees + size_t(slice) * L.bytes) : nullptr;
-    const unsigned cast_blocks = unsigned(std::min<int64_t>((n * n_feats + 255) / 256, 4096));
-    with_real_type(dtype, [&](auto t) {
-        forest_cast_kernel<<<cast_blocks, 256, 0, st>>>(static_cast<const decltype(t) *>(d_X), n, n_feats, row_stride, Xf);
-    });
-    CK_LAUNCH("forest_cast_kernel");
+    int32_t *w = h_weights ? reinterpret_cast<int32_t *>(trees + size_t(slice) * L.s.bytes) : nullptr;
+    if ((rc = cast_to_f32(d_X, dtype, n, n_feats, row_stride, Xf, st)) != B200AA_OK) return rc;
     CK(cudaMemcpyAsync(y, h_y, size_t(n) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
-    int64_t written = 0;
-    std::vector<int64_t> meta(size_t(slice) * 2);
+    TreesOut out{h_nodes, h_values, n_classes, node_capacity, h_node_count, h_max_depth, 0};
     for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
         const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
         if (w) CK(cudaMemcpyAsync(w, h_weights + t0 * n, size_t(nt * n) * 4, cudaMemcpyHostToDevice, st));
         forest_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(Xf, y, n, n_feats, n_classes, max_features, kind,
                                                                          w, seeds + t0, trees, L);
         CK_LAUNCH("forest_build_kernel");
-        for (int64_t i = 0; i < nt; ++i)
-            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], trees + size_t(i) * L.bytes + L.meta, 16,
-                               cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        for (int64_t i = 0; i < nt; ++i) {
-            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
-            h_node_count[t] = nc;
-            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
-            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
-            const char *tb = trees + size_t(i) * L.bytes;
-            CK(cudaMemcpyAsync(h_nodes + written, tb + L.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(h_values + written * n_classes, tb + L.values, size_t(nc) * n_classes * 8,
-                               cudaMemcpyDeviceToHost, st));
-            written += nc;
-        }
-        CK(cudaStreamSynchronize(st));    // the next slice reuses the scratch the copies read
+        if ((rc = read_trees(st, trees, L.s, t0, nt, out)) != B200AA_OK) return scratch.done(rc);
     }
     return scratch.done(B200AA_OK);
 }
@@ -175,11 +250,11 @@ __global__ void forest_cv_scale_kernel(const double *__restrict__ X, int F, cons
     for (int64_t i = 0; i < n_test; ++i) Xte[i * F + f] = __double2float_rn(knn::standardise(X[int64_t(test[i]) * F + f], sc));
 }
 
-// One thread per test row: walk every tree of the slice (left iff x <= threshold, tree/_tree.pyx _apply_dense) and add
+// One thread per test row: walk every tree of the slice (forest::tree_apply) and add
 // its leaf's values to the row's class sums in tree order (forest predict_proba); after the last slice P = sum / T, the
 // first maximum is the prediction (classes_.take(argmax)), mapped to its class over all problems and counted.
 __global__ void forest_cv_classify_kernel(const float *__restrict__ Xte, int64_t n_test, int F, int C, const char *__restrict__ trees,
-                                          TreeLayout L, int nt, bool first, bool last, int n_trees,
+                                          Slot S, int nt, bool first, bool last, int n_trees,
                                           double *__restrict__ acc, const int32_t *__restrict__ to_global,
                                           const int32_t *__restrict__ y_test, int n_classes, int32_t *__restrict__ pred,
                                           unsigned long long *__restrict__ counts)
@@ -191,10 +266,9 @@ __global__ void forest_cv_classify_kernel(const float *__restrict__ Xte, int64_t
     if (first)
         for (int c = 0; c < C; ++c) a[c] = 0.0;
     for (int t = 0; t < nt; ++t) {
-        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * L.bytes + L.nodes);
-        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * L.bytes + L.values);
-        int32_t i = 0;
-        while (nodes[i].left != forest::kTreeLeaf) i = double(x[nodes[i].feature]) <= nodes[i].threshold ? nodes[i].left : nodes[i].right;
+        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * S.bytes + S.nodes);
+        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * S.bytes + S.values);
+        const int32_t i = forest::tree_apply(nodes, [x](int f) { return x[f]; });
         for (int c = 0; c < C; ++c) a[c] = forest::dadd(a[c], values[int64_t(i) * C + c]);
     }
     if (!last) return;
@@ -225,26 +299,18 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
         !d_counts || n < 1 || n > (int64_t(1) << 29) || n_feats < 1 || n_classes < 1 || n_problems < 1 ||
         (kind != forest::kBest && kind != forest::kRandom) || (kind == forest::kBest) != (h_weights != nullptr))
         return B200AA_ERR_INVALID;
-    for (int64_t i = 0; i < n; ++i)
-        if (h_y[i] < 0 || h_y[i] >= n_classes) return B200AA_ERR_INVALID;
-    if (h_train_off[0] != 0 || h_test_off[0] != 0) return B200AA_ERR_INVALID;
-    int64_t ntr_max = 0, nte_max = 0, trees_total = 0, weights_total = 0, t_max = 0;
+    if (!valid_labels(h_y, n, n_classes) || !valid_splits(n, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx))
+        return B200AA_ERR_INVALID;
+    int64_t ntr_max = 0, nte_max = 0, weights_total = 0, t_max = 0;
     for (int64_t p = 0; p < n_problems; ++p) {
         const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
-        if (ntr < 1 || ntr > n || nte < 0 || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
-        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
-            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
-        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
-            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
+        if (ntr > n || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
         ntr_max = std::max(ntr_max, ntr);
         nte_max = std::max(nte_max, nte);
         t_max = std::max<int64_t>(t_max, h_n_trees[p]);
-        trees_total += h_n_trees[p];
         weights_total += int64_t(h_n_trees[p]) * ntr;
     }
-    if (h_weights)
-        for (int64_t i = 0; i < weights_total; ++i)
-            if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (h_weights && !valid_weights(h_weights, weights_total)) return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats || n_classes > forest::kMaxClasses) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int C = n_classes, F = n_feats, max_features = forest::sqrt_features(F);
@@ -256,9 +322,8 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
                  b_acc = align256(size_t(std::max<int64_t>(nte_max, 1)) * C * 8), b_seeds = align256(size_t(t_max) * 4),
                  b_yt = b_te;
     const size_t fixed = b_y + b_tr + b_te + b_map + b_xtr + b_xte + b_acc + b_seeds + b_yt;
-    const size_t per_tree = Lmax.bytes + (h_weights ? align256(size_t(ntr_max) * 4) : 0);
-    const int64_t slice = std::max<int64_t>(
-        1, std::min<int64_t>(t_max, fixed + per_tree < kScratchSliceBytes ? int64_t((kScratchSliceBytes - fixed) / per_tree) : 1));
+    const size_t per_tree = Lmax.s.bytes + (h_weights ? align256(size_t(ntr_max) * 4) : 0);
+    const int64_t slice = std::max<int64_t>(1, trees_per_launch(fixed, per_tree, t_max));    // never refused for scratch
     StreamScratch scratch(st);
     const int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
     if (rc != B200AA_OK) return rc;
@@ -273,7 +338,7 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
     uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
     int32_t *d_ytest = reinterpret_cast<int32_t *>(q); q += b_yt;
     char *d_trees = q;
-    int32_t *d_w = h_weights ? reinterpret_cast<int32_t *>(d_trees + size_t(slice) * Lmax.bytes) : nullptr;
+    int32_t *d_w = h_weights ? reinterpret_cast<int32_t *>(d_trees + size_t(slice) * Lmax.s.bytes) : nullptr;
     CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * C * C * sizeof(int64_t), st));
     std::vector<int32_t> ylocal(ntr_max), ytest(std::max<int64_t>(nte_max, 1)), map(forest::kMaxClasses);
     int64_t tree0 = 0, w0 = 0;
@@ -313,7 +378,7 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
             CK_LAUNCH("forest_build_kernel");
             if (nte) {
                 forest_cv_classify_kernel<<<unsigned((nte + 127) / 128), 128, 0, st>>>(
-                    d_xte, nte, F, Cl, d_trees, L, int(nt), t0 == 0, t0 + nt == T, T, d_acc, d_map, d_ytest, C,
+                    d_xte, nte, F, Cl, d_trees, L.s, int(nt), t0 == 0, t0 + nt == T, T, d_acc, d_map, d_ytest, C,
                     d_pred + h_test_off[p], reinterpret_cast<unsigned long long *>(d_counts + p * C * C));
                 CK_LAUNCH("forest_cv_classify_kernel");
             }
@@ -330,25 +395,20 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// the global scratch of one regression tree of at most n samples: [samples | idx | fv | keys | stack | nodes | values |
-// meta | weights]
+// a regression tree's slot of at most n samples, from offset `at`: [samples | idx | fv | keys | weights | tail]
 struct RegLayout {
-    size_t samples, idx, fv, keys, stack, nodes, values, meta, weights, bytes;
+    size_t samples, idx, fv, keys, weights;
+    Slot s;
 };
-RegLayout reg_layout(int64_t n, int F)
+RegLayout reg_layout(int64_t n, int F, size_t at = 0)
 {
-    const int64_t cap = 2 * n - 1;
     RegLayout L;
-    L.samples = 0;
+    L.samples = at;
     L.idx = L.samples + align256(size_t(n) * 4);
     L.fv = L.idx + align256(size_t(n) * 4);
     L.keys = L.fv + align256(size_t(n) * 4);
-    L.stack = L.keys + align256(size_t(F) * size_t(forest::pow2_at_least(n)) * 8);
-    L.nodes = L.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
-    L.values = L.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
-    L.meta = L.values + align256(size_t(cap) * 8);
-    L.weights = L.meta + 256;
-    L.bytes = L.weights + align256(size_t(n) * 4);
+    L.weights = L.keys + align256(size_t(F) * size_t(forest::pow2_at_least(n)) * 8);
+    L.s = slot_after(L.weights + align256(size_t(n) * 4), n, 1);
     return L;
 }
 
@@ -361,7 +421,7 @@ struct RegJob {
 }  // namespace
 
 // One CTA per tree of the launch: build_regression_tree with the block as its team.  Tree i's scratch (its weights
-// included) starts at scratch + i * L.bytes.
+// included) starts at scratch + i * L.s.bytes.
 __global__ void __launch_bounds__(forest::kThreads) forest_reg_build_kernel(const float *__restrict__ X,
                                                                            const double *__restrict__ y, int F,
                                                                            const RegJob *__restrict__ jobs,
@@ -370,47 +430,17 @@ __global__ void __launch_bounds__(forest::kThreads) forest_reg_build_kernel(cons
 {
     extern __shared__ __align__(16) unsigned char forest_reg_smem[];
     const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
-    char *base = scratch + size_t(blockIdx.x) * L.bytes;
-    unsigned char *s = forest_reg_smem;
-    forest::RegShared *st = reinterpret_cast<forest::RegShared *>(s);
-    s += (sizeof(forest::RegShared) + 15) & ~size_t(15);
-    double *vproxy = reinterpret_cast<double *>(s);
-    s += size_t(F) * 8;
-    int64_t *vpos = reinterpret_cast<int64_t *>(s);
-    s += size_t(F) * 8;
-    float *mn = reinterpret_cast<float *>(s);
-    float *mx = mn + F;
-    int32_t *features = reinterpret_cast<int32_t *>(mx + F);
-    int32_t *constf = features + F, *drawn = constf + F, *vis = drawn + F, *tied = vis + F;
+    char *base = scratch + size_t(blockIdx.x) * L.s.bytes;
     const RegJob job = jobs[blockIdx.x];
-    const forest::RegTree T{X, y, job.rows, reinterpret_cast<const int32_t *>(base + L.weights), job.n, F,
-                            reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.idx),
-                            reinterpret_cast<float *>(base + L.fv), reinterpret_cast<uint64_t *>(base + L.keys),
-                            reinterpret_cast<forest::StackRec *>(base + L.stack), reinterpret_cast<forest::NodeOut *>(base + L.nodes),
-                            reinterpret_cast<double *>(base + L.values), features, constf, drawn, vis, tied, mn, mx, vproxy,
-                            vpos, st};
+    forest::RegTree T{X, y, job.rows, reinterpret_cast<const int32_t *>(base + L.weights), job.n, F,
+                      reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.idx),
+                      reinterpret_cast<float *>(base + L.fv), reinterpret_cast<uint64_t *>(base + L.keys),
+                      reinterpret_cast<forest::StackRec *>(base + L.s.stack), reinterpret_cast<forest::NodeOut *>(base + L.s.nodes),
+                      reinterpret_cast<double *>(base + L.s.values)};
+    forest::carve_reg_smem(forest_reg_smem, T);
     forest::build_regression_tree(T, tm, seeds[blockIdx.x]);
-    if (threadIdx.x == 0) {
-        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
-        meta[0] = st->node_count;
-        meta[1] = st->max_depth;
-    }
+    put_meta(base + L.s.meta, T.st);
 }
-
-namespace {
-
-bool y_finite(double v) { return v - v == 0.0; }
-
-// trees per launch: as many as keep fixed + trees under the scratch slice bound, or 0 when not even one tree fits (the
-// entry points then refuse with B200AA_ERR_UNSUPPORTED before any CUDA call).  A tree's sort keys take 8 F pow2(n)
-// bytes, so at F = 136 one tree fits for n up to 131 072.
-int64_t reg_slice(size_t fixed, size_t per_tree, int64_t n_trees)
-{
-    if (fixed + per_tree > kScratchSliceBytes) return 0;
-    return std::min<int64_t>(n_trees, int64_t((kScratchSliceBytes - fixed) / per_tree));
-}
-
-}  // namespace
 
 extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n, int n_feats, int64_t row_stride,
                                            const double *h_y, int n_trees, const int32_t *h_weights,
@@ -424,22 +454,19 @@ extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n
         n > (int64_t(1) << 29) || n_feats < 1 || row_stride < n_feats || n_trees < 1 || node_capacity < 0 ||
         (dtype != B200AA_DTYPE_F32 && dtype != B200AA_DTYPE_F64))
         return B200AA_ERR_INVALID;
-    for (int64_t i = 0; i < n; ++i)
-        if (!y_finite(h_y[i])) return B200AA_ERR_INVALID;
-    for (int64_t i = 0; i < int64_t(n_trees) * n; ++i)
-        if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (!finite_targets(h_y, n) || !valid_weights(h_weights, int64_t(n_trees) * n)) return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
     const RegLayout L = reg_layout(n, n_feats);
     const size_t b_x = align256(size_t(n) * n_feats * 4), b_y = align256(size_t(n) * 8), b_seeds = align256(size_t(n_trees) * 4),
                  b_jobs = align256(size_t(n_trees) * sizeof(RegJob));
     const size_t fixed = b_x + b_y + b_seeds + b_jobs;
-    const int64_t slice = reg_slice(fixed, L.bytes, n_trees);
+    const int64_t slice = trees_per_launch(fixed, L.s.bytes, n_trees);
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::reg_smem_bytes(n_feats);
     CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
+    int rc = scratch.alloc(fixed + size_t(slice) * L.s.bytes);
     if (rc != B200AA_OK) return rc;
     char *base = static_cast<char *>(scratch.get());
     float *Xf = reinterpret_cast<float *>(base);
@@ -447,38 +474,20 @@ extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n
     uint32_t *seeds = reinterpret_cast<uint32_t *>(base + b_x + b_y);
     RegJob *jobs = reinterpret_cast<RegJob *>(base + b_x + b_y + b_seeds);
     char *trees = base + fixed;
-    const unsigned cast_blocks = unsigned(std::min<int64_t>((n * n_feats + 255) / 256, 4096));
-    with_real_type(dtype, [&](auto t) {
-        forest_cast_kernel<<<cast_blocks, 256, 0, st>>>(static_cast<const decltype(t) *>(d_X), n, n_feats, row_stride, Xf);
-    });
-    CK_LAUNCH("forest_cast_kernel");
+    if ((rc = cast_to_f32(d_X, dtype, n, n_feats, row_stride, Xf, st)) != B200AA_OK) return rc;
     std::vector<RegJob> hjobs(size_t(slice), RegJob{nullptr, n});
     CK(cudaMemcpyAsync(y, h_y, size_t(n) * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(jobs, hjobs.data(), size_t(slice) * sizeof(RegJob), cudaMemcpyHostToDevice, st));
-    int64_t written = 0;
-    std::vector<int64_t> meta(size_t(slice) * 2);
+    TreesOut out{h_nodes, h_values, 1, node_capacity, h_node_count, h_max_depth, 0};
     for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
         const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
         for (int64_t i = 0; i < nt; ++i)
-            CK(cudaMemcpyAsync(trees + size_t(i) * L.bytes + L.weights, h_weights + (t0 + i) * n, size_t(n) * 4,
+            CK(cudaMemcpyAsync(trees + size_t(i) * L.s.bytes + L.weights, h_weights + (t0 + i) * n, size_t(n) * 4,
                                cudaMemcpyHostToDevice, st));
         forest_reg_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(Xf, y, n_feats, jobs, seeds + t0, trees, L);
         CK_LAUNCH("forest_reg_build_kernel");
-        for (int64_t i = 0; i < nt; ++i)
-            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], trees + size_t(i) * L.bytes + L.meta, 16, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        for (int64_t i = 0; i < nt; ++i) {
-            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
-            h_node_count[t] = nc;
-            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
-            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
-            const char *tb = trees + size_t(i) * L.bytes;
-            CK(cudaMemcpyAsync(h_nodes + written, tb + L.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(h_values + written, tb + L.values, size_t(nc) * 8, cudaMemcpyDeviceToHost, st));
-            written += nc;
-        }
-        CK(cudaStreamSynchronize(st));    // the next slice reuses the scratch the copies read
+        if ((rc = read_trees(st, trees, L.s, t0, nt, out)) != B200AA_OK) return scratch.done(rc);
     }
     return scratch.done(B200AA_OK);
 }
@@ -503,11 +512,11 @@ struct RegPredJob {
 };
 }  // namespace
 
-// One thread per (problem, row), blockIdx.y the problem: walk its trees of this launch in tree order (left iff x <=
-// threshold) and add their leaf values to the row's sum (ForestRegressor.predict: out += tree.predict(X)); after the
+// One thread per (problem, row), blockIdx.y the problem: walk its trees of this launch in tree order (forest::tree_apply)
+// and add their leaf values to the row's sum (ForestRegressor.predict: out += tree.predict(X)); after the
 // problem's last tree, the sum / n_trees in its place (y_hat /= len(estimators_)).
 __global__ void forest_reg_predict_kernel(const float *__restrict__ Xs, int F, const RegPredJob *__restrict__ pjobs,
-                                          const char *__restrict__ trees, RegLayout L, double *__restrict__ acc)
+                                          const char *__restrict__ trees, Slot S, double *__restrict__ acc)
 {
     const RegPredJob J = pjobs[blockIdx.y];
     const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -515,11 +524,9 @@ __global__ void forest_reg_predict_kernel(const float *__restrict__ Xs, int F, c
     const float *x = Xs + int64_t(J.rows[r]) * F;
     double a = J.first ? 0.0 : acc[J.acc_off + r];
     for (int t = J.t0; t < J.t0 + J.nt; ++t) {
-        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * L.bytes + L.nodes);
-        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * L.bytes + L.values);
-        int32_t i = 0;
-        while (nodes[i].left != forest::kTreeLeaf) i = double(x[nodes[i].feature]) <= nodes[i].threshold ? nodes[i].left : nodes[i].right;
-        a = forest::dadd(a, values[i]);
+        const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(trees + size_t(t) * S.bytes + S.nodes);
+        const double *values = reinterpret_cast<const double *>(trees + size_t(t) * S.bytes + S.values);
+        a = forest::dadd(a, values[forest::tree_apply(nodes, [x](int f) { return x[f]; })]);
     }
     acc[J.acc_off + r] = J.last ? forest::ddiv(a, double(J.n_trees)) : a;
 }
@@ -536,23 +543,17 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
     if (!d_X || !h_y || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !h_n_trees || !h_weights ||
         !h_seeds || !d_pred_test || !d_pred_train || n < 1 || n > (int64_t(1) << 29) || n_feats < 1 || n_problems < 1)
         return B200AA_ERR_INVALID;
-    for (int64_t i = 0; i < n; ++i)
-        if (!y_finite(h_y[i])) return B200AA_ERR_INVALID;
-    if (h_train_off[0] != 0 || h_test_off[0] != 0) return B200AA_ERR_INVALID;
+    if (!finite_targets(h_y, n) || !valid_splits(n, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx))
+        return B200AA_ERR_INVALID;
     int64_t ntr_max = 0, trees_total = 0, weights_total = 0;
     for (int64_t p = 0; p < n_problems; ++p) {
-        const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off[p + 1] - h_test_off[p];
-        if (ntr < 1 || ntr > n || nte < 0 || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
-        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
-            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
-        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
-            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
+        const int64_t ntr = h_train_off[p + 1] - h_train_off[p];
+        if (ntr > n || h_n_trees[p] < 1) return B200AA_ERR_INVALID;
         ntr_max = std::max(ntr_max, ntr);
         trees_total += h_n_trees[p];
         weights_total += int64_t(h_n_trees[p]) * ntr;
     }
-    for (int64_t i = 0; i < weights_total; ++i)
-        if (h_weights[i] < 0 || h_weights[i] > (1 << 29)) return B200AA_ERR_INVALID;
+    if (!valid_weights(h_weights, weights_total)) return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
     const int F = n_feats;
     const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems], n_rows = n_tr + n_te;
@@ -563,13 +564,13 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
                  b_seeds = align256(size_t(trees_total) * 4), b_jobs = align256(size_t(trees_total) * sizeof(RegJob)),
                  b_pjobs = align256(size_t(n_problems) * sizeof(RegPredJob));
     const size_t fixed = b_xs + b_y + b_tr + b_rows + b_acc + b_seeds + b_jobs + b_pjobs;
-    const int64_t slice = std::min<int64_t>(reg_slice(fixed, L.bytes, trees_total), 65535);    // problems per launch: grid y
+    const int64_t slice = std::min<int64_t>(trees_per_launch(fixed, L.s.bytes, trees_total), 65535);    // problems per launch: grid y
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::reg_smem_bytes(F);
     CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * L.bytes);
+    const int rc = scratch.alloc(fixed + size_t(slice) * L.s.bytes);
     if (rc != B200AA_OK) return rc;
     char *q = static_cast<char *>(scratch.get());
     float *d_xs = reinterpret_cast<float *>(q); q += b_xs;
@@ -613,7 +614,7 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
         for (int64_t i = 0; i < nt; ++i) {
             const int64_t g = g0 + i, p = prob_of[size_t(g)];
             const int64_t ntr = h_train_off[p + 1] - h_train_off[p];
-            CK(cudaMemcpyAsync(d_trees + size_t(i) * L.bytes + L.weights, h_weights + w0[p] + (g - tree0[p]) * ntr,
+            CK(cudaMemcpyAsync(d_trees + size_t(i) * L.s.bytes + L.weights, h_weights + w0[p] + (g - tree0[p]) * ntr,
                                size_t(ntr) * 4, cudaMemcpyHostToDevice, st));
         }
         forest_reg_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(d_xs, d_y, F, d_jobs + g0, d_seeds + g0,
@@ -630,7 +631,7 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
         }
         CK(cudaMemcpyAsync(d_pjobs, pj.data(), size_t(np) * sizeof(RegPredJob), cudaMemcpyHostToDevice, st));
         forest_reg_predict_kernel<<<dim3(unsigned((max_rows + 127) / 128), unsigned(np)), 128, 0, st>>>(
-            d_xs, F, d_pjobs, d_trees, L, d_acc);
+            d_xs, F, d_pjobs, d_trees, L.s, d_acc);
         CK_LAUNCH("forest_reg_predict_kernel");
         CK(cudaStreamSynchronize(st));    // the next launch reuses the scratch and the host job arrays
     }
@@ -663,18 +664,17 @@ struct BoostJob {
     double *raw_test;
 };
 
-// a boosting tree's scratch: the regression tree's, then leaf_of [n] and leaf_rows [n]
+// a boosting tree's slot: [leaf_of | leaf_rows | the regression tree's slot]
 struct BoostLayout {
+    size_t leaf_of, leaf_rows;
     RegLayout reg;
-    size_t leaf_of, leaf_rows, bytes;
 };
 BoostLayout boost_layout(int64_t n, int F)
 {
     BoostLayout B;
-    B.reg = reg_layout(n, F);
-    B.leaf_of = B.reg.bytes;
+    B.leaf_of = 0;
     B.leaf_rows = B.leaf_of + align256(size_t(n) * 4);
-    B.bytes = B.leaf_rows + align256(size_t(n) * 4);
+    B.reg = reg_layout(n, F, B.leaf_rows + align256(size_t(n) * 4));
     return B;
 }
 
@@ -690,7 +690,10 @@ __global__ void __launch_bounds__(forest::kThreads) boost_build_kernel(const flo
     extern __shared__ __align__(16) unsigned char boost_smem[];
     const forest::Team tm{int(threadIdx.x), int(blockDim.x)};
     const RegLayout &L = B.reg;
-    char *base = scratch + size_t(blockIdx.x) * B.bytes;
+    char *base = scratch + size_t(blockIdx.x) * L.s.bytes;
+    // forest::carve_reg_smem's carve with part [kThreads] after vpos (boost_smem_bytes), written out: calling the carve
+    // here swaps two local arrays in the kernel's stack frame, which costs 16 bytes of stack and 4 / 8 bytes of spill
+    // stores / loads
     unsigned char *s = boost_smem;
     forest::RegShared *st = reinterpret_cast<forest::RegShared *>(s);
     s += (sizeof(forest::RegShared) + 15) & ~size_t(15);
@@ -711,17 +714,13 @@ __global__ void __launch_bounds__(forest::kThreads) boost_build_kernel(const flo
     const forest::RegTree T{X, J.neg_g + J.k, J.rows, w, J.n, F,
                             reinterpret_cast<int32_t *>(base + L.samples), reinterpret_cast<int32_t *>(base + L.idx),
                             reinterpret_cast<float *>(base + L.fv), reinterpret_cast<uint64_t *>(base + L.keys),
-                            reinterpret_cast<forest::StackRec *>(base + L.stack), reinterpret_cast<forest::NodeOut *>(base + L.nodes),
-                            reinterpret_cast<double *>(base + L.values), features, constf, drawn, vis, tied, mn, mx, vproxy,
+                            reinterpret_cast<forest::StackRec *>(base + L.s.stack), reinterpret_cast<forest::NodeOut *>(base + L.s.nodes),
+                            reinterpret_cast<double *>(base + L.s.values), features, constf, drawn, vis, tied, mn, mx, vproxy,
                             vpos, st, J.K, forest::kBoostDepth};
     forest::build_regression_tree(T, tm, seeds[blockIdx.x]);
     forest::boost_leaves(T, forest::BoostTree{J.y, J.k, J.K, J.raw, lr, reinterpret_cast<int32_t *>(base + B.leaf_of),
                                               reinterpret_cast<int32_t *>(base + B.leaf_rows), part}, tm);
-    if (threadIdx.x == 0) {
-        int64_t *meta = reinterpret_cast<int64_t *>(base + L.meta);
-        meta[0] = st->node_count;
-        meta[1] = st->max_depth;
-    }
+    put_meta(base + L.s.meta, T.st);
 }
 
 // One thread per (tree, test row), blockIdx.y the tree of the launch: the row's leaf, and raw_test[:, k] += lr * value
@@ -732,9 +731,9 @@ __global__ void boost_test_kernel(const float *__restrict__ X, int F, const Boos
     const BoostJob J = jobs[blockIdx.y];
     const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (r >= J.n_test) return;
-    const char *base = scratch + size_t(blockIdx.y) * B.bytes;
-    const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(base + B.reg.nodes);
-    const double *values = reinterpret_cast<const double *>(base + B.reg.values);
+    const char *base = scratch + size_t(blockIdx.y) * B.reg.s.bytes;
+    const forest::NodeOut *nodes = reinterpret_cast<const forest::NodeOut *>(base + B.reg.s.nodes);
+    const double *values = reinterpret_cast<const double *>(base + B.reg.s.values);
     const float *x = X + int64_t(J.test_rows[r]) * F;
     const int32_t leaf = forest::tree_apply(nodes, [x](int f) { return x[f]; });
     double &o = J.raw_test[r * J.K + J.k];
@@ -760,18 +759,13 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
         !h_seeds || n_rows < 1 || n_rows > (int64_t(1) << 29) || n_feats < 1 || n_problems < 1 ||
         !(learning_rate - learning_rate == 0.0) || (h_test_off == nullptr) != (h_test_rows == nullptr) ||
         out != (h_values != nullptr) || out != (h_node_count != nullptr) || out != (h_max_depth != nullptr) ||
-        node_capacity < 0 || h_train_off[0] != 0 || (h_test_off && h_test_off[0] != 0))
+        node_capacity < 0 || !valid_splits(n_rows, n_problems, h_train_off, h_train_rows, h_test_off, h_test_rows))
         return B200AA_ERR_INVALID;
     int64_t ntr_max = 0, nte_max = 0, n_trees = 0;
     for (int64_t p = 0; p < n_problems; ++p) {
         const int64_t ntr = h_train_off[p + 1] - h_train_off[p], nte = h_test_off ? h_test_off[p + 1] - h_test_off[p] : 0;
-        if (ntr < 1 || nte < 0 || !valid_trees_per_stage(h_n_trees[p]) || (h_active[p] != 0 && h_active[p] != 1))
+        if (!valid_trees_per_stage(h_n_trees[p]) || (h_active[p] != 0 && h_active[p] != 1) || (nte > 0 && !d_raw_test))
             return B200AA_ERR_INVALID;
-        if (nte > 0 && !d_raw_test) return B200AA_ERR_INVALID;
-        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
-            if (h_train_rows[i] < 0 || h_train_rows[i] >= n_rows) return B200AA_ERR_INVALID;
-        for (int64_t i = h_test_off ? h_test_off[p] : 0; i < (h_test_off ? h_test_off[p + 1] : 0); ++i)
-            if (h_test_rows[i] < 0 || h_test_rows[i] >= n_rows) return B200AA_ERR_INVALID;
         if (!h_active[p]) continue;
         ntr_max = std::max(ntr_max, ntr);
         nte_max = std::max(nte_max, nte);
@@ -785,14 +779,14 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
                  b_seeds = align256(size_t(std::max<int64_t>(n_trees, 1)) * 4),
                  b_jobs = align256(size_t(std::max<int64_t>(n_trees, 1)) * sizeof(BoostJob));
     const size_t fixed = b_tr + b_te + b_seeds + b_jobs;
-    const int64_t slice = std::min<int64_t>(reg_slice(fixed, B.bytes, std::max<int64_t>(n_trees, 1)), 65535);    // grid y
+    const int64_t slice = std::min<int64_t>(trees_per_launch(fixed, B.reg.s.bytes, std::max<int64_t>(n_trees, 1)), 65535);    // grid y
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     if (n_trees == 0) return B200AA_OK;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::boost_smem_bytes(n_feats);
     CK(cudaFuncSetAttribute(boost_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kBoostSmemCap)));
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * B.bytes);
+    int rc = scratch.alloc(fixed + size_t(slice) * B.reg.s.bytes);
     if (rc != B200AA_OK) return rc;
     char *q = static_cast<char *>(scratch.get());
     int32_t *d_tr = reinterpret_cast<int32_t *>(q); q += b_tr;
@@ -818,8 +812,7 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
     if (n_te) CK(cudaMemcpyAsync(d_te, h_test_rows, size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_jobs, jobs.data(), size_t(n_trees) * sizeof(BoostJob), cudaMemcpyHostToDevice, st));
-    int64_t written = 0;
-    std::vector<int64_t> meta(size_t(slice) * 2);
+    TreesOut trees_out{h_nodes, h_values, 1, node_capacity, h_node_count, h_max_depth, 0};
     for (int64_t t0 = 0; t0 < n_trees; t0 += slice) {
         const int64_t nt = std::min<int64_t>(slice, n_trees - t0);
         boost_build_kernel<<<unsigned(nt), forest::kThreads, smem, st>>>(d_X, n_feats, d_jobs + t0, d_seeds + t0,
@@ -832,21 +825,8 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
                                                                                                 learning_rate, d_trees, B);
             CK_LAUNCH("boost_test_kernel");
         }
-        if (!out) continue;             // the next launch reuses the scratch in stream order
-        for (int64_t i = 0; i < nt; ++i)
-            CK(cudaMemcpyAsync(&meta[size_t(i) * 2], d_trees + size_t(i) * B.bytes + B.reg.meta, 16, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        for (int64_t i = 0; i < nt; ++i) {
-            const int64_t nc = meta[size_t(i) * 2], t = t0 + i;
-            h_node_count[t] = nc;
-            h_max_depth[t] = int32_t(meta[size_t(i) * 2 + 1]);
-            if (written + nc > node_capacity) return scratch.done(B200AA_ERR_INVALID);
-            const char *tb = d_trees + size_t(i) * B.bytes;
-            CK(cudaMemcpyAsync(h_nodes + written, tb + B.reg.nodes, size_t(nc) * sizeof(forest::NodeOut), cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(h_values + written, tb + B.reg.values, size_t(nc) * 8, cudaMemcpyDeviceToHost, st));
-            written += nc;
-        }
-        CK(cudaStreamSynchronize(st));
+        // without trees to return, the next launch reuses the scratch in stream order
+        if (out && (rc = read_trees(st, d_trees, B.reg.s, t0, nt, trees_out)) != B200AA_OK) return scratch.done(rc);
     }
     return scratch.done(B200AA_OK);
 }
@@ -858,15 +838,8 @@ extern "C" int b200aa_boosting_scale(const double *d_X, int64_t n, int n_feats, 
     NvtxRange nvtx_("b200aa_boosting_scale");
     REFUSE_CAPTURE(stream, "b200aa_boosting_scale", kWhyHostArrays);
     if (!d_X || !h_train_off || !h_train_idx || !h_test_off || !h_test_idx || !d_Xs || n < 1 || n > (int64_t(1) << 29) ||
-        n_feats < 1 || n_problems < 1 || h_train_off[0] != 0 || h_test_off[0] != 0)
+        n_feats < 1 || n_problems < 1 || !valid_splits(n, n_problems, h_train_off, h_train_idx, h_test_off, h_test_idx))
         return B200AA_ERR_INVALID;
-    for (int64_t p = 0; p < n_problems; ++p) {
-        if (h_train_off[p + 1] - h_train_off[p] < 1 || h_test_off[p + 1] < h_test_off[p]) return B200AA_ERR_INVALID;
-        for (int64_t i = h_train_off[p]; i < h_train_off[p + 1]; ++i)
-            if (h_train_idx[i] < 0 || h_train_idx[i] >= n) return B200AA_ERR_INVALID;
-        for (int64_t i = h_test_off[p]; i < h_test_off[p + 1]; ++i)
-            if (h_test_idx[i] < 0 || h_test_idx[i] >= n) return B200AA_ERR_INVALID;
-    }
     const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems];
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StreamScratch scratch(st);

@@ -187,6 +187,28 @@ constexpr size_t smem_bytes(int F, int C)
 }
 constexpr size_t kSmemCap = smem_bytes(kMaxFeats, kMaxClasses);
 
+// forest_build_kernel's dynamic shared memory at s (16-aligned) carved into T's team-shared arrays for a team of `team`
+// threads, in the order smem_bytes counts them (T.F and T.C set).  Returns the end of the carve.
+__host__ __device__ inline unsigned char *carve_smem(unsigned char *s, size_t team, Tree &T)
+{
+    T.st = reinterpret_cast<Shared *>(s);
+    s += (sizeof(Shared) + 15) & ~size_t(15);
+    T.thr = reinterpret_cast<double *>(s);
+    s += size_t(T.F) * 8;
+    T.cnt = reinterpret_cast<int64_t *>(s);
+    s += team * T.C * 8;
+    T.red_proxy = reinterpret_cast<double *>(s);
+    s += team * 8;
+    T.red_pos = reinterpret_cast<int64_t *>(s);
+    s += team * 8;
+    T.mn = reinterpret_cast<float *>(s);
+    T.mx = T.mn + T.F;
+    T.features = reinterpret_cast<int32_t *>(T.mx + T.F);
+    T.constf = T.features + T.F;
+    T.drawn = T.constf + T.F;
+    return reinterpret_cast<unsigned char *>(T.drawn + T.F);
+}
+
 // The team building one tree: on the device the CTA (sync = __syncthreads); on the host, tid / n of threads that meet at
 // wait(wait_ctx), a barrier (tests/ run the builders on std::threads), or a team of one with no wait.
 struct Team {
@@ -715,11 +737,6 @@ struct RegShared {
     uint32_t rng;
 };
 
-// Dynamic shared memory of forest_reg_build_kernel: st, vproxy / vpos [F], mn / mx / features / constf / drawn / vis /
-// tied [F]; the attribute is set to kRegSmemCap (as kSmemCap)
-constexpr size_t reg_smem_bytes(int F) { return sizeof(RegShared) + size_t(F) * (5 * 4 + 2 * 4 + 16) + 64; }
-constexpr size_t kRegSmemCap = reg_smem_bytes(kMaxFeats);
-
 // Everything one regression tree reads and writes.  Global: X [rows, F] and y [rows] (shared by every tree; rows[s] is
 // local sample s's row, or s when rows is NULL), w [n] (bootstrap counts), samples / idx [n] and fv [n] (the replay's
 // indices and values), keys [F * pow2_at_least(n)], stack [n + 1], nodes [2 n - 1], values [2 n - 1].  Team-shared:
@@ -751,6 +768,32 @@ struct RegTree {
     __host__ __device__ double yv(int32_t s) const { return y_stride ? y[int64_t(s) * y_stride] : y[row(s)]; }
     __host__ __device__ double wv(int32_t s) const { return double(w[s]); }
 };
+
+// Dynamic shared memory of forest_reg_build_kernel: st, vproxy / vpos [F], mn / mx / features / constf / drawn / vis /
+// tied [F]; the attribute is set to kRegSmemCap (as kSmemCap)
+constexpr size_t reg_smem_bytes(int F) { return sizeof(RegShared) + size_t(F) * (5 * 4 + 2 * 4 + 16) + 64; }
+constexpr size_t kRegSmemCap = reg_smem_bytes(kMaxFeats);
+
+// forest_reg_build_kernel's dynamic shared memory at s (16-aligned) carved into T's team-shared arrays, in the order
+// reg_smem_bytes counts them (T.F set).  Returns the end of the carve.  boost_build_kernel carves the same with part
+// [kThreads] after vpos (boost_smem_bytes).
+__host__ __device__ inline unsigned char *carve_reg_smem(unsigned char *s, RegTree &T)
+{
+    T.st = reinterpret_cast<RegShared *>(s);
+    s += (sizeof(RegShared) + 15) & ~size_t(15);
+    T.vproxy = reinterpret_cast<double *>(s);
+    s += size_t(T.F) * 8;
+    T.vpos = reinterpret_cast<int64_t *>(s);
+    s += size_t(T.F) * 8;
+    T.mn = reinterpret_cast<float *>(s);
+    T.mx = T.mn + T.F;
+    T.features = reinterpret_cast<int32_t *>(T.mx + T.F);
+    T.constf = T.features + T.F;
+    T.drawn = T.constf + T.F;
+    T.vis = T.drawn + T.F;
+    T.tied = T.vis + T.F;
+    return reinterpret_cast<unsigned char *>(T.tied + T.F);
+}
 
 // Sets a flag that several of the team's threads may set between two syncs: a plain store on the device, a relaxed
 // atomic one on the host, where concurrent plain stores (even of one value) are a data race to C++ and ThreadSanitizer.

@@ -370,6 +370,25 @@ def test_stage_argument_checks():
         assert _stage(lib, a) == L.ERR_INVALID, kw
     a = _stage_args(F=513)
     assert _stage(lib, a) == L.ERR_UNSUPPORTED
+    # a training split of more rows than X has (here 7 of 6, one repeated) is accepted: F = 513 refuses it next
+    a = _stage_args(F=513)
+    a.update(tro=np.array([0, 7], np.int64), tr=np.array([0, 1, 2, 3, 4, 5, 0], np.int32))
+    assert _stage(lib, a) == L.ERR_UNSUPPORTED
+    # an input both invalid and over the feature limit is invalid
+    for kw in (dict(tr=np.array([0, 1, 2, 6], np.int32)), dict(K=np.array([2], np.int32)), dict(rawte=None)):
+        a = _stage_args(F=513)
+        a.update(kw)
+        assert _stage(lib, a) == L.ERR_INVALID, kw
+    # an inactive problem's rows are checked, but it counts toward no size limit: nothing to build returns B200AA_OK
+    # before any CUDA call, even for a training set over the scratch bound
+    a = _stage_args(F=513)
+    a.update(act=np.array([0], np.int32), te=np.array([4, 6], np.int32))
+    assert _stage(lib, a) == L.ERR_INVALID
+    n = 131073
+    a = _stage_args(n=n, F=136)
+    a.update(tro=np.array([0, n], np.int64), tr=np.arange(n, dtype=np.int32), teo=None, te=None, rawte=None,
+             K=np.array([1], np.int32), act=np.array([0], np.int32), seeds=np.ones(1, np.uint32))
+    assert _stage(lib, a) == L.OK
 
 
 def test_scale_and_count_argument_checks():

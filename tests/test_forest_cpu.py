@@ -244,6 +244,10 @@ def test_abi_argument_checks():
     assert call(F=513, stride=513, mf=1) == L.ERR_UNSUPPORTED
     ybig = np.arange(n, dtype=np.int32) % 33
     assert call(y=p(ybig), C=33) == L.ERR_UNSUPPORTED
+    # an input both invalid and over the feature or class limit is invalid
+    assert call(F=513, stride=513, mf=1, w=p(wneg)) == L.ERR_INVALID
+    assert call(F=513, stride=513, mf=1, C=1) == L.ERR_INVALID
+    assert call(y=p(ybig), C=33, w=p(wneg)) == L.ERR_INVALID
 
 
 def test_cross_validate_argument_checks():
@@ -275,3 +279,9 @@ def test_cross_validate_argument_checks():
                dict(tro=p(empty))):
         assert call(**kw) == L.ERR_INVALID, kw
     assert call(F=513) == L.ERR_UNSUPPORTED
+    # a training split of more rows than X has (here 7 of 6, one repeated) is invalid
+    long_off, long_tr = np.array([0, 7], np.int64), np.array([0, 1, 2, 3, 4, 5, 0], np.int32)
+    assert call(tro=p(long_off), tr=p(long_tr), w=p(np.ones((2, 7), np.int32))) == L.ERR_INVALID
+    # an input both invalid and over the feature limit is invalid
+    assert call(F=513, tr=p(bad_tr)) == L.ERR_INVALID
+    assert call(F=513, te=p(np.array([4, 6], np.int32))) == L.ERR_INVALID

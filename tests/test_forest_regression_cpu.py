@@ -280,6 +280,9 @@ def test_abi_argument_checks():
                dict(y=p(ynan)), dict(y=p(yinf)), dict(w=p(wneg))):
         assert call(**kw) == L.ERR_INVALID, kw
     assert call(F=513, stride=513) == L.ERR_UNSUPPORTED
+    # an input both invalid and over the feature limit is invalid
+    assert call(F=513, stride=513, y=p(ynan)) == L.ERR_INVALID
+    assert call(F=513, stride=513, w=p(wneg)) == L.ERR_INVALID
 
 
 def test_cross_validate_argument_checks():
@@ -316,6 +319,13 @@ def test_cross_validate_argument_checks():
                dict(tro=p(empty)), dict(w=p(wneg))):
         assert call(**kw) == L.ERR_INVALID, kw
     assert call(F=513) == L.ERR_UNSUPPORTED
+    # a training split of more rows than X has (here 7 of 6, one repeated) is invalid
+    long_off, long_tr = np.array([0, 7], np.int64), np.array([0, 1, 2, 3, 4, 5, 0], np.int32)
+    assert call(tro=p(long_off), tr=p(long_tr), w=p(np.ones((2, 7), np.int32))) == L.ERR_INVALID
+    # an input both invalid and over the feature limit is invalid
+    assert call(F=513, y=p(ynan)) == L.ERR_INVALID
+    assert call(F=513, te=p(bad_te)) == L.ERR_INVALID
+    assert call(F=513, w=p(wneg)) == L.ERR_INVALID
 
 
 def test_scratch_bound_refused_before_any_cuda_call():

@@ -271,3 +271,26 @@ def test_final_fit_through_rebound_train_gradient_boosting():
     np.random.seed(13)
     ref = GradientBoostingClassifier(n_estimators=10).fit(Xn, y)
     BC.compare(got, ref, BC.held_out(Xn))
+
+
+def test_scale_accepts_a_training_split_longer_than_X():
+    """b200aa_boosting_scale accepts a training split of more rows than X has (repeated rows), as the stage does, and
+    standardises both splits with the training rows' StandardScaler fit."""
+    import ctypes
+    from sklearn.preprocessing import StandardScaler
+    from pyaudioanalysis_b200 import _lib as L
+    r = np.random.RandomState(4)
+    X = r.randn(6, 3)
+    tr, te = np.array([0, 1, 2, 3, 4, 5, 0, 1], np.int32), np.array([4, 5], np.int32)
+    tro, teo = np.array([0, tr.size], np.int64), np.array([0, te.size], np.int64)
+    d_X = torch.from_numpy(X).cuda()
+    out = torch.empty((tr.size + te.size, 3), dtype=torch.float32, device="cuda")
+
+    def p(a):
+        return ctypes.c_void_p(a.ctypes.data)
+    assert L.lib().b200aa_boosting_scale(ctypes.c_void_p(d_X.data_ptr()), 6, 3, 1, p(tro), p(tr), p(teo), p(te),
+                                         ctypes.c_void_p(out.data_ptr()), None) == L.OK
+    torch.cuda.synchronize()
+    sc = StandardScaler().fit(X[tr])
+    want = np.concatenate([sc.transform(X[tr]), sc.transform(X[te])]).astype(np.float32)
+    np.testing.assert_allclose(out.cpu().numpy(), want, rtol=1e-6, atol=1e-6)

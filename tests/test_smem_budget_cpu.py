@@ -60,9 +60,11 @@ SM90_OPTIN = 227 * 1024
 
 def test_kernel13_shared_memory_caps(tmp_path_factory):
     """Kernel 13's three build kernels: every accepted shape (F <= 512, C <= 32) fits under the kernel's cap, the cap is
-    the size at the largest shape, every cap is below sm_90's opt-in maximum, and every cudaFuncSetAttribute in forest.cu
-    passes a cap constant.  A launcher that set its own call's size instead would let a concurrent call of a smaller shape
-    lower the limit between another thread's set and launch, and that launch would fail."""
+    the size at the largest shape, every cap is below sm_90's opt-in maximum, at every accepted shape the carve of the
+    shared memory (forest.cuh carve_smem / carve_reg_smem) ends within the size formula the launchers pass, and every
+    cudaFuncSetAttribute in forest.cu passes a cap constant, with at least one per build kernel.  A launcher that set its
+    own call's size instead would let a concurrent call of a smaller shape lower the limit between another thread's set
+    and launch, and that launch would fail."""
     csrc = os.path.join(host_exe.ROOT, "pyaudioanalysis_b200", "csrc")
     exe = host_exe.build(tmp_path_factory, "forest_smem_host.cu", "-I" + csrc)
     lines = [ln.split() for ln in subprocess.run([exe], capture_output=True, text=True, check=True).stdout.splitlines()]
@@ -72,6 +74,8 @@ def test_kernel13_shared_memory_caps(tmp_path_factory):
         assert largest == cap, (kern, cap, largest, shape)
         assert cap <= SM90_OPTIN, (kern, cap)
     assert caps["forest_build_kernel"] == (49832, 49832, "512:32")          # past the 48 KB default
+    past = {ln[0]: int(ln[4]) for ln in lines}
+    assert past == dict.fromkeys(caps, 0), past
     src = open(os.path.join(csrc, "forest.cu")).read()
     calls = re.findall(r"cudaFuncSetAttribute\(\s*(\w+)\s*,\s*cudaFuncAttributeMaxDynamicSharedMemorySize\s*,\s*([^;]*?)\)\);", src)
     assert len(calls) == src.count("cudaFuncSetAttribute(") == 5, calls
@@ -79,3 +83,4 @@ def test_kernel13_shared_memory_caps(tmp_path_factory):
             "boost_build_kernel": "int(forest::kBoostSmemCap)"}
     for kern, arg in calls:
         assert want[kern] == arg.strip(), (kern, arg)
+    assert {kern for kern, _ in calls} == set(want), calls
