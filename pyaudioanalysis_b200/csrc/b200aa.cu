@@ -672,7 +672,7 @@ static int launch_clipped(const b200aa_plan *pl, StParams p, int64_t per_clip, c
     }
     // large windows: the arrays of every resident CTA in stream-ordered scratch, CTAs loop over the items
     const int64_t grid = std::min<int64_t>(p.n_items, int64_t(pl->sm_count) * 2);
-    p.scratch_stride = (bytes + 255) & ~size_t(255);
+    p.scratch_stride = align256(bytes);
     StreamScratch scratch(st);
     const int rc = scratch.alloc(p.scratch_stride * size_t(grid));
     if (rc != B200AA_OK) return rc;

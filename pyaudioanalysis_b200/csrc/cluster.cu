@@ -181,33 +181,32 @@ extern "C" int b200aa_cluster_distance_means(const double *d_X, int64_t n, int n
     std::vector<int32_t> mean_of(size_t(n_slots), -1);
     for (size_t m = 0; m < plan.means.size(); ++m) mean_of[size_t(plan.means[m].slot)] = int32_t(m);
 
-    // scratch: [perm | segments | means | mean_of] uploaded at once, then G, the segment sums, a pass's distances and leaf sums
-    const size_t perm_b = align256(perm.size() * sizeof(int64_t)), segs_b = align256(plan.segs.size() * sizeof(cluster::Segment));
-    const size_t means_b = align256(plan.means.size() * sizeof(cluster::Mean)), slots_b = align256(mean_of.size() * sizeof(int32_t));
-    const size_t head_b = perm_b + segs_b + means_b + slots_b;
-    const size_t g_b = align256(size_t(n) * D * sizeof(double)), sums_b = align256(plan.segs.size() * sizeof(double));
-    const size_t dist_b = align256(size_t(*std::max_element(plan.pass_dist.begin(), plan.pass_dist.end())) * sizeof(double));
-    const size_t leaf_b = size_t(*std::max_element(plan.pass_leaves.begin(), plan.pass_leaves.end())) * sizeof(double);
-    std::vector<char> head(head_b, 0);
-    std::memcpy(head.data(), perm.data(), perm.size() * sizeof(int64_t));
-    std::memcpy(head.data() + perm_b, plan.segs.data(), plan.segs.size() * sizeof(cluster::Segment));
-    std::memcpy(head.data() + perm_b + segs_b, plan.means.data(), plan.means.size() * sizeof(cluster::Mean));
-    std::memcpy(head.data() + perm_b + segs_b + means_b, mean_of.data(), mean_of.size() * sizeof(int32_t));
+    // the permutation, segments, means and mean_of, uploaded at once as one head
+    Layout L;
+    const size_t perm_at = L.add(perm.size() * sizeof(int64_t)), segs_at = L.add(plan.segs.size() * sizeof(cluster::Segment)),
+                 means_at = L.add(plan.means.size() * sizeof(cluster::Mean)), mean_of_at = L.add(mean_of.size() * sizeof(int32_t));
+    std::vector<char> head(L.bytes(), 0);
+    std::memcpy(head.data() + perm_at, perm.data(), perm.size() * sizeof(int64_t));
+    std::memcpy(head.data() + segs_at, plan.segs.data(), plan.segs.size() * sizeof(cluster::Segment));
+    std::memcpy(head.data() + means_at, plan.means.data(), plan.means.size() * sizeof(cluster::Mean));
+    std::memcpy(head.data() + mean_of_at, mean_of.data(), mean_of.size() * sizeof(int32_t));
+    // then G, the segment sums, and the largest pass's distances and leaf sums
+    const size_t g_at = L.add(size_t(n) * D * sizeof(double)), sums_at = L.add(plan.segs.size() * sizeof(double)),
+                 dist_at = L.add(size_t(*std::max_element(plan.pass_dist.begin(), plan.pass_dist.end())) * sizeof(double)),
+                 leaf_at = L.add(size_t(*std::max_element(plan.pass_leaves.begin(), plan.pass_leaves.end())) * sizeof(double));
 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(head_b + g_b + sums_b + dist_b + leaf_b);
+    const int rc = scratch.alloc(L.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const int64_t *d_perm = reinterpret_cast<const int64_t *>(base);
-    const cluster::Segment *d_segs = reinterpret_cast<const cluster::Segment *>(base + perm_b);
-    const cluster::Mean *d_means = reinterpret_cast<const cluster::Mean *>(base + perm_b + segs_b);
-    const int32_t *d_mean_of = reinterpret_cast<const int32_t *>(base + perm_b + segs_b + means_b);
-    double *G = reinterpret_cast<double *>(base + head_b);
-    double *seg_sum = reinterpret_cast<double *>(base + head_b + g_b);
-    double *dist = reinterpret_cast<double *>(base + head_b + g_b + sums_b);
-    double *leaf_sum = reinterpret_cast<double *>(base + head_b + g_b + sums_b + dist_b);
-    CK(cudaMemcpyAsync(base, head.data(), head_b, cudaMemcpyHostToDevice, st));
+    void *base = scratch.get();
+    const int64_t *d_perm = Layout::at<const int64_t>(base, perm_at);
+    const cluster::Segment *d_segs = Layout::at<const cluster::Segment>(base, segs_at);
+    const cluster::Mean *d_means = Layout::at<const cluster::Mean>(base, means_at);
+    const int32_t *d_mean_of = Layout::at<const int32_t>(base, mean_of_at);
+    double *G = Layout::at<double>(base, g_at), *seg_sum = Layout::at<double>(base, sums_at);
+    double *dist = Layout::at<double>(base, dist_at), *leaf_sum = Layout::at<double>(base, leaf_at);
+    CK(cudaMemcpyAsync(base, head.data(), head.size(), cudaMemcpyHostToDevice, st));
     const int64_t cells = n * D;
     cluster_gather_kernel<<<unsigned(std::min<int64_t>((cells + 255) / 256, 1 << 16)), 256, 0, st>>>(d_X, x_stride, D, d_perm,
                                                                                                      n, G);

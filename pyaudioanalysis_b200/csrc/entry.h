@@ -121,6 +121,29 @@ constexpr size_t kScratchSliceBytes = size_t(256) << 20;
 
 inline size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
 
+// The regions of one block of scratch, in order from offset `at`, each padded to a multiple of 256 bytes: add() returns a
+// region's byte offset, bytes() the end of the last.  One layout places both the host image of a head and the device block
+// it is uploaded to, so the two cannot disagree.
+class Layout {
+  public:
+    explicit Layout(size_t at = 0) : end_(at) {}
+    size_t add(size_t bytes)
+    {
+        const size_t at = end_;
+        end_ += align256(bytes);
+        return at;
+    }
+    size_t bytes() const { return end_; }
+    template <class T>
+    static T *at(void *base, size_t offset)
+    {
+        return reinterpret_cast<T *>(static_cast<char *>(base) + offset);
+    }
+
+  private:
+    size_t end_;
+};
+
 // f(float{}) for B200AA_DTYPE_F32, f(double{}) for B200AA_DTYPE_F64 (the caller has checked dtype): a launch over either
 // element type written once
 template <class F>

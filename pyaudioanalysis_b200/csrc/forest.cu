@@ -70,34 +70,36 @@ bool valid_splits(int64_t n, int64_t n_problems, const int64_t *train_off, const
 }
 
 // One tree's slot of global scratch: its builder's own arrays (the head), then the tail every builder writes: stack
-// [n + 1], nodes [2 n - 1], values [(2 n - 1) per_node], meta (node_count, max_depth).  Every part starts 256-aligned.
+// [n + 1], nodes [2 n - 1], values [(2 n - 1) per_node], meta (node_count, max_depth).
 struct Slot {
     size_t stack, nodes, values, meta, bytes;
 };
 Slot slot_after(size_t head, int64_t n, int per_node)
 {
     const int64_t cap = 2 * n - 1;
+    Layout A(head);
     Slot S;
-    S.stack = head;
-    S.nodes = S.stack + align256(size_t(n + 1) * sizeof(forest::StackRec));
-    S.values = S.nodes + align256(size_t(cap) * sizeof(forest::NodeOut));
-    S.meta = S.values + align256(size_t(cap) * per_node * 8);
-    S.bytes = S.meta + 256;
+    S.stack = A.add(size_t(n + 1) * sizeof(forest::StackRec));
+    S.nodes = A.add(size_t(cap) * sizeof(forest::NodeOut));
+    S.values = A.add(size_t(cap) * per_node * 8);
+    S.meta = A.add(2 * sizeof(int64_t));
+    S.bytes = A.bytes();
     return S;
 }
 
-// a classification tree's slot: [samples | tmp | keys | tail]
+// a classification tree's slot
 struct TreeLayout {
     size_t samples, tmp, keys;
     Slot s;
 };
 TreeLayout tree_layout(int64_t n, int C)
 {
+    Layout A;
     TreeLayout L;
-    L.samples = 0;
-    L.tmp = L.samples + align256(size_t(n) * 4);
-    L.keys = L.tmp + align256(size_t(n) * 4);
-    L.s = slot_after(L.keys + align256(size_t(forest::pow2_at_least(n)) * 8), n, C);
+    L.samples = A.add(size_t(n) * 4);
+    L.tmp = A.add(size_t(n) * 4);
+    L.keys = A.add(size_t(forest::pow2_at_least(n)) * 8);
+    L.s = slot_after(A.bytes(), n, C);
     return L;
 }
 
@@ -207,18 +209,20 @@ extern "C" int b200aa_forest_fit(const void *d_X, int dtype, int64_t n, int n_fe
     const size_t smem = forest::smem_bytes(n_feats, n_classes);
     CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kSmemCap)));
     const TreeLayout L = tree_layout(n, n_classes);
-    const size_t per_tree = L.s.bytes + (h_weights ? align256(size_t(n) * 4) : 0);
-    const size_t fixed = align256(size_t(n) * n_feats * 4) + align256(size_t(n) * 4) + align256(size_t(n_trees) * 4);
-    const int64_t slice = std::max<int64_t>(1, trees_per_launch(fixed, per_tree, n_trees));    // never refused for scratch
+    Layout A;
+    const size_t x_at = A.add(size_t(n) * n_feats * 4), y_at = A.add(size_t(n) * 4), seeds_at = A.add(size_t(n_trees) * 4);
+    const size_t w_row = h_weights ? align256(size_t(n) * 4) : 0;    // a tree's weights: one padded row per tree
+    const int64_t slice = std::max<int64_t>(1, trees_per_launch(A.bytes(), L.s.bytes + w_row, n_trees));    // never refused
+    const size_t trees_at = A.add(size_t(slice) * L.s.bytes), w_at = A.add(size_t(slice) * w_row);
     StreamScratch scratch(st);
-    int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
+    int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    float *Xf = reinterpret_cast<float *>(base);
-    int32_t *y = reinterpret_cast<int32_t *>(base + align256(size_t(n) * n_feats * 4));
-    uint32_t *seeds = reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(y) + align256(size_t(n) * 4));
-    char *trees = base + fixed;
-    int32_t *w = h_weights ? reinterpret_cast<int32_t *>(trees + size_t(slice) * L.s.bytes) : nullptr;
+    void *base = scratch.get();
+    float *Xf = Layout::at<float>(base, x_at);
+    int32_t *y = Layout::at<int32_t>(base, y_at);
+    uint32_t *seeds = Layout::at<uint32_t>(base, seeds_at);
+    char *trees = Layout::at<char>(base, trees_at);
+    int32_t *w = h_weights ? Layout::at<int32_t>(base, w_at) : nullptr;
     if ((rc = cast_to_f32(d_X, dtype, n, n_feats, row_stride, Xf, st)) != B200AA_OK) return rc;
     CK(cudaMemcpyAsync(y, h_y, size_t(n) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(seeds, h_seeds, size_t(n_trees) * 4, cudaMemcpyHostToDevice, st));
@@ -315,30 +319,29 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int C = n_classes, F = n_feats, max_features = forest::sqrt_features(F);
     CK(cudaFuncSetAttribute(forest_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kSmemCap)));
-    // scratch: [y_local | train | test | map | Xtr | Xte | acc | seeds | weights of a slice | trees of a slice]
+    // every region sized by the largest problem
     const TreeLayout Lmax = tree_layout(ntr_max, C);
-    const size_t b_y = align256(size_t(ntr_max) * 4), b_tr = b_y, b_te = align256(size_t(std::max<int64_t>(nte_max, 1)) * 4),
-                 b_map = 256, b_xtr = align256(size_t(ntr_max) * F * 4), b_xte = align256(size_t(std::max<int64_t>(nte_max, 1)) * F * 4),
-                 b_acc = align256(size_t(std::max<int64_t>(nte_max, 1)) * C * 8), b_seeds = align256(size_t(t_max) * 4),
-                 b_yt = b_te;
-    const size_t fixed = b_y + b_tr + b_te + b_map + b_xtr + b_xte + b_acc + b_seeds + b_yt;
-    const size_t per_tree = Lmax.s.bytes + (h_weights ? align256(size_t(ntr_max) * 4) : 0);
-    const int64_t slice = std::max<int64_t>(1, trees_per_launch(fixed, per_tree, t_max));    // never refused for scratch
+    const int64_t nte1 = std::max<int64_t>(nte_max, 1);
+    Layout A;
+    const size_t ylocal_at = A.add(size_t(ntr_max) * 4), train_at = A.add(size_t(ntr_max) * 4), test_at = A.add(size_t(nte1) * 4),
+                 map_at = A.add(forest::kMaxClasses * 4), xtr_at = A.add(size_t(ntr_max) * F * 4),
+                 xte_at = A.add(size_t(nte1) * F * 4), acc_at = A.add(size_t(nte1) * C * 8), seeds_at = A.add(size_t(t_max) * 4),
+                 ytest_at = A.add(size_t(nte1) * 4);
+    const size_t w_row = h_weights ? align256(size_t(ntr_max) * 4) : 0;    // a tree's weights: one padded row per tree
+    const int64_t slice = std::max<int64_t>(1, trees_per_launch(A.bytes(), Lmax.s.bytes + w_row, t_max));    // never refused
+    const size_t trees_at = A.add(size_t(slice) * Lmax.s.bytes), w_at = A.add(size_t(slice) * w_row);
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * per_tree);
+    const int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *q = static_cast<char *>(scratch.get());
-    int32_t *d_ylocal = reinterpret_cast<int32_t *>(q); q += b_y;
-    int32_t *d_train = reinterpret_cast<int32_t *>(q); q += b_tr;
-    int32_t *d_test = reinterpret_cast<int32_t *>(q); q += b_te;
-    int32_t *d_map = reinterpret_cast<int32_t *>(q); q += b_map;
-    float *d_xtr = reinterpret_cast<float *>(q); q += b_xtr;
-    float *d_xte = reinterpret_cast<float *>(q); q += b_xte;
-    double *d_acc = reinterpret_cast<double *>(q); q += b_acc;
-    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
-    int32_t *d_ytest = reinterpret_cast<int32_t *>(q); q += b_yt;
-    char *d_trees = q;
-    int32_t *d_w = h_weights ? reinterpret_cast<int32_t *>(d_trees + size_t(slice) * Lmax.s.bytes) : nullptr;
+    void *base = scratch.get();
+    int32_t *d_ylocal = Layout::at<int32_t>(base, ylocal_at), *d_train = Layout::at<int32_t>(base, train_at);
+    int32_t *d_test = Layout::at<int32_t>(base, test_at), *d_map = Layout::at<int32_t>(base, map_at);
+    float *d_xtr = Layout::at<float>(base, xtr_at), *d_xte = Layout::at<float>(base, xte_at);
+    double *d_acc = Layout::at<double>(base, acc_at);
+    uint32_t *d_seeds = Layout::at<uint32_t>(base, seeds_at);
+    int32_t *d_ytest = Layout::at<int32_t>(base, ytest_at);
+    char *d_trees = Layout::at<char>(base, trees_at);
+    int32_t *d_w = h_weights ? Layout::at<int32_t>(base, w_at) : nullptr;
     CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * C * C * sizeof(int64_t), st));
     std::vector<int32_t> ylocal(ntr_max), ytest(std::max<int64_t>(nte_max, 1)), map(forest::kMaxClasses);
     int64_t tree0 = 0, w0 = 0;
@@ -395,20 +398,21 @@ extern "C" int b200aa_forest_cross_validate(const double *d_X, int64_t n, int n_
 // ------------------------------------------------------------------------------------------------
 namespace {
 
-// a regression tree's slot of at most n samples, from offset `at`: [samples | idx | fv | keys | weights | tail]
+// a regression tree's slot of at most n samples, from offset `at`
 struct RegLayout {
     size_t samples, idx, fv, keys, weights;
     Slot s;
 };
 RegLayout reg_layout(int64_t n, int F, size_t at = 0)
 {
+    Layout A(at);
     RegLayout L;
-    L.samples = at;
-    L.idx = L.samples + align256(size_t(n) * 4);
-    L.fv = L.idx + align256(size_t(n) * 4);
-    L.keys = L.fv + align256(size_t(n) * 4);
-    L.weights = L.keys + align256(size_t(F) * size_t(forest::pow2_at_least(n)) * 8);
-    L.s = slot_after(L.weights + align256(size_t(n) * 4), n, 1);
+    L.samples = A.add(size_t(n) * 4);
+    L.idx = A.add(size_t(n) * 4);
+    L.fv = A.add(size_t(n) * 4);
+    L.keys = A.add(size_t(F) * size_t(forest::pow2_at_least(n)) * 8);
+    L.weights = A.add(size_t(n) * 4);
+    L.s = slot_after(A.bytes(), n, 1);
     return L;
 }
 
@@ -457,23 +461,24 @@ extern "C" int b200aa_forest_regressor_fit(const void *d_X, int dtype, int64_t n
     if (!finite_targets(h_y, n) || !valid_weights(h_weights, int64_t(n_trees) * n)) return B200AA_ERR_INVALID;
     if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
     const RegLayout L = reg_layout(n, n_feats);
-    const size_t b_x = align256(size_t(n) * n_feats * 4), b_y = align256(size_t(n) * 8), b_seeds = align256(size_t(n_trees) * 4),
-                 b_jobs = align256(size_t(n_trees) * sizeof(RegJob));
-    const size_t fixed = b_x + b_y + b_seeds + b_jobs;
-    const int64_t slice = trees_per_launch(fixed, L.s.bytes, n_trees);
+    Layout A;
+    const size_t x_at = A.add(size_t(n) * n_feats * 4), y_at = A.add(size_t(n) * 8), seeds_at = A.add(size_t(n_trees) * 4),
+                 jobs_at = A.add(size_t(n_trees) * sizeof(RegJob));
+    const int64_t slice = trees_per_launch(A.bytes(), L.s.bytes, n_trees);
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
+    const size_t trees_at = A.add(size_t(slice) * L.s.bytes);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::reg_smem_bytes(n_feats);
     CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
-    int rc = scratch.alloc(fixed + size_t(slice) * L.s.bytes);
+    int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    float *Xf = reinterpret_cast<float *>(base);
-    double *y = reinterpret_cast<double *>(base + b_x);
-    uint32_t *seeds = reinterpret_cast<uint32_t *>(base + b_x + b_y);
-    RegJob *jobs = reinterpret_cast<RegJob *>(base + b_x + b_y + b_seeds);
-    char *trees = base + fixed;
+    void *base = scratch.get();
+    float *Xf = Layout::at<float>(base, x_at);
+    double *y = Layout::at<double>(base, y_at);
+    uint32_t *seeds = Layout::at<uint32_t>(base, seeds_at);
+    RegJob *jobs = Layout::at<RegJob>(base, jobs_at);
+    char *trees = Layout::at<char>(base, trees_at);
     if ((rc = cast_to_f32(d_X, dtype, n, n_feats, row_stride, Xf, st)) != B200AA_OK) return rc;
     std::vector<RegJob> hjobs(size_t(slice), RegJob{nullptr, n});
     CK(cudaMemcpyAsync(y, h_y, size_t(n) * 8, cudaMemcpyHostToDevice, st));
@@ -557,31 +562,30 @@ extern "C" int b200aa_forest_regression_cross_validate(const double *d_X, int64_
     if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
     const int F = n_feats;
     const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems], n_rows = n_tr + n_te;
-    // scratch: [Xs | y | train | rows (test then train, per problem) | acc | seeds | jobs | pjobs | trees of a launch]
     const RegLayout L = reg_layout(ntr_max, F);
-    const size_t b_xs = align256(size_t(n) * F * 4), b_y = align256(size_t(n) * 8), b_tr = align256(size_t(n_tr) * 4),
-                 b_rows = align256(size_t(n_rows) * 4), b_acc = align256(size_t(std::max<int64_t>(n_rows, 1)) * 8),
-                 b_seeds = align256(size_t(trees_total) * 4), b_jobs = align256(size_t(trees_total) * sizeof(RegJob)),
-                 b_pjobs = align256(size_t(n_problems) * sizeof(RegPredJob));
-    const size_t fixed = b_xs + b_y + b_tr + b_rows + b_acc + b_seeds + b_jobs + b_pjobs;
-    const int64_t slice = std::min<int64_t>(trees_per_launch(fixed, L.s.bytes, trees_total), 65535);    // problems per launch: grid y
+    Layout A;
+    const size_t xs_at = A.add(size_t(n) * F * 4), y_at = A.add(size_t(n) * 8), train_at = A.add(size_t(n_tr) * 4),
+                 rows_at = A.add(size_t(n_rows) * 4), acc_at = A.add(size_t(std::max<int64_t>(n_rows, 1)) * 8),
+                 seeds_at = A.add(size_t(trees_total) * 4), jobs_at = A.add(size_t(trees_total) * sizeof(RegJob)),
+                 pjobs_at = A.add(size_t(n_problems) * sizeof(RegPredJob));
+    const int64_t slice = std::min<int64_t>(trees_per_launch(A.bytes(), L.s.bytes, trees_total), 65535);    // problems per launch: grid y
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
+    const size_t trees_at = A.add(size_t(slice) * L.s.bytes);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::reg_smem_bytes(F);
     CK(cudaFuncSetAttribute(forest_reg_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kRegSmemCap)));
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(fixed + size_t(slice) * L.s.bytes);
+    const int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *q = static_cast<char *>(scratch.get());
-    float *d_xs = reinterpret_cast<float *>(q); q += b_xs;
-    double *d_y = reinterpret_cast<double *>(q); q += b_y;
-    int32_t *d_train = reinterpret_cast<int32_t *>(q); q += b_tr;
-    int32_t *d_rows = reinterpret_cast<int32_t *>(q); q += b_rows;
-    double *d_acc = reinterpret_cast<double *>(q); q += b_acc;
-    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
-    RegJob *d_jobs = reinterpret_cast<RegJob *>(q); q += b_jobs;
-    RegPredJob *d_pjobs = reinterpret_cast<RegPredJob *>(q); q += b_pjobs;
-    char *d_trees = q;
+    void *base = scratch.get();
+    float *d_xs = Layout::at<float>(base, xs_at);
+    double *d_y = Layout::at<double>(base, y_at);
+    int32_t *d_train = Layout::at<int32_t>(base, train_at), *d_rows = Layout::at<int32_t>(base, rows_at);
+    double *d_acc = Layout::at<double>(base, acc_at);
+    uint32_t *d_seeds = Layout::at<uint32_t>(base, seeds_at);
+    RegJob *d_jobs = Layout::at<RegJob>(base, jobs_at);
+    RegPredJob *d_pjobs = Layout::at<RegPredJob>(base, pjobs_at);
+    char *d_trees = Layout::at<char>(base, trees_at);
     // every tree's job, and every problem's rows: its test rows, then its training rows
     std::vector<RegJob> jobs(static_cast<size_t>(trees_total));
     std::vector<int32_t> rows(size_t(std::max<int64_t>(n_rows, 1)));
@@ -664,17 +668,18 @@ struct BoostJob {
     double *raw_test;
 };
 
-// a boosting tree's slot: [leaf_of | leaf_rows | the regression tree's slot]
+// a boosting tree's slot: its leaf arrays, then a regression tree's slot
 struct BoostLayout {
     size_t leaf_of, leaf_rows;
     RegLayout reg;
 };
 BoostLayout boost_layout(int64_t n, int F)
 {
+    Layout A;
     BoostLayout B;
-    B.leaf_of = 0;
-    B.leaf_rows = B.leaf_of + align256(size_t(n) * 4);
-    B.reg = reg_layout(n, F, B.leaf_rows + align256(size_t(n) * 4));
+    B.leaf_of = A.add(size_t(n) * 4);
+    B.leaf_rows = A.add(size_t(n) * 4);
+    B.reg = reg_layout(n, F, A.bytes());
     return B;
 }
 
@@ -774,26 +779,25 @@ extern "C" int b200aa_boosting_stage(const float *d_X, int64_t n_rows, int n_fea
     if (n_feats > forest::kMaxFeats) return B200AA_ERR_UNSUPPORTED;
     const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off ? h_test_off[n_problems] : 0;
     const BoostLayout B = boost_layout(std::max<int64_t>(ntr_max, 1), n_feats);
-    // scratch: [train rows | test rows | seeds | jobs | trees of a launch]
-    const size_t b_tr = align256(size_t(n_tr) * 4), b_te = align256(size_t(std::max<int64_t>(n_te, 1)) * 4),
-                 b_seeds = align256(size_t(std::max<int64_t>(n_trees, 1)) * 4),
-                 b_jobs = align256(size_t(std::max<int64_t>(n_trees, 1)) * sizeof(BoostJob));
-    const size_t fixed = b_tr + b_te + b_seeds + b_jobs;
-    const int64_t slice = std::min<int64_t>(trees_per_launch(fixed, B.reg.s.bytes, std::max<int64_t>(n_trees, 1)), 65535);    // grid y
+    const int64_t n_trees1 = std::max<int64_t>(n_trees, 1);
+    Layout A;
+    const size_t tr_at = A.add(size_t(n_tr) * 4), te_at = A.add(size_t(std::max<int64_t>(n_te, 1)) * 4),
+                 seeds_at = A.add(size_t(n_trees1) * 4), jobs_at = A.add(size_t(n_trees1) * sizeof(BoostJob));
+    const int64_t slice = std::min<int64_t>(trees_per_launch(A.bytes(), B.reg.s.bytes, n_trees1), 65535);    // grid y
     if (slice < 1) return B200AA_ERR_UNSUPPORTED;
     if (n_trees == 0) return B200AA_OK;
+    const size_t trees_at = A.add(size_t(slice) * B.reg.s.bytes);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = forest::boost_smem_bytes(n_feats);
     CK(cudaFuncSetAttribute(boost_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(forest::kBoostSmemCap)));
     StreamScratch scratch(st);
-    int rc = scratch.alloc(fixed + size_t(slice) * B.reg.s.bytes);
+    int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *q = static_cast<char *>(scratch.get());
-    int32_t *d_tr = reinterpret_cast<int32_t *>(q); q += b_tr;
-    int32_t *d_te = reinterpret_cast<int32_t *>(q); q += b_te;
-    uint32_t *d_seeds = reinterpret_cast<uint32_t *>(q); q += b_seeds;
-    BoostJob *d_jobs = reinterpret_cast<BoostJob *>(q); q += b_jobs;
-    char *d_trees = q;
+    void *base = scratch.get();
+    int32_t *d_tr = Layout::at<int32_t>(base, tr_at), *d_te = Layout::at<int32_t>(base, te_at);
+    uint32_t *d_seeds = Layout::at<uint32_t>(base, seeds_at);
+    BoostJob *d_jobs = Layout::at<BoostJob>(base, jobs_at);
+    char *d_trees = Layout::at<char>(base, trees_at);
     // every active problem's trees, k inner
     std::vector<BoostJob> jobs;
     jobs.reserve(size_t(n_trees));
@@ -842,12 +846,12 @@ extern "C" int b200aa_boosting_scale(const double *d_X, int64_t n, int n_feats, 
         return B200AA_ERR_INVALID;
     const int64_t n_tr = h_train_off[n_problems], n_te = h_test_off[n_problems];
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    Layout A;
+    const size_t tr_at = A.add(size_t(n_tr) * 4), te_at = A.add(size_t(std::max<int64_t>(n_te, 1)) * 4);
     StreamScratch scratch(st);
-    const size_t b_tr = align256(size_t(n_tr) * 4);
-    const int rc = scratch.alloc(b_tr + align256(size_t(std::max<int64_t>(n_te, 1)) * 4));
+    const int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    int32_t *d_tr = static_cast<int32_t *>(scratch.get());
-    int32_t *d_te = reinterpret_cast<int32_t *>(static_cast<char *>(scratch.get()) + b_tr);
+    int32_t *d_tr = Layout::at<int32_t>(scratch.get(), tr_at), *d_te = Layout::at<int32_t>(scratch.get(), te_at);
     CK(cudaMemcpyAsync(d_tr, h_train_idx, size_t(n_tr) * 4, cudaMemcpyHostToDevice, st));
     if (n_te) CK(cudaMemcpyAsync(d_te, h_test_idx, size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
     for (int64_t p = 0; p < n_problems; ++p) {
@@ -906,20 +910,18 @@ extern "C" int b200aa_boosting_count(const double *d_raw_test, int64_t n_problem
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * n_classes * n_classes * sizeof(int64_t), st));
     if (n_te == 0) return B200AA_OK;
-    // scratch: [prob | raw_off | test_off | trees | classes | y_test]
-    const size_t b_prob = align256(size_t(n_te) * 4), b_off = align256(size_t(n_problems) * 8),
-                 b_toff = align256(size_t(n_problems + 1) * 8), b_trees = align256(size_t(n_problems) * 4),
-                 b_cls = align256(size_t(n_problems) * forest::kMaxClasses * 4), b_y = align256(size_t(n_te) * 4);
+    Layout A;
+    const size_t prob_at = A.add(size_t(n_te) * 4), off_at = A.add(size_t(n_problems) * 8),
+                 toff_at = A.add(size_t(n_problems + 1) * 8), trees_at = A.add(size_t(n_problems) * 4),
+                 cls_at = A.add(size_t(n_problems) * forest::kMaxClasses * 4), y_at = A.add(size_t(n_te) * 4);
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(b_prob + b_off + b_toff + b_trees + b_cls + b_y);
+    const int rc = scratch.alloc(A.bytes());
     if (rc != B200AA_OK) return rc;
-    char *q = static_cast<char *>(scratch.get());
-    int32_t *d_prob = reinterpret_cast<int32_t *>(q); q += b_prob;
-    int64_t *d_off = reinterpret_cast<int64_t *>(q); q += b_off;
-    int64_t *d_toff = reinterpret_cast<int64_t *>(q); q += b_toff;
-    int32_t *d_trees = reinterpret_cast<int32_t *>(q); q += b_trees;
-    int32_t *d_cls = reinterpret_cast<int32_t *>(q); q += b_cls;
-    int32_t *d_y = reinterpret_cast<int32_t *>(q);
+    void *base = scratch.get();
+    int32_t *d_prob = Layout::at<int32_t>(base, prob_at);
+    int64_t *d_off = Layout::at<int64_t>(base, off_at), *d_toff = Layout::at<int64_t>(base, toff_at);
+    int32_t *d_trees = Layout::at<int32_t>(base, trees_at), *d_cls = Layout::at<int32_t>(base, cls_at);
+    int32_t *d_y = Layout::at<int32_t>(base, y_at);
     CK(cudaMemcpyAsync(d_prob, prob.data(), size_t(n_te) * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_off, raw_off.data(), size_t(n_problems) * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_toff, h_test_off, size_t(n_problems + 1) * 8, cudaMemcpyHostToDevice, st));

@@ -77,17 +77,17 @@ extern "C" int b200aa_standard_scale(const void *d_X, int dtype, int64_t n_mats,
     }
     // NumPy reduces over axis 0 along the axis of smaller stride: pairwise down each column of a column-major matrix
     const bool pairwise = D == 1 || row_stride < col_stride;
-    const size_t rows_b = align256(size_t(n_mats) * sizeof(int64_t));
-    std::vector<char> head(2 * rows_b, 0);
-    std::memcpy(head.data(), h_rows, size_t(n_mats) * sizeof(int64_t));
-    std::memcpy(head.data() + rows_b, h_out_off, size_t(n_mats) * sizeof(int64_t));
+    Layout L;
+    const size_t rows_at = L.add(size_t(n_mats) * sizeof(int64_t)), off_at = L.add(size_t(n_mats) * sizeof(int64_t));
+    std::vector<char> head(L.bytes(), 0);
+    std::memcpy(head.data() + rows_at, h_rows, size_t(n_mats) * sizeof(int64_t));
+    std::memcpy(head.data() + off_at, h_out_off, size_t(n_mats) * sizeof(int64_t));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StreamScratch scratch(st);
     const int rc = scratch.alloc(head.size());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const int64_t *d_rows = reinterpret_cast<const int64_t *>(base);
-    const int64_t *d_off = reinterpret_cast<const int64_t *>(base + rows_b);
+    void *base = scratch.get();
+    const int64_t *d_rows = Layout::at<const int64_t>(base, rows_at), *d_off = Layout::at<const int64_t>(base, off_at);
     CK(cudaMemcpyAsync(base, head.data(), head.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_bad, 0, size_t(n_mats) * sizeof(int32_t), st));
     const unsigned grid_y = unsigned(std::min<int64_t>(n_mats, 65535));
@@ -141,14 +141,15 @@ extern "C" int b200aa_outlier_columns(const double *d_X, int64_t n_rows, int n_f
     seg.n_feat = n_rows;
     seg.len = int64_t(D) * D;
     seg.kind = cluster::kBlock;
-    const size_t seg_b = align256(sizeof seg), dist_b = size_t(D) * D * sizeof(double);
+    Layout L;
+    const size_t seg_at = L.add(sizeof seg), dist_at = L.add(size_t(D) * D * sizeof(double));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(seg_b + dist_b);
+    const int rc = scratch.alloc(L.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const cluster::Segment *d_seg = reinterpret_cast<const cluster::Segment *>(base);
-    double *dist = reinterpret_cast<double *>(base + seg_b);
+    void *base = scratch.get();
+    const cluster::Segment *d_seg = Layout::at<const cluster::Segment>(base, seg_at);
+    double *dist = Layout::at<double>(base, dist_at);
     CK(cudaMemcpyAsync(base, &seg, sizeof seg, cudaMemcpyHostToDevice, st));
     cluster_dist_kernel<<<unsigned(cluster::tiles_of(seg)), cluster::kThreads, 0, st>>>(d_seg, 0, 1, d_X, int(col_stride),
                                                                                        dist);

@@ -181,14 +181,16 @@ int hmm_decode(const T *d_mid, int64_t n_clips, int n_feats, int64_t m_stride, c
     cuts.push_back(n_clips);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t smem = 2 * size_t(n_states) * sizeof(double);
-    const size_t clips_b = align256(clips.size() * sizeof(int64_t)), e_b = align256(size_t(max_rows) * n_states * sizeof(double));
+    Layout L;
+    const size_t clips_at = L.add(clips.size() * sizeof(int64_t)), e_at = L.add(size_t(max_rows) * n_states * sizeof(double)),
+                 bp_at = L.add(size_t(max_rows) * n_states * sizeof(int32_t));
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(clips_b + e_b + size_t(max_rows) * n_states * sizeof(int32_t));
+    const int rc = scratch.alloc(L.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const int64_t *d_clips = reinterpret_cast<const int64_t *>(base);
-    double *e = reinterpret_cast<double *>(base + clips_b);
-    int32_t *bp = reinterpret_cast<int32_t *>(base + clips_b + e_b);
+    void *base = scratch.get();
+    const int64_t *d_clips = Layout::at<const int64_t>(base, clips_at);
+    double *e = Layout::at<double>(base, e_at);
+    int32_t *bp = Layout::at<int32_t>(base, bp_at);
     CK(cudaMemcpyAsync(base, clips.data(), clips.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_bad, 0, size_t(n_clips) * sizeof(int32_t), st));
     for (size_t s = 0; s + 1 < cuts.size(); ++s) {

@@ -323,37 +323,37 @@ extern "C" int b200aa_knn_cross_validate(const double *d_X, const int32_t *d_y, 
     }
     slices.push_back(cur);
 
-    // scratch: [items | training indices | test indices] uploaded once, then one slice's matrices, slots, classes, keys
-    size_t train_b = 0, query_b = 0, slots_b = 0, truth_b = 0, keys_b = 0;
+    // the items and the training and test indices, uploaded once as one head
+    Layout L;
+    const size_t items_at = L.add(items.size() * sizeof(knn::Problem)), tr_at = L.add(size_t(n_train_all) * sizeof(int32_t)),
+                 te_at = L.add(size_t(n_test_all) * sizeof(int32_t));
+    std::vector<char> head(te_at + size_t(n_test_all) * sizeof(int32_t));
+    std::memcpy(head.data() + items_at, items.data(), items.size() * sizeof(knn::Problem));
+    std::memcpy(head.data() + tr_at, h_train_idx, size_t(n_train_all) * sizeof(int32_t));
+    std::memcpy(head.data() + te_at, h_test_idx, size_t(n_test_all) * sizeof(int32_t));
+    // then one slice's matrices, slots, classes and keys, each sized by the largest slice
+    int64_t train_rows = 0, query_rows = 0, n_keys = 0;
     for (const CvSlice &s : slices) {
-        train_b = std::max(train_b, align256(size_t(s.train_rows) * n_feats * sizeof(double)));
-        query_b = std::max(query_b, align256(size_t(s.query_rows) * n_feats * sizeof(double)));
-        slots_b = std::max(slots_b, align256(size_t(s.train_rows) * sizeof(int32_t)));
-        truth_b = std::max(truth_b, align256(size_t(s.query_rows) * sizeof(int32_t)));
-        keys_b = std::max(keys_b, align256(size_t(s.keys) * sizeof(uint64_t)));
+        train_rows = std::max(train_rows, s.train_rows);
+        query_rows = std::max(query_rows, s.query_rows);
+        n_keys = std::max(n_keys, s.keys);
     }
-    const size_t items_b = align256(items.size() * sizeof(knn::Problem));
-    const size_t tr_b = align256(size_t(n_train_all) * sizeof(int32_t)), te_b = size_t(n_test_all) * sizeof(int32_t);
-    std::vector<char> blob(items_b + tr_b + te_b);
-    std::memcpy(blob.data(), items.data(), items.size() * sizeof(knn::Problem));
-    std::memcpy(blob.data() + items_b, h_train_idx, size_t(n_train_all) * sizeof(int32_t));
-    std::memcpy(blob.data() + items_b + tr_b, h_test_idx, te_b);
+    const size_t train_at = L.add(size_t(train_rows) * n_feats * sizeof(double)),
+                 query_at = L.add(size_t(query_rows) * n_feats * sizeof(double)),
+                 slots_at = L.add(size_t(train_rows) * sizeof(int32_t)), truth_at = L.add(size_t(query_rows) * sizeof(int32_t)),
+                 keys_at = L.add(size_t(n_keys) * sizeof(uint64_t));
 
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t head_b = align256(blob.size());
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(head_b + train_b + query_b + slots_b + truth_b + keys_b);
+    const int rc = scratch.alloc(L.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const knn::Problem *d_items = reinterpret_cast<const knn::Problem *>(base);
-    const int32_t *d_tr = reinterpret_cast<const int32_t *>(base + items_b);
-    const int32_t *d_te = reinterpret_cast<const int32_t *>(base + items_b + tr_b);
-    double *train = reinterpret_cast<double *>(base + head_b);
-    double *query = reinterpret_cast<double *>(base + head_b + train_b);
-    int32_t *slots = reinterpret_cast<int32_t *>(base + head_b + train_b + query_b);
-    int32_t *truth = reinterpret_cast<int32_t *>(base + head_b + train_b + query_b + slots_b);
-    uint64_t *keys = reinterpret_cast<uint64_t *>(base + head_b + train_b + query_b + slots_b + truth_b);
-    CK(cudaMemcpyAsync(base, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+    void *base = scratch.get();
+    const knn::Problem *d_items = Layout::at<const knn::Problem>(base, items_at);
+    const int32_t *d_tr = Layout::at<const int32_t>(base, tr_at), *d_te = Layout::at<const int32_t>(base, te_at);
+    double *train = Layout::at<double>(base, train_at), *query = Layout::at<double>(base, query_at);
+    int32_t *slots = Layout::at<int32_t>(base, slots_at), *truth = Layout::at<int32_t>(base, truth_at);
+    uint64_t *keys = Layout::at<uint64_t>(base, keys_at);
+    CK(cudaMemcpyAsync(base, head.data(), head.size(), cudaMemcpyHostToDevice, st));
     CK(cudaMemsetAsync(d_counts, 0, size_t(n_problems) * n_classes * n_classes * sizeof(int64_t), st));
 
     KnnVotes out{};

@@ -284,19 +284,19 @@ extern "C" int b200aa_music_thumbnail(const double *d_X, int n_feats, int64_t x_
 
     // slices of whole tracks whose S and NaN windows fit kScratchSliceBytes; a larger track is a slice of its own
     std::vector<int64_t> cut(1, 0);
-    size_t slice_b = 0, max_slice_b = 0;
+    Layout slice_l;
+    size_t largest_slice = 0;
     for (int64_t b = 0; b < n_tracks; ++b) {
         Track &t = tracks[size_t(b)];
-        const size_t sb = sim_only ? 0 : align256(size_t(t.T * t.T) * sizeof(double));
-        const size_t hb = sim_only ? 0 : align256(size_t(t.T * t.R));
-        if (b > cut.back() && (slice_b + sb + hb > kScratchSliceBytes || b - cut.back() == 65535)) {
+        const size_t sb = sim_only ? 0 : size_t(t.T * t.T) * sizeof(double), hb = sim_only ? 0 : size_t(t.T * t.R);
+        if (b > cut.back() && (slice_l.bytes() + align256(sb) + align256(hb) > kScratchSliceBytes || b - cut.back() == 65535)) {
             cut.push_back(b);
-            slice_b = 0;
+            slice_l = Layout();
         }
-        t.s0 = sim_only ? t.c0 : int64_t(slice_b / sizeof(double));
-        t.h0 = int64_t(slice_b + sb);
-        slice_b += sb + hb;
-        max_slice_b = std::max(max_slice_b, slice_b);
+        const size_t s_at = slice_l.add(sb);
+        t.s0 = sim_only ? t.c0 : int64_t(s_at / sizeof(double));
+        t.h0 = int64_t(slice_l.add(hb));
+        largest_slice = std::max(largest_slice, slice_l.bytes());
     }
     cut.push_back(n_tracks);
     int64_t max_part = 0;
@@ -307,25 +307,26 @@ extern "C" int b200aa_music_thumbnail(const double *d_X, int n_feats, int64_t x_
         max_part = std::max(max_part, n * blocks_per_track((maxR * maxR + thumb::kMaskThreads - 1) / thumb::kMaskThreads, n));
     }
 
-    // scratch: [tracks | norms | NaN flags | min keys | argmax parts | a slice's S and NaN windows]
-    const size_t tracks_b = align256(tracks.size() * sizeof(Track)), nrm_b = align256(size_t(rows) * sizeof(double));
-    const size_t flag_b = align256(size_t(n_tracks) * sizeof(int32_t)), key_b = align256(size_t(n_tracks) * sizeof(uint64_t));
-    const size_t part_b = sim_only ? 0 : align256(size_t(max_part) * sizeof(Best));
+    // the memsets of the NaN flags and min keys cover their regions' padding too
+    Layout L;
+    const size_t tracks_at = L.add(tracks.size() * sizeof(Track)), nrm_at = L.add(size_t(rows) * sizeof(double)),
+                 flag_at = L.add(size_t(n_tracks) * sizeof(int32_t)), key_at = L.add(size_t(n_tracks) * sizeof(uint64_t)),
+                 part_at = L.add(sim_only ? 0 : size_t(max_part) * sizeof(Best)), slice_at = L.add(largest_slice);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     StreamScratch scratch(st);
-    const int rc = scratch.alloc(tracks_b + nrm_b + flag_b + key_b + part_b + max_slice_b);
+    const int rc = scratch.alloc(L.bytes());
     if (rc != B200AA_OK) return rc;
-    char *base = static_cast<char *>(scratch.get());
-    const Track *d_tracks = reinterpret_cast<const Track *>(base);
-    double *nrm = reinterpret_cast<double *>(base + tracks_b);
-    int32_t *flag = reinterpret_cast<int32_t *>(base + tracks_b + nrm_b);
-    unsigned long long *keys = reinterpret_cast<unsigned long long *>(base + tracks_b + nrm_b + flag_b);
-    Best *part = reinterpret_cast<Best *>(base + tracks_b + nrm_b + flag_b + key_b);
-    char *slice = base + tracks_b + nrm_b + flag_b + key_b + part_b;
+    void *base = scratch.get();
+    const Track *d_tracks = Layout::at<const Track>(base, tracks_at);
+    double *nrm = Layout::at<double>(base, nrm_at);
+    int32_t *flag = Layout::at<int32_t>(base, flag_at);
+    unsigned long long *keys = Layout::at<unsigned long long>(base, key_at);
+    Best *part = Layout::at<Best>(base, part_at);
+    char *slice = Layout::at<char>(base, slice_at);
     double *S = sim_only ? d_sim : reinterpret_cast<double *>(slice);
     CK(cudaMemcpyAsync(base, tracks.data(), tracks.size() * sizeof(Track), cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(flag, 0, flag_b, st));
-    CK(cudaMemsetAsync(keys, 0xff, key_b, st));
+    CK(cudaMemsetAsync(flag, 0, key_at - flag_at, st));
+    CK(cudaMemsetAsync(keys, 0xff, part_at - key_at, st));
     thumb_norm_kernel<<<unsigned(std::min<int64_t>((rows + 255) / 256, 1 << 16)), 256, 0, st>>>(d_X, x_stride, F, rows, nrm);
     CK_LAUNCH("thumb_norm_kernel");
     for (size_t s = 0; s + 1 < cut.size(); ++s) {

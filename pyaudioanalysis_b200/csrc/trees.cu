@@ -115,25 +115,27 @@ extern "C" int b200aa_trees_create(b200aa_trees **out, const b200aa_tree_node *h
     }
     if (trees::warp_bytes(n_feats, n_classes) * kTreeWarps > 48 * 1024) return B200AA_ERR_UNSUPPORTED;
     const size_t vals = size_t(n_leaves) * (mode == trees::kForestMean ? size_t(n_classes) : 1);
-    const size_t nodes_b = align256(size_t(n_nodes) * sizeof(trees::Node)), roots_b = align256(size_t(n_trees) * sizeof(int32_t));
     const bool has_init = mode == trees::kBoostSum;         // a forest's sums start at 0: h_init is not read
-    const size_t values_b = align256(vals * sizeof(double)), init_b = has_init ? size_t(n_classes) * sizeof(double) : 0;
+    Layout L;
+    const size_t nodes_at = L.add(size_t(n_nodes) * sizeof(trees::Node)), roots_at = L.add(size_t(n_trees) * sizeof(int32_t)),
+                 values_at = L.add(vals * sizeof(double)), init_at = L.add(has_init ? size_t(n_classes) * sizeof(double) : 0);
     std::unique_ptr<b200aa_trees> m(new b200aa_trees{});
     CK(cudaGetDevice(&m->device));
-    CK(cudaMalloc(&m->blob, nodes_b + roots_b + values_b + init_b));
+    CK(cudaMalloc(&m->blob, L.bytes()));
     char *base = static_cast<char *>(m->blob);
     // The upload goes through a stream of its own and is waited for, so the model is on the device when create returns:
     // a copy from pageable memory may return before its DMA lands, and a caller's non-blocking stream is not ordered
     // after the legacy default stream.
     cudaStream_t up = nullptr;
     cudaError_t e = cudaStreamCreateWithFlags(&up, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(base, h_nodes, size_t(n_nodes) * sizeof(trees::Node), cudaMemcpyHostToDevice, up);
     if (e == cudaSuccess)
-        e = cudaMemcpyAsync(base + nodes_b, h_roots, size_t(n_trees) * sizeof(int32_t), cudaMemcpyHostToDevice, up);
+        e = cudaMemcpyAsync(base + nodes_at, h_nodes, size_t(n_nodes) * sizeof(trees::Node), cudaMemcpyHostToDevice, up);
     if (e == cudaSuccess)
-        e = cudaMemcpyAsync(base + nodes_b + roots_b, h_values, vals * sizeof(double), cudaMemcpyHostToDevice, up);
+        e = cudaMemcpyAsync(base + roots_at, h_roots, size_t(n_trees) * sizeof(int32_t), cudaMemcpyHostToDevice, up);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(base + values_at, h_values, vals * sizeof(double), cudaMemcpyHostToDevice, up);
     if (e == cudaSuccess && has_init)
-        e = cudaMemcpyAsync(base + nodes_b + roots_b + values_b, h_init, init_b, cudaMemcpyHostToDevice, up);
+        e = cudaMemcpyAsync(base + init_at, h_init, size_t(n_classes) * sizeof(double), cudaMemcpyHostToDevice, up);
     if (up) {
         const cudaError_t es = cudaStreamSynchronize(up);
         if (e == cudaSuccess) e = es;
@@ -150,10 +152,10 @@ extern "C" int b200aa_trees_create(b200aa_trees **out, const b200aa_tree_node *h
     m->n_feats = n_feats;
     m->mode = mode;
     m->allow_nan = allow_nan ? 1 : 0;
-    m->nodes = reinterpret_cast<const trees::Node *>(base);
-    m->roots = reinterpret_cast<const int32_t *>(base + nodes_b);
-    m->values = reinterpret_cast<const double *>(base + nodes_b + roots_b);
-    m->init = has_init ? reinterpret_cast<const double *>(base + nodes_b + roots_b + values_b) : nullptr;
+    m->nodes = Layout::at<const trees::Node>(base, nodes_at);
+    m->roots = Layout::at<const int32_t>(base, roots_at);
+    m->values = Layout::at<const double>(base, values_at);
+    m->init = has_init ? Layout::at<const double>(base, init_at) : nullptr;
     *out = m.release();
     return B200AA_OK;
 }
